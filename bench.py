@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- images/sec of a MobileViTv2-1.0 bf16 256x256 training step (BASELINE.json metric) on N B200s.
+"""bench.py -- images/sec of a MobileViTv2-1.0 bf16 256x256 training step (BASELINE.json metric) on N H100s.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--batch B] [--impl ours|reference]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P bench.py --gpus N ...
@@ -13,6 +13,8 @@ step's images+labels copied from pinned host memory and the loss read back insid
 algorithmic bytes of the pointwise-conv GEMM kernel family (the dominant kernel) / their CUDA-event time vs measured HBM
 peak; ``cpu_baseline`` = the oracle (CPU restatement of the reference path) timed on a bounded sample on the host cores.
 ``--impl reference`` times that CPU path alone (the reference is pure Python/PyTorch; its nn.Module path == the oracle).
+``--dump-outputs DIR`` writes what the last step of the first timed region computed -- the loss and the updated parameters -- as
+float32 ``DIR/<name>.npy``; the inputs and the initial weights are seeded, so two builds can be compared output for output.
 """
 import argparse
 import json
@@ -62,11 +64,11 @@ def measured_peaks():
         with open(p) as f:
             d = json.load(f)
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s)"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md 'clocks line')."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, gpu_index=0):
         self.proc, self.lines, self.gpu = None, [], gpu_index
@@ -111,6 +113,27 @@ class ClockSampler:
         return {"sm_mhz": sm[len(sm) // 2] if sm else None, "sm_max_mhz": mx, "reasons": sorted(reasons), "samples": len(sm)}
 
 
+DUMP_MAX_PARAMS = 8 * 1024 * 1024  # 32 MB of float32: larger models dump a fixed seeded sample of their parameters
+
+
+def output_snapshot(loss, model):
+    """What a caller of the timed step receives: the step's loss and the updated parameters (flattened in model.parameters() order;
+    beyond DUMP_MAX_PARAMS elements, the same seeded sample of positions on every run)."""
+    with torch.no_grad():
+        flat = torch.cat([p.detach().float().flatten() for p in model.parameters()])
+        if flat.numel() > DUMP_MAX_PARAMS:
+            idx = torch.randperm(flat.numel(), generator=torch.Generator().manual_seed(0))[:DUMP_MAX_PARAMS].sort().values
+            flat = flat[idx.to(flat.device)]
+        return {"loss": loss.detach().float().reshape(1).clone(), "params": flat.clone()}
+
+
+def write_outputs(out_dir, outputs):
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in outputs.items():
+        np.save(os.path.join(out_dir, name + ".npy"), t.cpu().numpy().astype(np.float32))
+
+
 # ------------------------------------------------------------------------------------------------ CPU (reference) arm
 ALGO_MB_PER_IMAGE = {1.0: 190.8, 2.0: 380.5}  # SURVEY.md 8d: 3 x (sum of conv/linear in+out activation elements) x 2 B
 
@@ -121,7 +144,7 @@ def workload_config(width, B, world):
     return {"workload": f"MobileViTv2-{width:.1f} bf16 training step, synthetic ImageNet 256x256"
                         + (f" (BASELINE.json configs[{cfg_no}])" if cfg_no is not None else ""),
             "per_gpu_batch": B, "global_batch": B * world, "parallelism": f"dp{world}", "resolution": RES,
-            "l2": "activations per step (>7 GB at batch 128) exceed the 126 MB L2; no explicit flush"}
+            "l2": "activations per step (>7 GB at batch 128) exceed the 50 MB L2; no explicit flush"}
 
 
 def usable_cores():
@@ -508,9 +531,8 @@ def run_ours(args, rank, world, local_rank):
         optimer.install()
     sampler = ClockSampler(local_rank)
     # ---------------- timed region 1: inputs resident in HBM
-    # The sampler is started BEFORE the barrier: spawning nvidia-smi takes 10-100 ms of host time on rank 0; after the barrier that delay made
-    # every other rank wait at its first all-reduce inside ITS timed region (max over ranks then reported 33.3 ms/step for steps that took
-    # 27.9 ms on every rank -- the N = 8 inconsistency of round 1 as well).
+    # The sampler is started BEFORE the barrier: spawning nvidia-smi takes 10-100 ms of host time on rank 0; after the barrier that delay would
+    # make every other rank wait at its first all-reduce inside ITS timed region and inflate the max over ranks.
     if rank == 0:
         sampler.start()
     sync_all()
@@ -527,6 +549,7 @@ def run_ours(args, rank, world, local_rank):
         marks[i + 1].record()
     ev0, ev1 = marks[0], marks[-1]
     sync_all()
+    outputs = output_snapshot(loss, model) if args.dump_outputs else None
     per_step = sorted(marks[i].elapsed_time(marks[i + 1]) for i in range(args.steps))
     step_stats = {"min": per_step[0], "median": per_step[len(per_step) // 2], "p90": per_step[min(len(per_step) - 1, int(0.9 * len(per_step)))],
                   "max": per_step[-1], "note": "rank 0's CUDA-event time of each timed step"}
@@ -620,27 +643,17 @@ def run_ours(args, rank, world, local_rank):
                             "(includes ~5 us of event overhead per launch: a lower bound)", "bound": "hbm", "achieved": ach, "peak": peak,
                   "unit": "GB/s", "frac": ach / peak, "launches_per_step": n // nsteps_t, "kernel_ms_per_step": per_step_ms,
                   "share_of_step": per_step_ms / ms_step, "algorithmic_bytes_per_step": gbytes / nsteps_t, "tflops": gflops / (gms * 1e-3) / 1e12}
-    # The dominant "kernel" of this path is the step itself: ONE CUDA-graph launch per step (~370 kernel nodes, no kernel above 6 % of it).
+    # The dominant "kernel" of this path is the step itself: ONE CUDA-graph launch per step.
     # achieved = SURVEY.md 8d's algorithmic bytes per image x the images one launch processes / the launch's CUDA-event duration (the timed
-    # region above); traffic = DRAM bytes of one step summed over its kernels from the committed ncu launch list (profiles/step_dram.json).
+    # region above).
     algo_mb = ALGO_MB_PER_IMAGE.get(args.width)
     roof = None
     if algo_mb:
         algo_bytes = algo_mb * 1e6 * B
         ach = algo_bytes / (ms_step * 1e-3) / 1e9
-        traffic, traffic_src = None, None
-        try:
-            with open(os.path.join(ROOT, "profiles", "step_dram.json")) as f:
-                sd = json.load(f)
-            if abs(sd.get("width", 1.0) - args.width) < 1e-9 and sd.get("per_gpu_batch") == B:
-                traffic, traffic_src = sd["dram_bytes_per_step"], sd.get("source")
-        except Exception:
-            pass
         roof = {"kernel": ("one CUDA-graph launch = the whole training step" if use_graph else "the whole training step (eager launches)"),
                 "bound": "hbm", "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak, "peak_source": peak_src,
-                "algorithmic_bytes_per_launch": algo_bytes, "traffic": traffic,
-                "traffic_over_algorithmic": (traffic / algo_bytes) if traffic else None, "traffic_source": traffic_src,
-                "kernels_per_launch": launches // max(args.steps, 1)}
+                "algorithmic_bytes_per_launch": algo_bytes, "kernels_per_launch": launches // max(args.steps, 1)}
     cpu = None
     if not args.no_cpu_baseline and world == 1:
         r = cpu_training_throughput(args.width, 3, 1, budget_s=min(60.0, args.cpu_budget))
@@ -677,6 +690,8 @@ def run_ours(args, rank, world, local_rank):
         line["op_ms"] = op_ms
         if timer.records:
             line["gemm_shapes"] = timer.per_shape(3 if use_graph else args.steps)
+    if outputs is not None:
+        write_outputs(args.dump_outputs, outputs)
     emit(line)
 
 
@@ -780,6 +795,7 @@ def run_vit(args, rank, world, local_rank):
         loss = ts.step(x_dev, y_dev)
         marks[i + 1].record()
     sync_all()
+    outputs = output_snapshot(loss, model) if args.dump_outputs else None
     clocks = sampler.stop() if rank == 0 else None
     ms_step = max_over_ranks(marks[0].elapsed_time(marks[-1])) / args.steps
     per = sorted(marks[i].elapsed_time(marks[i + 1]) for i in range(args.steps))
@@ -810,7 +826,7 @@ def run_vit(args, rank, world, local_rank):
             peaks = json.load(f)
     except Exception:
         pass
-    peak_tf = float(peaks.get("bf16_tflops_sustained", 1440.0))
+    peak_tf = float(peaks.get("bf16_tflops_sustained", 989.0))  # fallback: H100 SXM data sheet, dense bf16
     gflop = (CLIP_GFLOP_PER_PAIR if clip else VIT_GFLOP_PER_IMAGE).get(mode)
     ach = (value / world) * gflop / 1e3 if gflop else None
     eager = None
@@ -820,6 +836,8 @@ def run_vit(args, rank, world, local_rank):
             eager["ours_over_eager"] = value / eager["value"]
         except Exception as e:
             eager = {"error": repr(e)[:300]}
+    if outputs is not None:
+        write_outputs(args.dump_outputs, outputs)
     emit({
         "metric": (f"image-text pairs/sec contrastive training step, CLIP ViT-{mode}/16 bf16 224x224" if clip else
                    f"images/sec training step, ViT-{mode}/16 bf16 224x224"), "value": value, "unit": "images/sec", "n_gpus": world, "steps": args.steps,
@@ -827,13 +845,13 @@ def run_vit(args, rank, world, local_rank):
         "config": {"workload": (f"CLIP ViT-{mode}/16 image + 12-layer text tower, contrastive loss with feature all-gather, fwd + bwd + clip + AdamW, "
                                 "synthetic pairs (BASELINE.json configs[4])" if clip else
                                 f"ViT-{mode}/16 bf16 forward + loss + backward + clip + AdamW, synthetic 224x224 (BASELINE.json configs[2])"), "per_gpu_batch": B,
-                   "global_batch": B * world, "parallelism": f"dp{world}", "resolution": 224, "l2": "activations per step (> 10 GB) exceed the 126 MB L2"},
+                   "global_batch": B * world, "parallelism": f"dp{world}", "resolution": 224, "l2": "activations per step (> 10 GB) exceed the 50 MB L2"},
         "step_ms": {"min": per[0], "median": per[len(per) // 2], "max": per[-1]}, "clocks": clocks,
         "e2e": {"value": world * B / (e2e_ms * 1e-3), "unit": "images/sec", "h2d_bytes_per_step": world * (hx.numel() * 4 + hy.numel() * 8), "d2h_bytes_per_step": world * 4,
                 "ms_per_step": e2e_ms},
         "gpu_launches": launches,
         "roofline": {"kernel": "whole step (one CUDA-graph launch): tensor-bound GEMMs + attention", "bound": "tensor", "achieved": ach, "peak": peak_tf,
-                     "unit": "TFLOP/s", "frac": (ach / peak_tf) if ach else None, "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained", "traffic": None,
+                     "unit": "TFLOP/s", "frac": (ach / peak_tf) if ach else None, "peak_source": ("MEASURED_PEAKS.json bf16_tflops_sustained" if "bf16_tflops_sustained" in peaks else "H100 SXM data sheet"), "traffic": None,
                      "algorithmic_gflop_per_image": gflop},
         "gpu_eager_baseline": eager, "loss": float(loss.detach()),
     })
@@ -858,6 +876,8 @@ def main():
     ap.add_argument("--buckets", type=int, default=3, help="gradient all-reduce buckets (N > 1)")
     ap.add_argument("--no-pdl", action="store_true", help="diagnostics: plain stream-ordered launches instead of programmatic dependent launch")
     ap.add_argument("--no-graph", action="store_true", help="run the step eagerly instead of replaying one captured CUDA graph (N=1)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the loss and the updated parameters of the last timed step as float32 DIR/<name>.npy (rank 0)")
     args = ap.parse_args()
     rank, world, local_rank = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1)), int(os.environ.get("LOCAL_RANK", 0))
     quiet_stdout()

@@ -1,5 +1,5 @@
 /*
- * cvnets_b200.h -- C ABI of libcvnets_b200.so: the sm_100a kernels behind the apple/ml-cvnets vision-backbone hot path.
+ * cvnets_b200.h -- C ABI of libcvnets_b200.so: the sm_90a kernels behind the apple/ml-cvnets vision-backbone hot path.
  *
  * The reference (apple/ml-cvnets) is pure Python and has NO native operator / FFI boundary (SURVEY.md 8b); its hot
  * path bottoms out in torch.nn.functional calls.  This header is therefore the boundary a maintainer would bind with
@@ -86,12 +86,12 @@ typedef struct {
   double* col_sum; double* col_sq;   /* fp64 [N] accumulators or NULL (BatchNorm statistics of the stored output) */
   double* samp_sum; double* samp_sq; /* fp64 [M/rows_per_sample] or NULL (GroupNorm statistics of the stored output) */
   double* gn_ws;            /* CVB_E_GN_BWD only, optional: ZEROED fp64 workspace [2][M/rows_per_sample][N].  When given (and
-                               rows_per_sample % 64 == 0) the epilogue runs on the tcgen05 kernel: it accumulates the per-(sample, channel)
+                               rows_per_sample % 64 == 0) the epilogue runs on the wgmma kernel: it accumulates the per-(sample, channel)
                                sums of v and v*x there and a finalize kernel derives col_sum/col_sq/samp_sum/samp_sq from them. */
 } cvb_gemm_args;
 CVB_API int cvb_pw_gemm(const cvb_gemm_args* args, cvb_stream_t stream);
-/* Two kernels implement cvb_pw_gemm (and two cvb_pw_wgrad): warp-specialised tcgen05/TMEM/TMA kernels (N >= 96 resp. K % 64 == 0)
- * and mma.sync kernels (narrow / odd shapes).  Testing hook: disable (0) / enable (1) the tcgen05 kernels so the two can be compared
+/* Two kernels implement cvb_pw_gemm (and two cvb_pw_wgrad): warp-specialised wgmma/TMA kernels (N >= 96 resp. K % 64 == 0)
+ * and mma.sync kernels (narrow / odd shapes).  Testing hook: disable (0) / enable (1) the wgmma kernels so the two can be compared
  * on identical inputs; returns the previous setting. */
 CVB_API int cvb_set_tc_enabled(int on);
 /* Every kernel is launched with programmatic dependent launch (its set-up overlaps the previous kernel's tail; the kernel
@@ -108,8 +108,8 @@ typedef struct {
   const void* A; int lda; int a_mode;
   const float* a_p0; const float* a_p1;                    /* per-K */
   const float* row_mean; const float* row_rstd; int rows_per_sample;
-  float* dW; int lddw; /* fp32 [N, lddw], atomically accumulated: caller zeroes */
-  float* dbias;        /* fp32 [N] or NULL, atomically accumulated */
+  float* dW; int lddw; /* fp32 [N, lddw], accumulated (+=): caller zeroes */
+  float* dbias;        /* fp32 [N] or NULL, accumulated (+=) */
 } cvb_wgrad_args;
 CVB_API int cvb_pw_wgrad(const cvb_wgrad_args* args, cvb_stream_t stream);
 
@@ -146,7 +146,7 @@ typedef struct {
   const float* Wt;
   void* DX;         /* bf16 [B,H,W,C] */
   double* col_sum; double* col_sq; /* may be NULL when x_mode == RAW */
-  float* dWt;       /* fp32 [9][C], atomically accumulated */
+  float* dWt;       /* fp32 [9][C], accumulated (+=) */
   int dilation;     /* 0 or 1: none */
 } cvb_dw_bwd_args;
 CVB_API int cvb_dw_bwd(const cvb_dw_bwd_args* args, cvb_stream_t stream);
@@ -240,16 +240,16 @@ CVB_API int cvb_linattn_cross_bwd(const void* QK_prev, int ldq, const void* V_x,
  * O: bf16 [B*S, ldo] with head h at columns h*c.. (the layout out_proj reads, :236).  scale = head_dim^-0.5 (:70, :187).
  * attn_mask: fp32 [B, S, S] additive (or NULL, :197-208); key_padding_mask: uint8 [B, S], non-zero = masked with -inf (:210-224).
  * Softmax in fp32 (:226-228).  LSE: fp32 [B, H, S] log-sum-exp (base 2) saved for the backward.  S <= 256, even c <= 64.
- * head_dim == 64 (ViT-B / CLIP image tower, key-padding masks included) runs on tcgen05 tensor cores (mha_tc.cu: TMA-staged operands, scores in
- * TMEM, one thread per query row); every other head_dim, and heads with an additive mask, on the mma.sync kernels (mha.cu).
+ * head_dim == 64 (ViT-B / CLIP image tower, key-padding masks included) runs on wgmma tensor cores (mha_tc.cu: TMA-staged operands, whole
+ * score rows in registers); every other head_dim, and heads with an additive mask, on the mma.sync kernels (mha.cu).
  * ------------------------------------------------------------------------------------------------------------- */
 CVB_API int cvb_mha_fwd(const void* QKV, int ldq, int B, int S, int H, int head_dim, float scale, const float* attn_mask,
                 const unsigned char* key_padding_mask, void* O, int ldo, float* LSE, cvb_stream_t stream);
 /* dQKV (bf16 [B*S, lddq], same column layout as QKV) from dO; recomputes the probabilities from LSE. */
 CVB_API int cvb_mha_bwd(const void* QKV, int ldq, const void* O, const void* DO, int ldo, const float* LSE, int B, int S, int H, int head_dim,
                 float scale, const float* attn_mask, const unsigned char* key_padding_mask, void* DQKV, int lddq, cvb_stream_t stream);
-/* Diagnostics / A-B timing: which head_dim == 64 implementation runs.  bit 0: tcgen05 forward, bit 1: tcgen05 backward, bit 2: tcgen05 also
- * for heads with an additive attn_mask (default 3: additive-mask heads -- the causal CLIP text tower, S = 77 -- measured faster on mma.sync;
+/* Diagnostics / A-B timing: which head_dim == 64 implementation runs.  bit 0: wgmma forward, bit 1: wgmma backward, bit 2: wgmma also
+ * for heads with an additive attn_mask (default 3: additive-mask heads -- the causal CLIP text tower, S = 77 -- stay on mma.sync;
  * the environment variable CVB_MHA_TC sets the initial value).  Returns the previous mask. */
 CVB_API int cvb_set_mha_impl(int mask);
 /* per-token LayerNorm statistics of a bf16 [M, C] matrix: mean[m], rstd[m] = 1/sqrt(var + eps) (biased variance, fp32 math like

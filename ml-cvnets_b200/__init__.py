@@ -1,5 +1,5 @@
 """ml-cvnets_b200: the apple/ml-cvnets vision-backbone hot path (MobileViTv2: InvertedResidual, MobileViTBlockv2,
-LinearSelfAttention, LinearAttnFFN, conv+BN+SiLU; plus the ViT-style MultiHeadAttention / TransformerEncoder / LayerNorm) as hand-written sm_100a CUDA kernels behind a C ABI
+LinearSelfAttention, LinearAttnFFN, conv+BN+SiLU; plus the ViT-style MultiHeadAttention / TransformerEncoder / LayerNorm) as hand-written sm_90a CUDA kernels behind a C ABI
 (include/cvnets_b200.h) with drop-in ``nn.Module``s on top.  Import name: ``ml_cvnets_b200`` (alias package at the repo root).
 """
 from . import _lib  # noqa: F401

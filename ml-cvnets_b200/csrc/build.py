@@ -1,4 +1,4 @@
-"""Build libcvnets_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libcvnets_b200.so in-tree with nvcc for sm_90a (cross-compiles without a GPU).
 
     python ml-cvnets_b200/csrc/build.py [--force] [--verbose]
 """
@@ -12,7 +12,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 SOURCES = ["gemm.cu", "gemm_tc.cu", "wgrad_tc.cu", "dwconv.cu", "dwconv_dilated.cu", "norm.cu", "linattn.cu", "mha.cu", "mha_tc.cu", "optim.cu", "loss.cu", "conv.cu", "clip.cu", "se.cu", "dropout.cu"]
 LIB = os.path.join(HERE, "libcvnets_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "--use_fast_math",
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+FLAGS = ARCH + ["-O3", "-lineinfo", "-std=c++17", "--use_fast_math",
          "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--expt-relaxed-constexpr"]
 
 
@@ -43,7 +44,7 @@ def build(force=False, verbose=False):
 
     with ThreadPoolExecutor(max_workers=min(8, len(SOURCES))) as ex:
         objs = list(ex.map(compile_one, SOURCES))
-    cmd = [NVCC, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-lcudart"]
+    cmd = [NVCC, "-shared", "-o", LIB] + objs + ARCH + ["-lcudart"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError("link failed:\n%s\n%s" % (r.stdout, r.stderr))

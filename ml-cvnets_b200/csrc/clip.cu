@@ -1,4 +1,4 @@
-// CLIP text tower edges and feature normalisation (BASELINE.json configs[4]; SURVEY.md 8f row 2), sm_100a.
+// CLIP text tower edges and feature normalisation (BASELINE.json configs[4]; SURVEY.md 8f row 2), sm_90a.
 //   cvb_embedding_{fwd,bwd} : token embedding + learnable positional embedding (cvnets/text_encoders/transformer.py:328-341,
 //                             cvnets/layers/embedding.py, positional_embedding.py:53-110)
 //   cvb_eot_gather_{fwd,bwd}: features of the end-of-text token = the highest token id of each sequence (transformer.py:413-421)

@@ -1,4 +1,4 @@
-// Shared device/host helpers for libcvnets_b200 (sm_100a only).
+// Shared device/host helpers for libcvnets_b200 (sm_90a only).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -8,8 +8,8 @@
 
 #include "../../include/cvnets_b200.h"
 
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 1000)
-#error "libcvnets_b200 targets sm_100a (B200) only"
+#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ != 900)
+#error "libcvnets_b200 targets sm_90a (H100) only"
 #endif
 
 typedef __nv_bfloat16 bf16;
@@ -37,10 +37,17 @@ void cvb_set_error(const char* fmt, ...);
 
 static inline bool cvb_aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 int cvb_num_sms();
+// Order-independent gradient accumulation.  Partial sums that many CTAs (or warps) contribute are added in fp64: the few fp32 addends of
+// one element sum exactly there, so the result does not depend on the order in which they arrive and two runs of a step are bitwise equal.
+// cvb_det_alloc: zeroed fp64 scratch of n elements (stream-ordered, capturable); cvb_det_add: dst[r * ld + c] += scratch[r * cols + c];
+// cvb_det_free: release it after the adds.
+int cvb_det_alloc(double** scratch, size_t n, cudaStream_t st);
+int cvb_det_add(const double* scratch, float* dst, int rows, int cols, int ld, cudaStream_t st);
+int cvb_det_free(double* scratch, cudaStream_t st);
 
 // ---------------------------------------------------------------------------------------------- small device helpers
 // SiLU through ONE special-function op: sigmoid(z) = 0.5 + 0.5 tanh(z/2) with tanh.approx.f32 (MUFU.TANH, max abs error 2^-11), instead of
-// ex2 + rcp (two MUFU ops: 16 / clk / SM on B200, which made the SiLU of a 268 M-element tensor cost ~120 us of MUFU pipe alone).  The
+// ex2 + rcp (two MUFU ops at 16 / clk / SM: the SiLU of a large activation tensor would be bound by the MUFU pipe).  The
 // absolute error of silu is <= |z| * 2.5e-4 -- below bf16 resolution of every value that is not itself negligible.  -DCVB_SILU_EXP=1
 // restores the exp formulation (A/B and accuracy checks).
 #ifndef CVB_SILU_EXP
@@ -81,28 +88,11 @@ __device__ __forceinline__ float2 unpack_bf162(uint32_t u) {
   bf162 v = *reinterpret_cast<bf162*>(&u);
   return __bfloat1622float2(v);
 }
-// packed fp32 arithmetic on a register pair (sm_100: FFMA2 / FMUL2 / FADD2): halves the issue slots of pair-wise fp32 math
-__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
-  float2 r;
-  asm("{ .reg .b64 a,b,c,d; mov.b64 a,{%2,%3}; mov.b64 b,{%4,%5}; mov.b64 c,{%6,%7}; fma.rn.f32x2 d,a,b,c; mov.b64 {%0,%1}, d; }"
-      : "=f"(r.x), "=f"(r.y)
-      : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y), "f"(c.x), "f"(c.y));
-  return r;
-}
-__device__ __forceinline__ float2 fmul2(float2 a, float2 b) {
-  float2 r;
-  asm("{ .reg .b64 a,b,d; mov.b64 a,{%2,%3}; mov.b64 b,{%4,%5}; mul.rn.f32x2 d,a,b; mov.b64 {%0,%1}, d; }"
-      : "=f"(r.x), "=f"(r.y)
-      : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y));
-  return r;
-}
-__device__ __forceinline__ float2 fadd2(float2 a, float2 b) {
-  float2 r;
-  asm("{ .reg .b64 a,b,d; mov.b64 a,{%2,%3}; mov.b64 b,{%4,%5}; add.rn.f32x2 d,a,b; mov.b64 {%0,%1}, d; }"
-      : "=f"(r.x), "=f"(r.y)
-      : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y));
-  return r;
-}
+// fp32 arithmetic on a register pair.  Hopper has no packed f32x2 instructions: these are two scalar ops each, with the same
+// round-to-nearest results (fma stays fused), so callers written for pairs keep their numerics.
+__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
+__device__ __forceinline__ float2 fmul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 fadd2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
 // 8 bf16 <-> 8 floats
 __device__ __forceinline__ void unpack8(const uint4& u, float* f) {
   float2 a = unpack_bf162(u.x), b = unpack_bf162(u.y), c = unpack_bf162(u.z), d = unpack_bf162(u.w);
@@ -170,7 +160,7 @@ __device__ __forceinline__ float apply_mode(int mode, float x, float p0, float p
 
 // ---------------------------------------------------------------------------------------------- programmatic dependent launch
 // Every kernel of the library is launched with the programmatic-stream-serialization attribute: its CTAs may become resident
-// while the previous kernel in the stream is still draining, run their private set-up (mbarrier init, TMEM allocation,
+// while the previous kernel in the stream is still draining, run their private set-up (mbarrier init,
 // tensor-map prefetch), and block in pdl_wait() until the previous grid has completed and flushed its memory.  RULES: nothing
 // produced by an earlier kernel is read, and no global memory is written, before pdl_wait(); every kernel executes
 // pdl_wait() in every thread (so "grid B complete" always implies "grid A complete" along the stream).
@@ -193,7 +183,7 @@ static inline cudaError_t cvb_launch(void (*kernel)(KArgs...), dim3 grid, dim3 b
   return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
 
-// ---------------------------------------------------------------------------------------------- TMA + mbarrier (sm_90+/sm_100a)
+// ---------------------------------------------------------------------------------------------- TMA + mbarrier (sm_90a)
 #include <cuda.h>  // CUtensorMap (types only; the encoder is fetched through cudaGetDriverEntryPoint, no -lcuda)
 
 // Host: tensor map of a channels-last bf16 feature map [B, H, W, C] with a [1, boxH, boxW, boxC] box (boxC * 2 bytes <= 128),
@@ -202,7 +192,7 @@ int cvb_make_tmap_nhwc(CUtensorMap* map, const void* base, int B, int H, int W, 
 // Host: tensor map of a row-major bf16 matrix [rows, cols] (leading dimension ld elements) with a [box_rows, 32 cols] box and
 // 64-byte swizzle: the shared-memory image is exactly the 64-byte-row XOR layout (swz64) the GEMM's ldmatrix addressing uses.
 int cvb_make_tmap_2d_k32(CUtensorMap* map, const void* base, int64_t rows, int cols, int ld, int box_rows);
-// Same matrix view with a [box_rows, 64 cols] box and 128-byte swizzle: the image is the canonical MN-major SWIZZLE_128B UMMA
+// Same matrix view with a [box_rows, 64 cols] box and 128-byte swizzle: the image is the canonical MN-major SWIZZLE_128B wgmma
 // operand layout (8-row x 128-byte atoms) when the ROWS are the reduction dimension (weight-gradient GEMM).
 int cvb_make_tmap_2d_c64(CUtensorMap* map, const void* base, int64_t rows, int cols, int ld, int box_rows);
 
@@ -233,6 +223,71 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
                "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(col), "r"(row)
                : "memory");
 }
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory"); }
+
+// ---------------------------------------------------------------------------------------------- wgmma (sm_90a warpgroup MMA)
+// Shared-memory matrix descriptor: start address, leading / stride byte offsets (16-byte units), layout type in bits [62,64)
+// (1 = 128-byte swizzle, 2 = 64-byte swizzle).  K-major swizzled operands ignore the leading offset; MN-major SWIZZLE_128B
+// operands use it as the distance between 64-element groups of the M/N dimension and the stride offset between 8-row k groups.
+enum { WG_SW128 = 1, WG_SW64 = 2 };
+__device__ __forceinline__ uint64_t wgmma_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes, int layout) {
+  uint64_t d = 0;
+  d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
+  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
+  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
+  d |= (uint64_t)layout << 62;
+  return d;
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keep the accumulator registers live and ordered around the asynchronous MMAs
+template <int R>
+__device__ __forceinline__ void wgmma_reg_fence(float* d) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// D[64 x N] (+)= A[64 x 16] * B[16 x N], bf16 operands from shared memory, fp32 accumulator in registers (N / 2 per thread).
+// TA / TB: operand is MN-major (transposed) instead of K-major.  Accumulator fragment: thread t of the warpgroup holds, for every
+// 8-column block j, rows 16 (t / 32) + (t % 32) / 4 (+ 8 for the odd pair) and columns 8 j + 2 (t % 4) + {0, 1}.
+#define CVB_WG_R8(b) "+f"(d[b + 0]), "+f"(d[b + 1]), "+f"(d[b + 2]), "+f"(d[b + 3]), "+f"(d[b + 4]), "+f"(d[b + 5]), "+f"(d[b + 6]), "+f"(d[b + 7])
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n64(float* d, uint64_t da, uint64_t db, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, "
+      "%32, %33, p, 1, 1, %35, %36;\n\t}"
+      : CVB_WG_R8(0), CVB_WG_R8(8), CVB_WG_R8(16), CVB_WG_R8(24)
+      : "l"(da), "l"(db), "r"(accumulate), "n"(TA), "n"(TB));
+}
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n128(float* d, uint64_t da, uint64_t db, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
+      "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, "
+      "%64, %65, p, 1, 1, %67, %68;\n\t}"
+      : CVB_WG_R8(0), CVB_WG_R8(8), CVB_WG_R8(16), CVB_WG_R8(24), CVB_WG_R8(32), CVB_WG_R8(40), CVB_WG_R8(48), CVB_WG_R8(56)
+      : "l"(da), "l"(db), "r"(accumulate), "n"(TA), "n"(TB));
+}
+// Same with A [64 x 16] from registers: a[0..3] = bf16 pairs (row g, cols 2t..), (g + 8, 2t..), (g, 2t + 8..), (g + 8, 2t + 8..) of warp w's
+// 16 rows, g = lane / 4, t = lane % 4 -- i.e. accumulator columns 16 kk .. 16 kk + 15 of an m64nN result, packed, feed k-step kk directly.
+template <int TB>
+__device__ __forceinline__ void wgmma_m64n64_rs(float* d, const uint32_t* a, uint64_t db, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, "
+      "{%32,%33,%34,%35}, %36, p, 1, 1, %38;\n\t}"
+      : CVB_WG_R8(0), CVB_WG_R8(8), CVB_WG_R8(16), CVB_WG_R8(24)
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate), "n"(TB));
+}
+#undef CVB_WG_R8
+
 // 4-D tiled TMA load: coordinates innermost first (c, w, h, b); completes `bytes of the box` on the mbarrier
 __device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c, int w, int h, int b) {
   asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];" ::"r"(

@@ -1,4 +1,4 @@
-// Dense (groups = 1) k x k convolution as im2col + the pointwise GEMM, and the ViT token assembly (sm_100a).
+// Dense (groups = 1) k x k convolution as im2col + the pointwise GEMM, and the ViT token assembly (sm_90a).
 //
 // The MobileViTv2 path has exactly one dense k x k conv (the stem, cvb_stem_im2col).  The other hot-path models need a few more:
 // the ViT / CLIP conv stem ("patch embedding": 4x4 s4 p1, 2x2 s2, 2x2 s2 -- cvnets/models/classification/vit.py:90-121) and

@@ -1,5 +1,5 @@
 // Dropout / stochastic depth on the residual stream (cvnets/layers/dropout.py == nn.Dropout; torchvision.ops.StochasticDepth(mode="row") as used by
-// cvnets/modules/transformer.py:97-100,139-156), sm_100a.
+// cvnets/modules/transformer.py:97-100,139-156), sm_90a.
 //
 //   forward   Y[m, c] = R[m, c] + V[m, c] * e(m, c) * r(m / rows_per_sample)        (R optional)
 //   backward  DV[m, c] = DY[m, c] * e(m, c) * r(...)                                   (the gradient of R is DY itself)

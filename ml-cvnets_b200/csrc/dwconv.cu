@@ -1,11 +1,11 @@
-// Depthwise 3x3 convolution (pad 1, stride 1|2), NHWC bf16, forward and fused backward (sm_100a).
+// Depthwise 3x3 convolution (pad 1, stride 1|2), NHWC bf16, forward and fused backward (sm_90a).
 //
 // HBM-bound stencils whose first implementation was instruction-issue bound (~85 instructions per element).  This version is
 // built around the instruction count:
 //   * a warp spans the CTA's 64 channels (lane = channel pair, one 4-byte bf16x2 access per lane = one conflict-free 128-byte
 //     shared-memory wavefront per warp) and WALKS along a strip of pixels, keeping the 3x3 neighbourhood of the strip's rows in
 //     registers (sliding window: each neighbour is loaded (R+2)/R times instead of 9);
-//   * all arithmetic is packed fp32 (FFMA2 = fma.rn.f32x2 on the channel pair), weights / dW accumulators / BN statistics stay in
+//   * all arithmetic is fp32 on channel pairs (ffma2 / fmul2 helpers), weights / dW accumulators / BN statistics stay in
 //     registers for the whole batch loop of the CTA;
 //   * backward: for every INPUT pixel p the same neighbourhood dy[p - tap] feeds both products,
 //         dX[p] = sum_t W[t] * dy[p - t]        dW[t] += act(x[p]) * dy[p - t],
@@ -59,7 +59,7 @@ __device__ __forceinline__ void transform_tile(uint8_t* tile, int TH_, int TW_, 
       const uint32_t rw[4] = {raw.x, raw.y, raw.z, raw.w};
       uint32_t ow[4];
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {  // packed fp32 pairs: 2 FFMA2 + 2 MUFU per channel pair
+      for (int j = 0; j < 4; ++j) {  // fp32 channel pairs: 2 ffma2 + 2 MUFU per channel pair
         float2 z = ffma2(make_float2(sc[2 * j], sc[2 * j + 1]), up2(rw[j]), make_float2(sh[2 * j], sh[2 * j + 1]));
         if (XMODE == CVB_A_AFF_SILU) {
 #if CVB_SILU_EXP
@@ -85,7 +85,7 @@ __global__ void __launch_bounds__(NT, 2) dw_fwd_kernel(const __grid_constant__ C
   constexpr int WR = (S == 1) ? 4 : 3;  // window rows
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  __shared__ float s_cs[CB], s_cq[CB];
+  __shared__ double s_cs[CB], s_cq[CB];  // fp64: the warps' fp32 partials sum exactly, whatever their order
   __shared__ __align__(16) float s_xp[2 * CB];
   __shared__ __align__(8) uint64_t bar[2];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -97,7 +97,7 @@ __global__ void __launch_bounds__(NT, 2) dw_fwd_kernel(const __grid_constant__ C
   const uint32_t tile_bytes = (uint32_t)IH * IW * 128;
   const int n_img = (p.B - (int)blockIdx.z + (int)gridDim.z - 1) / (int)gridDim.z;
 
-  if (tid < CB) { s_cs[tid] = 0.f; s_cq[tid] = 0.f; }
+  if (tid < CB) { s_cs[tid] = 0.0; s_cq[tid] = 0.0; }
   if (tid == 0) {
     mbar_init(&bar[0], 1);
     mbar_init(&bar[1], 1);
@@ -138,7 +138,7 @@ __global__ void __launch_bounds__(NT, 2) dw_fwd_kernel(const __grid_constant__ C
     }
     bf16* __restrict__ Y = static_cast<bf16*>(p.Y) + (size_t)b * Ho * Wo * p.C + cl;
     // interior tiles (every output pixel and channel of the tile exists): no per-pixel predicates, statistics straight from the fp32
-    // accumulators (the rounding error of the stored bf16 averages out over the >= 10^5 values per channel, as in the tcgen05 GEMM epilogue)
+    // accumulators (the rounding error of the stored bf16 averages out over the >= 10^5 values per channel, as in the wgmma GEMM epilogue)
     auto strips = [&](auto interior_tag) {
     constexpr bool INTERIOR = decltype(interior_tag)::value;
     for (int st = warp; st < n_strips; st += NT / 32) {
@@ -205,13 +205,13 @@ __global__ void __launch_bounds__(NT, 2) dw_fwd_kernel(const __grid_constant__ C
   }
   if (p.col_sum) {
     if (lane_ok) {
-      atomicAdd(&s_cs[2 * lane], cs.x); atomicAdd(&s_cs[2 * lane + 1], cs.y);
-      atomicAdd(&s_cq[2 * lane], cq.x); atomicAdd(&s_cq[2 * lane + 1], cq.y);
+      atomicAdd(&s_cs[2 * lane], (double)cs.x); atomicAdd(&s_cs[2 * lane + 1], (double)cs.y);
+      atomicAdd(&s_cq[2 * lane], (double)cq.x); atomicAdd(&s_cq[2 * lane + 1], (double)cq.y);
     }
     __syncthreads();
     if (tid < CB && c0 + tid < p.C) {
-      atomicAdd(p.col_sum + c0 + tid, (double)s_cs[tid]);
-      atomicAdd(p.col_sq + c0 + tid, (double)s_cq[tid]);
+      atomicAdd(p.col_sum + c0 + tid, s_cs[tid]);
+      atomicAdd(p.col_sq + c0 + tid, s_cq[tid]);
     }
   }
 }
@@ -281,8 +281,8 @@ __global__ void __launch_bounds__(NTB, 1) dw_bwd_kernel(const __grid_constant__ 
   constexpr bool BNB = (GMODE == CVB_A_BNB);
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  __shared__ float s_cs[CB], s_cq[CB];
-  __shared__ float s_dw[9][CB];
+  __shared__ double s_cs[CB], s_cq[CB];  // fp64: the warps' fp32 partials sum exactly, whatever their order
+  __shared__ double s_dw[9][CB];
   __shared__ __align__(16) float s_gp[3 * CB];
   __shared__ __align__(8) uint64_t bar[2], ybar;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -310,8 +310,8 @@ __global__ void __launch_bounds__(NTB, 1) dw_bwd_kernel(const __grid_constant__ 
     tma_load_4d(sY2, &tmY2, &ybar, c0, gw_base, gh_base, (int)blockIdx.z + i * (int)gridDim.z);
   };
 
-  for (int i = tid; i < 9 * CB; i += NTB) (&s_dw[0][0])[i] = 0.f;
-  if (tid < CB) { s_cs[tid] = 0.f; s_cq[tid] = 0.f; }
+  for (int i = tid; i < 9 * CB; i += NTB) (&s_dw[0][0])[i] = 0.0;
+  if (tid < CB) { s_cs[tid] = 0.0; s_cq[tid] = 0.0; }
   if (tid == 0) {
     mbar_init(&bar[0], 1);
     mbar_init(&bar[1], 1);
@@ -500,22 +500,22 @@ __global__ void __launch_bounds__(NTB, 1) dw_bwd_kernel(const __grid_constant__ 
   if (lane_ok) {
 #pragma unroll
     for (int t = 0; t < 9; ++t) {
-      atomicAdd(&s_dw[t][2 * lane], accw[t].x);
-      atomicAdd(&s_dw[t][2 * lane + 1], accw[t].y);
+      atomicAdd(&s_dw[t][2 * lane], (double)accw[t].x);
+      atomicAdd(&s_dw[t][2 * lane + 1], (double)accw[t].y);
     }
     if (p.col_sum) {
-      atomicAdd(&s_cs[2 * lane], cs.x); atomicAdd(&s_cs[2 * lane + 1], cs.y);
-      atomicAdd(&s_cq[2 * lane], cq.x); atomicAdd(&s_cq[2 * lane + 1], cq.y);
+      atomicAdd(&s_cs[2 * lane], (double)cs.x); atomicAdd(&s_cs[2 * lane + 1], (double)cs.y);
+      atomicAdd(&s_cq[2 * lane], (double)cq.x); atomicAdd(&s_cq[2 * lane + 1], (double)cq.y);
     }
   }
   __syncthreads();
   for (int i = tid; i < 9 * CB; i += NTB) {
     int tp = i / CB, c = i % CB;
-    if (c0 + c < p.C) atomicAdd(p.dWt + tp * p.C + c0 + c, s_dw[tp][c]);
+    if (c0 + c < p.C) atomicAdd(reinterpret_cast<double*>(p.dWt) + tp * p.C + c0 + c, s_dw[tp][c]);  // fp64 scratch (cvb_dw_bwd)
   }
   if (p.col_sum && tid < CB && c0 + tid < p.C) {
-    atomicAdd(p.col_sum + c0 + tid, (double)s_cs[tid]);
-    atomicAdd(p.col_sq + c0 + tid, (double)s_cq[tid]);
+    atomicAdd(p.col_sum + c0 + tid, s_cs[tid]);
+    atomicAdd(p.col_sq + c0 + tid, s_cq[tid]);
   }
 }
 
@@ -610,11 +610,16 @@ extern "C" int cvb_dw_bwd(const cvb_dw_bwd_args* args, cvb_stream_t stream) {
   if (cvb_make_tmap_nhwc(&tmDZ, a.DZ, a.B, Ho, Wo, a.C, GH, GW, CB, 0)) return 1;
   if (cvb_make_tmap_nhwc(&tmY2, bnb ? a.Y2 : a.DZ, a.B, Ho, Wo, a.C, GH, GW, CB, 0)) return 1;
   if (cvb_make_tmap_nhwc(&tmX, a.X, a.B, a.H, a.W, a.C, XH, XW, CB, 0)) return 1;
+  // the CTAs' dW partials meet in an fp64 scratch (order-independent), added to dWt afterwards
+  double* ws = nullptr;
+  if (cvb_det_alloc(&ws, (size_t)9 * a.C, st)) return 2;
+  cvb_dw_bwd_args b = a;
+  b.dWt = reinterpret_cast<float*>(ws);
 #define CVB_DW_BWD(GM, XM, S)                                                                                             \
   {                                                                                                                      \
     static bool attr = false;                                                                                            \
     if (!attr) { CVB_CUDA(cudaFuncSetAttribute(dw_bwd_kernel<GM, XM, S>, cudaFuncAttributeMaxDynamicSharedMemorySize, 216 * 1024)); attr = true; } \
-    CVB_CUDA(cvb_launch(dw_bwd_kernel<GM, XM, S>, grid, NTB, smem, st, tmDZ, tmY2, tmX, a, Ho, Wo, TH, TW, tiles_w, g_bytes, x_bytes));   \
+    CVB_CUDA(cvb_launch(dw_bwd_kernel<GM, XM, S>, grid, NTB, smem, st, tmDZ, tmY2, tmX, b, Ho, Wo, TH, TW, tiles_w, g_bytes, x_bytes));   \
   }
 #define CVB_DW_BWD_X(GM, S)                                                   \
   {                                                                          \
@@ -630,5 +635,6 @@ extern "C" int cvb_dw_bwd(const cvb_dw_bwd_args* args, cvb_stream_t stream) {
 #undef CVB_DW_BWD_X
 #undef CVB_DW_BWD
   CVB_LAUNCH_CHECK();
-  return 0;
+  if (cvb_det_add(ws, a.dWt, 9, a.C, a.C, st)) return 2;
+  return cvb_det_free(ws, st);
 }

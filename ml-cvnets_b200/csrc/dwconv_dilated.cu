@@ -1,4 +1,4 @@
-// Dilated depthwise 3x3 convolution (stride 1, pad = dilation), NHWC bf16, forward and fused backward (sm_100a).
+// Dilated depthwise 3x3 convolution (stride 1, pad = dilation), NHWC bf16, forward and fused backward (sm_90a).
 //
 // SURVEY.md 8f row 4: segmentation backbones run MobileViTv2 with output_stride 8 / 16, which replaces the stride of layer_4 / layer_5
 // by dilation 2 / 4 in their depthwise convs (cvnets/models/classification/base_image_encoder.py:38-47, mobilevit_v2.py:176-191;

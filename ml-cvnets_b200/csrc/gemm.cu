@@ -1,15 +1,15 @@
-// Pointwise-conv / linear GEMMs for the MobileViTv2 hot path (sm_100a).
+// Pointwise-conv / linear GEMMs for the MobileViTv2 hot path (sm_90a).
 //
 //   cvb_pw_gemm : C[M,N] = epi( load(A)[M,K] * W[N,K]^T + bias )      forward and input-gradient GEMMs
 //   cvb_pw_wgrad: dW[N,K] += sum_m load(G)[m,n] * load(A)[m,k]        weight-gradient GEMM (reduction over pixels)
 //
-// Every layer here is HBM-bound (K,N <= 768: <= 170 FLOP/B, B200 ridge ~250 FLOP/B; SURVEY.md 8d), so the design goal is
+// Every layer here is HBM-bound (K,N <= 768: <= 170 FLOP/B, H100 ridge ~295 FLOP/B from the data sheet's 989 TFLOP/s / 3.35 TB/s; SURVEY.md 8d), so the design goal is
 // "read each activation once, write each activation once": the producer's BatchNorm/SiLU/GroupNorm (or the BN-backward of the
 // consumer) is a LOAD MODE of the A operand, and bias / activation / residual / BN statistics / GN statistics / activation
 // backward / GroupNorm backward are EPILOGUE modes, so no stand-alone normalisation or activation pass exists inside a module.
 // This file holds the mma.sync.m16n8k16 (bf16 -> fp32) kernels: the forward / input-gradient GEMM for narrow layers (N < 96) and
-// shapes the tcgen05 kernels do not take, the 64x64-tile weight-gradient kernel (K % 64 != 0 or tiny N, K), and the C-ABI entry
-// points that route to the tcgen05 / TMEM kernels in gemm_tc.cu and wgrad_tc.cu first.
+// shapes the wgmma kernels do not take, the 64x64-tile weight-gradient kernel (K % 64 != 0 or tiny N, K), and the C-ABI entry
+// points that route to the wgmma kernels in gemm_tc.cu and wgrad_tc.cu first.
 #include "common.cuh"
 
 namespace {
@@ -22,7 +22,7 @@ __device__ __forceinline__ uint32_t swz64(int row, int ch) {  // 64-byte rows, 4
   return static_cast<uint32_t>(row * 64 + ((ch ^ ((row >> 1) & 3)) << 4));
 }
 
-// The kernel is INSTRUCTION-ISSUE / latency bound, not tensor bound (ncu, profiles/): K <= 768 gives few MMAs per output
+// The kernel is INSTRUCTION-ISSUE / latency bound, not tensor bound: K <= 768 gives few MMAs per output
 // element, so the design minimises issued instructions per tile and maximises bytes in flight:
 //   * operands arrive by TMA (cp.async.bulk.tensor.2d, 64-byte swizzle == the ldmatrix XOR layout): ONE elected thread feeds a
 //     ring of A stages that runs across ALL M tiles of the persistent CTA (mbarrier completion); the weight panel [BN, K] is
@@ -70,12 +70,12 @@ __global__ void __launch_bounds__(NTHREADS, 2) pw_gemm_kernel(const __grid_const
   uint8_t* sA2 = sA + NST * A_STAGE;                   // second operand of the BN-backward prologue
   uint8_t* sO = sA + (TWO_A ? 2 : 1) * NST * A_STAGE;  // bf16 [BM][LDO] aux-in / result-out staging
   float* sP = reinterpret_cast<float*>(sO + BM * LDO * 2);
-  __shared__ float s_col[2][128];
+  __shared__ double s_col[2][128];
   __shared__ double s_samp[2][128];  // fp64: cross-thread order must not change the GroupNorm statistics
   __shared__ __align__(8) uint64_t full[MAX_STAGES];
   __shared__ __align__(8) uint64_t wbar;
 
-  if (tid < 128) { s_col[0][tid] = 0.f; s_col[1][tid] = 0.f; s_samp[0][tid] = 0.0; s_samp[1][tid] = 0.0; }
+  if (tid < 128) { s_col[0][tid] = 0.0; s_col[1][tid] = 0.0; s_samp[0][tid] = 0.0; s_samp[1][tid] = 0.0; }
   if (tid == 0) {
     for (int i = 0; i < NST; ++i) mbar_init(&full[i], 1);
     mbar_init(&wbar, 1);
@@ -386,14 +386,14 @@ __global__ void __launch_bounds__(NTHREADS, 2) pw_gemm_kernel(const __grid_const
       }
       if (g == 0) {
         const int col = wn0 + (j >> 1) * 8 + 2 * t + (j & 1);
-        atomicAdd(&s_col[0][col], a);
-        atomicAdd(&s_col[1][col], q);
+        atomicAdd(&s_col[0][col], (double)a);
+        atomicAdd(&s_col[1][col], (double)q);
       }
     }
     __syncthreads();
     if (tid < BN && n0 + tid < p.N) {
-      atomicAdd(p.col_sum + n0 + tid, (double)s_col[0][tid]);
-      atomicAdd(p.col_sq + n0 + tid, (double)s_col[1][tid]);
+      atomicAdd(p.col_sum + n0 + tid, s_col[0][tid]);
+      atomicAdd(p.col_sq + n0 + tid, s_col[1][tid]);
     }
   }
 }
@@ -489,7 +489,7 @@ __global__ void __launch_bounds__(NTHREADS, 2) pw_wgrad_kernel(const cvb_wgrad_a
   uint8_t* sG = smem;
   uint8_t* sG2 = smem + NST * T_STAGE;
   uint8_t* sA = smem + (TWO_G ? 2 : 1) * NST * T_STAGE;
-  __shared__ float s_db[WG_TN];
+  __shared__ double s_db[WG_TN];
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int g = lane >> 2, t = lane & 3;
@@ -508,7 +508,7 @@ __global__ void __launch_bounds__(NTHREADS, 2) pw_wgrad_kernel(const cvb_wgrad_a
   const bf16* __restrict__ G2 = static_cast<const bf16*>(p.G2);
   const bf16* __restrict__ A = static_cast<const bf16*>(p.A);
   const bool want_db = (p.dbias != nullptr) && (blockIdx.x == 0);
-  if (tid < WG_TN) s_db[tid] = 0.f;
+  if (tid < WG_TN) s_db[tid] = 0.0;
 
   // loader / transformer role: this thread owns chunk column `lch` (8 channels) of rows (tid>>3) + 32*i of every stage
   const int lch = tid & 7;
@@ -637,7 +637,7 @@ __global__ void __launch_bounds__(NTHREADS, 2) pw_wgrad_kernel(const cvb_wgrad_a
       for (int e = 0; e < 4; ++e) {
         int n = n0 + wn0 + ni * 16 + g + (e >> 1) * 8;
         int k = k0 + wk0 + kj * 8 + 2 * t + (e & 1);
-        if (n < p.N && k < p.K) atomicAdd(p.dW + (size_t)n * p.lddw + k, acc[ni][kj][e]);
+        if (n < p.N && k < p.K) atomicAdd(reinterpret_cast<double*>(p.dW) + (size_t)n * p.lddw + k, (double)acc[ni][kj][e]);
       }
   if (want_db) {
 #pragma unroll
@@ -645,10 +645,10 @@ __global__ void __launch_bounds__(NTHREADS, 2) pw_wgrad_kernel(const cvb_wgrad_a
       float v = db[e];  // reduce over the 4 row-lanes of this warp that share the chunk column (lane bits 3,4)
       v += __shfl_xor_sync(0xffffffffu, v, 8);
       v += __shfl_xor_sync(0xffffffffu, v, 16);
-      if (lane < 8) atomicAdd(&s_db[lch * 8 + e], v);
+      if (lane < 8) atomicAdd(&s_db[lch * 8 + e], (double)v);
     }
     __syncthreads();
-    if (tid < WG_TN && n0 + tid < p.N) atomicAdd(p.dbias + n0 + tid, s_db[tid]);
+    if (tid < WG_TN && n0 + tid < p.N) atomicAdd(reinterpret_cast<double*>(p.dbias) + n0 + tid, s_db[tid]);
   }
 }
 
@@ -688,8 +688,8 @@ int dispatch_wgrad_a(const cvb_wgrad_args& a, cudaStream_t st) {
 
 }  // namespace
 
-int cvb_pw_wgrad_tc(const cvb_wgrad_args& a, cudaStream_t st);  // wgrad_tc.cu: tcgen05 / TMEM weight-gradient kernel
-int cvb_pw_gemm_tc(const cvb_gemm_args& a, cudaStream_t st);  // gemm_tc.cu: tcgen05 / TMEM kernel (all load modes; STORE / residual / SiLU-backward / GroupNorm-backward epilogues)
+int cvb_pw_wgrad_tc(const cvb_wgrad_args& a, cudaStream_t st);  // wgrad_tc.cu: wgmma weight-gradient kernel
+int cvb_pw_gemm_tc(const cvb_gemm_args& a, cudaStream_t st);  // gemm_tc.cu: wgmma kernel (all load modes; STORE / residual / SiLU-backward / GroupNorm-backward epilogues)
 static int g_tc_enabled = 1;
 extern "C" int cvb_set_tc_enabled(int on) {
   int old = g_tc_enabled;
@@ -721,7 +721,7 @@ extern "C" int cvb_pw_gemm(const cvb_gemm_args* args, cvb_stream_t stream) {
   if (a.a_mode == CVB_A_BNB)
     CVB_CHECK(a.A2 && a.a_p0 && a.a_p1 && a.a_p2 && a.lda2 % 8 == 0 && cvb_aligned16(a.A2), "cvb_pw_gemm: BNB needs A2 and p0/p1/p2");
   if (g_tc_enabled) {
-    int rc = cvb_pw_gemm_tc(a, st);  // tcgen05 / TMEM kernel: STORE / residual / SiLU-backward epilogues, N >= 96
+    int rc = cvb_pw_gemm_tc(a, st);  // wgmma kernel: STORE / residual / SiLU-backward epilogues, N >= 96
     if (rc != -1) return rc;
   }
   const int epi = a.e_mode == CVB_E_STORE ? (a.R ? EPI_STORE_R : EPI_STORE) : a.e_mode == CVB_E_SILU ? EPI_SILU
@@ -750,15 +750,20 @@ extern "C" int cvb_pw_wgrad(const cvb_wgrad_args* args, cvb_stream_t stream) {
   if (a.a_mode == CVB_A_GN) CVB_CHECK(a.row_mean && a.row_rstd && a.rows_per_sample > 0 && a.a_p0 && a.a_p1, "cvb_pw_wgrad: GN needs statistics");
   if (a.a_mode == CVB_A_AFF || a.a_mode == CVB_A_AFF_SILU) CVB_CHECK(a.a_p0 && a.a_p1, "cvb_pw_wgrad: AFF needs p0/p1");
   if (a.g_mode == CVB_A_BNB) CVB_CHECK(a.G2 && a.g_p0 && a.g_p1 && a.g_p2 && a.ldg2 % 8 == 0 && cvb_aligned16(a.G2), "cvb_pw_wgrad: BNB needs G2 and p0/p1/p2");
-  if (g_tc_enabled && (a.g_mode == CVB_A_RAW || a.g_mode == CVB_A_BNB)) {
-    int rc = cvb_pw_wgrad_tc(a, st);  // tcgen05 kernel: whole [128 x 256] dW blocks in TMEM, operands read once
-    if (rc >= 0) return rc;
-  }
-  if (a.g_mode == CVB_A_RAW) return dispatch_wgrad_a<CVB_A_RAW>(a, st);
-  if (a.g_mode == CVB_A_BNB) {
-    CVB_CHECK(a.G2 && a.g_p0 && a.g_p1 && a.g_p2 && a.ldg2 % 8 == 0 && cvb_aligned16(a.G2), "cvb_pw_wgrad: BNB needs G2 and p0/p1/p2");
-    return dispatch_wgrad_a<CVB_A_BNB>(a, st);
-  }
-  cvb_set_error("cvb_pw_wgrad: unsupported g_mode %d", a.g_mode);
-  return 1;
+  CVB_CHECK(a.g_mode == CVB_A_RAW || a.g_mode == CVB_A_BNB, "cvb_pw_wgrad: unsupported g_mode %d", a.g_mode);
+  // the kernels reduce split partials with fp64 atomics into a scratch (order-independent), which is then added to dW / dbias
+  double* ws = nullptr;
+  const size_t nW = (size_t)a.N * a.K;
+  if (cvb_det_alloc(&ws, nW + (a.dbias ? a.N : 0), st)) return 2;
+  cvb_wgrad_args b = a;
+  b.dW = reinterpret_cast<float*>(ws);
+  b.lddw = a.K;
+  b.dbias = a.dbias ? reinterpret_cast<float*>(ws + nW) : nullptr;
+  int rc = -1;
+  if (g_tc_enabled) rc = cvb_pw_wgrad_tc(b, st);  // wgmma kernel: whole [128 x 128] dW blocks in registers, operands read once
+  if (rc < 0) rc = a.g_mode == CVB_A_RAW ? dispatch_wgrad_a<CVB_A_RAW>(b, st) : dispatch_wgrad_a<CVB_A_BNB>(b, st);
+  if (rc == 0) rc = cvb_det_add(ws, a.dW, a.N, a.K, a.lddw, st);
+  if (rc == 0 && a.dbias) rc = cvb_det_add(ws + nW, a.dbias, 1, a.N, a.N, st);
+  const int rf = cvb_det_free(ws, st);
+  return rc ? rc : rf;
 }

@@ -1,91 +1,47 @@
-// tcgen05 / TMEM / TMA pointwise-conv GEMM (sm_100a): every load mode, STORE / residual / SiLU-backward / GroupNorm-backward epilogues.
+// wgmma / TMA pointwise-conv GEMM (sm_90a): every load mode, STORE / residual / SiLU-backward / GroupNorm-backward epilogues.
 //
 //   C[M,N] = epi( A[M,K] * W[N,K]^T + bias )          same contract as the mma.sync kernel in gemm.cu
 //
 // Warp-specialised, one persistent CTA per SM:
-//   warp 0    TMA producer : ring of A stages [128 pixels x 32 k] (cp.async.bulk.tensor.2d, 64-byte swizzle) across ALL tiles
-//   warp 1    MMA issuer   : one elected thread issues tcgen05.mma.cta_group::1.kind::f16; the accumulator lives in TMEM,
-//                            double buffered (2 x 128 columns), completion is signalled with tcgen05.commit -> mbarrier
-//   warps 2-17 epilogue    : tcgen05.ld (32 lanes x 32 columns), bias / residual / activation-backward / BatchNorm statistics,
-//                            bf16 staging tile in smem, 16-byte row-contiguous stores
-//   warps 18-21 transform  : (layers with a prologue) apply the producer's BN(+SiLU) / GroupNorm / BN-backward to the landed A
-//                            stage in place, fence.proxy.async, then hand the stage to the MMA warp through a second mbarrier
-// The product is computed TRANSPOSED, D[channel, pixel] = W[channel, :] . A[pixel, :], i.e. the weight panel is the UMMA
-// "A" operand (M = 128 output channels = TMEM lanes) and the activation tile the "B" operand (N = 128 pixels = TMEM columns).
-// Each epilogue thread then owns ONE output channel: bias is a scalar, the per-channel BatchNorm sums are thread-local (no
-// shuffles, no smem atomics) and are flushed with one fp64 atomic per channel per CTA.  The epilogue of tile j overlaps the
-// MMAs of tile j+1 and the TMA loads of tiles j+2...
+//   warps 0-7  two consumer warpgroups: warpgroup g issues wgmma.m64n128k16 for output channels [64 g, 64 g + 64) of the tile
+//              (fp32 accumulator in registers), then runs the epilogue on those registers: bias / residual / activation-backward /
+//              BatchNorm statistics, bf16 staging tile in smem, 16-byte row-contiguous stores
+//   warp 8     TMA producer : ring of A stages [128 pixels x 32 k] (cp.async.bulk.tensor.2d, 64-byte swizzle) across ALL tiles
+//   warps 9-   transform    : (layers with a prologue) apply the producer's BN(+SiLU) / GroupNorm / BN-backward to the landed A
+//                             stage in place, fence.proxy.async, then hand the stage to the consumers through a second mbarrier
+// The product is computed TRANSPOSED, D[channel, pixel] = W[channel, :] . A[pixel, :], i.e. the weight panel is the wgmma "A"
+// operand (M = 64 output channels per warpgroup) and the activation tile the "B" operand (N = 128 pixels).  Each consumer thread
+// owns two output channels and 32 pixels of each: bias is a pair of scalars and the per-channel BatchNorm sums stay in registers
+// until the CTA's last tile (one quad shuffle, then one fp64 atomic per channel per CTA).  The TMA loads of tiles j+1... overlap
+// the epilogue of tile j.
 #include "common.cuh"
 #include <cstdlib>
 
 namespace {
 
-constexpr int TC_BM = 128;      // pixels per tile  (UMMA N)
-constexpr int TC_BN = 128;      // channels per tile (UMMA M)
+constexpr int TC_BM = 128;      // pixels per tile  (wgmma N)
+constexpr int TC_BN = 128;      // channels per tile (2 warpgroups x wgmma M 64)
 constexpr int TC_BK = 32;       // k per stage (64-byte rows)
 constexpr int TC_STAGE = TC_BM * TC_BK * 2;   // 8 KB
 constexpr int TC_WBLK = TC_BN * TC_BK * 2;    // 8 KB per k-block of the weight panel
 constexpr int TC_LDO = TC_BN + 8;             // bf16 staging row stride (elements)
-constexpr int TC_EPI_WARPS = 16;            // four warps per TMEM lane quadrant, each draining a quarter (32) of the pixel columns: the
-                                            // epilogue, not HBM, bounded round 1's kernel (2 warps / scheduler, ~3000 cycles per tile)
-constexpr int TC_EPI_THREADS = TC_EPI_WARPS * 32;
-constexpr int TC_THREADS = 64 + TC_EPI_THREADS;
+constexpr int TC_EPI_THREADS = 256;           // the two consumer warpgroups
+constexpr int TC_PRODUCER_WARP = TC_EPI_THREADS / 32;
+constexpr int TC_THREADS = TC_EPI_THREADS + 32;
 constexpr int TC_XF_THREADS_MAX = 256;      // transform warps (only launched for layers with a prologue).  Each warp is a latency-bound
-                                            // chain (LDS -> convert -> FMA -> MUFU -> pack -> STS): with 4 warps the MMA issuer spent most of its
-                                            // time waiting for transformed stages (ncu source view, round 2), so the prologue layers run 8
-                                            // (same-box A/B: AFF_SILU 100.9 -> 85.9 us, GN 48.3 -> 43.4 us); the BNB prologue (two operand
-                                            // tiles per stage, SiLU-backward epilogue) was 4 % faster with 4 and keeps them
+                                            // chain (LDS -> convert -> FMA -> MUFU -> pack -> STS), so the prologue layers run 8 warps; the
+                                            // BNB prologue (two operand tiles per stage, SiLU-backward epilogue) runs 4
 template <int AMODE>
 struct XfCfg {
   static constexpr int THREADS = (AMODE == CVB_A_RAW) ? 0 : (AMODE == CVB_A_BNB ? 128 : TC_XF_THREADS_MAX);
   static constexpr int IT = THREADS ? (TC_BM * 4) / THREADS : 1;  // 16-byte chunks of a [128 x 32] bf16 stage per transform thread
 };
 constexpr int TC_MAX_STAGES = 12;
-constexpr int TC_TMEM_COLS = 256;             // 2 accumulators x 128 fp32 columns
 
 enum { TEPI_STORE = 0, TEPI_STORE_R = 1, TEPI_SILU_BWD = 2, TEPI_GN_BWD = 3 };
 
-__device__ __forceinline__ uint64_t umma_desc_sw64(uint32_t saddr) {
-  // K-major operand, 64-byte swizzle: rows of 64 B, 8-row groups 512 B apart (cute::UMMA::SmemDescriptor, mma_sm100_desc.hpp)
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);  // start address            bits [0,14)
-  d |= (uint64_t)1 << 16;                    // leading byte offset (16 B; unused for swizzled K-major) bits [16,30)
-  d |= (uint64_t)(512 >> 4) << 32;           // stride byte offset = 512 B bits [32,46)
-  d |= (uint64_t)1 << 46;                    // descriptor version 1 (Blackwell)
-  d |= (uint64_t)4 << 61;                    // layout type: SWIZZLE_64B
-  return d;
-}
-// kind::f16 instruction descriptor: D = F32, A = B = BF16, both K-major, N = 128 (>>3), M = 128 (>>4)
-constexpr uint32_t TC_IDESC = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(TC_BM >> 3) << 17) | ((uint32_t)(TC_BN >> 4) << 24);
-
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(TC_IDESC), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,"
-      "%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]),
-        "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]),
-        "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
+// K-major operand, 64-byte swizzle: rows of 64 B (32 k), 8-row groups 512 B apart; a k-step of 16 advances the start by 32 B
+__device__ __forceinline__ uint64_t desc_sw64(uint32_t saddr) { return wgmma_desc(saddr, 16, 512, WG_SW64); }
 __device__ __forceinline__ void epi_bar_sync() { asm volatile("bar.sync 1, %0;" ::"n"(TC_EPI_THREADS) : "memory"); }
 
 // WRES: the weight panel [128 ch, K] stays resident in smem (loaded once); otherwise (large K) its k-blocks stream through the
@@ -113,29 +69,20 @@ __global__ void __launch_bounds__(TC_THREADS + XfCfg<AMODE>::THREADS, 1)
   uint8_t* sO = sA + NST * RING_STAGE;              // bf16 [128 pix][TC_LDO] staging (aux in / result out)
   float* sP = reinterpret_cast<float*>(sO + TC_BM * TC_LDO * 2);  // prologue parameters [3][Kpad]
   __shared__ __align__(8) uint64_t full[TC_MAX_STAGES], empty[TC_MAX_STAGES], ready[TC_MAX_STAGES];
-  __shared__ __align__(8) uint64_t wbar, tfull[2], tempty[2];
-  __shared__ uint32_t tmem_base_smem;
+  __shared__ __align__(8) uint64_t wbar;
   __shared__ double s_samp[2][128];
 
   if (tid == 0) {
-    for (int i = 0; i < NST; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); mbar_init(&ready[i], XfCfg<AMODE>::THREADS ? XfCfg<AMODE>::THREADS / 32 : 1); }
+    for (int i = 0; i < NST; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 2); mbar_init(&ready[i], XfCfg<AMODE>::THREADS ? XfCfg<AMODE>::THREADS / 32 : 1); }
     mbar_init(&wbar, 1);
-    for (int i = 0; i < 2; ++i) { mbar_init(&tfull[i], 1); mbar_init(&tempty[i], TC_EPI_WARPS); }
     fence_mbar_init();
   }
   if (tid < 128) { s_samp[0][tid] = 0.0; s_samp[1][tid] = 0.0; }
-  if (warp == 1) {  // TMEM allocation (whole warp), address published through smem
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_smem)), "r"(TC_TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
-  pdl_wait();  // barriers, TMEM allocation and CTA scheduling overlapped the previous kernel's tail; data accesses start here
+  pdl_wait();  // barriers and CTA scheduling overlapped the previous kernel's tail; data accesses start here
   pdl_trigger();
 
-  if (warp == 0) {
+  if (warp == TC_PRODUCER_WARP) {
     // ===================================================== TMA producer
     if (lane == 0) {
       if (WRES) {
@@ -153,31 +100,7 @@ __global__ void __launch_bounds__(TC_THREADS + XfCfg<AMODE>::THREADS, 1)
         if (!WRES) tma_load_2d(sA + stage * RING_STAGE + A_BYTES, &tmW, &full[stage], kt * TC_BK, n0);
       }
     }
-  } else if (warp == 1) {
-    // ===================================================== MMA issuer
-    if (lane == 0) {
-      if (WRES) mbar_wait(&wbar, 0);
-      int it = 0;
-      for (int j = 0; j < my_tiles; ++j) {
-        const int buf = j & 1;
-        if (j >= 2) mbar_wait(&tempty[buf], ((j >> 1) - 1) & 1);  // epilogue has drained this accumulator
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + (uint32_t)(buf * TC_BM);
-        for (int kt = 0; kt < KT; ++kt, ++it) {
-          const int stage = it % NST;
-          mbar_wait(XF ? &ready[stage] : &full[stage], (it / NST) & 1);  // landed (and transformed in place)
-          tc_fence_after();
-          const uint32_t aa = smem_u32(sA + stage * RING_STAGE);
-          const uint32_t wa = WRES ? smem_u32(sW + kt * TC_WBLK) : aa + A_BYTES;
-#pragma unroll
-          for (int k = 0; k < TC_BK / 16; ++k)
-            umma_f16(tmem_d, umma_desc_sw64(wa + k * 32), umma_desc_sw64(aa + k * 32), (kt | k) ? 1u : 0u);
-          umma_commit(&empty[stage]);  // frees the smem slot once these MMAs have read it
-        }
-        umma_commit(&tfull[buf]);      // accumulator complete
-      }
-    }
-  } else if (warp >= 2 + TC_EPI_WARPS) {
+  } else if (warp > TC_PRODUCER_WARP) {
     // ===================================================== transform warps: producer's normalisation / activation, in place
     if (XF) {
       constexpr int TC_XF_THREADS = XfCfg<AMODE>::THREADS > 0 ? XfCfg<AMODE>::THREADS : 128;
@@ -217,7 +140,7 @@ __global__ void __launch_bounds__(TC_THREADS + XfCfg<AMODE>::THREADS, 1)
           const int c = tt + i * TC_XF_THREADS;
           const int row = c >> 2, ch = c & 3;
           const int k = k0 + ch * 8;
-          const uint32_t off = (uint32_t)(row * 64 + ((ch ^ ((row >> 1) & 3)) << 4));  // 64-byte swizzle (TMA == UMMA layout)
+          const uint32_t off = (uint32_t)(row * 64 + ((ch ^ ((row >> 1) & 3)) << 4));  // 64-byte swizzle (TMA == wgmma layout)
           uint4* pa = reinterpret_cast<uint4*>(st + off);
           float f[8], q0[8], q1[8];
           unpack8(*pa, f);
@@ -256,26 +179,32 @@ __global__ void __launch_bounds__(TC_THREADS + XfCfg<AMODE>::THREADS, 1)
       }
     }
   } else {
-    // ===================================================== epilogue warps (threads 64..319): one output channel per thread
-    const int et = tid - 64;                 // 0..TC_EPI_THREADS-1
-    const int quad = warp & 3;               // TMEM lane quadrant this warp may access
-    const int cquart = (warp - 2) >> 2;      // which quarter (32) of the pixel columns this warp drains
-    const int ch_local = quad * 32 + lane;   // output channel within the tile == TMEM lane
-    const int ch = n0 + ch_local;
-    const bool ch_ok = ch < p.N;
-    const float bias = (ch_ok && p.bias) ? __ldg(p.bias + ch) : 0.f;
-    const float ep0 = ((EPI == TEPI_SILU_BWD || EPI == TEPI_GN_BWD) && ch_ok && p.e_p0) ? __ldg(p.e_p0 + ch) : 1.f;
-    const float ep1 = (EPI == TEPI_SILU_BWD && ch_ok && p.e_p1) ? __ldg(p.e_p1 + ch) : 0.f;
+    // ===================================================== consumer warpgroups: MMA, then the epilogue on the accumulator registers
+    const int et = tid;                       // 0..TC_EPI_THREADS-1
+    const int wg = tid >> 7;                  // channel half of the tile
+    const int r0 = wg * 64 + ((tid & 127) >> 5) * 16 + (lane >> 2);  // local channel of acc[4j + {0,1}]; r0 + 8 holds acc[4j + {2,3}]
+    const int pc = 2 * (lane & 3);            // pixel column of acc[4j] within the 8-column block j
+    int chn[2];
+    bool ch_ok[2];
+    float bias[2], ep0[2], ep1[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      chn[h] = n0 + r0 + 8 * h;
+      ch_ok[h] = chn[h] < p.N;
+      bias[h] = (ch_ok[h] && p.bias) ? __ldg(p.bias + chn[h]) : 0.f;
+      ep0[h] = ((EPI == TEPI_SILU_BWD || EPI == TEPI_GN_BWD) && ch_ok[h] && p.e_p0) ? __ldg(p.e_p0 + chn[h]) : 1.f;
+      ep1[h] = (EPI == TEPI_SILU_BWD && ch_ok[h] && p.e_p1) ? __ldg(p.e_p1 + chn[h]) : 0.f;
+    }
     constexpr bool has_aux = (EPI != TEPI_STORE);
     const bf16* __restrict__ AUX = static_cast<const bf16*>(EPI == TEPI_STORE_R ? p.R : p.Y);
     const int ldaux = EPI == TEPI_STORE_R ? p.ldr : p.ldy;
     const bool want_samp = (p.samp_sum != nullptr) && (EPI != TEPI_GN_BWD);  // GN_BWD: the sample sums come from the workspace finalize
     const bool lin_bwd = (p.e_mode == CVB_E_LIN_BWD);  // SiLU-backward epilogue without the activation factor (BatchNorm with no act)
     const int rps = p.rows_per_sample > 0 ? p.rows_per_sample : 1;
-    float cs = 0.f, cq = 0.f;  // this channel's statistics over all tiles of the CTA
-    float2 cs2 = make_float2(0.f, 0.f), cq2 = make_float2(0.f, 0.f);  // hot-path partials (even / odd pixel columns), folded in at the end
+    float cs[2] = {0.f, 0.f}, cq[2] = {0.f, 0.f};  // statistics of this thread's two channels over its pixels of all tiles of the CTA
     bf16* __restrict__ Cg = static_cast<bf16*>(p.C);
     constexpr int CGS = TC_BN / 8;
+    const uint32_t w_off = (uint32_t)wg * 64 * 64;  // this warpgroup's 64 weight rows (8 swizzle atoms of 512 B)
 
     auto issue_aux = [&](int j) {
       const int m0 = ((int)blockIdx.y + j * (int)gridDim.y) * TC_BM;
@@ -288,76 +217,99 @@ __global__ void __launch_bounds__(TC_THREADS + XfCfg<AMODE>::THREADS, 1)
       cp_async_commit();
     };
     if (has_aux && my_tiles > 0) issue_aux(0);
+    if (WRES) mbar_wait(&wbar, 0);
 
+    float acc[64];
+    int it = 0;
     for (int j = 0; j < my_tiles; ++j) {
-      const int buf = j & 1;
       const int m0 = ((int)blockIdx.y + j * (int)gridDim.y) * TC_BM;
+      for (int kt = 0; kt < KT; ++kt, ++it) {
+        const int stage = it % NST;
+        mbar_wait(XF ? &ready[stage] : &full[stage], (it / NST) & 1);  // landed (and transformed in place)
+        const uint32_t aa = smem_u32(sA + stage * RING_STAGE);
+        const uint32_t wa = (WRES ? smem_u32(sW + kt * TC_WBLK) : aa + A_BYTES) + w_off;
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < TC_BK / 16; ++k) wgmma_m64n128<0, 0>(acc, desc_sw64(wa + k * 32), desc_sw64(aa + k * 32), (kt | k) ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<1>();  // the previous k-block's MMAs have read their stage
+        if (kt > 0 && (tid & 127) == 0) mbar_arrive(&empty[(it - 1) % NST]);
+      }
+      wgmma_wait<0>();
+      wgmma_reg_fence<64>(acc);
+      if ((tid & 127) == 0) mbar_arrive(&empty[(it - 1) % NST]);
+
       if (has_aux) {
         cp_async_wait<0>();
         epi_bar_sync();  // aux tile visible to all epilogue threads
       }
-      mbar_wait(&tfull[buf], (j >> 1) & 1);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(buf * TC_BM);
       const bool full_tile = (m0 + TC_BM <= p.M);  // rows >= M have zero A rows; only their bias must be masked (last tile)
-      {
-        const int cc = cquart;
-        uint32_t r[32];
-        tmem_ld32(taddr + cc * 32, r);
-        uint16_t* so = reinterpret_cast<uint16_t*>(sO) + (cc * 32) * TC_LDO + ch_local;
-        if (full_tile && !has_aux) {
-          // hot path (conv -> BN statistics): ~5 instructions per value.  The BatchNorm sums are taken from the fp32 values
-          // (before bf16 rounding): the rounding error averages out over the >= 128 pixels of the tile.
-          // packed fp32 pairs (adjacent pixel columns are adjacent registers of the tcgen05.ld result): 7 instructions per 2 values
-          const float2 b2 = make_float2(bias, bias);
+      float gs[2][2] = {{0.f, 0.f}, {0.f, 0.f}}, gq[2][2] = {{0.f, 0.f}, {0.f, 0.f}};  // GN_BWD: per channel, per 64-pixel half
 #pragma unroll
-          for (int i = 0; i < 32; i += 2) {
-            const float2 v = fadd2(make_float2(__uint_as_float(r[i]), __uint_as_float(r[i + 1])), b2);
-            const uint32_t pk = pack_bf162(v.x, v.y);
-            so[i * TC_LDO] = (uint16_t)pk;
-            so[(i + 1) * TC_LDO] = (uint16_t)(pk >> 16);
-            cs2 = fadd2(cs2, v);
-            cq2 = ffma2(v, v, cq2);
+      for (int h = 0; h < 2; ++h) {
+        bf16* so = reinterpret_cast<bf16*>(sO) + r0 + 8 * h;
+        if (full_tile && !has_aux) {
+          // hot path (conv -> BN statistics).  The BatchNorm sums are taken from the fp32 values (before bf16 rounding): the
+          // rounding error averages out over the >= 128 pixels of the tile.
+#pragma unroll
+          for (int jb = 0; jb < 16; ++jb) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const float v = acc[4 * jb + 2 * h + e] + bias[h];
+              so[(8 * jb + pc + e) * TC_LDO] = __float2bfloat16_rn(v);
+              cs[h] += v;
+              cq[h] = fmaf(v, v, cq[h]);
+            }
           }
         } else {
 #pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            float v = __uint_as_float(r[i]) + ((full_tile || m0 + cc * 32 + i < p.M) ? bias : 0.f);
-            float y = 0.f;
-            if (has_aux) y = __bfloat162float(reinterpret_cast<const bf16*>(so)[i * TC_LDO]);
-            if (EPI == TEPI_STORE_R) v += y;
-            if (EPI == TEPI_SILU_BWD && !lin_bwd) v *= silu_grad_f(fmaf(ep0, y, ep1));
-            if (EPI == TEPI_GN_BWD) {
-              // GroupNorm backward, phase 1 in sum form: per (sample, channel) A = sum v, Bx = sum v*x (raw x); everything else
-              // (dgamma, dbeta, per-sample sums of g and g*xhat) is linear in A and Bx and is derived by the finalize kernel
-              cs += v;
-              cq = fmaf(v, y, cq);
-              reinterpret_cast<bf16*>(so)[i * TC_LDO] = __float2bfloat16_rn(v * ep0);
-            } else {
-              const bf16 vb = __float2bfloat16_rn(v);
-              reinterpret_cast<bf16*>(so)[i * TC_LDO] = vb;
-              const float vr = __bfloat162float(vb);  // statistics of the STORED values
-              cs += vr;
-              cq = fmaf(vr, EPI == TEPI_SILU_BWD ? y : vr, cq);
+          for (int jb = 0; jb < 16; ++jb) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int i = 8 * jb + pc + e;  // pixel within the tile
+              float v = acc[4 * jb + 2 * h + e] + ((full_tile || m0 + i < p.M) ? bias[h] : 0.f);
+              float y = 0.f;
+              if (has_aux) y = __bfloat162float(so[i * TC_LDO]);
+              if (EPI == TEPI_STORE_R) v += y;
+              if (EPI == TEPI_SILU_BWD && !lin_bwd) v *= silu_grad_f(fmaf(ep0[h], y, ep1[h]));
+              if (EPI == TEPI_GN_BWD) {
+                // GroupNorm backward, phase 1 in sum form: per (sample, channel) A = sum v, Bx = sum v*x (raw x); everything else
+                // (dgamma, dbeta, per-sample sums of g and g*xhat) is linear in A and Bx and is derived by the finalize kernel
+                gs[h][jb >> 3] += v;
+                gq[h][jb >> 3] = fmaf(v, y, gq[h][jb >> 3]);
+                so[i * TC_LDO] = __float2bfloat16_rn(v * ep0[h]);
+              } else {
+                const bf16 vb = __float2bfloat16_rn(v);
+                so[i * TC_LDO] = vb;
+                const float vr = __bfloat162float(vb);  // statistics of the STORED values
+                cs[h] += vr;
+                cq[h] = fmaf(vr, EPI == TEPI_SILU_BWD ? y : vr, cq[h]);
+              }
             }
           }
         }
       }
-      if (EPI == TEPI_GN_BWD) {  // this thread's 32 pixel columns never straddle samples (rows_per_sample % 64 == 0, checked on the host)
-        const int mh = m0 + cquart * 32;
-        if (ch_ok && mh < p.M) {
-          const int nsamples = (p.M + rps - 1) / rps;
-          double* wsA = p.gn_ws + (size_t)(mh / rps) * p.N + ch;
-          atomicAdd(wsA, (double)cs);
-          atomicAdd(wsA + (size_t)nsamples * p.N, (double)cq);
+      if (EPI == TEPI_GN_BWD) {  // a 64-pixel half tile never straddles samples (rows_per_sample % 64 == 0, checked on the host)
+        const int nsamples = (p.M + rps - 1) / rps;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+#pragma unroll
+          for (int hf = 0; hf < 2; ++hf) {
+            float a = gs[h][hf], bx = gq[h][hf];
+            a += __shfl_xor_sync(0xffffffffu, a, 1);
+            a += __shfl_xor_sync(0xffffffffu, a, 2);
+            bx += __shfl_xor_sync(0xffffffffu, bx, 1);
+            bx += __shfl_xor_sync(0xffffffffu, bx, 2);
+            const int mh = m0 + hf * 64;
+            if ((lane & 3) == 0 && ch_ok[h] && mh < p.M) {
+              double* wsA = p.gn_ws + (size_t)(mh / rps) * p.N + chn[h];
+              atomicAdd(wsA, (double)a);
+              atomicAdd(wsA + (size_t)nsamples * p.N, (double)bx);
+            }
+          }
         }
-        cs = 0.f;
-        cq = 0.f;
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty[buf]);  // one arrival per epilogue warp releases the accumulator
-      epi_bar_sync();                            // staged tile complete
+      epi_bar_sync();  // staged tile complete
       const int first_sample = m0 / rps;
       for (int c = et; c < TC_BM * CGS; c += TC_EPI_THREADS) {
         const int row = c / CGS, cgc = c % CGS;
@@ -394,20 +346,20 @@ __global__ void __launch_bounds__(TC_THREADS + XfCfg<AMODE>::THREADS, 1)
       }
       if (has_aux && j + 1 < my_tiles) issue_aux(j + 1);
     }
-    cs += cs2.x + cs2.y;
-    cq += cq2.x + cq2.y;
-    if (EPI != TEPI_GN_BWD && p.col_sum && ch_ok) {
-      atomicAdd(p.col_sum + ch, (double)cs);
-      atomicAdd(p.col_sq + ch, (double)cq);
+    if (EPI != TEPI_GN_BWD) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {  // the four threads of a quad share a channel
+        float s = cs[h], q = cq[h];
+        s += __shfl_xor_sync(0xffffffffu, s, 1);
+        s += __shfl_xor_sync(0xffffffffu, s, 2);
+        q += __shfl_xor_sync(0xffffffffu, q, 1);
+        q += __shfl_xor_sync(0xffffffffu, q, 2);
+        if (p.col_sum && ch_ok[h] && (lane & 3) == 0) {
+          atomicAdd(p.col_sum + chn[h], (double)s);
+          atomicAdd(p.col_sq + chn[h], (double)q);
+        }
+      }
     }
-  }
-
-  // ---- teardown
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TC_TMEM_COLS) : "memory");
   }
 }
 
@@ -423,8 +375,8 @@ int launch_tc_impl(const cvb_gemm_args& a, cudaStream_t st, size_t fixed, int st
     attr = true;
   }
   const int n_tiles = (a.N + TC_BN - 1) / TC_BN, m_tiles = (a.M + TC_BM - 1) / TC_BM;
-  // one persistent CTA per SM, never more CTAs than SMs: rounding UP (3 x 50 = 150 CTAs on 148 SMs) put two CTAs into a second wave and doubled
-  // the time of every N = 264 / 392 / 520 / 768-wide late-stage layer (profiles/r2_step_launches_v2_lazybn_dram.csv)
+  // one persistent CTA per SM, never more CTAs than SMs: rounding UP (e.g. 3 N tiles x 45 = 135 CTAs on 132 SMs) would put a few CTAs
+  // into a second wave and double the time of the layer
   int gy = cvb_num_sms() / n_tiles;
   if (gy > m_tiles) gy = m_tiles;
   if (gy < 1) gy = 1;
@@ -504,11 +456,11 @@ int dispatch_tc_epi(const cvb_gemm_args& a, cudaStream_t st) {
 
 }  // namespace
 
-// Returns -1 when the shape / mode is not handled by the tcgen05 kernel (caller uses the mma.sync kernel), 0 on success, > 0 on error.
+// Returns -1 when the shape / mode is not handled by the wgmma kernel (caller uses the mma.sync kernel), 0 on success, > 0 on error.
 int cvb_pw_gemm_tc(const cvb_gemm_args& a, cudaStream_t st) {
-  // every epilogue thread owns one of 128 output channels: narrow layers would idle most of them -> mma.sync kernel
+  // a CTA computes 128 output channels: narrow layers would idle most of them -> mma.sync kernel
   static const int min_n = [] { const char* e = getenv("CVB_TC_MIN_N"); return e ? atoi(e) : 96; }();  // diagnostics: route narrower layers here
-  if (a.N < min_n || (a.N >= 96 && a.N % 128 != 0 && a.N % 128 < 64 && a.N < 256)) return -1;  // N = 64 on this kernel measured slower than mma.sync (round 1)
+  if (a.N < min_n || (a.N >= 96 && a.N % 128 != 0 && a.N % 128 < 64 && a.N < 256)) return -1;  // narrow / ragged N would leave most of a 128-channel tile idle
   switch (a.a_mode) {
     case CVB_A_RAW: return dispatch_tc_epi<CVB_A_RAW>(a, st);
     case CVB_A_AFF: return dispatch_tc_epi<CVB_A_AFF>(a, st);

@@ -1,4 +1,4 @@
-// LinearSelfAttention core (MobileViTv2) between qkv_proj and out_proj, forward and backward (sm_100a).
+// LinearSelfAttention core (MobileViTv2) between qkv_proj and out_proj, forward and backward (sm_90a).
 // Reference: cvnets/layers/linear_attention.py:134-161; math: SURVEY.md Appendix A5.
 //
 // unfold / fold (cvnets/modules/mobilevit_block.py:526-555) never materialise: the tensor stays the channels-last feature
@@ -125,25 +125,26 @@ __global__ void __launch_bounds__(NT) linattn_fwd_kernel(const bf16* __restrict_
 // dynamic smem: s[N] | ds[N] | ctx[d] | dctx[d] | dbk[d] | dbv[d]
 __global__ void __launch_bounds__(NT) linattn_bwd_kernel(const bf16* __restrict__ QKV, int ldq, const bf16* __restrict__ DO, int ldo,
                                                          const float* __restrict__ S, const float* __restrict__ CTX, int H, int W, int d,
-                                                         bf16* __restrict__ DQKV, float* __restrict__ dbias, int unf, const bf16* __restrict__ VX,
+                                                         bf16* __restrict__ DQKV, double* __restrict__ dbias, int unf, const bf16* __restrict__ VX,
                                                          int ldvx, int Nv, bf16* __restrict__ DVX) {
   pdl_wait();
   pdl_trigger();
-  extern __shared__ float sm[];
+  extern __shared__ double smd[];
   __shared__ float ws[NT / 32];
   const int N = unf ? W : (H >> 1) * (W >> 1);
   const int P = unf ? H : 4;
   const int Wv = (VX == QKV) ? W : Nv;
-  float* s_s = sm;
-  float* s_ds = sm + N;
-  float* s_ctx = sm + 2 * N;
-  float* s_dctx = s_ctx + d;
-  float* s_dbk = s_dctx + d;
-  float* s_dbv = s_dbk + d;
+  // the sums the warps contribute to are fp64: their fp32 partials add exactly, whatever the order
+  double* s_ds = smd;
+  double* s_dctx = s_ds + N;
+  double* s_dbk = s_dctx + d;
+  double* s_dbv = s_dbk + d;
+  float* s_s = reinterpret_cast<float*>(s_dbv + d);
+  float* s_ctx = s_s + N;
   const int b = blockIdx.x / P, p = blockIdx.x % P;
   const int tid = threadIdx.x;
-  for (int n = tid; n < N; n += blockDim.x) { s_s[n] = S[((int64_t)b * P + p) * N + n]; s_ds[n] = 0.f; }
-  for (int i = tid; i < d; i += blockDim.x) { s_ctx[i] = CTX[((int64_t)b * P + p) * d + i]; s_dctx[i] = 0.f; s_dbk[i] = 0.f; s_dbv[i] = 0.f; }
+  for (int n = tid; n < N; n += blockDim.x) { s_s[n] = S[((int64_t)b * P + p) * N + n]; s_ds[n] = 0.0; }
+  for (int i = tid; i < d; i += blockDim.x) { s_ctx[i] = CTX[((int64_t)b * P + p) * d + i]; s_dctx[i] = 0.0; s_dbk[i] = 0.0; s_dbv[i] = 0.0; }
   __syncthreads();
 
   const int cgs = d >> 3;
@@ -170,7 +171,7 @@ __global__ void __launch_bounds__(NT) linattn_bwd_kernel(const bf16* __restrict_
     }
     if (grp < ngrp) {
 #pragma unroll
-      for (int j = 0; j < 8; ++j) { atomicAdd(&s_dctx[cg * 8 + j], acc[j]); atomicAdd(&s_dbv[cg * 8 + j], dbv[j]); }
+      for (int j = 0; j < 8; ++j) { atomicAdd(&s_dctx[cg * 8 + j], (double)acc[j]); atomicAdd(&s_dbv[cg * 8 + j], (double)dbv[j]); }
     }
   }
   __syncthreads();
@@ -178,7 +179,7 @@ __global__ void __launch_bounds__(NT) linattn_bwd_kernel(const bf16* __restrict_
   {
     float dctx[8], dbk[8];
 #pragma unroll
-    for (int j = 0; j < 8; ++j) { dctx[j] = s_dctx[cg * 8 + j]; dbk[j] = 0.f; }
+    for (int j = 0; j < 8; ++j) { dctx[j] = (float)s_dctx[cg * 8 + j]; dbk[j] = 0.f; }
     for (int n = n_first; n < N; n += ngrp) {
       const int64_t m = pix_index(b, p, n, H, W, unf);
       float k[8], dk[8];
@@ -191,24 +192,24 @@ __global__ void __launch_bounds__(NT) linattn_bwd_kernel(const bf16* __restrict_
         dk[j] = bf16_round(dctx[j] * sv);
         dbk[j] += dk[j];
       }
-      atomicAdd(&s_ds[n], part);
+      atomicAdd(&s_ds[n], (double)part);
       stg16(DQKV + m * ldq + cg * 8, pack8(dk));
     }
     if (grp < ngrp) {
 #pragma unroll
-      for (int j = 0; j < 8; ++j) atomicAdd(&s_dbk[cg * 8 + j], dbk[j]);
+      for (int j = 0; j < 8; ++j) atomicAdd(&s_dbk[cg * 8 + j], (double)dbk[j]);
     }
   }
   __syncthreads();
   // dq = s * (ds - sum_n ds*s); written with the zero pad of the last 16-byte chunk
   float ldot = 0.f;
-  for (int n = tid; n < N; n += blockDim.x) ldot += s_ds[n] * s_s[n];
+  for (int n = tid; n < N; n += blockDim.x) ldot += (float)s_ds[n] * s_s[n];
   const float dot = block_reduce_sum(ldot, ws);
   float ldq_sum = 0.f;
   for (int n = tid; n < N; n += blockDim.x) {
     const int64_t m = pix_index(b, p, n, H, W, unf);
     float f[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-    f[0] = bf16_round(s_s[n] * (s_ds[n] - dot));
+    f[0] = bf16_round(s_s[n] * ((float)s_ds[n] - dot));
     ldq_sum += f[0];
     for (int c = 2 * d; c < ldq; c += 8) {
       stg16(DQKV + m * ldq + c, pack8(f));
@@ -218,7 +219,7 @@ __global__ void __launch_bounds__(NT) linattn_bwd_kernel(const bf16* __restrict_
   if (dbias) {
     const float dq_sum = block_reduce_sum(ldq_sum, ws);
     for (int i = tid; i < d; i += blockDim.x) { atomicAdd(dbias + i, s_dbk[i]); atomicAdd(dbias + d + i, s_dbv[i]); }
-    if (tid == 0) atomicAdd(dbias + 2 * d, dq_sum);
+    if (tid == 0) atomicAdd(dbias + 2 * d, (double)dq_sum);
   }
 }
 
@@ -273,15 +274,20 @@ static int linattn_bwd_impl(const void* QKV, int ldq, const void* DO, int ldo, c
   CVB_CHECK(VX == QKV || patch == 0, "cvb_linattn_bwd: cross-attention needs the unfolded layout (patch = 0)");
   CVB_CHECK(DVX && ldvx % 8 == 0 && ldvx >= 2 * d && Nv > 0, "cvb_linattn_bwd: bad value tensor");
   const int nthreads = NT;
-  size_t smem = (size_t)(2 * N + 4 * d) * sizeof(float);
+  size_t smem = (size_t)(N + 3 * d) * sizeof(double) + (size_t)(N + d) * sizeof(float);
   CVB_CHECK(smem <= 200 * 1024, "cvb_linattn_bwd: N=%d too large", N);
   static bool attr = false;
   if (!attr) { CVB_CUDA(cudaFuncSetAttribute(linattn_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); attr = true; }
-  CVB_CUDA(cvb_launch(linattn_bwd_kernel, B * P, nthreads, smem, static_cast<cudaStream_t>(stream), static_cast<const bf16*>(QKV), ldq,
-                      static_cast<const bf16*>(DO), ldo, S, CTX, H, W, d, static_cast<bf16*>(DQKV), dbias, patch == 0 ? 1 : 0,
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  double* ws = nullptr;  // the CTAs' bias-gradient partials meet in fp64 (order-independent), added to dbias afterwards
+  if (dbias && cvb_det_alloc(&ws, (size_t)2 * d + 1, st)) return 2;
+  CVB_CUDA(cvb_launch(linattn_bwd_kernel, B * P, nthreads, smem, st, static_cast<const bf16*>(QKV), ldq,
+                      static_cast<const bf16*>(DO), ldo, S, CTX, H, W, d, static_cast<bf16*>(DQKV), ws, patch == 0 ? 1 : 0,
                       static_cast<const bf16*>(VX), ldvx, Nv, static_cast<bf16*>(DVX)));
   CVB_LAUNCH_CHECK();
-  return 0;
+  if (!dbias) return 0;
+  if (cvb_det_add(ws, dbias, 1, 2 * d + 1, 2 * d + 1, st)) return 2;
+  return cvb_det_free(ws, st);
 }
 
 extern "C" int cvb_linattn_bwd(const void* QKV, int ldq, const void* DO, int ldo, const float* S, const float* CTX, int B, int H, int W, int d, int patch,

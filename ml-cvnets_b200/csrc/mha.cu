@@ -1,4 +1,4 @@
-// Multi-head self-attention core (cvnets/layers/multi_head_attention.py:135-239), forward and backward, sm_100a.
+// Multi-head self-attention core (cvnets/layers/multi_head_attention.py:135-239), forward and backward, sm_90a.
 //
 //   O[b, s, h*c + :] = softmax_t( scale * Q[b,h,s,:] . K[b,h,t,:] + attn_mask[b,s,t]  (-inf where key_padding_mask[b,t]) ) @ V[b,h,t,:]
 //
@@ -7,7 +7,7 @@
 // tensor in HBM (the reference materialises it twice, bf16 and fp32: 477 MB per ViT-B layer, SURVEY.md 8a a11).
 // One CTA per (sample, head); the whole K / V (and Q, dO in the backward) of that head live in shared memory (S <= 256,
 // head_dim in {16, 32, 64}: every hot-path config of SURVEY.md 8a: ViT-B 197x64, CLIP text 77x64, MobileViT-v1 256x16..).
-// Tensor cores: mma.sync.m16n8k16 bf16 -> fp32 (the score tiles are 16 x 64 per warp: far below a tcgen05 tile), online softmax
+// Tensor cores: mma.sync.m16n8k16 bf16 -> fp32 (the score tiles are 16 x 64 per warp: far below a wgmma tile), online softmax
 // in the exp2 domain, probabilities kept in registers and re-used as the A operand of P.V.
 // Backward = two passes without atomics: pass A owns query rows (dQ), pass B owns key rows (dK, dV); P is recomputed from the
 // saved log-sum-exp.
@@ -412,7 +412,7 @@ int check_common(const char* who, const void* QKV, int ldq, int B, int S, int H,
 
 }  // namespace
 
-// head_dim == 64: tcgen05 kernels (mha_tc.cu); -1 = not handled there
+// head_dim == 64: wgmma kernels (mha_tc.cu); -1 = not handled there
 int cvb_mha_fwd_tc(const void* QKV, int ldq, int B, int S, int H, int head_dim, float scale, const float* amask, const unsigned char* kpm, void* O,
                    int ldo, float* LSE, cudaStream_t st);
 int cvb_mha_bwd_tc(const void* QKV, int ldq, const void* O, const void* DO, int ldo, const float* LSE, int B, int S, int H, int head_dim, float scale,

@@ -1,24 +1,17 @@
-// tcgen05 / TMEM / TMA multi-head attention core for head_dim == 64, S <= 256 (ViT-B 197 x 64, CLIP text 77 x 64), sm_100a.
+// wgmma / TMA multi-head attention core for head_dim == 64, S <= 256 (ViT-B 197 x 64, CLIP text 77 x 64), sm_90a.
 // Same contract as mha.cu (cvnets/layers/multi_head_attention.py:187-237): packed projection in, O / LSE out, dQKV in the backward.
 //
 // Every operand of a head -- Q, K, V, dO [rows x 64 bf16] -- is ONE TMA box [64 cols x rows] with 128-byte swizzle.  That shared-memory
 // image (128-byte rows, 8-row swizzle atoms of 1 KB) is at the same time
-//   * the canonical K-major  SWIZZLE_128B UMMA operand  (rows = M/N, the 64 channels = K)        -> S = Q K^T, dP = dO V^T
-//   * the canonical MN-major SWIZZLE_128B UMMA operand  (the 64 channels = M/N, rows = K)        -> O = P V, dQ = dS K, dK = dS^T Q, dV = P^T dO
-// so nothing is transposed or loaded twice.  P and dS are written by the softmax threads as [query rows x 64-key boxes] in the same
-// image and are consumed K-major (A of P V / dS K) and MN-major (A of P^T dO / dS^T Q).
+//   * the canonical K-major  SWIZZLE_128B wgmma operand  (rows = M/N, the 64 channels = K)        -> S = Q K^T, dP^T = V dO^T
+//   * the canonical MN-major SWIZZLE_128B wgmma operand  (the 64 channels = N, rows = K)           -> O = P V, dV = P^T dO, dK = dS^T Q, dQ = dS K
+// so nothing is transposed or loaded twice.  A whole score row (S <= 256) stays in the accumulator registers of its warpgroup: the
+// softmax needs no second pass over memory, and P / dS^T go straight from those registers into the A operand of the next wgmma.
 //
-// Scores live in TMEM with lanes = query rows: one thread owns one query row (tcgen05.ld 32x32b), so row max / row sum / log-sum-exp
-// are thread-local -- no shuffles, no shared-memory reductions.
-//
-// Forward, one CTA per (sample, head, 128-query tile), 2-3 CTAs per SM:
-//   warp 0   TMA: Q tile, K, V
-//   warp 1   MMA issuer: S = Q K^T (M 128, N = Sp, K 64) -> TMEM[0, Sp);  O += P_j V_j per 64-key chunk -> TMEM[0, 64) (the score columns of
-//            chunk 0 have been consumed by then)
-//   warps 2-5 softmax: pass 1 row max over TMEM, pass 2 exp2 / row sum / bf16 P chunks into a 2-slot smem ring; epilogue O / l -> global
-// Backward, one CTA per (sample, head), blocks of 128 queries x 128 keys, TMEM: S | dP | dQ_0 | dQ_1 | dK | dV = 512 columns:
-//   warp 1   per block: S = Q K^T, dP = dO V^T;  then dQ_q += dS K, dK_t += dS^T Q, dV_t += P^T dO
-//   warps 2-9 (two threads per query row, 64 key columns each): P = exp2(s - lse), dS = P (dP - D) -> smem images; dK / dV / dQ epilogues
+// Forward, one CTA per (sample, head, 128-query tile): two warpgroups of 64 query rows each; thread 0 issues the TMA loads.
+// Backward, one CTA per (sample, head): the two warpgroups take alternate 64-key blocks; per (key block, 64-query block)
+//   S^T = K Q^T, dP^T = V dO^T (registers) -> P^T, dS^T -> dV += P^T dO, dK += dS^T Q (register A operands), dQ_q += dS K (dS^T staged
+//   in shared memory, fp32 dQ accumulated in shared memory across the key blocks of both warpgroups)
 #include "common.cuh"
 
 #include <math_constants.h>
@@ -27,60 +20,10 @@
 namespace {
 
 constexpr float LOG2E = 1.4426950408889634f;
-constexpr int BOX128 = 128 * 128;  // bytes of a [128 rows x 64 ch] image
+constexpr int BOX64 = 64 * 128;  // bytes of a [64 rows x 64 ch] image
 
-__device__ __forceinline__ uint64_t desc_k_sw128(uint32_t saddr) {
-  // K-major, 128-byte swizzle: ((8,n),2):((8,SBO),1) in 16-byte units (cute::UMMA::make_umma_desc<Major::K>): rows of 128 B, 8-row groups 1 KB apart;
-  // a k-step of 16 elements advances the start address by 32 B inside the swizzle atom
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-__device__ __forceinline__ uint64_t desc_mn_sw128(uint32_t saddr, uint32_t lbo_bytes) {
-  // MN-major, 128-byte swizzle: ((8,n),(8,k)):((1,LBO),(8,SBO)): 64 contiguous M/N elements per row, LBO between 64-element groups, SBO = 1 KB
-  // between 8-row (k) groups; a k-step of 16 rows advances the start address by 2 KB (same construction as wgrad_tc.cu)
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-// kind::f16 instruction descriptor: D = F32, A = B = BF16; bits 15 / 16: A / B is MN-major
-__device__ __forceinline__ uint32_t make_idesc(int M, int N, int a_mn, int b_mn) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)a_mn << 15) | ((uint32_t)b_mn << 16) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-__device__ __forceinline__ void umma(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void arrive(uint64_t* bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory"); }
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,"
-      "%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]),
-        "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]),
-        "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
+__device__ __forceinline__ uint64_t desc_k(uint32_t saddr) { return wgmma_desc(saddr, 16, 1024, WG_SW128); }      // K-major: +32 B per k-step
+__device__ __forceinline__ uint64_t desc_mn(uint32_t saddr) { return wgmma_desc(saddr, BOX64, 1024, WG_SW128); }  // MN-major: +2 KB per k-step
 __device__ __forceinline__ float ex2(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
@@ -94,202 +37,169 @@ __device__ __forceinline__ float mask_add(const float* amask, const uint8_t* kpm
   if (amask && q < S) return amask[((size_t)b * S + q) * S + t] * LOG2E;
   return 0.f;
 }
-// write 32 consecutive values of one row (columns c32 * 32 .. + 31 of a 64-column box) as bf16 into a SWIZZLE_128B image
-__device__ __forceinline__ void store_row32(uint8_t* box, int row, int c32, const float* v) {
+__device__ __forceinline__ void wg_bar(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); }
+// accumulator columns [16 kk, 16 kk + 16) of an m64n64 fp32 result, scaled, as the bf16 A operand of k-step kk
+__device__ __forceinline__ void to_a_frag(const float* acc, int kk, uint32_t* a) {
 #pragma unroll
-  for (int i = 0; i < 4; ++i) *reinterpret_cast<uint4*>(box + sw128(row, c32 * 4 + i)) = pack8(v + i * 8);
+  for (int i = 0; i < 4; ++i) a[i] = pack_bf162(acc[8 * kk + 2 * i], acc[8 * kk + 2 * i + 1]);
 }
-// 64 fp32 accumulator columns of this thread's TMEM lane -> one 128-byte bf16 row in global memory
-__device__ __forceinline__ void store_acc64(bf16* dst, uint32_t taddr, float mul, bool ok) {
+// m64n64 fp32 accumulator * mul -> bf16 rows row0 + r (r < 64, row0 + r < S) of a [.. x 64] global matrix with leading dimension ld
+__device__ __forceinline__ void store_acc(bf16* dst, int ld, const float* acc, float mul, int row0, int S) {
+  const int lane = threadIdx.x & 31, r = ((threadIdx.x & 127) >> 5) * 16 + (lane >> 2);
 #pragma unroll
-  for (int hlf = 0; hlf < 2; ++hlf) {
-    uint32_t r[32];
-    tmem_ld32(taddr + hlf * 32, r);
-    if (ok) {
+  for (int h = 0; h < 2; ++h) {
+    const int row = row0 + r + 8 * h;
+    if (row < S) {
 #pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        float f[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) f[e] = __uint_as_float(r[i * 8 + e]) * mul;
-        stg16(dst + hlf * 32 + i * 8, pack8(f));
-      }
+      for (int j = 0; j < 8; ++j)
+        *reinterpret_cast<uint32_t*>(dst + (size_t)row * ld + 8 * j + 2 * (lane & 3)) = pack_bf162(acc[4 * j + 2 * h] * mul, acc[4 * j + 2 * h + 1] * mul);
     }
   }
 }
 
 // ------------------------------------------------------------------------------------------------------------- forward
-constexpr int FW_THREADS = 64 + 128;
+constexpr int FW_THREADS = 256;
 
-__global__ void __launch_bounds__(FW_THREADS, 3)
-    mha_tc_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV, int S, int Sp, int H, int NQT, float scale,
-                      const float* __restrict__ amask, const uint8_t* __restrict__ kpm, bf16* __restrict__ O, int ldo, float* __restrict__ LSE,
-                      uint32_t tmem_cols) {
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+__global__ void __launch_bounds__(FW_THREADS, 1)
+    mha_tc_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV, int S, int NCH, int H, int NQT, float scale,
+                      const float* __restrict__ amask, const uint8_t* __restrict__ kpm, bf16* __restrict__ O, int ldo, float* __restrict__ LSE) {
+  const int tid = threadIdx.x, lane = tid & 31, wg = tid >> 7;
   int bid = blockIdx.x;
   const int qt = bid % NQT;
   bid /= NQT;
   const int h = bid % H, b = bid / H;
   const int C = H * 64;
+  const int Sk = NCH * 64;  // key rows loaded (zero-filled past the tensor)
 
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* sQ = smem;                 // [128 q][64]
-  uint8_t* sK = sQ + BOX128;          // [Sp t][64]
-  uint8_t* sV = sK + Sp * 128;        // [Sp t][64]
-  uint8_t* sP = sV + Sp * 128;        // 2 slots x [128 q][64 t]
-  __shared__ __align__(8) uint64_t bar_qk, bar_v, s_full, o_full, p_full[2], p_empty[2];
-  __shared__ uint32_t tmem_base_smem;
+  uint8_t* sK = sQ + 2 * BOX64;       // [Sk t][64]
+  uint8_t* sV = sK + Sk * 128;        // [Sk t][64]
+  __shared__ __align__(8) uint64_t bar_qk, bar_v;
 
   if (tid == 0) {
-    mbar_init(&bar_qk, 1); mbar_init(&bar_v, 1); mbar_init(&s_full, 1); mbar_init(&o_full, 1);
-    for (int i = 0; i < 2; ++i) { mbar_init(&p_full[i], 4); mbar_init(&p_empty[i], 1); }
+    mbar_init(&bar_qk, 1);
+    mbar_init(&bar_v, 1);
     fence_mbar_init();
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_smem)), "r"(tmem_cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  fence_before();
   __syncthreads();
-  fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
   pdl_wait();
   pdl_trigger();
-
-  const int nsteps = Sp / 16;             // 16-key MMA steps of P V
-  const int nchunks = (nsteps + 3) / 4;   // 64-key P chunks
-
-  if (warp == 0) {
-    if (lane == 0) {
-      const int row0 = b * S;
-      mbar_expect_tx(&bar_qk, (uint32_t)(BOX128 + Sp * 128));
-      tma_load_2d(sQ, &tmQ, &bar_qk, h * 64, row0 + qt * 128);
-      tma_load_2d(sK, &tmKV, &bar_qk, C + h * 64, row0);
-      mbar_expect_tx(&bar_v, (uint32_t)(Sp * 128));
-      tma_load_2d(sV, &tmKV, &bar_v, 2 * C + h * 64, row0);
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      mbar_wait(&bar_qk, 0);
-      fence_after();
-      const uint32_t id_s = make_idesc(128, Sp, 0, 0);
-#pragma unroll
-      for (int k = 0; k < 4; ++k) umma(tmem_base, desc_k_sw128(smem_u32(sQ) + k * 32), desc_k_sw128(smem_u32(sK) + k * 32), id_s, k ? 1u : 0u);
-      commit(&s_full);
-      mbar_wait(&bar_v, 0);
-      const uint32_t id_o = make_idesc(128, 64, 0, 1);
-      for (int j = 0; j < nchunks; ++j) {
-        const int slot = j & 1;
-        mbar_wait(&p_full[slot], (j >> 1) & 1);
-        fence_after();
-        const int steps = min(4, nsteps - 4 * j);
-        for (int kk = 0; kk < steps; ++kk)
-          umma(tmem_base, desc_k_sw128(smem_u32(sP) + slot * BOX128 + kk * 32), desc_mn_sw128(smem_u32(sV) + (4 * j + kk) * 2048, BOX128), id_o,
-               (j | kk) ? 1u : 0u);
-        commit(&p_empty[slot]);
-      }
-      commit(&o_full);
-    }
-  } else {
-    const int quad = warp & 3;
-    const int row = quad * 32 + lane;   // TMEM lane == query row of the tile
-    const int q = qt * 128 + row;
-    const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16);
-    const float sc2 = scale * LOG2E;
-    const bool masked = (amask != nullptr) || (kpm != nullptr);
-    mbar_wait(&s_full, 0);
-    fence_after();
-    // ---- pass 1: row maximum (exp2 domain; scale > 0, so the unmasked chunks take the maximum of the raw scores)
-    float mraw = -CUDART_INF_F, m = -CUDART_INF_F;
-    for (int c0 = 0; c0 < Sp; c0 += 32) {
-      uint32_t r[32];
-      tmem_ld32(taddr + c0, r);
-      if (!masked && c0 + 32 <= S) {
-#pragma unroll
-        for (int i = 0; i < 32; ++i) mraw = fmaxf(mraw, __uint_as_float(r[i]));
-      } else {
-#pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          const int t = c0 + i;
-          if (t < S) {
-            float v = __uint_as_float(r[i]) * sc2;
-            if (masked) v += mask_add(amask, kpm, b, S, q, t);
-            m = fmaxf(m, v);
-          }
-        }
-      }
-    }
-    m = fmaxf(m, mraw * sc2);
-    const float msafe = (m == -CUDART_INF_F) ? 0.f : m;  // a fully masked row must not produce inf - inf
-    // ---- pass 2: P = exp2(sc2 * s + mask - m), row sum, bf16 chunks for the tensor core
-    float l = 0.f;
-    for (int j = 0; j < nchunks; ++j) {
-      const int slot = j & 1;
-      if (j >= 2) mbar_wait(&p_empty[slot], ((j >> 1) - 1) & 1);
-      uint8_t* box = sP + slot * BOX128;
-#pragma unroll
-      for (int hlf = 0; hlf < 2; ++hlf) {
-        const int c0 = j * 64 + hlf * 32;
-        if (c0 < Sp) {
-          uint32_t r[32];
-          float p[32];
-          tmem_ld32(taddr + c0, r);
-          if (!masked && c0 + 32 <= S) {
-#pragma unroll
-            for (int i = 0; i < 32; ++i) {
-              p[i] = ex2(fmaf(__uint_as_float(r[i]), sc2, -msafe));
-              l += p[i];
-            }
-          } else {
-#pragma unroll
-            for (int i = 0; i < 32; ++i) {
-              const int t = c0 + i;
-              float pv = 0.f;
-              if (t < S) {
-                float v = fmaf(__uint_as_float(r[i]), sc2, -msafe);
-                if (masked) v += mask_add(amask, kpm, b, S, q, t);
-                pv = ex2(v);
-              }
-              p[i] = pv;
-              l += pv;
-            }
-          }
-          store_row32(box, row, hlf, p);
-        }
-      }
-      fence_proxy_async();  // generic-proxy writes of P -> visible to the tensor core's async-proxy reads
-      fence_before();       // this thread's TMEM reads of the chunk's score columns are complete (P V overwrites columns [0, 64))
-      __syncwarp();
-      if (lane == 0) arrive(&p_full[slot]);
-    }
-    // ---- epilogue: O / l
-    mbar_wait(&o_full, 0);
-    fence_after();
-    const bool ok = q < S;
-    const float inv = 1.0f / l;  // a fully masked row gives 0 * inf = NaN, like softmax over an all -inf row in the reference
-    store_acc64(O + ((size_t)b * S + (ok ? q : 0)) * ldo + h * 64, taddr, inv, ok);
-    if (ok) LSE[((size_t)b * H + h) * S + q] = m + log2f(l);
-    fence_before();
+  if (tid == 0) {
+    const int row0 = b * S;
+    mbar_expect_tx(&bar_qk, (uint32_t)(2 * BOX64 + Sk * 128));
+    tma_load_2d(sQ, &tmQ, &bar_qk, h * 64, row0 + qt * 128);
+    tma_load_2d(sK, &tmKV, &bar_qk, C + h * 64, row0);
+    mbar_expect_tx(&bar_v, (uint32_t)(Sk * 128));
+    tma_load_2d(sV, &tmKV, &bar_v, 2 * C + h * 64, row0);
   }
-  __syncthreads();
-  if (warp == 1) {
-    fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(tmem_cols) : "memory");
+
+  const int rl = ((tid & 127) >> 5) * 16 + (lane >> 2);  // query row (within the warpgroup's 64) of acc[4j + {0,1}]; + 8 for {2,3}
+  const int q0 = qt * 128 + wg * 64;
+  const float sc2 = scale * LOG2E;
+  const bool masked = (amask != nullptr) || (kpm != nullptr);
+  const uint32_t aQ = smem_u32(sQ) + wg * BOX64, aK = smem_u32(sK), aV = smem_u32(sV);
+
+  // ---- S = Q K^T, 64-key chunks
+  float sacc[4][32];
+  mbar_wait(&bar_qk, 0);
+  wgmma_fence();
+#pragma unroll
+  for (int c = 0; c < 4; ++c)
+    if (c < NCH) {
+#pragma unroll
+      for (int k = 0; k < 4; ++k) wgmma_m64n64<0, 0>(sacc[c], desc_k(aQ + k * 32), desc_k(aK + c * BOX64 + k * 32), k ? 1u : 0u);
+    }
+  wgmma_commit();
+  wgmma_wait<0>();
+#pragma unroll
+  for (int c = 0; c < 4; ++c) wgmma_reg_fence<32>(sacc[c]);
+
+  // ---- softmax in the exp2 domain; a row is spread over the 4 threads of a quad
+  float m[2] = {-CUDART_INF_F, -CUDART_INF_F};
+#pragma unroll
+  for (int c = 0; c < 4; ++c)
+    if (c < NCH) {
+#pragma unroll
+      for (int i = 0; i < 32; ++i) {
+        const int hh = (i >> 1) & 1, q = q0 + rl + 8 * hh, t = c * 64 + 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+        float v = -CUDART_INF_F;
+        if (t < S) {
+          v = sacc[c][i] * sc2;
+          if (masked) v += mask_add(amask, kpm, b, S, q, t);
+        }
+        sacc[c][i] = v;
+        m[hh] = fmaxf(m[hh], v);
+      }
+    }
+  float l[2] = {0.f, 0.f}, msafe[2];
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    m[hh] = fmaxf(m[hh], __shfl_xor_sync(0xffffffffu, m[hh], 1));
+    m[hh] = fmaxf(m[hh], __shfl_xor_sync(0xffffffffu, m[hh], 2));
+    msafe[hh] = (m[hh] == -CUDART_INF_F) ? 0.f : m[hh];  // a fully masked row must not produce inf - inf
+  }
+#pragma unroll
+  for (int c = 0; c < 4; ++c)
+    if (c < NCH) {
+#pragma unroll
+      for (int i = 0; i < 32; ++i) {
+        const int hh = (i >> 1) & 1;
+        const float pv = ex2(sacc[c][i] - msafe[hh]);
+        sacc[c][i] = pv;
+        l[hh] += pv;
+      }
+    }
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    l[hh] += __shfl_xor_sync(0xffffffffu, l[hh], 1);
+    l[hh] += __shfl_xor_sync(0xffffffffu, l[hh], 2);
+  }
+
+  // ---- O = P V (P as bf16 register operand, V MN-major)
+  float oacc[32];
+  mbar_wait(&bar_v, 0);
+  wgmma_fence();
+#pragma unroll
+  for (int c = 0; c < 4; ++c)
+    if (c < NCH) {
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) {
+        uint32_t a[4];
+        to_a_frag(sacc[c], kk, a);
+        wgmma_m64n64_rs<1>(oacc, a, desc_mn(aV + (c * 64 + kk * 16) * 128), (c | kk) ? 1u : 0u);
+      }
+    }
+  wgmma_commit();
+  wgmma_wait<0>();
+  wgmma_reg_fence<32>(oacc);
+
+  // ---- epilogue: O / l (a fully masked row gives 0 * inf = NaN, like softmax over an all -inf row in the reference), LSE
+  const float inv[2] = {1.0f / l[0], 1.0f / l[1]};
+#pragma unroll
+  for (int i = 0; i < 32; ++i) oacc[i] *= inv[(i >> 1) & 1];
+  store_acc(O + (size_t)b * S * ldo + h * 64, ldo, oacc, 1.0f, q0, S);
+  if ((lane & 3) == 0) {
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const int q = q0 + rl + 8 * hh;
+      if (q < S) LSE[((size_t)b * H + h) * S + q] = m[hh] + log2f(l[hh]);
+    }
   }
 }
 
 // ------------------------------------------------------------------------------------------------------------ backward
-constexpr int BW_THREADS = 64 + 256;
-constexpr uint32_t T_S = 0, T_DP = 128, T_DQ = 256, T_DK = 384, T_DV = 448;
+constexpr int BW_THREADS = 256;
 
 __global__ void __launch_bounds__(BW_THREADS, 1)
     mha_tc_bwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmDO, const bf16* __restrict__ O,
-                      const bf16* __restrict__ DO, int ldo, const float* __restrict__ LSE, int S, int Sp, int H, int NT, float scale,
+                      const bf16* __restrict__ DO, int ldo, const float* __restrict__ LSE, int S, int H, int NB, float scale,
                       const float* __restrict__ amask, const uint8_t* __restrict__ kpm, bf16* __restrict__ DQKV, int lddq) {
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int tid = threadIdx.x, lane = tid & 31, wg = tid >> 7;
   const int h = blockIdx.x % H, b = blockIdx.x / H;
   const int C = H * 64;
-  const int R = NT * 128;  // rows of every operand image
+  const int R = NB * 64;  // rows of every operand image
 
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -297,187 +207,133 @@ __global__ void __launch_bounds__(BW_THREADS, 1)
   uint8_t* sK = sQ + R * 128;
   uint8_t* sV = sK + R * 128;
   uint8_t* sdO = sV + R * 128;
-  uint8_t* sP = sdO + R * 128;     // [128 q][128 t] = two 64-key boxes
-  uint8_t* sdS = sP + 2 * BOX128;
-  __shared__ __align__(8) uint64_t bar_ld, sdp_full, pds_full, pds_empty, dkv_full, dkv_free, dq_full;
-  __shared__ uint32_t tmem_base_smem;
+  uint8_t* sdST = sdO + R * 128;                              // per warpgroup: dS^T [64 keys][64 queries]
+  float* sdQ = reinterpret_cast<float*>(sdST + 2 * BOX64);    // fp32 [R][64]
+  float* sLSE = sdQ + R * 64;                                 // [R]
+  float* sD = sLSE + R;                                       // [R]: D = sum_c dO O
+  __shared__ __align__(8) uint64_t bar_ld;
 
   if (tid == 0) {
-    mbar_init(&bar_ld, 1); mbar_init(&sdp_full, 1); mbar_init(&pds_full, 8); mbar_init(&pds_empty, 1);
-    mbar_init(&dkv_full, 1); mbar_init(&dkv_free, 8); mbar_init(&dq_full, 1);
+    mbar_init(&bar_ld, 1);
     fence_mbar_init();
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_smem)), "r"(512) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  fence_before();
   __syncthreads();
-  fence_after();
-  const uint32_t tb = tmem_base_smem;
   pdl_wait();
   pdl_trigger();
-
-  if (warp == 0) {
-    if (lane == 0) {
-      const int row0 = b * S;
-      mbar_expect_tx(&bar_ld, (uint32_t)(4 * R * 128));
-      tma_load_2d(sQ, &tmQKV, &bar_ld, h * 64, row0);
-      tma_load_2d(sK, &tmQKV, &bar_ld, C + h * 64, row0);
-      tma_load_2d(sV, &tmQKV, &bar_ld, 2 * C + h * 64, row0);
-      tma_load_2d(sdO, &tmDO, &bar_ld, h * 64, row0);
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      mbar_wait(&bar_ld, 0);
-      fence_after();
-      const uint32_t aQ = smem_u32(sQ), aK = smem_u32(sK), aV = smem_u32(sV), aDO = smem_u32(sdO), aP = smem_u32(sP), aDS = smem_u32(sdS);
-      const uint32_t id_q = make_idesc(128, 64, 0, 1), id_kv = make_idesc(128, 64, 1, 1);
-      int i = 0;
-      for (int tt = 0; tt < NT; ++tt) {
-        const int NB = min(128, Sp - tt * 128);
-        const uint32_t id_s = make_idesc(128, NB, 0, 0);
-        for (int qt = 0; qt < NT; ++qt, ++i) {
-          // S = Q K^T, dP = dO V^T  (the softmax threads have drained the previous block: pds_full(i-1) was awaited below)
+  if (tid == 0) {
+    const int row0 = b * S;
+    mbar_expect_tx(&bar_ld, (uint32_t)(4 * R * 128));
+    tma_load_2d(sQ, &tmQKV, &bar_ld, h * 64, row0);
+    tma_load_2d(sK, &tmQKV, &bar_ld, C + h * 64, row0);
+    tma_load_2d(sV, &tmQKV, &bar_ld, 2 * C + h * 64, row0);
+    tma_load_2d(sdO, &tmDO, &bar_ld, h * 64, row0);
+  }
+  for (int i = tid; i < R * 64; i += BW_THREADS) sdQ[i] = 0.f;
+  for (int q = tid; q < R; q += BW_THREADS) {
+    float lv = 0.f, d = 0.f;
+    if (q < S) {
+      lv = LSE[((size_t)b * H + h) * S + q];
+      const bf16* orow = O + ((size_t)b * S + q) * ldo + h * 64;
+      const bf16* drow = DO + ((size_t)b * S + q) * ldo + h * 64;
 #pragma unroll
-          for (int k = 0; k < 4; ++k) umma(tb + T_S, desc_k_sw128(aQ + qt * BOX128 + k * 32), desc_k_sw128(aK + tt * BOX128 + k * 32), id_s, k ? 1u : 0u);
+      for (int ch = 0; ch < 8; ++ch) {
+        float a[8], c[8];
+        unpack8(ldg16(orow + ch * 8), a);
+        unpack8(ldg16(drow + ch * 8), c);
 #pragma unroll
-          for (int k = 0; k < 4; ++k) umma(tb + T_DP, desc_k_sw128(aDO + qt * BOX128 + k * 32), desc_k_sw128(aV + tt * BOX128 + k * 32), id_s, k ? 1u : 0u);
-          commit(&sdp_full);
-          mbar_wait(&pds_full, i & 1);
-          fence_after();
-          if (qt == 0 && tt > 0) {  // dK / dV of the previous key tile have been read out
-            mbar_wait(&dkv_free, (tt - 1) & 1);
-            fence_after();
-          }
-          // dQ_q += dS K_t   (A = dS K-major over the keys, B = K MN-major)
-          for (int kk = 0; kk < NB / 16; ++kk)
-            umma(tb + T_DQ + 64 * qt, desc_k_sw128(aDS + (kk >> 2) * BOX128 + (kk & 3) * 32), desc_mn_sw128(aK + (tt * 128 + kk * 16) * 128, BOX128), id_q,
-                 (tt | kk) ? 1u : 0u);
-          // dK_t += dS^T Q_q,  dV_t += P^T dO_q   (A MN-major over the keys: two 64-key boxes, reduction over the 128 query rows)
-#pragma unroll
-          for (int kk = 0; kk < 8; ++kk)
-            umma(tb + T_DK, desc_mn_sw128(aDS + kk * 2048, BOX128), desc_mn_sw128(aQ + (qt * 128 + kk * 16) * 128, BOX128), id_kv, (qt | kk) ? 1u : 0u);
-#pragma unroll
-          for (int kk = 0; kk < 8; ++kk)
-            umma(tb + T_DV, desc_mn_sw128(aP + kk * 2048, BOX128), desc_mn_sw128(aDO + (qt * 128 + kk * 16) * 128, BOX128), id_kv, (qt | kk) ? 1u : 0u);
-          commit(&pds_empty);
-          if (qt == NT - 1) commit(&dkv_full);
-        }
-      }
-      commit(&dq_full);
-    }
-  } else {
-    const int quad = warp & 3, half = (warp - 2) >> 2;
-    const int row = quad * 32 + lane;
-    const uint32_t taddr = tb + ((uint32_t)(quad * 32) << 16);
-    const float sc2 = scale * LOG2E;
-    const bool masked = (amask != nullptr) || (kpm != nullptr);
-    // per query row of each tile: log-sum-exp and D = sum_c dO O
-    float lse0 = 0.f, lse1 = 0.f, D0 = 0.f, D1 = 0.f;
-    for (int qt = 0; qt < NT; ++qt) {
-      const int q = qt * 128 + row;
-      if (q < S) {
-        const float lv = LSE[((size_t)b * H + h) * S + q];
-        const bf16* orow = O + ((size_t)b * S + q) * ldo + h * 64;
-        const bf16* drow = DO + ((size_t)b * S + q) * ldo + h * 64;
-        float d = 0.f;
-#pragma unroll
-        for (int ch = 0; ch < 8; ++ch) {
-          float a[8], c[8];
-          unpack8(ldg16(orow + ch * 8), a);
-          unpack8(ldg16(drow + ch * 8), c);
-#pragma unroll
-          for (int e = 0; e < 8; ++e) d = fmaf(a[e], c[e], d);
-        }
-        if (qt == 0) { lse0 = lv; D0 = d; } else { lse1 = lv; D1 = d; }
+        for (int e = 0; e < 8; ++e) d = fmaf(a[e], c[e], d);
       }
     }
-    bf16* dbase = DQKV + (size_t)b * S * lddq + h * 64;
-    int i = 0;
-    for (int tt = 0; tt < NT; ++tt) {
-      const int NB = min(128, Sp - tt * 128);
-      for (int qt = 0; qt < NT; ++qt, ++i) {
-        const int q = qt * 128 + row;
-        const bool q_ok = q < S;
-        const float lse_q = qt ? lse1 : lse0, D_q = qt ? D1 : D0;
-        mbar_wait(&sdp_full, i & 1);
-        fence_after();
-        if (i > 0) mbar_wait(&pds_empty, (i - 1) & 1);  // the previous block's output MMAs have read sP / sdS
-#pragma unroll
-        for (int cc = 0; cc < 2; ++cc) {
-          const int c0 = half * 64 + cc * 32;
-          if (c0 < NB) {
-            uint32_t rs[32], rd[32];
-            float p[32], ds[32];
-            tmem_ld32(taddr + T_S + c0, rs);
-            tmem_ld32(taddr + T_DP + c0, rd);
-            const int t0 = tt * 128 + c0;
-            const bool fast = !masked && q_ok && (t0 + 32 <= S);
-            if (fast) {
-#pragma unroll
-              for (int e = 0; e < 32; ++e) {
-                const float pv = ex2(fmaf(__uint_as_float(rs[e]), sc2, -lse_q));
-                p[e] = pv;
-                ds[e] = pv * (__uint_as_float(rd[e]) - D_q);
-              }
-            } else {
-#pragma unroll
-              for (int e = 0; e < 32; ++e) {
-                const int t = t0 + e;
-                float pv = 0.f, dv = 0.f;
-                if (q_ok && t < S) {
-                  float v = fmaf(__uint_as_float(rs[e]), sc2, -lse_q);
-                  if (masked) v += mask_add(amask, kpm, b, S, q, t);
-                  pv = ex2(v);
-                  dv = pv * (__uint_as_float(rd[e]) - D_q);
-                  if (pv == 0.f) dv = 0.f;  // masked keys: exactly zero whatever dP holds
-                }
-                p[e] = pv;
-                ds[e] = dv;
-              }
-            }
-            store_row32(sP + half * BOX128, row, cc, p);
-            store_row32(sdS + half * BOX128, row, cc, ds);
-          }
-        }
-        fence_proxy_async();
-        fence_before();
-        __syncwarp();
-        if (lane == 0) arrive(&pds_full);
-        if (qt == NT - 1) {  // this key tile is complete: dK (first four warps) / dV (last four), one key row per thread
-          mbar_wait(&dkv_full, tt & 1);
-          fence_after();
-          const int t = tt * 128 + row;
-          const bool ok = t < S;
-          bf16* dst = dbase + (size_t)(ok ? t : 0) * lddq + (half ? 2 * C : C);
-          store_acc64(dst, taddr + (half ? T_DV : T_DK), half ? 1.0f : scale, ok);
-          fence_before();
-          __syncwarp();
-          if (lane == 0) arrive(&dkv_free);
-        }
-      }
-    }
-    mbar_wait(&dq_full, 0);
-    fence_after();
-    if (half < NT) {
-      const int q = half * 128 + row;
-      const bool ok = q < S;
-      store_acc64(dbase + (size_t)(ok ? q : 0) * lddq, taddr + T_DQ + 64 * half, scale, ok);
-    }
-    fence_before();
+    sLSE[q] = lv;
+    sD[q] = d;
   }
   __syncthreads();
-  if (warp == 1) {
-    fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tb), "r"(512) : "memory");
+  mbar_wait(&bar_ld, 0);
+
+  const int rl = ((tid & 127) >> 5) * 16 + (lane >> 2);  // key row (within the block) of acc[4j + {0,1}]; + 8 for {2,3}
+  const float sc2 = scale * LOG2E;
+  const bool masked = (amask != nullptr) || (kpm != nullptr);
+  const uint32_t aQ = smem_u32(sQ), aK = smem_u32(sK), aV = smem_u32(sV), aDO = smem_u32(sdO), aDS = smem_u32(sdST) + wg * BOX64;
+  uint8_t* my_dST = sdST + wg * BOX64;
+  bf16* dbase = DQKV + (size_t)b * S * lddq + h * 64;
+
+  for (int kb = wg; kb < NB; kb += 2) {
+    float dk[32], dv[32];
+    for (int qb = 0; qb < NB; ++qb) {
+      float st[32], dpt[32];
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k) wgmma_m64n64<0, 0>(st, desc_k(aK + kb * BOX64 + k * 32), desc_k(aQ + qb * BOX64 + k * 32), k ? 1u : 0u);
+#pragma unroll
+      for (int k = 0; k < 4; ++k) wgmma_m64n64<0, 0>(dpt, desc_k(aV + kb * BOX64 + k * 32), desc_k(aDO + qb * BOX64 + k * 32), k ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_reg_fence<32>(st);
+      wgmma_reg_fence<32>(dpt);
+      // P^T = exp2(s sc2 + mask - lse), dS^T = P^T (dP^T - D); zero outside the sequence and for masked keys
+#pragma unroll
+      for (int i = 0; i < 32; ++i) {
+        const int t = kb * 64 + rl + 8 * ((i >> 1) & 1), q = qb * 64 + 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+        float pv = 0.f, dv2 = 0.f;
+        if (q < S && t < S) {
+          float v = fmaf(st[i], sc2, -sLSE[q]);
+          if (masked) v += mask_add(amask, kpm, b, S, q, t);
+          pv = ex2(v);
+          dv2 = pv * (dpt[i] - sD[q]);
+          if (pv == 0.f) dv2 = 0.f;  // masked keys: exactly zero whatever dP holds
+        }
+        st[i] = pv;
+        dpt[i] = dv2;
+      }
+      // dS^T as bf16 [64 keys][64 queries] SWIZZLE_128B image: the MN-major A operand of dQ = dS K
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const int row = rl + 8 * hh;
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+          *reinterpret_cast<uint32_t*>(my_dST + sw128(row, j) + 4 * (lane & 3)) = pack_bf162(dpt[4 * j + 2 * hh], dpt[4 * j + 2 * hh + 1]);
+      }
+      fence_proxy_async();
+      wg_bar(wg);
+      float dq[32];
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) {  // reduction over the 64 queries of the block
+        uint32_t a[4];
+        to_a_frag(st, kk, a);
+        wgmma_m64n64_rs<1>(dv, a, desc_mn(aDO + (qb * 64 + kk * 16) * 128), (qb | kk) ? 1u : 0u);
+        to_a_frag(dpt, kk, a);
+        wgmma_m64n64_rs<1>(dk, a, desc_mn(aQ + (qb * 64 + kk * 16) * 128), (qb | kk) ? 1u : 0u);
+      }
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk)  // reduction over the 64 keys of the block
+        wgmma_m64n64<1, 1>(dq, desc_mn(aDS + kk * 2048), desc_mn(aK + (kb * 64 + kk * 16) * 128), kk ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_reg_fence<32>(dv);
+      wgmma_reg_fence<32>(dk);
+      wgmma_reg_fence<32>(dq);
+#pragma unroll
+      for (int i = 0; i < 32; ++i)  // dQ rows = queries of the block, columns = channels
+        atomicAdd(sdQ + (qb * 64 + rl + 8 * ((i >> 1) & 1)) * 64 + 8 * (i >> 2) + 2 * (lane & 3) + (i & 1), dq[i]);
+      wg_bar(wg);  // every thread's reads of the dS^T image are complete before it is rewritten
+    }
+    store_acc(dbase + C, lddq, dk, scale, kb * 64, S);
+    store_acc(dbase + 2 * C, lddq, dv, 1.0f, kb * 64, S);
+  }
+  __syncthreads();
+  for (int i = tid; i < S * 8; i += BW_THREADS) {  // dQ: 8 chunks of 8 channels per query row
+    const int q = i >> 3, c8 = (i & 7) * 8;
+    float f[8];
+#pragma unroll
+    for (int e = 0; e < 8; ++e) f[e] = sdQ[q * 64 + c8 + e] * scale;
+    stg16(dbase + (size_t)q * lddq + c8, pack8(f));
   }
 }
 
-// bit 0: tcgen05 forward, bit 1: tcgen05 backward, bit 2: also for heads with an ADDITIVE mask.  Default 3: additive masks (the causal mask of the
-// CLIP text tower, S = 77) stay on the mma.sync kernels -- one thread owns one query row here, so the mask is read row-per-thread (32 cache
-// lines per load instruction) and the short sequences leave too few warps to hide that latency: measured 216 / 407 us (fwd / bwd, B 256, S 77,
-// 8 heads, causal) against 65 / 305 us on mma.sync, while the unmasked ViT-B shape (S 197, 12 heads) runs 156 / 462 us against 213 / 907 us.
+// bit 0: wgmma forward, bit 1: wgmma backward, bit 2: also for heads with an ADDITIVE mask.  Default 3: additive masks (the causal mask of
+// the CLIP text tower, S = 77) stay on the mma.sync kernels, which read the [S, S] mask in coalesced tiles; here every thread gathers
+// single mask values of its score fragment.
 int g_impl = -1;
 int impl() {
   if (g_impl < 0) {
@@ -499,16 +355,15 @@ extern "C" int cvb_set_mha_impl(int mask) {
 int cvb_mha_fwd_tc(const void* QKV, int ldq, int B, int S, int H, int head_dim, float scale, const float* amask, const unsigned char* kpm, void* O,
                    int ldo, float* LSE, cudaStream_t st) {
   if (head_dim != 64 || !(impl() & 1) || S > 256 || (amask && !(impl() & 4))) return -1;
-  const int Sp = (S + 15) / 16 * 16;
+  const int NCH = (S + 63) / 64;
   const int NQT = (S + 127) / 128;
   CUtensorMap tmQ, tmKV;
   if (cvb_make_tmap_2d_c64(&tmQ, QKV, (int64_t)B * S, 3 * H * 64, ldq, 128)) return 1;
-  if (cvb_make_tmap_2d_c64(&tmKV, QKV, (int64_t)B * S, 3 * H * 64, ldq, Sp)) return 1;
-  const size_t smem = (size_t)BOX128 + (size_t)2 * Sp * 128 + 2 * BOX128 + 1024;
-  const uint32_t cols = Sp <= 64 ? 64u : (Sp <= 128 ? 128u : 256u);
+  if (cvb_make_tmap_2d_c64(&tmKV, QKV, (int64_t)B * S, 3 * H * 64, ldq, NCH * 64)) return 1;
+  const size_t smem = (size_t)2 * BOX64 + (size_t)2 * NCH * BOX64 + 1024;
   static bool attr = false;
-  if (!attr) { CVB_CUDA(cudaFuncSetAttribute(mha_tc_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024)); attr = true; }
-  CVB_CUDA(cvb_launch(mha_tc_fwd_kernel, B * H * NQT, FW_THREADS, smem, st, tmQ, tmKV, S, Sp, H, NQT, scale, amask, kpm, static_cast<bf16*>(O), ldo, LSE, cols));
+  if (!attr) { CVB_CUDA(cudaFuncSetAttribute(mha_tc_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024)); attr = true; }
+  CVB_CUDA(cvb_launch(mha_tc_fwd_kernel, B * H * NQT, FW_THREADS, smem, st, tmQ, tmKV, S, NCH, H, NQT, scale, amask, kpm, static_cast<bf16*>(O), ldo, LSE));
   CVB_LAUNCH_CHECK();
   return 0;
 }
@@ -516,17 +371,17 @@ int cvb_mha_fwd_tc(const void* QKV, int ldq, int B, int S, int H, int head_dim, 
 int cvb_mha_bwd_tc(const void* QKV, int ldq, const void* O, const void* DO, int ldo, const float* LSE, int B, int S, int H, int head_dim, float scale,
                    const float* amask, const unsigned char* kpm, void* DQKV, int lddq, cudaStream_t st) {
   if (head_dim != 64 || !(impl() & 2) || S > 256 || (amask && !(impl() & 4))) return -1;
-  const int Sp = (S + 15) / 16 * 16;
-  const int NT = (S + 127) / 128;
-  const int R = NT * 128;
+  const int NB = (S + 63) / 64;
+  const int R = NB * 64;
   CUtensorMap tmQKV, tmDO;
   if (cvb_make_tmap_2d_c64(&tmQKV, QKV, (int64_t)B * S, 3 * H * 64, ldq, R)) return 1;
   if (cvb_make_tmap_2d_c64(&tmDO, DO, (int64_t)B * S, H * 64, ldo, R)) return 1;
-  const size_t smem = (size_t)4 * R * 128 + 4 * BOX128 + 1024;
+  // Q, K, V, dO images + two dS^T images + fp32 dQ + LSE / D
+  const size_t smem = (size_t)4 * R * 128 + 2 * BOX64 + (size_t)R * 64 * 4 + (size_t)2 * R * 4 + 1024;
   static bool attr = false;
-  if (!attr) { CVB_CUDA(cudaFuncSetAttribute(mha_tc_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); attr = true; }
-  CVB_CUDA(cvb_launch(mha_tc_bwd_kernel, B * H, BW_THREADS, smem, st, tmQKV, tmDO, static_cast<const bf16*>(O), static_cast<const bf16*>(DO), ldo, LSE, S, Sp,
-                      H, NT, scale, amask, kpm, static_cast<bf16*>(DQKV), lddq));
+  if (!attr) { CVB_CUDA(cudaFuncSetAttribute(mha_tc_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024)); attr = true; }
+  CVB_CUDA(cvb_launch(mha_tc_bwd_kernel, B * H, BW_THREADS, smem, st, tmQKV, tmDO, static_cast<const bf16*>(O), static_cast<const bf16*>(DO), ldo, LSE, S,
+                      H, NB, scale, amask, kpm, static_cast<bf16*>(DQKV), lddq));
   CVB_LAUNCH_CHECK();
   return 0;
 }

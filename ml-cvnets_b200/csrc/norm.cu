@@ -1,4 +1,4 @@
-// BatchNorm / GroupNorm bookkeeping, materialisation, reductions, pooling, stem im2col and weight preparation (sm_100a).
+// BatchNorm / GroupNorm bookkeeping, materialisation, reductions, pooling, stem im2col and weight preparation (sm_90a).
 // All tensor passes are 16-byte vectorised over the channel dimension of the [M, C] channels-last matrix; per-channel
 // reductions keep a fixed channel chunk per thread (threads = multiple of C/8), reduce in smem, then one fp64 atomic per
 // channel per CTA.
@@ -28,9 +28,44 @@ int cvb_num_sms() {
   static int sms = 0;
   if (sms == 0) {
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 148;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
   }
   return sms;
+}
+__global__ void __launch_bounds__(256) det_add_kernel(const double* __restrict__ s, float* __restrict__ dst, int rows, int cols, int ld) {
+  pdl_wait();
+  pdl_trigger();
+  const int64_t n = (int64_t)rows * cols;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const int r = (int)(i / cols), c = (int)(i % cols);
+    dst[(size_t)r * ld + c] += (float)s[i];
+  }
+}
+int cvb_det_alloc(double** scratch, size_t n, cudaStream_t st) {
+  static bool pool_set = false;
+  if (!pool_set) {  // keep freed scratch in the device's default pool instead of returning it to the driver at every synchronisation
+    int dev = 0;
+    cudaMemPool_t pool;
+    CVB_CUDA(cudaGetDevice(&dev));
+    CVB_CUDA(cudaDeviceGetDefaultMemPool(&pool, dev));
+    uint64_t keep = UINT64_MAX;
+    CVB_CUDA(cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep));
+    pool_set = true;
+  }
+  CVB_CUDA(cudaMallocAsync(reinterpret_cast<void**>(scratch), n * sizeof(double), st));
+  CVB_CUDA(cudaMemsetAsync(*scratch, 0, n * sizeof(double), st));
+  return 0;
+}
+int cvb_det_add(const double* scratch, float* dst, int rows, int cols, int ld, cudaStream_t st) {
+  const int64_t n = (int64_t)rows * cols;
+  const int grid = (int)std::min<int64_t>((n + 255) / 256, 4 * (int64_t)cvb_num_sms());
+  CVB_CUDA(cvb_launch(det_add_kernel, grid, 256, 0, st, scratch, dst, rows, cols, ld));
+  CVB_LAUNCH_CHECK();
+  return 0;
+}
+int cvb_det_free(double* scratch, cudaStream_t st) {
+  CVB_CUDA(cudaFreeAsync(scratch, st));
+  return 0;
 }
 extern "C" int cvb_device_info(int* sm_count, int* cc_major, int* cc_minor) {
   int dev = 0;
@@ -298,9 +333,9 @@ __global__ void __launch_bounds__(NT) bn_bwd_reduce_kernel(const bf16* __restric
                                                            int64_t M, int C, int cgs, int rpp, int rows_per_cta) {
   pdl_wait();
   pdl_trigger();
-  extern __shared__ float sred[];  // [2][C]
+  extern __shared__ double sdred[];  // fp64: the threads' fp32 partials add exactly, whatever the order; [2][C]
   const int tid = threadIdx.x;
-  for (int i = tid; i < 2 * C; i += blockDim.x) sred[i] = 0.f;
+  for (int i = tid; i < 2 * C; i += blockDim.x) sdred[i] = 0.0;
   __syncthreads();
   const int cg = tid % cgs, rr = tid / cgs;
   const int c = cg * 8;
@@ -322,9 +357,9 @@ __global__ void __launch_bounds__(NT) bn_bwd_reduce_kernel(const bf16* __restric
     if (DZ) stg16(DZ + r * C + c, pack8(d));
   }
 #pragma unroll
-  for (int j = 0; j < 8; ++j) { atomicAdd(&sred[c + j], a0[j]); atomicAdd(&sred[C + c + j], a1[j]); }
+  for (int j = 0; j < 8; ++j) { atomicAdd(&sdred[c + j], (double)a0[j]); atomicAdd(&sdred[C + c + j], (double)a1[j]); }
   __syncthreads();
-  for (int i = tid; i < C; i += blockDim.x) { atomicAdd(s0 + i, (double)sred[i]); atomicAdd(s1 + i, (double)sred[C + i]); }
+  for (int i = tid; i < C; i += blockDim.x) { atomicAdd(s0 + i, sdred[i]); atomicAdd(s1 + i, sdred[C + i]); }
 }
 
 // column sums of a bf16 / fp32 [M, ld] matrix into fp32
@@ -386,10 +421,10 @@ __global__ void __launch_bounds__(NT) gn_bwd_stats_kernel(const bf16* __restrict
                                                           int cgs, int rpp, int rows_per_cta, double* dgamma, double* dbeta, double* sg, double* sgx) {
   pdl_wait();
   pdl_trigger();
-  extern __shared__ float sred[];  // [2][C]
+  extern __shared__ double sdred[];  // fp64: the threads' fp32 partials add exactly, whatever the order; [2][C]
   __shared__ float ws[2][NT / 32];
   const int tid = threadIdx.x, b = blockIdx.y;
-  for (int i = tid; i < 2 * C; i += blockDim.x) sred[i] = 0.f;
+  for (int i = tid; i < 2 * C; i += blockDim.x) sdred[i] = 0.0;
   __syncthreads();
   const int cg = tid % cgs, rr = tid / cgs, c = cg * 8;
   const float mu = mean[b], rs = rstd[b];
@@ -414,12 +449,12 @@ __global__ void __launch_bounds__(NT) gn_bwd_stats_kernel(const bf16* __restrict
       }
     }
 #pragma unroll
-    for (int j = 0; j < 8; ++j) { atomicAdd(&sred[c + j], db[j]); atomicAdd(&sred[C + c + j], dg[j]); }
+    for (int j = 0; j < 8; ++j) { atomicAdd(&sdred[c + j], (double)db[j]); atomicAdd(&sdred[C + c + j], (double)dg[j]); }
   }
   s1 = warp_sum(s1); s2 = warp_sum(s2);
   if ((tid & 31) == 0) { ws[0][tid >> 5] = s1; ws[1][tid >> 5] = s2; }
   __syncthreads();
-  for (int i = tid; i < C; i += blockDim.x) { atomicAdd(dbeta + i, (double)sred[i]); atomicAdd(dgamma + i, (double)sred[C + i]); }
+  for (int i = tid; i < C; i += blockDim.x) { atomicAdd(dbeta + i, sdred[i]); atomicAdd(dgamma + i, sdred[C + i]); }
   if (tid == 0) {
     float a = 0.f, q = 0.f;
     for (int i = 0; i < (int)(blockDim.x + 31) / 32; ++i) { a += ws[0][i]; q += ws[1][i]; }
@@ -447,7 +482,7 @@ __global__ void __launch_bounds__(NT) ln_bwd_kernel(const bf16* __restrict__ V, 
   __syncthreads();
   const int nch = C / 8;
   // The per-channel sums go to shared memory with one reduction per (row, channel): keeping them in registers (96 accumulators per lane at C = 768)
-  // cost 246 registers = 8 warps per SM, and the kernel ran at 1.3 TB/s on the ViT-B shape (profiles/r2_step_launches_vit_b16.csv)
+  // cost 246 registers = 8 warps per SM
   const float invC = 1.0f / (float)C;
   for (int64_t row = (int64_t)blockIdx.x * (NT / 32) + warp; row < M; row += (int64_t)gridDim.x * (NT / 32)) {
     const float mu = mean[row], rs = rstd[row];
@@ -598,9 +633,9 @@ __global__ void __launch_bounds__(NT) gn_bwd_apply_kernel(const bf16* __restrict
                                                           const float* __restrict__ gamma) {
   pdl_wait();
   pdl_trigger();
-  extern __shared__ float sred[];  // [C]
+  extern __shared__ double sdred[];  // fp64: the threads' fp32 partials add exactly, whatever the order; [C]
   const int tid = threadIdx.x;
-  if (col_sum) { for (int i = tid; i < C; i += blockDim.x) sred[i] = 0.f; __syncthreads(); }
+  if (col_sum) { for (int i = tid; i < C; i += blockDim.x) sdred[i] = 0.0; __syncthreads(); }
   const int cg = tid % cgs, rr = tid / cgs;
   const int c = cg * 8;
   float a0[8], gm[8];
@@ -632,9 +667,9 @@ __global__ void __launch_bounds__(NT) gn_bwd_apply_kernel(const bf16* __restrict
   }
   if (col_sum) {
 #pragma unroll
-    for (int j = 0; j < 8; ++j) atomicAdd(&sred[c + j], a0[j]);
+    for (int j = 0; j < 8; ++j) atomicAdd(&sdred[c + j], (double)a0[j]);
     __syncthreads();
-    for (int i = tid; i < C; i += blockDim.x) atomicAdd(col_sum + i, (double)sred[i]);
+    for (int i = tid; i < C; i += blockDim.x) atomicAdd(col_sum + i, sdred[i]);
   }
 }
 
@@ -643,11 +678,11 @@ __global__ void __launch_bounds__(NT) pool_fwd_kernel(const bf16* __restrict__ X
   pdl_wait();
   pdl_trigger();
   // grid: (C/8 chunks rounded to blocks of 32 lanes..., B); thread = (chunk, row group)
-  extern __shared__ float sred[];  // [C]
+  extern __shared__ double sdred[];  // fp64: the threads' fp32 partials add exactly, whatever the order; [C]
   const int b = blockIdx.x;
   const int cgs = C / 8;
   const int tid = threadIdx.x;
-  for (int i = tid; i < C; i += blockDim.x) sred[i] = 0.f;
+  for (int i = tid; i < C; i += blockDim.x) sdred[i] = 0.0;
   __syncthreads();
   const int cg = tid % cgs, rr = tid / cgs, rpp = blockDim.x / cgs;
   float a[8];
@@ -660,9 +695,9 @@ __global__ void __launch_bounds__(NT) pool_fwd_kernel(const bf16* __restrict__ X
     for (int j = 0; j < 8; ++j) a[j] += f[j];
   }
 #pragma unroll
-  for (int j = 0; j < 8; ++j) atomicAdd(&sred[cg * 8 + j], a[j]);
+  for (int j = 0; j < 8; ++j) atomicAdd(&sdred[cg * 8 + j], (double)a[j]);
   __syncthreads();
-  for (int i = tid; i < C; i += blockDim.x) OUT[(int64_t)b * C + i] = __float2bfloat16_rn(sred[i] / (float)HW);
+  for (int i = tid; i < C; i += blockDim.x) OUT[(int64_t)b * C + i] = __float2bfloat16_rn((float)sdred[i] / (float)HW);
 }
 
 __global__ void __launch_bounds__(NT) pool_bwd_kernel(const bf16* __restrict__ DOUT, int HW, int C, bf16* __restrict__ DX, int64_t nvec) {
@@ -862,7 +897,7 @@ extern "C" int cvb_bn_bwd_reduce(const void* DOUT, const void* Y, const float* s
   CVB_CHECK(DOUT && Y && sum_dz && sum_dzy && M > 0 && C > 0 && C % 8 == 0 && C <= 2048, "cvb_bn_bwd_reduce: bad arguments");
   if (act) CVB_CHECK(scale && shift, "cvb_bn_bwd_reduce: act needs scale/shift");
   RowGeom g = row_geom(M, C);
-  CVB_CUDA(cvb_launch(bn_bwd_reduce_kernel, g.ctas, g.nthreads, 2 * C * sizeof(float), static_cast<cudaStream_t>(stream), 
+  CVB_CUDA(cvb_launch(bn_bwd_reduce_kernel, g.ctas, g.nthreads, 2 * C * sizeof(double), static_cast<cudaStream_t>(stream), 
       static_cast<const bf16*>(DOUT), static_cast<const bf16*>(Y), scale, shift, act, static_cast<bf16*>(DZ), sum_dz, sum_dzy, M, C, g.cgs, g.rpp,
       g.rows_per_cta));
   CVB_LAUNCH_CHECK();
@@ -933,7 +968,7 @@ extern "C" int cvb_gn_bwd_apply(const void* G, const void* X, const float* mean,
             "cvb_gn_bwd_apply: bad arguments");
   int64_t M = (int64_t)B * rows_per_sample;
   RowGeom g = row_geom(M, C);
-  CVB_CUDA(cvb_launch(gn_bwd_apply_kernel, g.ctas, g.nthreads, C * sizeof(float), static_cast<cudaStream_t>(stream), 
+  CVB_CUDA(cvb_launch(gn_bwd_apply_kernel, g.ctas, g.nthreads, C * sizeof(double), static_cast<cudaStream_t>(stream), 
       static_cast<const bf16*>(G), static_cast<const bf16*>(X), mean, rstd, sg, sgx, count, static_cast<const bf16*>(DRES), static_cast<bf16*>(DX), M,
       rows_per_sample, C, col_sum, g.cgs, g.rpp, g.rows_per_cta, static_cast<const float*>(nullptr)));
   CVB_LAUNCH_CHECK();
@@ -950,12 +985,12 @@ extern "C" int cvb_gn_bwd(const void* V, const void* X, const float* mean, const
   const int cap = (6 * cvb_num_sms() + B - 1) / B;
   int rows_per_cta = g1.rows_per_cta;
   if (chunks > cap) { rows_per_cta = ((rows_per_sample + cap - 1) / cap + g1.rpp - 1) / g1.rpp * g1.rpp; chunks = (rows_per_sample + rows_per_cta - 1) / rows_per_cta; }
-  CVB_CUDA(cvb_launch(gn_bwd_stats_kernel, dim3(chunks, B), g1.nthreads, 2 * C * sizeof(float), static_cast<cudaStream_t>(stream),
+  CVB_CUDA(cvb_launch(gn_bwd_stats_kernel, dim3(chunks, B), g1.nthreads, 2 * C * sizeof(double), static_cast<cudaStream_t>(stream),
                       static_cast<const bf16*>(V), static_cast<const bf16*>(X), mean, rstd, gamma, rows_per_sample, C, g1.cgs, g1.rpp, rows_per_cta, dgamma,
                       dbeta, samp_ws, samp_ws + B));
   CVB_LAUNCH_CHECK();
   RowGeom g = row_geom(M, C);
-  CVB_CUDA(cvb_launch(gn_bwd_apply_kernel, g.ctas, g.nthreads, C * sizeof(float), static_cast<cudaStream_t>(stream), static_cast<const bf16*>(V),
+  CVB_CUDA(cvb_launch(gn_bwd_apply_kernel, g.ctas, g.nthreads, C * sizeof(double), static_cast<cudaStream_t>(stream), static_cast<const bf16*>(V),
                       static_cast<const bf16*>(X), mean, rstd, static_cast<const double*>(samp_ws), static_cast<const double*>(samp_ws + B), count,
                       static_cast<const bf16*>(DRES), static_cast<bf16*>(DX), M, rows_per_sample, C, static_cast<double*>(nullptr), g.cgs, g.rpp,
                       g.rows_per_cta, gamma));
@@ -967,7 +1002,7 @@ extern "C" int cvb_global_pool_fwd(const void* X, int B, int HW, int C, void* OU
   CVB_CHECK(X && OUT && B > 0 && HW > 0 && C > 0 && C % 8 == 0 && C <= 2048, "cvb_global_pool_fwd: bad arguments");
   int cgs = C / 8;
   int rpp = NT / cgs; if (rpp < 1) rpp = 1;
-  CVB_CUDA(cvb_launch(pool_fwd_kernel, B, cgs * rpp, C * sizeof(float), static_cast<cudaStream_t>(stream), static_cast<const bf16*>(X), HW, C, static_cast<bf16*>(OUT)));
+  CVB_CUDA(cvb_launch(pool_fwd_kernel, B, cgs * rpp, C * sizeof(double), static_cast<cudaStream_t>(stream), static_cast<const bf16*>(X), HW, C, static_cast<bf16*>(OUT)));
   CVB_LAUNCH_CHECK();
   return 0;
 }

@@ -1,4 +1,4 @@
-// Squeeze-excitation channel scaling (cvnets/modules/squeeze_excitation.py:82-83: `x * self.se_layer(x)`), sm_100a.
+// Squeeze-excitation channel scaling (cvnets/modules/squeeze_excitation.py:82-83: `x * self.se_layer(x)`), sm_90a.
 //
 //   forward   Y[b, p, c] = X[b, p, c] * S[b, c]                       X, Y: bf16 channels-last [B, HW, C]; S: bf16 [B, C]
 //   backward  DX[b, p, c] = DY[b, p, c] * S[b, c];   DS[b, c] += sum_p DY[b, p, c] * X[b, p, c]      (DS fp32, zero-initialised by the caller)

@@ -1,16 +1,16 @@
-// tcgen05 / TMEM / TMA weight-gradient GEMM (sm_100a):   dW[N,K] += sum_m load(G)[m,n] * load(A)[m,k],  dbias[n] += sum_m load(G)[m,n]
+// wgmma / TMA weight-gradient GEMM (sm_90a):   dW[N,K] += sum_m load(G)[m,n] * load(A)[m,k],  dbias[n] += sum_m load(G)[m,n]
 //
 // The reduction runs over PIXELS, so both operands are "MN-major" for the tensor core: a [pixels x channels] tile with the channels
 // contiguous is exactly the canonical MN-major SWIZZLE_128B layout (8 pixel rows x 128 B atoms) that TMA produces with a
-// [64 channel x rows] box -- no transposition anywhere.  One CTA owns a whole [128 x <=256] block of dW in TMEM (128 lanes = dW
-// rows, fp32 columns = dW columns) and streams its slice of the pixel range through a TMA ring, so every activation / gradient
-// element is read ONCE per (N-block, K-block) instead of once per 64x64 tile (the mma.sync kernel is L2-bandwidth bound on
-// exactly that re-reading).  Warp roles:
-//   warp 0      TMA producer  : per stage [64 pixels] x {G: 128 ch (+ G2 for BN-backward), A: <=256 ch}, 64-channel boxes
-//   warp 1      MMA issuer    : 4 x tcgen05.mma.kind::f16 (K = 16 pixels each) per stage, both operands MN-major, accumulate in TMEM
-//   warps 2-9   transform     : in-place operand prologues in shared memory (BN-backward on G, BN+SiLU / SiLU / GroupNorm on A),
-//                               bias-gradient column sums, fence.proxy.async, hand the stage to the MMA warp
-//               epilogue      : after the last MMA: tcgen05.ld -> vectorised fp32 reductions (red.global.add.v4.f32) into dW
+// [64 channel x rows] box -- wgmma reads it transposed, no transposition anywhere.  One CTA owns a whole [128 x <=128] block of dW
+// in the registers of two consumer warpgroups (64 dW rows each) and streams its slice of the pixel range through a TMA ring, so
+// every activation / gradient element is read ONCE per (N-block, K-block) instead of once per 64x64 tile (the mma.sync kernel is
+// L2-bandwidth bound on exactly that re-reading).  Warp roles:
+//   warps 0-7   consumers     : 4 x wgmma.m64nKBk16 (K = 16 pixels each) per stage, both operands MN-major; after the last stage
+//                               fp64 reductions of the accumulator registers into the dW scratch (see cvb_det_alloc)
+//   warp 8      TMA producer  : per stage [64 pixels] x {G: 128 ch (+ G2 for BN-backward), A: <=128 ch}, 64-channel boxes
+//   warps 9-16  transform     : in-place operand prologues in shared memory (BN-backward on G, BN+SiLU / SiLU / GroupNorm on A),
+//                               bias-gradient column sums, fence.proxy.async, hand the stage to the consumers
 // Split over the pixel range (grid.z) so that ~all SMs are busy; partial sums meet in dW through the fp32 reductions.
 #include "common.cuh"
 
@@ -18,92 +18,48 @@ namespace {
 
 constexpr int WT_BMP = 64;                 // pixels per stage
 constexpr int WT_BOX = WT_BMP * 128;       // bytes of one [64 pixels x 64 channels] box (8 swizzle atoms of 1 KB)
+constexpr int WT_KB = 128;                 // dW columns per CTA (at most; K = 64 layers use 64)
 constexpr int WT_XF_WARPS = 8;
-constexpr int WT_THREADS = 64 + WT_XF_WARPS * 32;
+constexpr int WT_CONSUMERS = 256;          // two warpgroups
+constexpr int WT_PRODUCER_WARP = WT_CONSUMERS / 32;
+constexpr int WT_XF0 = WT_CONSUMERS + 32;  // first transform thread
+constexpr int WT_THREADS = WT_XF0 + WT_XF_WARPS * 32;
 constexpr int WT_MAX_STAGES = 6;
-constexpr int WT_TMEM_COLS = 256;
 
-__device__ __forceinline__ uint64_t umma_desc_mn_sw128(uint32_t saddr) {
-  // MN-major operand, 128-byte swizzle (cute::UMMA::make_umma_desc<Major::MN>): ((8,n),(8,k)) : ((1,LBO),(8,SBO)) in 16-byte units;
-  // LBO = distance between 64-channel boxes (8 KB), SBO = distance between 8-pixel groups (1 KB)
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
-  d |= (uint64_t)(WT_BOX >> 4) << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;  // descriptor version 1 (Blackwell)
-  d |= (uint64_t)2 << 61;  // layout type: SWIZZLE_128B
-  return d;
-}
-__device__ __forceinline__ void umma_f16_idesc(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void wt_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void wt_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void wt_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void wt_arrive(uint64_t* bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory"); }
-__device__ __forceinline__ void wt_tmem_ld32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,"
-      "%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]),
-        "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]),
-        "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void red_add_v4(float* p, float a, float b, float c, float d) {
-  asm volatile("red.global.add.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(p), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
-}
+// MN-major operand, 128-byte swizzle: LBO = distance between 64-channel boxes (8 KB), SBO = distance between 8-pixel groups (1 KB)
+__device__ __forceinline__ uint64_t desc_mn_sw128(uint32_t saddr) { return wgmma_desc(saddr, WT_BOX, 1024, WG_SW128); }
 // byte offset of the 16-byte chunk `ch` (logical, 0..7) of pixel row `row` inside one [64 x 64ch] box (TMA SWIZZLE_128B image)
 __device__ __forceinline__ uint32_t sw128(int row, int ch) { return static_cast<uint32_t>(row * 128 + ((ch ^ (row & 7)) << 4)); }
 
-template <int GMODE, int AMODE>
+template <int GMODE, int AMODE, int KB>
 __global__ void __launch_bounds__(WT_THREADS, 1)
     pw_wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmG, const __grid_constant__ CUtensorMap tmG2, const __grid_constant__ CUtensorMap tmA,
-                       const cvb_wgrad_args p, int m_per_cta, int NST, int KB, int stage_bytes) {
+                       const cvb_wgrad_args p, int m_per_cta, int NST, int stage_bytes) {
   constexpr bool BNB = (GMODE == CVB_A_BNB);
   constexpr bool A_HAS_P = (AMODE == CVB_A_AFF || AMODE == CVB_A_AFF_SILU || AMODE == CVB_A_GN);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int n0 = blockIdx.x * 128, k0 = blockIdx.y * 256;
+  const int n0 = blockIdx.x * 128, k0 = blockIdx.y * WT_KB;
   const int m_begin = blockIdx.z * m_per_cta;
   const int m_end = min(p.M, m_begin + m_per_cta);
   const int NS = (m_end - m_begin + WT_BMP - 1) / WT_BMP;   // >= 1 by construction of the grid
-  const int a_boxes = (KB + 63) / 64;
+  constexpr int a_boxes = KB / 64;
   const int a_off = (BNB ? 2 : 1) * 2 * WT_BOX;             // stage layout: [G: 2 boxes][G2: 2 boxes (BNB)][A: a_boxes boxes]
 
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  __shared__ __align__(8) uint64_t full[WT_MAX_STAGES], ready[WT_MAX_STAGES], empty[WT_MAX_STAGES], accbar;
-  __shared__ uint32_t tmem_base_smem;
-  __shared__ float s_db[128];
+  __shared__ __align__(8) uint64_t full[WT_MAX_STAGES], ready[WT_MAX_STAGES], empty[WT_MAX_STAGES];
+  __shared__ double s_db[128];
 
   if (tid == 0) {
-    for (int i = 0; i < NST; ++i) { mbar_init(&full[i], 1); mbar_init(&ready[i], WT_XF_WARPS); mbar_init(&empty[i], 1); }
-    mbar_init(&accbar, 1);
+    for (int i = 0; i < NST; ++i) { mbar_init(&full[i], 1); mbar_init(&ready[i], WT_XF_WARPS); mbar_init(&empty[i], 2); }
     fence_mbar_init();
   }
-  if (tid < 128) s_db[tid] = 0.f;
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_smem)), "r"(WT_TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  wt_fence_before();
+  if (tid < 128) s_db[tid] = 0.0;
   __syncthreads();
-  wt_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
   pdl_wait();
   pdl_trigger();
 
-  if (warp == 0) {
+  if (warp == WT_PRODUCER_WARP) {
     // ===================================================== TMA producer
     if (lane == 0) {
       for (int s = 0; s < NS; ++s) {
@@ -121,27 +77,46 @@ __global__ void __launch_bounds__(WT_THREADS, 1)
         for (int bx = 0; bx < a_boxes; ++bx) tma_load_2d(st + a_off + bx * WT_BOX, &tmA, &full[slot], k0 + bx * 64, m);
       }
     }
-  } else if (warp == 1) {
-    // ===================================================== MMA issuer
-    if (lane == 0) {
-      // kind::f16: D = F32, A = B = BF16, both MN-major, N = KB (>>3), M = 128 (>>4)
-      const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | (1u << 16) | ((uint32_t)(KB >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-      for (int s = 0; s < NS; ++s) {
-        const int slot = s % NST;
-        mbar_wait(&ready[slot], (s / NST) & 1);
-        wt_fence_after();
-        const uint32_t sg = smem_u32(smem + slot * stage_bytes);
-        const uint32_t sa = sg + a_off;
+  } else if (warp < WT_PRODUCER_WARP) {
+    // ===================================================== consumers: dW rows [64 wg, 64 wg + 64) of the block
+    const int wg = tid >> 7;
+    float acc[KB / 2];
+    for (int s = 0; s < NS; ++s) {
+      const int slot = s % NST;
+      mbar_wait(&ready[slot], (s / NST) & 1);
+      const uint32_t sg = smem_u32(smem + slot * stage_bytes) + wg * WT_BOX;  // this warpgroup's 64 gradient channels
+      const uint32_t sa = smem_u32(smem + slot * stage_bytes) + a_off;
+      wgmma_fence();
 #pragma unroll
-        for (int kk = 0; kk < WT_BMP / 16; ++kk)  // 16 pixels = two 8-row swizzle atoms = 2 KB further into every box
-          umma_f16_idesc(tmem_base, umma_desc_mn_sw128(sg + kk * 2048), umma_desc_mn_sw128(sa + kk * 2048), idesc, (s > 0 || kk > 0) ? 1u : 0u);
-        wt_commit(&empty[slot]);  // the stage may be refilled once these MMAs have read it
+      for (int kk = 0; kk < WT_BMP / 16; ++kk) {  // 16 pixels = two 8-row swizzle atoms = 2 KB further into every box
+        if (KB == 128)
+          wgmma_m64n128<1, 1>(acc, desc_mn_sw128(sg + kk * 2048), desc_mn_sw128(sa + kk * 2048), (s > 0 || kk > 0) ? 1u : 0u);
+        else
+          wgmma_m64n64<1, 1>(acc, desc_mn_sw128(sg + kk * 2048), desc_mn_sw128(sa + kk * 2048), (s > 0 || kk > 0) ? 1u : 0u);
       }
-      wt_commit(&accbar);
+      wgmma_commit();
+      wgmma_wait<1>();  // the previous stage's MMAs have read it: it may be refilled
+      if (s > 0 && (tid & 127) == 0) mbar_arrive(&empty[(s - 1) % NST]);
+    }
+    wgmma_wait<0>();
+    wgmma_reg_fence<KB / 2>(acc);
+    // ---- epilogue: accumulator registers -> fp64 reductions into the dW scratch (fragment: rows 16 w + lane / 4 (+ 8), columns 8 j + 2 (lane % 4))
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int n = n0 + wg * 64 + ((tid & 127) >> 5) * 16 + (lane >> 2) + 8 * h;
+      if (n < p.N) {
+        double* __restrict__ dWrow = reinterpret_cast<double*>(p.dW) + (size_t)n * p.lddw;
+#pragma unroll
+        for (int j = 0; j < KB / 8; ++j) {
+          const int k = k0 + 8 * j + 2 * (lane & 3);
+          if (k < p.K) atomicAdd(dWrow + k, (double)acc[4 * j + 2 * h]);
+          if (k + 1 < p.K) atomicAdd(dWrow + k + 1, (double)acc[4 * j + 2 * h + 1]);
+        }
+      }
     }
   } else {
-    // ===================================================== transform warps, then epilogue
-    const int xt = tid - 64;  // 0..255
+    // ===================================================== transform warps
+    const int xt = tid - WT_XF0;  // 0..255
     // G role: fixed 16-byte chunk column gc (0..15) of the 128 channels, rows (xt>>4) + 16*i
     const int gc = xt & 15;
     const int gn = n0 + gc * 8;
@@ -217,58 +192,26 @@ __global__ void __launch_bounds__(WT_THREADS, 1)
       }
       fence_proxy_async();  // generic-proxy writes -> visible to the tensor core's async-proxy reads
       __syncwarp();
-      if (lane == 0) wt_arrive(&ready[slot]);
+      if (lane == 0) mbar_arrive(&ready[slot]);
     }
 
     // ---- bias gradient: reduce the thread-local column sums (16 row-threads share a chunk column)
     if (want_db) {
 #pragma unroll
-      for (int e = 0; e < 8; ++e) atomicAdd(&s_db[gc * 8 + e], db[e]);
+      for (int e = 0; e < 8; ++e) atomicAdd(&s_db[gc * 8 + e], (double)db[e]);
       asm volatile("bar.sync 1, %0;" ::"n"(WT_XF_WARPS * 32) : "memory");
-      if (xt < 128 && n0 + xt < p.N) atomicAdd(p.dbias + n0 + xt, s_db[xt]);
+      if (xt < 128 && n0 + xt < p.N) atomicAdd(reinterpret_cast<double*>(p.dbias) + n0 + xt, s_db[xt]);
     }
 
-    // ---- epilogue: TMEM -> fp32 reductions into dW.  Lane quadrant q = warp % 4 (hardware rule), two warps per quadrant split the columns
-    mbar_wait(&accbar, 0);
-    wt_fence_after();
-    const int q = warp & 3, half = (warp - 2) >> 2;
-    const int n = n0 + q * 32 + lane;
-    float* __restrict__ dWrow = static_cast<float*>(p.dW) + (size_t)n * p.lddw + k0;
-    const int kchunks = (KB + 31) / 32;
-    for (int c = half; c < kchunks; c += 2) {
-      uint32_t v[32];
-      wt_tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(c * 32), v);
-      if (n < p.N) {
-#pragma unroll
-        for (int j = 0; j < 32; j += 4) {
-          const int k = k0 + c * 32 + j;
-          if (k + 3 < p.K && (p.lddw & 3) == 0) {
-            red_add_v4(dWrow + c * 32 + j, __uint_as_float(v[j]), __uint_as_float(v[j + 1]), __uint_as_float(v[j + 2]), __uint_as_float(v[j + 3]));
-          } else {
-#pragma unroll
-            for (int e = 0; e < 4; ++e)
-              if (k + e < p.K) atomicAdd(dWrow + c * 32 + j + e, __uint_as_float(v[j + e]));
-          }
-        }
-      }
-    }
-    wt_fence_before();
-  }
-  __syncthreads();
-  if (warp == 1) {
-    wt_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(WT_TMEM_COLS) : "memory");
   }
 }
 
-template <int GMODE, int AMODE>
+template <int GMODE, int AMODE, int KB>
 int launch_wgrad_tc(const cvb_wgrad_args& a, cudaStream_t st) {
-  const int nb = (a.N + 127) / 128, kb = (a.K + 255) / 256;
-  // columns per CTA: a multiple of 16 (UMMA N), the last K block may be narrower; all K blocks of one launch use the same KB, so
-  // pad the narrow one with zero-filled boxes instead (K is a multiple of 64 here)
-  const int KB = a.K >= 256 ? 256 : a.K;
-  const int a_boxes = (KB + 63) / 64;
-  const int stage_bytes = ((GMODE == CVB_A_BNB ? 4 : 2) + a_boxes) * WT_BOX;
+  // all K blocks of one launch use the same width KB; the last one may be narrower and is padded with zero-filled boxes
+  // (K is a multiple of 64 here)
+  const int nb = (a.N + 127) / 128, kb = (a.K + WT_KB - 1) / WT_KB;
+  const int stage_bytes = ((GMODE == CVB_A_BNB ? 4 : 2) + KB / 64) * WT_BOX;
   int nst = (200 * 1024) / stage_bytes;
   if (nst > WT_MAX_STAGES) nst = WT_MAX_STAGES;
   const int sms = cvb_num_sms();
@@ -285,13 +228,18 @@ int launch_wgrad_tc(const cvb_wgrad_args& a, cudaStream_t st) {
   if (cvb_make_tmap_2d_c64(&tmA, a.A, a.M, a.K, a.lda, WT_BMP)) return 1;
   static bool attr = false;
   if (!attr) {
-    CVB_CUDA(cudaFuncSetAttribute(pw_wgrad_tc_kernel<GMODE, AMODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, 216 * 1024));
+    CVB_CUDA(cudaFuncSetAttribute(pw_wgrad_tc_kernel<GMODE, AMODE, KB>, cudaFuncAttributeMaxDynamicSharedMemorySize, 216 * 1024));
     attr = true;
   }
   dim3 grid(nb, kb, splits);
-  CVB_CUDA(cvb_launch(pw_wgrad_tc_kernel<GMODE, AMODE>, grid, WT_THREADS, smem, st, tmG, tmG2, tmA, a, m_per_cta, nst, KB, stage_bytes));
+  CVB_CUDA(cvb_launch(pw_wgrad_tc_kernel<GMODE, AMODE, KB>, grid, WT_THREADS, smem, st, tmG, tmG2, tmA, a, m_per_cta, nst, stage_bytes));
   CVB_LAUNCH_CHECK();
   return 0;
+}
+
+template <int GMODE, int AMODE>
+int launch_wgrad_tc(const cvb_wgrad_args& a, cudaStream_t st) {
+  return a.K >= WT_KB ? launch_wgrad_tc<GMODE, AMODE, WT_KB>(a, st) : launch_wgrad_tc<GMODE, AMODE, 64>(a, st);
 }
 
 template <int GMODE>
@@ -311,10 +259,8 @@ int dispatch_wgrad_tc_a(const cvb_wgrad_args& a, cudaStream_t st) {
 // Returns 0 when the launch was issued, -1 when the shape is left to the mma.sync kernel, > 0 on error.
 int cvb_pw_wgrad_tc(const cvb_wgrad_args& a, cudaStream_t st) {
   // 64-channel TMA boxes on the reduced-over operand: K must be a multiple of 64 (the 3x3 stem / K = 32 layers stay on mma.sync);
-  // fp32 vector reductions want 16-byte aligned dW rows
   if (a.K % 64 != 0 || a.K < 64 || a.N < 32) return -1;
-  if (a.N <= 64 && a.K <= 64) return -1;  // half-empty 128-lane block and one 64-column box: the 64x64-tile mma.sync kernel is faster (measured)
-  if ((reinterpret_cast<uintptr_t>(a.dW) & 15) != 0) return -1;
+  if (a.N <= 64 && a.K <= 64) return -1;  // half-empty 128-row block and one 64-column box: left to the 64x64-tile mma.sync kernel
   if (a.g_mode == CVB_A_RAW) return dispatch_wgrad_tc_a<CVB_A_RAW>(a, st);
   if (a.g_mode == CVB_A_BNB) return dispatch_wgrad_tc_a<CVB_A_BNB>(a, st);
   return -1;

@@ -1202,7 +1202,7 @@ class TransformerEncoderFn(torch.autograd.Function):
         ln1 = ops.ln_stats(x2, cfg.eps)
         # wide layers (ViT / CLIP: K = 768 under 18-24 N tiles): the LayerNorm prologue is applied ONCE by a pre-pass (ops.WIDE_K / WIDE_N policy, which
         # pw_gemm would apply internally) and the normalised tokens are KEPT for the weight gradient of the same projection, which would otherwise
-        # re-normalise them (profiles/r2_step_launches_vit_b16.csv: 24 extra passes of 80 us per step)
+        # re-normalise them (one extra pass over the tokens per weight-gradient block)
         keep_n = ops.KEEP_NORMALISED and C >= ops.WIDE_K and 3 * C >= ops.WIDE_N_WGRAD and ffn >= ops.WIDE_N_WGRAD
         xn1 = xn2 = None
         if keep_n:

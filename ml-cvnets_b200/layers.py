@@ -2,7 +2,7 @@
 and ``state_dict`` keys as the reference (SURVEY.md 8b / Appendix B), so published checkpoints load unchanged and the
 reference's isinstance/name based machinery (weight init, BN momentum annealing, weight-decay grouping, EMA deepcopy)
 keeps working.  Parameters are ordinary ``nn.Parameter``s inside ordinary ``nn.Conv2d`` / ``nn.BatchNorm2d`` /
-``nn.GroupNorm`` / ``nn.Linear`` children; only ``forward`` is ours and it runs hand-written sm_100a kernels.
+``nn.GroupNorm`` / ``nn.Linear`` children; only ``forward`` is ours and it runs hand-written sm_90a kernels.
 
 There is deliberately NO PyTorch fallback.  Inside InvertedResidual / MobileViTBlockv2 / TransformerEncoder the layers are parameter
 containers executed by the fused autograd functions; used on their own they run the stand-alone functions of functional.py (same
@@ -201,7 +201,7 @@ class AdaptiveAvgPool2d(nn.Module):
     def __init__(self, output_size=1, *args, **kwargs) -> None:
         super().__init__()
         if output_size not in (1, (1, 1)):
-            raise NotImplementedError("AdaptiveAvgPool2d: output_size = 1 is on the B200 hot path")
+            raise NotImplementedError("AdaptiveAvgPool2d: output_size = 1 is on the GPU hot path")
         self.output_size = output_size
 
     def forward(self, x: Tensor) -> Tensor:
@@ -217,7 +217,7 @@ _ACT_CLASSES = {}
 
 def _need_cuda(x: Tensor, who: str):
     if not x.is_cuda:
-        raise RuntimeError(f"{who}: ml-cvnets_b200 runs on CUDA (sm_100a) only and has no CPU fallback; got a {x.device} tensor")
+        raise RuntimeError(f"{who}: ml-cvnets_b200 runs on CUDA (sm_90a) only and has no CPU fallback; got a {x.device} tensor")
 
 
 def get_normalization_layer(opts, num_features: int, norm_type: Optional[str] = None, *args, **kwargs) -> nn.Module:
@@ -232,7 +232,7 @@ def get_normalization_layer(opts, num_features: int, norm_type: Optional[str] = 
         return LayerNorm(num_features)
     if norm_type == "layer_norm_fp32":
         return LayerNormFP32(num_features)
-    raise NotImplementedError(f"normalization '{norm_type}' is not on the B200 hot path (batch_norm, layer_norm_2d, layer_norm, layer_norm_fp32 are)")
+    raise NotImplementedError(f"normalization '{norm_type}' is not on the GPU hot path (batch_norm, layer_norm_2d, layer_norm, layer_norm_fp32 are)")
 
 
 def build_activation_layer(opts, act_type: Optional[str] = None, *args, **kwargs) -> nn.Module:
@@ -241,7 +241,7 @@ def build_activation_layer(opts, act_type: Optional[str] = None, *args, **kwargs
     table = {"swish": Swish, "silu": Swish, "gelu": GELU, "relu": ReLU, "hard_swish": Hardswish, "hard_sigmoid": Hardsigmoid, "sigmoid": Sigmoid}
     if name in table:
         return table[name]()
-    raise NotImplementedError(f"activation '{name}' is not on the B200 hot path ({', '.join(sorted(table))} are)")
+    raise NotImplementedError(f"activation '{name}' is not on the GPU hot path ({', '.join(sorted(table))} are)")
 
 
 class Conv2d(nn.Conv2d):
@@ -408,7 +408,7 @@ class GlobalPool(BaseLayer):
     def __init__(self, pool_type: Optional[str] = "mean", keep_dim: Optional[bool] = False, *args, **kwargs) -> None:
         super().__init__()
         if pool_type != "mean":
-            raise NotImplementedError("only mean pooling is on the B200 hot path")
+            raise NotImplementedError("only mean pooling is on the GPU hot path")
         self.pool_type, self.keep_dim = pool_type, keep_dim
 
     def forward(self, x: Tensor) -> Tensor:
@@ -520,7 +520,7 @@ class MultiHeadAttention(BaseLayer):
         from . import functional as Fn
         from .ops import PreparedWeights as PW
         if x_kv is not None:
-            raise NotImplementedError("cross-attention (x_kv) is not implemented on the B200 path")
+            raise NotImplementedError("cross-attention (x_kv) is not implemented on the GPU path")
         if not x_q.is_cuda:
             raise RuntimeError("MultiHeadAttention: ml-cvnets_b200 has no CPU path")
         if x_q.dim() != 3 or x_q.shape[1] > 256:

@@ -2,7 +2,7 @@
 
 ``InvertedResidual`` (cvnets/modules/mobilenetv2.py:141-246), ``LinearAttnFFN`` (cvnets/modules/transformer.py:159-264)
 and ``MobileViTBlockv2`` (cvnets/modules/mobilevit_block.py:329-667): identical constructor signatures, child tree and
-``state_dict`` keys; ``forward`` dispatches to the autograd Functions in functional.py (hand-written sm_100a kernels).
+``state_dict`` keys; ``forward`` dispatches to the autograd Functions in functional.py (hand-written sm_90a kernels).
 """
 from __future__ import annotations
 
@@ -31,7 +31,7 @@ def make_divisible(v, divisor: int = 8, min_value=None):
 
 def _require_cuda(x: Tensor, who: str):
     if not x.is_cuda:
-        raise RuntimeError(f"{who}: ml-cvnets_b200 runs on CUDA (sm_100a) only and has no CPU fallback; got a {x.device} tensor")
+        raise RuntimeError(f"{who}: ml-cvnets_b200 runs on CUDA (sm_90a) only and has no CPU fallback; got a {x.device} tensor")
 
 
 class BaseModule(nn.Module):
@@ -450,7 +450,7 @@ class TransformerEncoder(BaseModule):
                  stochastic_dropout: Optional[float] = 0.0, *args, **kwargs) -> None:
         super().__init__()
         if num_heads <= 1:
-            raise NotImplementedError("SingleHeadAttention (num_heads == 1) is not on the B200 path")
+            raise NotImplementedError("SingleHeadAttention (num_heads == 1) is not on the GPU path")
         attn_unit = MultiHeadAttention(embed_dim, num_heads, attn_dropout=attn_dropout, bias=True)
         self.pre_norm_mha = nn.Sequential(get_normalization_layer(opts=opts, norm_type=transformer_norm_layer, num_features=embed_dim),
                                           attn_unit, Dropout(p=dropout))
@@ -495,7 +495,7 @@ class TransformerEncoder(BaseModule):
                 attn_mask: Optional[Tensor] = None, *args, **kwargs) -> Tensor:
         _require_cuda(x, "TransformerEncoder")
         if x_prev is not None:
-            raise NotImplementedError("cross-attention (x_prev) is not implemented on the B200 path")
+            raise NotImplementedError("cross-attention (x_prev) is not implemented on the GPU path")
         if self.training and self.pre_norm_mha[1].attn_dropout.p:
             raise NotImplementedError("attention-probability dropout > 0 in training mode is not implemented (every recipe of the reference sets 0; "
                                       "it is the identity in eval mode, which works)")

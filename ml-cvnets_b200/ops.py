@@ -88,7 +88,7 @@ def _count(n=1):
 
 
 def set_tc_enabled(on: bool) -> bool:
-    """Testing hook: route prologue-free GEMMs to the tcgen05 kernel (default) or to the mma.sync kernel."""
+    """Testing hook: route prologue-free GEMMs to the wgmma kernel (default) or to the mma.sync kernel."""
     return bool(_lib().cvb_set_tc_enabled(int(on)))
 
 
@@ -104,8 +104,8 @@ def set_pdl_enabled(on: bool) -> bool:
 WIDE_K = int(os.environ.get("CVB_WIDE_K", "384"))
 WIDE_N = int(os.environ.get("CVB_WIDE_N", "1024"))
 # weight gradients: every 128-row block of dW (N / 128 CTAs per K block) re-applies the prologue to the SAME activation operand inside its transform
-# warps.  ViT-B (ncu launch list, profiles/r2_step_launches_vit_b16.csv): the LayerNorm-fused weight gradients of qkv_proj / ffn.1 (N = 2304 / 3072,
-# 18 / 24 blocks) ran at 234-312 TFLOP/s against 858 TFLOP/s for the prologue-free ones of the same size -> one pre-pass, then the RAW kernel.
+# warps.  For the LayerNorm-fused weight gradients of the ViT-B qkv_proj / ffn.1 (N = 2304 / 3072, 18 / 24 blocks) that repeated prologue costs
+# far more than one pre-pass -> one pre-pass, then the RAW kernel.
 WIDE_N_WGRAD = int(os.environ.get("CVB_WIDE_N_WGRAD", "1536"))
 # TransformerEncoderFn keeps the pre-pass output of its two LayerNorm-fused projections for their weight gradients (2 x [tokens, C] bf16 per layer)
 KEEP_NORMALISED = int(os.environ.get("CVB_KEEP_NORMALISED", "1")) != 0
@@ -122,7 +122,7 @@ def pw_gemm(A: Tensor, W: Tensor, N: int, *, K: Optional[int] = None, a_mode: in
     K = A.shape[1] if K is None else K
     if a_mode != A_RAW and K >= WIDE_K and N >= WIDE_N:
         # wide late-stage layer (small, L2-resident operand): apply the prologue once instead of once per N tile, then run the
-        # prologue-free (tcgen05) GEMM
+        # prologue-free (wgmma) GEMM
         A = apply_load_mode(A, a_mode, K, A2=A2, a_p=a_p, row_stats=row_stats, rows_per_sample=rows_per_sample)
         a_mode, A2, a_p = A_RAW, None, (None, None, None)
         if e_mode != E_GN_BWD:  # the GroupNorm-backward epilogue reads the same per-sample statistics

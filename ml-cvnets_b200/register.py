@@ -30,7 +30,7 @@ _KEEP_REFERENCE = {"get_trainable_parameters", "freeze_norm_layers", "info", "up
 
 def _make_shell(ours_cls, base_cls, shell_name: str):
     """A ``base_cls`` (the reference's own base encoder: utils/registry.py:111-167 only accepts BaseAnyNNModel subclasses) whose children,
-    parameters, buffers and private state are those of a B200 model, and whose forward / feature-extraction methods are the B200 ones."""
+    parameters, buffers and private state are those of this package's model, and whose forward / feature-extraction methods are this package's."""
     import types
 
     def __init__(self, opts, *args, **kwargs) -> None:
@@ -55,7 +55,7 @@ def _make_shell(ours_cls, base_cls, shell_name: str):
 
 
 def register_with_cvnets(name: str = "mobilevit_v2_b200"):
-    """Injection point 2: register the B200 assemblers under new model names: ``mobilevit_v2_b200`` (or ``name``), ``mobilevit_b200``, ``vit_b200``.
+    """Injection point 2: register this package's assemblers under new model names: ``mobilevit_v2_b200`` (or ``name``), ``mobilevit_b200``, ``vit_b200``.
     Returns the MobileViTv2 shell class."""
     from cvnets.models import MODEL_REGISTRY
     from cvnets.models.classification.base_image_encoder import BaseImageEncoder

@@ -13,6 +13,8 @@ import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
+sys.path.insert(0, os.path.dirname(HERE))
+from golden_sample import sample_large  # noqa: E402
 from make_golden import O, get_model, load_seeded, make_opts, torch  # noqa: E402
 
 
@@ -27,14 +29,14 @@ def main():
         model.train()
         x = O.seeded_input((B, 3, res, res), 381)
         ends = model.extract_end_points_all(x, use_l5=True, use_l5_exp=False)
-        rec = {"ends": {k: v.detach().clone() for k, v in ends.items() if k in ("out_l3", "out_l4", "out_l5")},
+        rec = {"ends": {k: sample_large(v.detach().clone()) for k, v in ends.items() if k in ("out_l3", "out_l4", "out_l5")},
                "dilations": {n: list(m.dilation) for n, m in model.named_modules() if isinstance(m, torch.nn.Conv2d) and m.dilation != (1, 1)}}
         if os_ == 8:
             gy4, gy5 = O.seeded_input(tuple(ends["out_l4"].shape), 481), O.seeded_input(tuple(ends["out_l5"].shape), 482)
             ((ends["out_l4"] * gy4).sum() + (ends["out_l5"] * gy5).sum()).backward()
             grads = {k: p.grad for k, p in model.named_parameters() if p.grad is not None}
             rec.update(gy_seeds=(481, 482), grad_norms={k: float(g.norm()) for k, g in grads.items()},
-                       grads={k: g.clone() for k, g in grads.items() if g.numel() <= 5000})
+                       grads={k: sample_large(g.clone()) for k, g in grads.items() if g.numel() <= 5000})
         fx[f"os{os_}"] = rec
         print(os_, {k: tuple(v.shape) for k, v in ends.items()}, rec["dilations"])
     torch.save(fx, os.path.join(HERE, "mobilevit_v2_dilated_fp32.pt"))

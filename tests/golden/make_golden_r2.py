@@ -12,6 +12,8 @@ import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
+sys.path.insert(0, os.path.dirname(HERE))
+from golden_sample import sample_large  # noqa: E402
 from make_golden import O, F, ConvLayer2d, LinearSelfAttention, LinearAttnFFN, get_model, load_seeded, make_opts, run_module, strip, torch  # noqa: E402
 
 from cvnets.layers import GlobalPool, LinearLayer  # noqa: E402
@@ -92,7 +94,8 @@ def main():
     grads = {k: p.grad for k, p in model.named_parameters()}
     fixture = dict(width=width, res=res, seed=seed, x_seed=300 + seed, batch=B, labels=labels, logits=logits.detach().clone(), loss=loss.detach().clone(),
                    grad_norms={k: float(g.norm()) for k, g in grads.items()},
-                   grads={k: g.clone().half() if g.numel() > 4096 else g.clone() for k, g in grads.items() if g.numel() <= 65536},
+                   grads={k: sample_large(g.clone().half() if g.numel() > 4096 else g.clone(), limit=2048, n=2048) for k, g in grads.items()
+                          if g.numel() <= 65536},
                    buffers_after={k: b.detach().clone() for k, b in model.named_buffers() if b.numel() <= 4096})
     torch.save(fixture, os.path.join(HERE, "mobilevit_v2_b16_fp32.pt"))
     # ---- VisionTransformer, "small" geometry (same code path as base: 12 layers, head_dim 64, S = 197), batch 2 @ 224

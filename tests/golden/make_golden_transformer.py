@@ -15,9 +15,11 @@ REPO = os.path.dirname(os.path.dirname(HERE))
 REF = "/root/reference"
 sys.path.insert(0, REPO)
 sys.path.insert(0, REF)
+sys.path.insert(0, os.path.dirname(HERE))
 os.chdir(REF)
 
 import torch  # noqa: E402
+from golden_sample import sample_large  # noqa: E402
 
 from cvnets import modeling_arguments  # noqa: E402
 from cvnets.layers import MultiHeadAttention  # noqa: E402
@@ -84,6 +86,8 @@ def main():
         eps = m.pre_norm_mha[0].eps
         fx[name] = dict(cfg=dict(c=c, ffn=ffn, heads=heads, act=act, eps=eps), seed=seed,
                         **run(m, O.seeded_input((n, s, c), 100 + seed), 200 + seed))
+    for rec in fx.values():
+        rec["grads"] = {k: sample_large(g) for k, g in rec["grads"].items()}
     torch.save(fx, os.path.join(HERE, "transformer_fp32.pt"))
     print("wrote", sorted(fx.keys()))
 

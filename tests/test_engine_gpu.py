@@ -54,8 +54,7 @@ def test_train_step_gradients_match_autograd_path(pkg):
     """Workspace mode (gradients written in place, Functions return None) == the plain autograd path of the same kernels.
 
     The kernels accumulate statistics / weight gradients with atomics, so two runs of the SAME path differ in the last bits, and train-mode
-    BatchNorm through ~60 bf16 layers amplifies that (measured on B200: up to 1e-1 rel-L2 per parameter at batch 8 / 64x64, where the
-    deepest maps are 2x2).  The test therefore (a) uses a better conditioned shape and (b) bounds the workspace-vs-autograd difference by
+    BatchNorm through ~60 bf16 layers amplifies that, worst at tiny shapes (batch 8 / 64x64, where the deepest maps are 2x2).  The test therefore (a) uses a better conditioned shape and (b) bounds the workspace-vs-autograd difference by
     the run-to-run difference of the autograd path itself."""
     B, res = 16, 128
     x = O.seeded_input((B, 3, res, res), 5).cuda()

@@ -1,6 +1,8 @@
 """CPU-only checks (-m "not gpu"): the C-ABI library loads and exports every symbol include/cvnets_b200.h declares, the
 host-side mirror keeps the reference's state_dict / signature contract, the product refuses to run without CUDA, the
-reference-side registration works when the reference checkout is present, and the N>1 host logic works under gloo."""
+drop-in modules match the reference classes' recorded contract (tests/golden/reference_contract.json), and the N>1 host logic
+works under gloo."""
+import hashlib
 import inspect
 import json
 import os
@@ -99,133 +101,83 @@ def test_product_does_not_import_the_oracle():
                 assert "oracle" not in src.replace("no oracle", ""), f"{fn} mentions the oracle"
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/cvnets"), reason="reference checkout not present (GPU box)")
-def test_registration_with_reference_checkout():
-    code = r"""
-import sys, os, argparse
-sys.path.insert(0, %r); sys.path.insert(0, "/root/reference"); os.chdir("/root/reference")
-import ml_cvnets_b200.register as r
-from cvnets import modeling_arguments, get_model
-r.register_with_cvnets()
-opts = modeling_arguments(argparse.ArgumentParser()).parse_args([])
-for k, v in {"dataset.category": "classification", "model.classification.name": "mobilevit_v2_b200",
-             "model.classification.mitv2.width_multiplier": 1.0, "model.activation.name": "swish"}.items():
-    setattr(opts, k, v)
-ours = get_model(opts)
-setattr(opts, "model.classification.name", "mobilevit_v2")
-ref = get_model(opts)
-assert list(ours.state_dict().keys()) == list(ref.state_dict().keys())
-ours.load_state_dict(ref.state_dict(), strict=True)
-assert type(ours.layer_3[1]).__module__.startswith("ml_cvnets_b200")
-g, _ = ours.get_trainable_parameters(weight_decay=0.05, no_decay_bn_filter_bias=True)
-import ml_cvnets_b200 as m
-assert type(ours).forward is m.MobileViTv2.forward and type(ours).extract_end_points_all is m.MobileViTv2.extract_end_points_all
-assert len(ours._chain) == 10 and ours.fuse_boundaries and ours._chain[0] is ours.conv_1          # private state of the B200 model travels
-seg = get_model(opts.__class__(**{**vars(opts), "model.classification.name": "mobilevit_v2_b200"}), category="classification", output_stride=8)
-assert seg.layer_5[1].local_rep[0].block.conv.dilation == (4, 4)                                   # segmentation heads: output_stride is honoured
-# the other registered assemblers: same keys / shapes as the reference models they replace
-for ours_name, ref_name, extra in (("mobilevit_b200", "mobilevit", {"model.classification.mit.mode": "xx_small"}),
-                                   ("vit_b200", "vit", {"model.classification.vit.mode": "tiny", "model.classification.vit.norm_layer": "layer_norm_fp32",
-                                                        "model.activation.name": "gelu", "model.classification.activation.name": "gelu"})):
-    for k, v in extra.items():
-        setattr(opts, k, v)
-    setattr(opts, "model.classification.name", ours_name)
-    a = get_model(opts)
-    setattr(opts, "model.classification.name", ref_name)
-    b = get_model(opts)
-    assert {k: tuple(v.shape) for k, v in a.state_dict().items()} == {k: tuple(v.shape) for k, v in b.state_dict().items()}, ours_name
-    a.load_state_dict(b.state_dict(), strict=True)
-print("OK", sum(p.numel() for p in ours.parameters()), [len(x["params"]) for x in g])
-""" % REPO
-    out = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, env=dict(os.environ, PYTHONDONTWRITEBYTECODE="1"))
-    assert out.returncode == 0, out.stderr[-2000:]
-    assert "OK 4901841" in out.stdout
+@pytest.fixture(scope="module")
+def ref_contract(golden_dir):
+    """Signatures, state_dict entries, child trees and reprs of the reference classes (tests/golden/make_golden_contract.py)."""
+    with open(os.path.join(golden_dir, "reference_contract.json")) as f:
+        return json.load(f)
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/cvnets"), reason="reference checkout not present (GPU box)")
-def test_transformer_dropins_match_reference_contract():
+def _sd_entries(mod):
+    return [[k, list(v.shape), str(v.dtype)] for k, v in mod.state_dict().items()]
+
+
+def _sd_digest(mod):
+    e = _sd_entries(mod)
+    return {"n_entries": len(e), "sha256": hashlib.sha256(json.dumps(e, separators=(",", ":")).encode()).hexdigest()}
+
+
+def _params(f):
+    return [p for p in inspect.signature(f).parameters if p not in ("args", "kwargs")]
+
+
+def test_registration_with_reference_checkout(ref_contract):
+    """The assemblers register.py registers with the reference (mobilevit_v2 / mobilevit / vit replacements) build the reference models'
+    exact state_dicts: keys, shapes, dtypes and parameter count."""
+    import ml_cvnets_b200 as m
+    ours = m.MobileViTv2(m.default_opts(width_multiplier=1.0, **{"model.activation.name": "swish"}))
+    ref = ref_contract["mobilevit_v2"]
+    assert _sd_digest(ours) == ref["state_dict"]
+    assert sum(p.numel() for p in ours.parameters()) == ref["n_params"] == 4901841
+    assert len(ours._chain) == 10 and ours.fuse_boundaries and ours._chain[0] is ours.conv_1
+    seg = m.MobileViTv2(m.default_opts(width_multiplier=1.0), output_stride=8)
+    assert seg.layer_5[1].local_rep[0].block.conv.dilation == (4, 4)                                   # segmentation heads: output_stride is honoured
+    assert _sd_digest(m.MobileViT(m.default_mit_opts("xx_small"))) == ref_contract["mobilevit_xx_small"]["state_dict"]
+    assert _sd_digest(m.VisionTransformer(m.default_vit_opts("tiny"))) == ref_contract["vit_tiny"]["state_dict"]
+
+
+def test_transformer_dropins_match_reference_contract(ref_contract):
     """MultiHeadAttention / TransformerEncoder: same constructor parameters, forward parameters, state_dict keys and shapes as the
-    reference classes (SURVEY.md 8b), checked against the reference checkout itself; rebind_modules() swaps them in."""
-    code = r"""
-import sys, os, argparse, inspect
-sys.path.insert(0, %r); sys.path.insert(0, "/root/reference"); os.chdir("/root/reference")
-import ml_cvnets_b200 as ours
-import ml_cvnets_b200.register as r
-from cvnets import modeling_arguments
-from cvnets.layers import MultiHeadAttention as RefMHA
-from cvnets.modules import TransformerEncoder as RefEnc
-def params(f): return [p for p in inspect.signature(f).parameters if p not in ("args", "kwargs")]
-assert params(ours.MultiHeadAttention.__init__) == params(RefMHA.__init__)
-assert params(ours.MultiHeadAttention.forward)[:5] == ["self", "x_q", "x_kv", "key_padding_mask", "attn_mask"]
-assert params(ours.TransformerEncoder.__init__) == params(RefEnc.__init__)
-assert params(ours.TransformerEncoder.forward) == params(RefEnc.forward)
-opts = modeling_arguments(argparse.ArgumentParser()).parse_args([])
-for act in ("swish", "gelu"):
-    setattr(opts, "model.activation.name", act)
-    a, b = ours.TransformerEncoder(opts, 64, 128, num_heads=4), RefEnc(opts, 64, 128, num_heads=4)
-    sa, sb = a.state_dict(), b.state_dict()
-    assert list(sa.keys()) == list(sb.keys()), (list(sa.keys()), list(sb.keys()))
-    assert all(sa[k].shape == sb[k].shape and sa[k].dtype == sb[k].dtype for k in sa)
-    a.load_state_dict(sb, strict=True)
-    assert float(a.pre_norm_mha[0].eps) == float(b.pre_norm_mha[0].eps)
-    assert repr(a).split("(")[0] == repr(b).split("(")[0]
-m1, m2 = ours.MultiHeadAttention(64, 4), RefMHA(64, 4)
-assert list(m1.state_dict().keys()) == list(m2.state_dict().keys())
-r.rebind_modules()
-import cvnets.modules as cm
-assert cm.TransformerEncoder is ours.TransformerEncoder and cm.MobileViTBlockv2 is ours.MobileViTBlockv2
-try:
-    a(__import__("torch").zeros(2, 5, 64))
-    raise SystemExit("CPU input must raise")
-except RuntimeError:
-    pass
-print("OK")
-""" % REPO
-    out = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, env=dict(os.environ, PYTHONDONTWRITEBYTECODE="1"))
-    assert out.returncode == 0, out.stderr[-2000:]
-    assert "OK" in out.stdout
+    reference classes (SURVEY.md 8b)."""
+    import ml_cvnets_b200 as ours
+    ref = ref_contract["transformer"]
+    assert _params(ours.MultiHeadAttention.__init__) == ref["params"]["mha_init"]
+    assert _params(ours.MultiHeadAttention.forward)[:5] == ["self", "x_q", "x_kv", "key_padding_mask", "attn_mask"]
+    assert _params(ours.TransformerEncoder.__init__) == ref["params"]["enc_init"]
+    assert _params(ours.TransformerEncoder.forward) == ref["params"]["enc_forward"]
+    for act in ("swish", "gelu"):
+        a = ours.TransformerEncoder(ours.default_opts(**{"model.activation.name": act}), 64, 128, num_heads=4)
+        assert _sd_entries(a) == ref[act]["state_dict"], act
+        assert float(a.pre_norm_mha[0].eps) == ref[act]["eps"]
+        assert repr(a).split("(")[0] == ref[act]["repr_head"]
+    assert list(ours.MultiHeadAttention(64, 4).state_dict().keys()) == ref["mha_state_dict"]
+    with pytest.raises(RuntimeError):
+        a(torch.zeros(2, 5, 64))  # CPU input must raise
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/cvnets"), reason="reference checkout not present (GPU box)")
-def test_se_block_and_dropout_children_match_reference_contract():
+def test_se_block_and_dropout_children_match_reference_contract(ref_contract):
     """InvertedResidualSE / SqueezeExcitation (SURVEY.md 8f row 4) and the dropout / stochastic-depth children of TransformerEncoder: constructor
-    parameters, child tree, state_dict keys / shapes and repr head against the reference checkout; rebind_modules() swaps the block in."""
-    code = r"""
-import sys, os, argparse, inspect
-sys.path.insert(0, %r); sys.path.insert(0, "/root/reference"); os.chdir("/root/reference")
-import ml_cvnets_b200 as ours
-import ml_cvnets_b200.register as r
-from cvnets import modeling_arguments
-from cvnets.modules import InvertedResidualSE as RefSE, SqueezeExcitation as RefSq, TransformerEncoder as RefEnc
-def params(f): return [p for p in inspect.signature(f).parameters if p not in ("args", "kwargs")]
-assert params(ours.InvertedResidualSE.__init__) == params(RefSE.__init__)
-assert params(ours.SqueezeExcitation.__init__) == params(RefSq.__init__)
-opts = modeling_arguments(argparse.ArgumentParser()).parse_args([])
-for kw in (dict(expand_ratio=4, stride=1, use_se=True, act_fn_name="hard_swish"), dict(expand_ratio=3, stride=2, use_se=True, act_fn_name="relu"),
-           dict(expand_ratio=1, stride=1, use_se=False, act_fn_name="relu"), dict(expand_ratio=2, stride=1, use_se=True, kernel_size=5)):
-    a, b = ours.InvertedResidualSE(opts, 24, 24, **kw), RefSE(opts, 24, 24, **kw)
-    sa, sb = a.state_dict(), b.state_dict()
-    assert list(sa.keys()) == list(sb.keys()), (list(sa.keys()), list(sb.keys()))
-    assert all(sa[k].shape == sb[k].shape and sa[k].dtype == sb[k].dtype for k in sa)
-    a.load_state_dict(sb, strict=True)
-    assert [n for n, _ in a.block.named_children()] == [n for n, _ in b.block.named_children()]
-    assert list(a.block._modules) == list(b.block._modules)                       # incl. the shared activation registered twice
-    assert repr(a) == repr(b), (repr(a), repr(b))
-    assert a.use_res_connect == b.use_res_connect
-e1, e2 = ours.TransformerEncoder(opts, 64, 128, num_heads=4, dropout=0.1, ffn_dropout=0.2), RefEnc(opts, 64, 128, num_heads=4, dropout=0.1, ffn_dropout=0.2)
-assert [type(m).__name__ for m in e1.pre_norm_ffn] == [type(m).__name__ for m in e2.pre_norm_ffn]
-assert (e1.pre_norm_mha[2].p, e1.pre_norm_ffn[3].p, e1.pre_norm_ffn[5].p) == (e2.pre_norm_mha[2].p, e2.pre_norm_ffn[3].p, e2.pre_norm_ffn[5].p)
-s1, s2 = ours.TransformerEncoder(opts, 64, 128, num_heads=4, stochastic_dropout=0.2), RefEnc(opts, 64, 128, num_heads=4, stochastic_dropout=0.2)
-assert type(s1.drop_path).__name__ == type(s2.drop_path).__name__ == "StochasticDepth" and s1.drop_path.p == s2.drop_path.p
-assert list(s1.state_dict().keys()) == list(s2.state_dict().keys())
-r.rebind_modules()
-import cvnets.modules as cm
-assert cm.InvertedResidualSE is ours.InvertedResidualSE and cm.SqueezeExcitation is ours.SqueezeExcitation
-print("OK")
-""" % REPO
-    out = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, env=dict(os.environ, PYTHONDONTWRITEBYTECODE="1"))
-    assert out.returncode == 0, out.stderr[-2000:]
-    assert "OK" in out.stdout
+    parameters, child tree, state_dict keys / shapes and repr against the reference classes."""
+    import ml_cvnets_b200 as ours
+    ref = ref_contract["inverted_residual_se"]
+    assert _params(ours.InvertedResidualSE.__init__) == ref["params"]["se_init"]
+    assert _params(ours.SqueezeExcitation.__init__) == ref["params"]["sq_init"]
+    opts = ours.default_opts(**{"model.activation.name": ref["activation"]})
+    assert len(ref["configs"]) == 4
+    for cfg in ref["configs"]:
+        a = ours.InvertedResidualSE(opts, 24, 24, **cfg["kwargs"])
+        assert _sd_entries(a) == cfg["state_dict"], cfg["kwargs"]
+        assert [n for n, _ in a.block.named_children()] == cfg["children"]
+        assert list(a.block._modules) == cfg["modules"]                       # incl. the shared activation registered twice
+        assert repr(a) == cfg["repr"], (repr(a), cfg["repr"])
+        assert a.use_res_connect == cfg["use_res_connect"]
+    enc = ref
+    e1 = ours.TransformerEncoder(opts, 64, 128, num_heads=4, dropout=0.1, ffn_dropout=0.2)
+    assert [type(m).__name__ for m in e1.pre_norm_ffn] == enc["dropout_children"]["pre_norm_ffn"]
+    assert [e1.pre_norm_mha[2].p, e1.pre_norm_ffn[3].p, e1.pre_norm_ffn[5].p] == enc["dropout_children"]["p"]
+    s1 = ours.TransformerEncoder(opts, 64, 128, num_heads=4, stochastic_dropout=0.2)
+    assert type(s1.drop_path).__name__ == enc["stochastic"]["drop_path"] == "StochasticDepth" and s1.drop_path.p == enc["stochastic"]["p"]
+    assert list(s1.state_dict().keys()) == enc["stochastic"]["state_dict_keys"]
 
 
 def _gloo_worker(rank, world, port, q):

@@ -125,7 +125,7 @@ def test_pw_gemm_small_m_large_k(ops, M, N, K, a_mode):
 @pytest.mark.parametrize("epi,a_mode", [("store", 0), ("store_r", 0), ("silu_bwd", 0), ("store", 2), ("store_r", 3), ("store", 4), ("store", 5),
                                          ("silu_bwd", 5), ("store", 1)])
 def test_pw_gemm_tcgen05_vs_mma_sync(ops, M, N, K, epi, a_mode):
-    """The tcgen05/TMEM kernel and the mma.sync kernel implement the same contract: same inputs -> same outputs / statistics
+    """The wgmma kernel and the mma.sync kernel implement the same contract: same inputs -> same outputs / statistics
     (up to fp32 accumulation order), and both match the fp32 restatement."""
     rps = 64
     nb = (M + rps - 1) // rps
@@ -155,12 +155,12 @@ def test_pw_gemm_tcgen05_vs_mma_sync(ops, M, N, K, epi, a_mode):
             ops.set_tc_enabled(prev)
     acc = load_ref(a_mode, A, pk, A2, row, rps) @ W.float().t()
     ref = acc + bias if epi == "store" else acc + bias + aux.float() if epi == "store_r" else acc * dsilu(sc * aux.float() + sh)
-    for name, (o, col, samp) in zip(("tcgen05", "mma.sync"), outs):
+    for name, (o, col, samp) in zip(("wgmma", "mma.sync"), outs):
         close(o, ref, what=f"{name} out")
         of = o.float()
         close_stat(col[0], of.sum(0), f"{name} col_sum")
         close_stat(col[1], (of * (aux.float() if epi == "silu_bwd" else of)).sum(0), f"{name} col_sq")
-    close(outs[0][0], outs[1][0], rtol=1e-2, atol=1e-2 * float(ref.abs().max()), what="tcgen05 vs mma.sync")
+    close(outs[0][0], outs[1][0], rtol=1e-2, atol=1e-2 * float(ref.abs().max()), what="wgmma vs mma.sync")
     if epi != "silu_bwd":
         close_stat(outs[0][2][0], outs[1][2][0], "samp_sum tc vs mma")
         close_stat(outs[0][2][1], outs[1][2][1], "samp_sq tc vs mma")
@@ -228,7 +228,7 @@ def test_pw_gemm_silu_bwd(ops, M, N, K):
 
 
 @pytest.mark.parametrize("M,N,K,rps,ws", [(512, 64, 136, 64, False), (768, 128, 256, 256, False), (160, 16, 40, 16, False),
-                                           # with a workspace and rows_per_sample % 64 == 0 the epilogue runs on the tcgen05 kernel (sum form)
+                                           # with a workspace and rows_per_sample % 64 == 0 the epilogue runs on the wgmma kernel (sum form)
                                            (768, 128, 256, 256, True), (4096, 192, 392, 1024, True), (1280, 256, 520, 128, True), (1344, 256, 512, 64, True)])
 @pytest.mark.parametrize("bnb", [False, True])
 def test_pw_gemm_gn_bwd(ops, M, N, K, rps, ws, bnb):
@@ -260,7 +260,7 @@ def test_pw_gemm_gn_bwd(ops, M, N, K, rps, ws, bnb):
 
 
 # ----------------------------------------------------------------------------------------------------------- GEMM wgrad
-# K % 64 == 0 shapes run on the tcgen05 kernel (wgrad_tc.cu: MN-major operands, dW block in TMEM), the others on mma.sync
+# K % 64 == 0 shapes run on the wgmma kernel (wgrad_tc.cu: MN-major operands, dW block in registers), the others on mma.sync
 @pytest.mark.parametrize("M,N,K", [(1000, 64, 32), (4096, 128, 64), (777, 264, 40), (300, 72, 200), (5000, 192, 192), (3001, 264, 128),
                                    (2500, 64, 384), (20000, 256, 256), (700, 512, 768), (64, 128, 64)])
 @pytest.mark.parametrize("g_mode,a_mode", [(0, 0), (5, 0), (5, 2), (0, 3), (0, 4), (5, 4), (0, 1)])
@@ -607,7 +607,7 @@ def test_mha_fwd_bwd(ops, B, S, H, c, mask):
 @pytest.mark.parametrize("B,S,H", [(2, 197, 3), (2, 77, 2), (1, 250, 2)])
 @pytest.mark.parametrize("mask", ["none", "causal", "padding"])
 def test_mha_tc_matches_mma(ops, B, S, H, mask):
-    """head_dim 64 has two implementations: tcgen05 (mha_tc.cu, the default) and mma.sync (mha.cu).  Same inputs -> same O / LSE / dQKV up to the
+    """head_dim 64 has two implementations: wgmma (mha_tc.cu, the default) and mma.sync (mha.cu).  Same inputs -> same O / LSE / dQKV up to the
     bf16 rounding of P (the tensor-core operand) and the accumulation order."""
     from ml_cvnets_b200 import _lib as L
     lib = L.load()
@@ -623,7 +623,7 @@ def test_mha_tc_matches_mma(ops, B, S, H, mask):
     res = {}
     old = lib.cvb_set_mha_impl(0)
     try:
-        for name, m in (("mma", 0), ("tc", 7)):  # 7: tcgen05 forward + backward, also with an additive mask
+        for name, m in (("mma", 0), ("tc", 7)):  # 7: wgmma forward + backward, also with an additive mask
             lib.cvb_set_mha_impl(m)
             O, LSE = ops.mha_fwd(qkv, B, S, H, 64, 0.125, attn_mask=amask, key_padding_mask=kpm)
             D = ops.mha_bwd(qkv, O, dO, LSE, B, S, H, 64, 0.125, attn_mask=amask, key_padding_mask=kpm)
@@ -633,7 +633,7 @@ def test_mha_tc_matches_mma(ops, B, S, H, mask):
     for i, what in enumerate(("O", "LSE", "dQKV")):
         a, b = res["tc"][i].double(), res["mma"][i].double()
         r = float((a - b).norm() / (b.norm() + 1e-30))
-        assert r <= 4e-3, f"{what}: tcgen05 vs mma.sync rel-L2 {r:.3g}"
+        assert r <= 4e-3, f"{what}: wgmma vs mma.sync rel-L2 {r:.3g}"
 
 
 @pytest.mark.parametrize("M,K", [(1000, 768), (333, 64), (70, 3072)])

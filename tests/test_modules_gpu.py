@@ -14,6 +14,7 @@ import torch
 import torch.nn.functional as F
 
 from oracle import cvnets_oracle as O
+from golden_sample import at_sample, ref_norm
 
 pytestmark = pytest.mark.gpu
 
@@ -55,7 +56,7 @@ def autocast_errors(oracle_fn, shapes, seed, fx):
     with torch.autocast("cuda", dtype=torch.bfloat16):
         y = oracle_fn(P, x)
     y.backward(fx["gy"].cuda().to(y.dtype))
-    return {k: rel_l2(P["m." + k].grad, g) for k, g in fx["grads"].items()}
+    return {k: rel_l2(*at_sample(P["m." + k].grad, g)) for k, g in fx["grads"].items()}
 
 
 def run_and_check(module, fx, out_tol=2e-2, gx_tol=4e-2, gp_tol=5e-2, check_gx=True, auto=None):
@@ -72,13 +73,14 @@ def run_and_check(module, fx, out_tol=2e-2, gx_tol=4e-2, gp_tol=5e-2, check_gx=T
     named = dict(module.named_parameters())
     for k, g in fx["grads"].items():
         assert named[k].grad is not None, k
-        e, c = rel_l2(named[k].grad, g), cosine(named[k].grad, g)
+        ours, gs = at_sample(named[k].grad, g)
+        e, c = rel_l2(ours, gs), cosine(ours, gs)
         errs[k] = e
         # bias-like gradients are sums over pixels of bf16 gradient tensors: their noise floor is set by bf16 rounding,
         # so the bound is the larger of the fixed tolerance and 3x the torch-autocast error on the same quantity
         tol = max(gp_tol, 3.0 * auto[k]) if auto is not None else gp_tol
-        small = float(g.norm()) < 1e-3 * float(fx["gy"].norm())  # e.g. d(query bias): softmax grads sum to ~0
-        assert (e <= tol and c >= 1 - tol) or small, f"{k}: rel-L2 {e:.4g} (tol {tol:.3g}) cos {c:.5f} |g|={float(g.norm()):.3g}"
+        small = ref_norm(g) < 1e-3 * float(fx["gy"].norm())  # e.g. d(query bias): softmax grads sum to ~0
+        assert (e <= tol and c >= 1 - tol) or small, f"{k}: rel-L2 {e:.4g} (tol {tol:.3g}) cos {c:.5f} |g|={ref_norm(g):.3g}"
     bufs = dict(module.named_buffers())
     for k, b in fx.get("buffers", {}).items():
         if k.endswith("num_batches_tracked"):

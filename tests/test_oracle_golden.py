@@ -1,6 +1,7 @@
 """Pin the oracle (oracle/cvnets_oracle.py) to the fixtures generated from the REAL reference
 (tests/golden/make_golden.py).  CPU only, fp32, tight tolerances."""
 import json
+import math
 import os
 
 import pytest
@@ -8,6 +9,7 @@ import torch
 import torch.nn.functional as F
 
 from oracle import cvnets_oracle as O
+from golden_sample import at_sample, ref_shape
 
 TOL = dict(atol=2e-5, rtol=2e-4)
 
@@ -28,7 +30,7 @@ def _check(P, fx, x, y, prefix="m."):
     torch.testing.assert_close(y, fx["y"], **TOL)
     torch.testing.assert_close(x.grad, fx["gx"], **TOL)
     for k, g in fx["grads"].items():
-        torch.testing.assert_close(P[prefix + k].grad, g, atol=5e-5, rtol=5e-4, msg=lambda m, k=k: f"{k}: {m}")
+        torch.testing.assert_close(*at_sample(P[prefix + k].grad, g), atol=5e-5, rtol=5e-4, msg=lambda m, k=k: f"{k}: {m}")
     for k, b in fx["buffers"].items():
         torch.testing.assert_close(P[prefix + k].detach(), b, **TOL, msg=lambda m, k=k: f"{k}: {m}")
 
@@ -120,6 +122,12 @@ def test_state_dict_contract(golden_dir):
                if not k.endswith(("running_mean", "running_var", "num_batches_tracked"))) == 4901841
 
 
+def _noise_floor(norms):
+    """Gradients below this norm are analytically zero (e.g. the bias of a BatchNorm whose output only feeds another normalisation): what the
+    fixture stores for them is the floating-point rounding of the CPU it was generated on, so only their smallness is checked."""
+    return 1e-6 * math.sqrt(sum(float(n) ** 2 for n in norms))
+
+
 @pytest.mark.parametrize("width", ["1.0", "0.5"])
 def test_mobilevit_v2_model(golden_dir, width):
     fx = torch.load(os.path.join(golden_dir, "mobilevit_v2_fp32.pt"), weights_only=False)[width]
@@ -138,7 +146,11 @@ def test_mobilevit_v2_model(golden_dir, width):
         torch.testing.assert_close(v.flatten()[:: max(1, v.numel() // 512)][:512], fx["stage_sample"][name], atol=1e-4, rtol=1e-3)
     for k, n in fx["grad_norms"].items():
         assert abs(float(P[k].grad.norm()) - n) <= 2e-3 * n + 1e-6, (k, float(P[k].grad.norm()), n)
+    floor = _noise_floor(fx["grad_norms"].values())
     for k, g in fx["grad_small"].items():
+        if float(g.norm()) < floor:
+            assert float(P[k].grad.norm()) < 2 * floor, k
+            continue
         torch.testing.assert_close(P[k].grad, g, atol=1e-4 * float(g.abs().max()) + 1e-7, rtol=2e-3, msg=lambda m, k=k: f"{k}: {m}")
     for k, b in fx["buffers_after"].items():
         torch.testing.assert_close(P[k].detach(), b, atol=1e-5, rtol=1e-4)
@@ -154,7 +166,7 @@ def _check_nobuf(P, fx, x, y, prefix="m."):
     torch.testing.assert_close(y, fx["y"], **TOL)
     torch.testing.assert_close(x.grad, fx["gx"], **TOL)
     for k, g in fx["grads"].items():
-        torch.testing.assert_close(P[prefix + k].grad, g, atol=5e-5, rtol=5e-4, msg=lambda m, k=k: f"{k}: {m}")
+        torch.testing.assert_close(*at_sample(P[prefix + k].grad, g), atol=5e-5, rtol=5e-4, msg=lambda m, k=k: f"{k}: {m}")
 
 
 @pytest.mark.parametrize("name", ["mha", "mha_hd32", "mha_causal", "mha_padding"])
@@ -221,8 +233,13 @@ def test_model_batch16_fixture(golden_dir):
     assert abs(float(loss) - float(fx["loss"])) <= 1e-5
     for k, n in fx["grad_norms"].items():
         assert abs(float(P[k].grad.norm()) - n) <= 2e-3 * n + 1e-7, k
+    floor = _noise_floor(fx["grad_norms"].values())
     for k, g in fx["grads"].items():
-        e = float((P[k].grad - g.float()).norm() / (g.float().norm() + 1e-12))
+        if fx["grad_norms"][k] < floor:
+            assert float(P[k].grad.norm()) < 2 * floor, k
+            continue
+        ours, g = at_sample(P[k].grad, g)
+        e = float((ours - g.float()).norm() / (g.float().norm() + 1e-12))
         assert e <= (2e-3 if g.dtype == torch.float16 else 2e-4), (k, e)
 
 
@@ -260,7 +277,11 @@ def test_mobilevit_v1_xxs_fixture(golden_dir):
     loss.backward()
     assert float((logits - fx["logits"]).norm() / fx["logits"].norm()) <= 5e-5
     assert abs(float(loss) - float(fx["loss"])) <= 1e-5
+    floor = _noise_floor(g.norm() for g in fx["grads"].values())
     for k, g in fx["grads"].items():
+        if float(g.norm()) < floor:
+            assert float(P[k].grad.norm()) < 2 * floor, k
+            continue
         assert float((P[k].grad - g).norm() / (g.norm() + 1e-12)) <= 2e-3, k
 
 
@@ -292,12 +313,14 @@ def test_dilated_backbone_fixture(golden_dir):
         _, st = O.mobilevit_v2_forward(P, x, width_multiplier=fx["width"], training=True, return_stages=True, output_stride=os_)
         ends = {"out_l3": st["layer_3.1"], "out_l4": st["layer_4.1"], "out_l5": st["layer_5.1"]}
         for k, v in rec["ends"].items():
-            assert ends[k].shape == v.shape, (os_, k, ends[k].shape, v.shape)
-            assert float((ends[k] - v).norm() / v.norm()) <= 2e-5, (os_, k)
+            assert tuple(ends[k].shape) == ref_shape(v), (os_, k, ends[k].shape, ref_shape(v))
+            ours, v = at_sample(ends[k], v)
+            assert float((ours - v).norm() / v.norm()) <= 2e-5, (os_, k)
         if "grads" in rec:
             gy4, gy5 = (O.seeded_input(tuple(ends[k].shape), sd) for k, sd in zip(("out_l4", "out_l5"), rec["gy_seeds"]))
             ((ends["out_l4"] * gy4).sum() + (ends["out_l5"] * gy5).sum()).backward()
             for k, n in rec["grad_norms"].items():
                 assert abs(float(P[k].grad.norm()) - n) <= 2e-3 * n + 1e-6, k
             for k, g in rec["grads"].items():
-                assert float((P[k].grad - g).norm() / (g.norm() + 1e-12)) <= 5e-4, k
+                ours, g = at_sample(P[k].grad, g)
+                assert float((ours - g).norm() / (g.norm() + 1e-12)) <= 5e-4, k

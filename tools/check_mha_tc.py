@@ -1,4 +1,4 @@
-"""tcgen05 attention core (csrc/mha_tc.cu) against the fp32 formula AND the mma.sync kernels (csrc/mha.cu), plus same-box A/B timing.
+"""wgmma attention core (csrc/mha_tc.cu) against the fp32 formula AND the mma.sync kernels (csrc/mha.cu), plus same-box A/B timing.
 
     python tools/check_mha_tc.py [--stage fwd|bwd|time] [--out gpurun_out/mha_tc_check.txt]
 
