@@ -31,7 +31,7 @@ typedef void* cvb_stream_t; /* cudaStream_t */
 #define CVB_API
 #endif
 
-#define CVB_ABI_VERSION 9
+#define CVB_ABI_VERSION 10
 
 /* operand "load modes": the normalisation / activation of the PRODUCER layer is applied while the CONSUMER loads it
  * (training-mode BatchNorm cannot be fused into its own conv: SURVEY.md section 7 "hard parts"). */
@@ -239,9 +239,11 @@ CVB_API int cvb_linattn_cross_bwd(const void* QK_prev, int ldq, const void* V_x,
  * QKV: bf16 [B*S, ldq] rows = tokens, columns [q (H*c) | k (H*c) | v (H*c)] exactly as qkv_proj writes them (:148-153);
  * O: bf16 [B*S, ldo] with head h at columns h*c.. (the layout out_proj reads, :236).  scale = head_dim^-0.5 (:70, :187).
  * attn_mask: fp32 [B, S, S] additive (or NULL, :197-208); key_padding_mask: uint8 [B, S], non-zero = masked with -inf (:210-224).
- * Softmax in fp32 (:226-228).  LSE: fp32 [B, H, S] log-sum-exp (base 2) saved for the backward.  S <= 256, even c <= 64.
- * head_dim == 64 (ViT-B / CLIP image tower, key-padding masks included) runs on wgmma tensor cores (mha_tc.cu: TMA-staged operands, whole
- * score rows in registers); every other head_dim, and heads with an additive mask, on the mma.sync kernels (mha.cu).
+ * Softmax in fp32 (:226-228).  LSE: fp32 [B, H, S] log-sum-exp (base 2) saved for the backward.  Even c <= 64; S <= 256, or any S for c = 64.
+ * head_dim == 64 (ViT-B / CLIP image tower, key-padding masks included) runs on wgmma tensor cores: S <= 256 in mha_tc.cu (TMA-staged operands,
+ * whole score rows in registers), S > 256 (ViT / CLIP at 256-512 px crops) in mha_long.cu (K/V and Q/dO streamed through shared memory in
+ * 64-row tiles, online softmax; a backward without atomics, bitwise reproducible).  Every other head_dim, and heads with an additive mask at
+ * S <= 256, run on the mma.sync kernels (mha.cu).
  * ------------------------------------------------------------------------------------------------------------- */
 CVB_API int cvb_mha_fwd(const void* QKV, int ldq, int B, int S, int H, int head_dim, float scale, const float* attn_mask,
                 const unsigned char* key_padding_mask, void* O, int ldo, float* LSE, cvb_stream_t stream);
@@ -250,7 +252,8 @@ CVB_API int cvb_mha_bwd(const void* QKV, int ldq, const void* O, const void* DO,
                 float scale, const float* attn_mask, const unsigned char* key_padding_mask, void* DQKV, int lddq, cvb_stream_t stream);
 /* Diagnostics / A-B timing: which head_dim == 64 implementation runs.  bit 0: wgmma forward, bit 1: wgmma backward, bit 2: wgmma also
  * for heads with an additive attn_mask (default 3: additive-mask heads -- the causal CLIP text tower, S = 77 -- stay on mma.sync;
- * the environment variable CVB_MHA_TC sets the initial value).  Returns the previous mask. */
+ * the environment variable CVB_MHA_TC sets the initial value).  bit 3: the streaming kernels (mha_long.cu) also for S <= 256, to cross-check
+ * them against the register-resident ones.  Returns the previous mask. */
 CVB_API int cvb_set_mha_impl(int mask);
 /* per-token LayerNorm statistics of a bf16 [M, C] matrix: mean[m], rstd[m] = 1/sqrt(var + eps) (biased variance, fp32 math like
  * nn.LayerNorm under autocast).  The normalisation itself is the GN load mode of the consuming GEMM with rows_per_sample = 1. */
@@ -398,6 +401,13 @@ CVB_API int cvb_concat2(const void* A, const void* B, int C1, int C2, int64_t M,
 CVB_API int cvb_split2(const void* G, int C1, int C2, int64_t M, void* DA, void* DB, cvb_stream_t stream);
 CVB_API int cvb_vit_tokens_fwd(const void* patch, const float* pos, const float* cls, void* out, int B, int N, int C, cvb_stream_t stream);
 CVB_API int cvb_vit_tokens_bwd(const void* dout, void* dpatch, float* dpos, float* dcls, int B, int N, int C, cvb_stream_t stream);
+/* The same with a positional table of n_pos != N rows (inputs other than 224 x 224; cvnets/layers/positional_embedding.py:90-95): the table is
+ * resampled to N rows as F.interpolate(pos [1, 1, n_pos, C], size=(N, C), mode="bilinear", align_corners=False) does -- a 1-D linear
+ * resample of the flattened patch index -- inside the kernel, in fp32, and added to the patch row with one bf16 rounding.  The backward sums
+ * dout over the batch per token and gathers the transposed stencil into dpos [n_pos, C] (+=) without atomics: bitwise reproducible. */
+CVB_API int cvb_vit_tokens_interp_fwd(const void* patch, const float* pos, int n_pos, const float* cls, void* out, int B, int N, int C,
+                                      cvb_stream_t stream);
+CVB_API int cvb_vit_tokens_interp_bwd(const void* dout, void* dpatch, float* dpos, int n_pos, float* dcls, int B, int N, int C, cvb_stream_t stream);
 
 #ifdef __cplusplus
 }

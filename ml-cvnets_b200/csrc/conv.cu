@@ -145,6 +145,86 @@ __global__ void __launch_bounds__(CNT) vit_tokens_bwd_kernel(const bf16* __restr
   }
 }
 
+// Interpolated positional embeddings (cvnets/layers/positional_embedding.py:90-95): the reference resizes the [1, 1, n_pos, C] table to
+// (N, C) with F.interpolate(mode="bilinear", align_corners=False).  The C axis maps onto itself, so this is a 1-D linear resample of the
+// flattened patch index (not a 2-D resample of the patch grid), with PyTorch's source-index rule: scale = n_pos / N,
+// src = max(scale (s + 0.5) - 0.5, 0), i0 = floor(src), i1 = i0 + (i0 < n_pos - 1), lambda = src - i0.  Unfused roundings: the products
+// are computed as PyTorch's CPU kernel does.
+__device__ __forceinline__ void interp_src(int s, float scale, int n_pos, int& i0, int& i1, float& lam) {
+  const float src = fmaxf(__fsub_rn(__fmul_rn(scale, __fadd_rn((float)s, 0.5f)), 0.5f), 0.f);
+  i0 = (int)src;
+  i1 = i0 + (i0 < n_pos - 1 ? 1 : 0);
+  lam = __fsub_rn(src, (float)i0);
+}
+
+// out[b, 0] = cls;  out[b, 1 + s] = patch[b, s] + (1 - lambda_s) pos[i0_s] + lambda_s pos[i1_s], in fp32, rounded once to bf16
+__global__ void __launch_bounds__(CNT) vit_tokens_interp_fwd_kernel(const bf16* __restrict__ patch, const float* __restrict__ pos, int n_pos, float scale,
+                                                                    const float* __restrict__ cls, bf16* __restrict__ out, int B, int N, int C, int has_cls) {
+  pdl_wait();
+  pdl_trigger();
+  const int cg = C >> 3, S = N + has_cls;
+  const int64_t total = (int64_t)B * S * cg;
+  for (int64_t idx = (int64_t)blockIdx.x * CNT + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * CNT) {
+    const int c8 = (int)(idx % cg);
+    const int64_t tok = idx / cg;
+    const int t = (int)(tok % S);
+    const int64_t b = tok / S;
+    float f[8];
+    if (has_cls && t == 0) {
+#pragma unroll
+      for (int q = 0; q < 8; ++q) f[q] = cls[c8 * 8 + q];
+    } else {
+      const int n = t - has_cls;
+      int i0, i1;
+      float lam;
+      interp_src(n, scale, n_pos, i0, i1, lam);
+      const float w0 = __fsub_rn(1.f, lam);
+      unpack8(ldg16(patch + (b * N + n) * C + c8 * 8), f);
+#pragma unroll
+      for (int q = 0; q < 8; ++q)
+        f[q] += __fadd_rn(__fmul_rn(w0, pos[(int64_t)i0 * C + c8 * 8 + q]), __fmul_rn(lam, pos[(int64_t)i1 * C + c8 * 8 + q]));
+    }
+    stg16(out + tok * C + c8 * 8, pack8(f));
+  }
+}
+
+// dpos[j] += sum over output tokens s (ascending) of (1 - lambda_s) [i0_s == j] g[s] + lambda_s [i1_s == j] g[s], g = the batch sum of dout
+// (fp32 [N, C]).  A gather over the few tokens whose stencil touches table row j: one thread per (j, 8 channels), no atomics.
+__global__ void __launch_bounds__(CNT) vit_pos_interp_bwd_kernel(const float* __restrict__ g, float* __restrict__ dpos, int n_pos, float scale, int N,
+                                                                 int C) {
+  pdl_wait();
+  pdl_trigger();
+  const int cg = C >> 3;
+  const int64_t total = (int64_t)n_pos * cg;
+  for (int64_t idx = (int64_t)blockIdx.x * CNT + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * CNT) {
+    const int c8 = (int)(idx % cg), j = (int)(idx / cg);
+    // tokens with i0 in {j - 1, j}: src in [j - 1, j + 1), i.e. s in ((j - 0.5) / scale - 0.5, (j + 1.5) / scale - 0.5), widened by 2
+    const int s_lo = max(0, (int)((j - 1.0f) / scale) - 2), s_hi = min(N - 1, (int)((j + 2.0f) / scale) + 2);
+    float acc[8];
+#pragma unroll
+    for (int q = 0; q < 8; ++q) acc[q] = 0.f;
+    for (int s = s_lo; s <= s_hi; ++s) {
+      int i0, i1;
+      float lam;
+      interp_src(s, scale, n_pos, i0, i1, lam);
+      if (i0 != j && i1 != j) continue;
+      const float* gs = g + (int64_t)s * C + c8 * 8;
+      if (i0 == j) {
+        const float w0 = __fsub_rn(1.f, lam);
+#pragma unroll
+        for (int q = 0; q < 8; ++q) acc[q] = __fadd_rn(acc[q], __fmul_rn(w0, gs[q]));
+      }
+      if (i1 == j) {
+#pragma unroll
+        for (int q = 0; q < 8; ++q) acc[q] = __fadd_rn(acc[q], __fmul_rn(lam, gs[q]));
+      }
+    }
+    float* dst = dpos + (int64_t)j * C + c8 * 8;
+#pragma unroll
+    for (int q = 0; q < 8; ++q) dst[q] += acc[q];
+  }
+}
+
 // MobileViT-v1 unfolding / folding (cvnets/modules/mobilevit_block.py:186-267) on channels-last rows: the feature map row (b, h, w) and the
 // token row (b*P + p, n) with p = (h % ph) * pw + (w % pw), n = (h / ph) * (W / pw) + (w / pw) hold the same C values: a row permutation.
 __global__ void __launch_bounds__(CNT) patch_permute_kernel(const bf16* __restrict__ X, bf16* __restrict__ OUT, int H, int W, int C, int ph, int pw,
@@ -272,4 +352,33 @@ extern "C" int cvb_split2(const void* G, int C1, int C2, int64_t M, void* DA, vo
                       static_cast<bf16*>(DB)));
   CVB_LAUNCH_CHECK();
   return 0;
+}
+
+extern "C" int cvb_vit_tokens_interp_fwd(const void* patch, const float* pos, int n_pos, const float* cls, void* out, int B, int N, int C,
+                                         cvb_stream_t stream) {
+  CVB_CHECK(patch && pos && out && B > 0 && N > 0 && n_pos > 0 && C > 0 && C % 8 == 0 && cvb_aligned16(patch) && cvb_aligned16(out),
+            "cvb_vit_tokens_interp_fwd: bad arguments");
+  const int has_cls = cls != nullptr;
+  CVB_CUDA(cvb_launch(vit_tokens_interp_fwd_kernel, cgrid((int64_t)B * (N + has_cls) * (C / 8)), CNT, 0, static_cast<cudaStream_t>(stream),
+                      static_cast<const bf16*>(patch), pos, n_pos, (float)n_pos / (float)N, cls, static_cast<bf16*>(out), B, N, C, has_cls));
+  CVB_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int cvb_vit_tokens_interp_bwd(const void* dout, void* dpatch, float* dpos, int n_pos, float* dcls, int B, int N, int C, cvb_stream_t stream) {
+  CVB_CHECK(dout && dpatch && dpos && B > 0 && N > 0 && n_pos > 0 && C > 0 && C % 8 == 0 && cvb_aligned16(dout) && cvb_aligned16(dpatch),
+            "cvb_vit_tokens_interp_bwd: bad arguments");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int has_cls = dcls != nullptr;
+  // batch sum per output token into a zeroed fp32 [N, C] scratch (the non-interpolating kernel, dpos = scratch), then the transposed stencil
+  double* ws = nullptr;
+  if (cvb_det_alloc(&ws, ((size_t)N * C + 1) / 2, st)) return 2;
+  float* g = reinterpret_cast<float*>(ws);
+  CVB_CUDA(cvb_launch(vit_tokens_bwd_kernel, cgrid((int64_t)(N + has_cls) * (C / 8)), CNT, 0, st, static_cast<const bf16*>(dout), static_cast<bf16*>(dpatch),
+                      g, dcls, B, N, C, has_cls));
+  CVB_LAUNCH_CHECK();
+  CVB_CUDA(cvb_launch(vit_pos_interp_bwd_kernel, cgrid((int64_t)n_pos * (C / 8)), CNT, 0, st, static_cast<const float*>(g), dpos, n_pos,
+                      (float)n_pos / (float)N, N, C));
+  CVB_LAUNCH_CHECK();
+  return cvb_det_free(ws, st);
 }

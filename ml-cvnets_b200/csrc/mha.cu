@@ -405,14 +405,19 @@ int launch_bwd(const void* QKV, int ldq, const void* O, const void* DO, int ldo,
 int check_common(const char* who, const void* QKV, int ldq, int B, int S, int H, int head_dim, int ldo) {
   CVB_CHECK(QKV && B > 0 && S > 0 && H > 0, "%s: bad arguments", who);
   CVB_CHECK(head_dim >= 2 && head_dim <= 64 && head_dim % 2 == 0, "%s: head_dim %d not supported (even values up to 64)", who, head_dim);
-  CVB_CHECK(S <= 256, "%s: sequence length %d > 256 is not supported in this round (K/V of one head are shared-memory resident)", who, S);
+  CVB_CHECK(S <= 256 || head_dim == 64, "%s: sequence length %d > 256 needs head_dim 64 (got %d): the streaming kernels are head_dim-64 only, the "
+            "other head dims keep K/V of one head in shared memory", who, S, head_dim);
   CVB_CHECK(ldq % 8 == 0 && ldo % 8 == 0 && ldq >= 3 * H * head_dim && ldo >= H * head_dim && cvb_aligned16(QKV), "%s: bad leading dimensions / alignment", who);
   return 0;
 }
 
 }  // namespace
 
-// head_dim == 64: wgmma kernels (mha_tc.cu); -1 = not handled there
+// head_dim == 64: streaming wgmma kernels for S > 256 (mha_long.cu), register-resident wgmma kernels (mha_tc.cu); -1 = not handled there
+int cvb_mha_fwd_long(const void* QKV, int ldq, int B, int S, int H, int head_dim, float scale, const float* amask, const unsigned char* kpm, void* O,
+                     int ldo, float* LSE, cudaStream_t st);
+int cvb_mha_bwd_long(const void* QKV, int ldq, const void* O, const void* DO, int ldo, const float* LSE, int B, int S, int H, int head_dim, float scale,
+                     const float* amask, const unsigned char* kpm, void* DQKV, int lddq, cudaStream_t st);
 int cvb_mha_fwd_tc(const void* QKV, int ldq, int B, int S, int H, int head_dim, float scale, const float* amask, const unsigned char* kpm, void* O,
                    int ldo, float* LSE, cudaStream_t st);
 int cvb_mha_bwd_tc(const void* QKV, int ldq, const void* O, const void* DO, int ldo, const float* LSE, int B, int S, int H, int head_dim, float scale,
@@ -423,6 +428,10 @@ extern "C" int cvb_mha_fwd(const void* QKV, int ldq, int B, int S, int H, int he
   if (check_common("cvb_mha_fwd", QKV, ldq, B, S, H, head_dim, ldo)) return 1;
   CVB_CHECK(O && LSE && cvb_aligned16(O), "cvb_mha_fwd: null / misaligned output");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
+  {
+    const int rc = cvb_mha_fwd_long(QKV, ldq, B, S, H, head_dim, scale, attn_mask, key_padding_mask, O, ldo, LSE, st);
+    if (rc >= 0) return rc;
+  }
   {
     const int rc = cvb_mha_fwd_tc(QKV, ldq, B, S, H, head_dim, scale, attn_mask, key_padding_mask, O, ldo, LSE, st);
     if (rc >= 0) return rc;
@@ -438,6 +447,10 @@ extern "C" int cvb_mha_bwd(const void* QKV, int ldq, const void* O, const void* 
   CVB_CHECK(O && DO && LSE && DQKV && cvb_aligned16(O) && cvb_aligned16(DO) && cvb_aligned16(DQKV) && lddq % 8 == 0 && lddq >= 3 * H * head_dim,
             "cvb_mha_bwd: null / misaligned operand");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
+  {
+    const int rc = cvb_mha_bwd_long(QKV, ldq, O, DO, ldo, LSE, B, S, H, head_dim, scale, attn_mask, key_padding_mask, DQKV, lddq, st);
+    if (rc >= 0) return rc;
+  }
   {
     const int rc = cvb_mha_bwd_tc(QKV, ldq, O, DO, ldo, LSE, B, S, H, head_dim, scale, attn_mask, key_padding_mask, DQKV, lddq, st);
     if (rc >= 0) return rc;

@@ -333,7 +333,7 @@ __global__ void __launch_bounds__(BW_THREADS, 1)
 
 // bit 0: wgmma forward, bit 1: wgmma backward, bit 2: also for heads with an ADDITIVE mask.  Default 3: additive masks (the causal mask of
 // the CLIP text tower, S = 77) stay on the mma.sync kernels, which read the [S, S] mask in coalesced tiles; here every thread gathers
-// single mask values of its score fragment.
+// single mask values of its score fragment.  bit 3: the streaming kernels of mha_long.cu also for S <= 256 (cross-checks only).
 int g_impl = -1;
 int impl() {
   if (g_impl < 0) {
@@ -345,9 +345,11 @@ int impl() {
 
 }  // namespace
 
+int cvb_mha_impl() { return impl(); }
+
 extern "C" int cvb_set_mha_impl(int mask) {
   const int old = impl();
-  g_impl = mask & 7;
+  g_impl = mask & 15;
   return old;
 }
 

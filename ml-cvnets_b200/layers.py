@@ -523,8 +523,11 @@ class MultiHeadAttention(BaseLayer):
             raise NotImplementedError("cross-attention (x_kv) is not implemented on the GPU path")
         if not x_q.is_cuda:
             raise RuntimeError("MultiHeadAttention: ml-cvnets_b200 has no CPU path")
-        if x_q.dim() != 3 or x_q.shape[1] > 256:
-            raise NotImplementedError("MultiHeadAttention expects [N, S, C] with S <= 256")
+        if x_q.dim() != 3:
+            raise NotImplementedError("MultiHeadAttention expects [N, S, C]")
+        if x_q.shape[1] > 256 and self.head_dim != 64:
+            raise NotImplementedError(f"MultiHeadAttention: S = {x_q.shape[1]} > 256 needs head_dim 64 (the streaming attention kernels); "
+                                      f"head_dim {self.head_dim} keeps a head in shared memory and supports S <= 256")
         if self._cfg is None:
             prep = PW()
             self._cfg = self.build_cfg(prep)

@@ -4,8 +4,11 @@
 Host code like the MobileViTv2 assembler: same attribute names / ``state_dict`` keys as the reference (``patch_emb.{0,1,2}.block.*``,
 ``cls_token``, ``pos_embed.pos_embed.pos_embed``, ``transformer.{i}.*``, ``post_transformer_norm.*``, ``classifier.*``), every forward /
 backward kernel is the library's.  BASELINE.json configs[2]: ViT-B/16, bf16, 224x224 (examples/vit/classification/vit_base.yaml).
-Not implemented (raises): SimpleFPN (detection), sinusoidal / interpolated positional embeddings (inputs other than 224x224 with the
-default 196 embeddings), output_stride, gradient checkpointing, attention-probability dropout > 0 in training.
+Any input resolution whose sides are multiples of 16 works, square or not (the multi-scale recipes feed 128-320 px crops): when the patch
+grid does not hold the table's 196 entries, the positional table is linearly resampled in the token-assembly kernel exactly as the
+reference's F.interpolate does (cvnets/layers/positional_embedding.py:90-95), and sequences over 256 tokens run on the streaming attention
+kernels (every ViT mode has head_dim 64).  Not implemented (raises): SimpleFPN (detection), sinusoidal positional embeddings,
+output_stride, gradient checkpointing, attention-probability dropout > 0 in training.
 """
 from __future__ import annotations
 
@@ -146,9 +149,7 @@ class VisionTransformer(nn.Module):
     def extract_patch_embeddings(self, x: Tensor) -> Tuple[Tensor, Tuple[int, int]]:
         patch = self.patch_emb(x)  # [B, d, nh, nw], channels-last == token-major [B*N, d]
         n_h, n_w = patch.shape[-2:]
-        pe = self.pos_embed.pos_embed.pos_embed
-        if n_h * n_w != pe.shape[2]:
-            raise NotImplementedError("interpolated positional embeddings (inputs other than 224x224) are not implemented")
+        pe = self.pos_embed.pos_embed.pos_embed  # resampled to n_h * n_w rows inside the token kernel when the counts differ
         tok = self._tok
         tok.ws = getattr(self, "_ws", None)
         tok.plist = [pe] + ([self.cls_token] if self.cls_token is not None else [])

@@ -499,8 +499,12 @@ class TransformerEncoder(BaseModule):
         if self.training and self.pre_norm_mha[1].attn_dropout.p:
             raise NotImplementedError("attention-probability dropout > 0 in training mode is not implemented (every recipe of the reference sets 0; "
                                       "it is the identity in eval mode, which works)")
-        if x.dim() != 3 or x.shape[1] > 256:
-            raise NotImplementedError("TransformerEncoder expects [N, S, C] with S <= 256")
+        if x.dim() != 3:
+            raise NotImplementedError("TransformerEncoder expects [N, S, C]")
+        hd = self.pre_norm_mha[1].head_dim
+        if x.shape[1] > 256 and hd != 64:
+            raise NotImplementedError(f"TransformerEncoder: S = {x.shape[1]} > 256 needs head_dim 64 (the streaming attention kernels); "
+                                      f"head_dim {hd} keeps a head in shared memory and supports S <= 256")
         if x.shape[1] == x.shape[2]:
             raise NotImplementedError("S == C: the reference's LayerNorm would take its channel-first branch (layer_norm.py:52-65)")
         if self._cfg is None:

@@ -370,6 +370,25 @@ def vit_tokens_bwd(dout: Tensor, dpos: Tensor, dcls: Optional[Tensor], B: int, N
     return dpatch
 
 
+def vit_tokens_interp_fwd(patch: Tensor, pos: Tensor, cls: Optional[Tensor], B: int, N: int, C: int) -> Tensor:
+    """Token assembly with the positional table ``pos`` ([.., n_pos, C] fp32) linearly resampled to N rows (F.interpolate, align_corners=False)."""
+    S = N + (1 if cls is not None else 0)
+    out = torch.empty((B, S, C), device=patch.device, dtype=torch.bfloat16)
+    L.check(_lib().cvb_vit_tokens_interp_fwd(patch.data_ptr(), pos.data_ptr(), pos.shape[-2], _p(cls), out.data_ptr(), B, N, C, _stream()),
+            "cvb_vit_tokens_interp_fwd")
+    _count()
+    return out
+
+
+def vit_tokens_interp_bwd(dout: Tensor, dpos: Tensor, dcls: Optional[Tensor], B: int, N: int, C: int) -> Tensor:
+    """Adjoint of vit_tokens_interp_fwd: returns dpatch, adds into dpos ([n_pos, C] fp32) and dcls."""
+    dpatch = torch.empty((B * N, C), device=dout.device, dtype=torch.bfloat16)
+    L.check(_lib().cvb_vit_tokens_interp_bwd(dout.data_ptr(), dpatch.data_ptr(), dpos.data_ptr(), dpos.shape[-2], _p(dcls), B, N, C, _stream()),
+            "cvb_vit_tokens_interp_bwd")
+    _count()
+    return dpatch
+
+
 def stem_im2col(x: Tensor, mix: Optional[Tensor] = None) -> Tensor:
     """fp32 image [B,3,H,W] (any strides) -> bf16 patch matrix [B*(H/2)*(W/2), 32]; ``mix`` (device float[6]) folds mixup / cutmix in."""
     lib = _lib()
