@@ -31,7 +31,7 @@ typedef void* cvb_stream_t; /* cudaStream_t */
 #define CVB_API
 #endif
 
-#define CVB_ABI_VERSION 10
+#define CVB_ABI_VERSION 11
 
 /* operand "load modes": the normalisation / activation of the PRODUCER layer is applied while the CONSUMER loads it
  * (training-mode BatchNorm cannot be fused into its own conv: SURVEY.md section 7 "hard parts"). */
@@ -250,11 +250,10 @@ CVB_API int cvb_mha_fwd(const void* QKV, int ldq, int B, int S, int H, int head_
 /* dQKV (bf16 [B*S, lddq], same column layout as QKV) from dO; recomputes the probabilities from LSE. */
 CVB_API int cvb_mha_bwd(const void* QKV, int ldq, const void* O, const void* DO, int ldo, const float* LSE, int B, int S, int H, int head_dim,
                 float scale, const float* attn_mask, const unsigned char* key_padding_mask, void* DQKV, int lddq, cvb_stream_t stream);
-/* Diagnostics / A-B timing: which head_dim == 64 implementation runs.  bit 0: wgmma forward, bit 1: wgmma backward, bit 2: wgmma also
- * for heads with an additive attn_mask (default 3: additive-mask heads -- the causal CLIP text tower, S = 77 -- stay on mma.sync;
- * the environment variable CVB_MHA_TC sets the initial value).  bit 3: the streaming kernels (mha_long.cu) also for S <= 256, to cross-check
- * them against the register-resident ones.  Returns the previous mask. */
-CVB_API int cvb_set_mha_impl(int mask);
+/* Testing hook: which kernel family serves a head, forward and backward alike.  0 = automatic (default, as described above);
+ * 1 = the mma.sync kernels wherever they can run (S <= 256); 2 = the streaming kernels for every head_dim-64 shape.  Modes 1 and 2
+ * cross-check the families against each other; any other value selects 0.  Returns the previous mode. */
+CVB_API int cvb_set_mha_impl(int mode);
 /* per-token LayerNorm statistics of a bf16 [M, C] matrix: mean[m], rstd[m] = 1/sqrt(var + eps) (biased variance, fp32 math like
  * nn.LayerNorm under autocast).  The normalisation itself is the GN load mode of the consuming GEMM with rows_per_sample = 1. */
 /* LayerNorm backward of a [M, C] token matrix in one pass (autograd of nn.LayerNorm as used at transformer.py:77-95):
@@ -388,9 +387,6 @@ CVB_API int cvb_unprep_grad(const float* src, float* dst, int rows, int cols, in
 CVB_API int cvb_im2col(const void* X, int x_fp32, int64_t sxn, int64_t sxc, int64_t sxh, int64_t sxw, int B, int Cin, int H, int W, int k, int stride,
                int pad, void* A, int lda, cvb_stream_t stream);
 CVB_API int cvb_col2im(const void* dA, int lda, int B, int Cin, int H, int W, int k, int stride, int pad, void* dX, cvb_stream_t stream);
-/* ViT token assembly (vit.py:476-507): out[b,0] = cls (no positional term), out[b,1+n] = patch[b,n] + pos[n]; patch bf16 [B*N, C] (the
- * channels-last output of the last stem conv IS token-major), pos fp32 [N, C], cls fp32 [C] or NULL, out bf16 [B, N(+1), C].
- * bwd: dpatch = dout[:, 1:], dpos += sum_b dout[:, 1:], dcls += sum_b dout[:, 0] (fp32, accumulated into caller-zeroed buffers). */
 /* MobileViT-v1 unfolding / folding (cvnets/modules/mobilevit_block.py:186-267) as a row permutation of the channels-last matrix:
  * feature-map row (b, h, w) <-> token row (b*P + p, n), p = (h % ph)*pw + (w % pw), n = (h / ph)*(W / pw) + (w / pw), P = ph*pw.
  * inverse = 0: X is the feature map [B*H*W, C], OUT the token matrix [B*P, N, C]; inverse = 1: the other way (folding).  The permutation
@@ -399,12 +395,13 @@ CVB_API int cvb_patch_permute(const void* X, void* OUT, int B, int H, int W, int
 /* OUT[m, :] = [A[m, :C1] | B[m, :C2]] (torch.cat((res, fm), dim=1) on channels-last maps, mobilevit_block.py:287) and the adjoint split */
 CVB_API int cvb_concat2(const void* A, const void* B, int C1, int C2, int64_t M, void* OUT, cvb_stream_t stream);
 CVB_API int cvb_split2(const void* G, int C1, int C2, int64_t M, void* DA, void* DB, cvb_stream_t stream);
-CVB_API int cvb_vit_tokens_fwd(const void* patch, const float* pos, const float* cls, void* out, int B, int N, int C, cvb_stream_t stream);
-CVB_API int cvb_vit_tokens_bwd(const void* dout, void* dpatch, float* dpos, float* dcls, int B, int N, int C, cvb_stream_t stream);
-/* The same with a positional table of n_pos != N rows (inputs other than 224 x 224; cvnets/layers/positional_embedding.py:90-95): the table is
- * resampled to N rows as F.interpolate(pos [1, 1, n_pos, C], size=(N, C), mode="bilinear", align_corners=False) does -- a 1-D linear
- * resample of the flattened patch index -- inside the kernel, in fp32, and added to the patch row with one bf16 rounding.  The backward sums
- * dout over the batch per token and gathers the transposed stencil into dpos [n_pos, C] (+=) without atomics: bitwise reproducible. */
+/* ViT token assembly (vit.py:476-507): out[b,0] = cls (no positional term), out[b,1+n] = patch[b,n] + pos'[n]; patch bf16 [B*N, C] (the
+ * channels-last output of the last stem conv IS token-major), pos fp32 [n_pos, C], cls fp32 [C] or NULL, out bf16 [B, N(+1), C].
+ * pos' is the table resampled to N rows as F.interpolate(pos [1, 1, n_pos, C], size=(N, C), mode="bilinear", align_corners=False) does
+ * (cvnets/layers/positional_embedding.py:90-95) -- a 1-D linear resample of the flattened patch index, the identity when N == n_pos
+ * (224 x 224 inputs) -- computed inside the kernel in fp32 and added to the patch row with one bf16 rounding.
+ * bwd: dpatch = dout[:, 1:], dcls += sum_b dout[:, 0], dpos [n_pos, C] += the transposed stencil applied to sum_b dout[:, 1:] (fp32,
+ * accumulated into caller-zeroed buffers; a gather without atomics: bitwise reproducible). */
 CVB_API int cvb_vit_tokens_interp_fwd(const void* patch, const float* pos, int n_pos, const float* cls, void* out, int B, int N, int C,
                                       cvb_stream_t stream);
 CVB_API int cvb_vit_tokens_interp_bwd(const void* dout, void* dpatch, float* dpos, int n_pos, float* dcls, int B, int N, int C, cvb_stream_t stream);

@@ -13,7 +13,7 @@ from ctypes import POINTER, Structure, c_char_p, c_double, c_float, c_int, c_int
 _HERE = os.path.dirname(os.path.abspath(__file__))
 # CVB_LIB: diagnostics only (A/B of two kernel builds on the same GPU box, tools/build_variant.sh); the product loads the in-tree library
 LIB_PATH = os.environ.get("CVB_LIB") or os.path.join(_HERE, "csrc", "libcvnets_b200.so")
-ABI_VERSION = 10
+ABI_VERSION = 11
 
 # load modes / epilogue modes (mirror include/cvnets_b200.h)
 A_RAW, A_AFF, A_AFF_SILU, A_SILU, A_GN, A_BNB = 0, 1, 2, 3, 4, 5
@@ -150,8 +150,6 @@ _SIGS = {
     "cvb_patch_permute": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "cvb_concat2": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int64, c_void_p, c_void_p]),
     "cvb_split2": (c_int, [c_void_p, c_int, c_int, c_int64, c_void_p, c_void_p, c_void_p]),
-    "cvb_vit_tokens_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
-    "cvb_vit_tokens_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "cvb_vit_tokens_interp_fwd": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "cvb_vit_tokens_interp_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_void_p]),
     "cvb_cast_f64_f32": (c_int, [c_void_p, c_int, c_int, c_void_p]),

@@ -19,7 +19,7 @@ FLAGS = ARCH + ["-O3", "-lineinfo", "-std=c++17", "--use_fast_math",
 
 def _digest():
     h = hashlib.sha256()
-    for fn in sorted(SOURCES + ["common.cuh", "../../include/cvnets_b200.h", "build.py"]):
+    for fn in sorted(SOURCES + ["common.cuh", "mha_wgmma.cuh", "../../include/cvnets_b200.h", "build.py"]):
         with open(os.path.join(HERE, fn), "rb") as f:
             h.update(f.read())
     return h.hexdigest()

@@ -93,32 +93,7 @@ __global__ void __launch_bounds__(CNT) col2im_nhwc_kernel(const bf16* __restrict
   }
 }
 
-// ViT token assembly (vit.py:476-507): out[b, 0] = cls;  out[b, 1 + n] = patch[b, n] + pos[n]   (no positional term on the cls token)
-__global__ void __launch_bounds__(CNT) vit_tokens_fwd_kernel(const bf16* __restrict__ patch, const float* __restrict__ pos, const float* __restrict__ cls,
-                                                             bf16* __restrict__ out, int B, int N, int C, int has_cls) {
-  pdl_wait();
-  pdl_trigger();
-  const int cg = C >> 3, S = N + has_cls;
-  const int64_t total = (int64_t)B * S * cg;
-  for (int64_t idx = (int64_t)blockIdx.x * CNT + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * CNT) {
-    const int c8 = (int)(idx % cg);
-    const int64_t tok = idx / cg;
-    const int t = (int)(tok % S);
-    const int64_t b = tok / S;
-    float f[8];
-    if (has_cls && t == 0) {
-#pragma unroll
-      for (int q = 0; q < 8; ++q) f[q] = cls[c8 * 8 + q];
-    } else {
-      const int n = t - has_cls;
-      unpack8(ldg16(patch + (b * N + n) * C + c8 * 8), f);
-#pragma unroll
-      for (int q = 0; q < 8; ++q) f[q] += pos[(int64_t)n * C + c8 * 8 + q];
-    }
-    stg16(out + tok * C + c8 * 8, pack8(f));
-  }
-}
-
+// ViT token assembly (vit.py:476-507), backward without the positional stencil:
 // dpatch[b, n] = dout[b, 1 + n];  dpos[n] += sum_b dout[b, 1 + n];  dcls += sum_b dout[b, 0].  One thread per (token position, 8 channels).
 __global__ void __launch_bounds__(CNT) vit_tokens_bwd_kernel(const bf16* __restrict__ dout, bf16* __restrict__ dpatch, float* __restrict__ dpos,
                                                              float* __restrict__ dcls, int B, int N, int C, int has_cls) {
@@ -157,7 +132,9 @@ __device__ __forceinline__ void interp_src(int s, float scale, int n_pos, int& i
   lam = __fsub_rn(src, (float)i0);
 }
 
-// out[b, 0] = cls;  out[b, 1 + s] = patch[b, s] + (1 - lambda_s) pos[i0_s] + lambda_s pos[i1_s], in fp32, rounded once to bf16
+// ViT token assembly (vit.py:476-507, no positional term on the cls token):
+// out[b, 0] = cls;  out[b, 1 + s] = patch[b, s] + (1 - lambda_s) pos[i0_s] + lambda_s pos[i1_s], in fp32, rounded once to bf16.
+// At N == n_pos (224 px) the stencil is the identity (scale 1, i0_s = s, lambda_s = 0): out = patch + pos.
 __global__ void __launch_bounds__(CNT) vit_tokens_interp_fwd_kernel(const bf16* __restrict__ patch, const float* __restrict__ pos, int n_pos, float scale,
                                                                     const float* __restrict__ cls, bf16* __restrict__ out, int B, int N, int C, int has_cls) {
   pdl_wait();
@@ -308,24 +285,6 @@ extern "C" int cvb_col2im(const void* dA, int lda, int B, int Cin, int H, int W,
   return 0;
 }
 
-extern "C" int cvb_vit_tokens_fwd(const void* patch, const float* pos, const float* cls, void* out, int B, int N, int C, cvb_stream_t stream) {
-  CVB_CHECK(patch && pos && out && B > 0 && N > 0 && C > 0 && C % 8 == 0 && cvb_aligned16(patch) && cvb_aligned16(out), "cvb_vit_tokens_fwd: bad arguments");
-  const int has_cls = cls != nullptr;
-  CVB_CUDA(cvb_launch(vit_tokens_fwd_kernel, cgrid((int64_t)B * (N + has_cls) * (C / 8)), CNT, 0, static_cast<cudaStream_t>(stream),
-                      static_cast<const bf16*>(patch), pos, cls, static_cast<bf16*>(out), B, N, C, has_cls));
-  CVB_LAUNCH_CHECK();
-  return 0;
-}
-
-extern "C" int cvb_vit_tokens_bwd(const void* dout, void* dpatch, float* dpos, float* dcls, int B, int N, int C, cvb_stream_t stream) {
-  CVB_CHECK(dout && dpatch && dpos && B > 0 && N > 0 && C > 0 && C % 8 == 0 && cvb_aligned16(dout) && cvb_aligned16(dpatch), "cvb_vit_tokens_bwd: bad arguments");
-  const int has_cls = dcls != nullptr;
-  CVB_CUDA(cvb_launch(vit_tokens_bwd_kernel, cgrid((int64_t)(N + has_cls) * (C / 8)), CNT, 0, static_cast<cudaStream_t>(stream),
-                      static_cast<const bf16*>(dout), static_cast<bf16*>(dpatch), dpos, dcls, B, N, C, has_cls));
-  CVB_LAUNCH_CHECK();
-  return 0;
-}
-
 extern "C" int cvb_patch_permute(const void* X, void* OUT, int B, int H, int W, int C, int patch_h, int patch_w, int inverse, cvb_stream_t stream) {
   CVB_CHECK(X && OUT && B > 0 && H > 0 && W > 0 && C > 0 && C % 8 == 0 && patch_h > 0 && patch_w > 0 && H % patch_h == 0 && W % patch_w == 0,
             "cvb_patch_permute: bad arguments (C %% 8 == 0, H, W multiples of the patch)");
@@ -370,7 +329,7 @@ extern "C" int cvb_vit_tokens_interp_bwd(const void* dout, void* dpatch, float* 
             "cvb_vit_tokens_interp_bwd: bad arguments");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int has_cls = dcls != nullptr;
-  // batch sum per output token into a zeroed fp32 [N, C] scratch (the non-interpolating kernel, dpos = scratch), then the transposed stencil
+  // batch sum per output token into a zeroed fp32 [N, C] scratch (vit_tokens_bwd_kernel, dpos = scratch), then the transposed stencil
   double* ws = nullptr;
   if (cvb_det_alloc(&ws, ((size_t)N * C + 1) / 2, st)) return 2;
   float* g = reinterpret_cast<float*>(ws);

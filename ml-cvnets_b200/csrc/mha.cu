@@ -411,31 +411,48 @@ int check_common(const char* who, const void* QKV, int ldq, int B, int S, int H,
   return 0;
 }
 
+// Which kernels serve a head.  Forward and backward ask the same question, so they always agree (the backward reads the forward's LSE).
+//   head_dim != 64                          mma.sync (this file; S <= 256, enforced by check_common)
+//   head_dim 64, S > 256                    streaming wgmma (mha_long.cu), with or without masks
+//   head_dim 64, S <= 256, additive mask    mma.sync: it reads the [S, S] mask in coalesced tiles, where the wgmma score fragments would
+//                                           gather single values (the causal CLIP text tower, S = 77)
+//   head_dim 64, S <= 256, otherwise        register-resident wgmma (mha_tc.cu)
+// g_mode (cvb_set_mha_impl, cross-checks only) overrides the choice where another family can run the shape.
+enum class MhaPath { Mma, Tc, Long };
+int g_mode = 0;  // 0 automatic, 1 mma.sync wherever it runs, 2 streaming for every head_dim-64 shape
+
+MhaPath route(int S, int head_dim, bool additive_mask) {
+  if (head_dim != 64) return MhaPath::Mma;
+  if (S > 256 || g_mode == 2) return MhaPath::Long;
+  if (additive_mask || g_mode == 1) return MhaPath::Mma;
+  return MhaPath::Tc;
+}
+
 }  // namespace
 
-// head_dim == 64: streaming wgmma kernels for S > 256 (mha_long.cu), register-resident wgmma kernels (mha_tc.cu); -1 = not handled there
-int cvb_mha_fwd_long(const void* QKV, int ldq, int B, int S, int H, int head_dim, float scale, const float* amask, const unsigned char* kpm, void* O,
-                     int ldo, float* LSE, cudaStream_t st);
-int cvb_mha_bwd_long(const void* QKV, int ldq, const void* O, const void* DO, int ldo, const float* LSE, int B, int S, int H, int head_dim, float scale,
+// head_dim 64 launchers: register-resident wgmma (mha_tc.cu: S <= 256, key-padding mask only) and streaming wgmma (mha_long.cu: any S)
+int cvb_mha_fwd_tc(const void* QKV, int ldq, int B, int S, int H, float scale, const unsigned char* kpm, void* O, int ldo, float* LSE, cudaStream_t st);
+int cvb_mha_bwd_tc(const void* QKV, int ldq, const void* O, const void* DO, int ldo, const float* LSE, int B, int S, int H, float scale,
+                   const unsigned char* kpm, void* DQKV, int lddq, cudaStream_t st);
+int cvb_mha_fwd_long(const void* QKV, int ldq, int B, int S, int H, float scale, const float* amask, const unsigned char* kpm, void* O, int ldo,
+                     float* LSE, cudaStream_t st);
+int cvb_mha_bwd_long(const void* QKV, int ldq, const void* O, const void* DO, int ldo, const float* LSE, int B, int S, int H, float scale,
                      const float* amask, const unsigned char* kpm, void* DQKV, int lddq, cudaStream_t st);
-int cvb_mha_fwd_tc(const void* QKV, int ldq, int B, int S, int H, int head_dim, float scale, const float* amask, const unsigned char* kpm, void* O,
-                   int ldo, float* LSE, cudaStream_t st);
-int cvb_mha_bwd_tc(const void* QKV, int ldq, const void* O, const void* DO, int ldo, const float* LSE, int B, int S, int H, int head_dim, float scale,
-                   const float* amask, const unsigned char* kpm, void* DQKV, int lddq, cudaStream_t st);
+
+extern "C" int cvb_set_mha_impl(int mode) {
+  const int old = g_mode;
+  g_mode = (mode == 1 || mode == 2) ? mode : 0;
+  return old;
+}
 
 extern "C" int cvb_mha_fwd(const void* QKV, int ldq, int B, int S, int H, int head_dim, float scale, const float* attn_mask,
                            const unsigned char* key_padding_mask, void* O, int ldo, float* LSE, cvb_stream_t stream) {
   if (check_common("cvb_mha_fwd", QKV, ldq, B, S, H, head_dim, ldo)) return 1;
   CVB_CHECK(O && LSE && cvb_aligned16(O), "cvb_mha_fwd: null / misaligned output");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  {
-    const int rc = cvb_mha_fwd_long(QKV, ldq, B, S, H, head_dim, scale, attn_mask, key_padding_mask, O, ldo, LSE, st);
-    if (rc >= 0) return rc;
-  }
-  {
-    const int rc = cvb_mha_fwd_tc(QKV, ldq, B, S, H, head_dim, scale, attn_mask, key_padding_mask, O, ldo, LSE, st);
-    if (rc >= 0) return rc;
-  }
+  const MhaPath path = route(S, head_dim, attn_mask != nullptr);
+  if (path == MhaPath::Long) return cvb_mha_fwd_long(QKV, ldq, B, S, H, scale, attn_mask, key_padding_mask, O, ldo, LSE, st);
+  if (path == MhaPath::Tc) return cvb_mha_fwd_tc(QKV, ldq, B, S, H, scale, key_padding_mask, O, ldo, LSE, st);
   if (head_dim <= 16) return launch_fwd<16>(QKV, ldq, B, S, H, scale, attn_mask, key_padding_mask, O, ldo, LSE, st, head_dim);
   if (head_dim <= 32) return launch_fwd<32>(QKV, ldq, B, S, H, scale, attn_mask, key_padding_mask, O, ldo, LSE, st, head_dim);
   return launch_fwd<64>(QKV, ldq, B, S, H, scale, attn_mask, key_padding_mask, O, ldo, LSE, st, head_dim);
@@ -447,14 +464,9 @@ extern "C" int cvb_mha_bwd(const void* QKV, int ldq, const void* O, const void* 
   CVB_CHECK(O && DO && LSE && DQKV && cvb_aligned16(O) && cvb_aligned16(DO) && cvb_aligned16(DQKV) && lddq % 8 == 0 && lddq >= 3 * H * head_dim,
             "cvb_mha_bwd: null / misaligned operand");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  {
-    const int rc = cvb_mha_bwd_long(QKV, ldq, O, DO, ldo, LSE, B, S, H, head_dim, scale, attn_mask, key_padding_mask, DQKV, lddq, st);
-    if (rc >= 0) return rc;
-  }
-  {
-    const int rc = cvb_mha_bwd_tc(QKV, ldq, O, DO, ldo, LSE, B, S, H, head_dim, scale, attn_mask, key_padding_mask, DQKV, lddq, st);
-    if (rc >= 0) return rc;
-  }
+  const MhaPath path = route(S, head_dim, attn_mask != nullptr);
+  if (path == MhaPath::Long) return cvb_mha_bwd_long(QKV, ldq, O, DO, ldo, LSE, B, S, H, scale, attn_mask, key_padding_mask, DQKV, lddq, st);
+  if (path == MhaPath::Tc) return cvb_mha_bwd_tc(QKV, ldq, O, DO, ldo, LSE, B, S, H, scale, key_padding_mask, DQKV, lddq, st);
   if (head_dim <= 16) return launch_bwd<16>(QKV, ldq, O, DO, ldo, LSE, B, S, H, scale, attn_mask, key_padding_mask, DQKV, lddq, st, head_dim);
   if (head_dim <= 32) return launch_bwd<32>(QKV, ldq, O, DO, ldo, LSE, B, S, H, scale, attn_mask, key_padding_mask, DQKV, lddq, st, head_dim);
   return launch_bwd<64>(QKV, ldq, O, DO, ldo, LSE, B, S, H, scale, attn_mask, key_padding_mask, DQKV, lddq, st, head_dim);

@@ -2,11 +2,12 @@
 //
 // mha_tc.cu keeps a whole head in shared memory and whole score rows in registers, which caps S at 256.  Here K / V (forward) and
 // Q / dO (backward) stream through a 3-stage shared-memory ring in 64-row tiles, so nothing on chip grows with S (ViT / CLIP at the
-// multi-scale recipes' 256-320 px crops: S = 257 .. 401; 384 px fine-tuning: S = 577; 512 px: S = 1025).
+// multi-scale recipes' 256-320 px crops: S = 257 .. 401; 384 px fine-tuning: S = 577; 512 px: S = 1025).  The router in mha.cu sends
+// every head_dim-64 head with S > 256 here, with or without masks; test mode 2 of cvb_set_mha_impl sends the shorter ones too.
 //
-// Operand images are the ones mha_tc.cu uses: one [64 rows x 64 ch] SWIZZLE_128B TMA box per tile, read as the K-major operand
-// (rows = M / N) or as the MN-major operand (rows = K) of a wgmma; P and dS go from the accumulator registers straight into the A operand
-// of the next wgmma.  Warp 8 of every CTA is the TMA producer (full / empty mbarrier pair per stage); warps 0-7 are two consumer
+// Operand images are the ones mha_tc.cu uses, from the same helpers (mha_wgmma.cuh): one [64 rows x 64 ch] SWIZZLE_128B TMA box per
+// tile, read as the K-major operand (rows = M / N) or as the MN-major operand (rows = K) of a wgmma; P and dS go from the accumulator
+// registers straight into the A operand of the next wgmma.  Warp 8 of every CTA is the TMA producer (full / empty mbarrier pair per stage); warps 0-7 are two consumer
 // warpgroups of 64 rows each.
 //
 // Forward, one CTA per (sample, head, 128 queries): online softmax in the exp2 domain (running row max and sum, O rescaled per key tile).
@@ -17,50 +18,13 @@
 //   mha_long_dkv_kernel   one CTA per (sample, head, 128 keys): streams Q / dO tiles, P^T and dS^T from LSE and D, dV += P^T dO, dK += dS^T Q
 //   mha_long_dq_kernel    one CTA per (sample, head, 128 queries): streams K / V tiles, recomputes P and dS, dQ += dS K
 // The price of determinism is the recompute of Q K^T and dO V^T in the dQ kernel: 7 instead of 5 m64n64 products per (64 x 64) block.
-#include "common.cuh"
-
-#include <math_constants.h>
-
-int cvb_mha_impl();
+#include "mha_wgmma.cuh"
 
 namespace {
 
-constexpr float LOG2E = 1.4426950408889634f;
-constexpr int BOX64 = 64 * 128;  // bytes of a [64 rows x 64 ch] image
 constexpr int NST = 3;           // ring stages
 constexpr int THREADS = 288;     // two consumer warpgroups + one producer warp
 constexpr int PRODUCER = 256;    // first thread of the producer warp
-
-__device__ __forceinline__ uint64_t desc_k(uint32_t saddr) { return wgmma_desc(saddr, 16, 1024, WG_SW128); }
-__device__ __forceinline__ uint64_t desc_mn(uint32_t saddr) { return wgmma_desc(saddr, BOX64, 1024, WG_SW128); }
-__device__ __forceinline__ float ex2(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-// additive mask term (exp2 domain) of score (q, t), t < S; -inf for padded keys (mha_tc.cu mask_add)
-__device__ __forceinline__ float mask_add(const float* amask, const uint8_t* kpm, int b, int S, int q, int t) {
-  if (kpm && kpm[(size_t)b * S + t]) return -CUDART_INF_F;
-  if (amask && q < S) return amask[((size_t)b * S + q) * S + t] * LOG2E;
-  return 0.f;
-}
-__device__ __forceinline__ void to_a_frag(const float* acc, int kk, uint32_t* a) {
-#pragma unroll
-  for (int i = 0; i < 4; ++i) a[i] = pack_bf162(acc[8 * kk + 2 * i], acc[8 * kk + 2 * i + 1]);
-}
-// m64n64 fp32 accumulator * mul -> bf16 rows row0 + r (row0 + r < S) of a [.. x 64] global matrix with leading dimension ld
-__device__ __forceinline__ void store_acc(bf16* dst, int ld, const float* acc, float mul, int row0, int S) {
-  const int lane = threadIdx.x & 31, r = ((threadIdx.x & 127) >> 5) * 16 + (lane >> 2);
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const int row = row0 + r + 8 * h;
-    if (row < S) {
-#pragma unroll
-      for (int j = 0; j < 8; ++j)
-        *reinterpret_cast<uint32_t*>(dst + (size_t)row * ld + 8 * j + 2 * (lane & 3)) = pack_bf162(acc[4 * j + 2 * h] * mul, acc[4 * j + 2 * h + 1] * mul);
-    }
-  }
-}
 
 // Shared layout of every kernel: two own [128 rows] operand images (Q, or K | V, or Q | dO: 4 boxes), then NST stages of two streamed boxes.
 struct Smem {
@@ -402,8 +366,6 @@ __global__ void __launch_bounds__(THREADS, 1)
   store_acc(DQKV + (size_t)b * S * lddq + h * 64, lddq, dq, scale, q0, S);
 }
 
-bool use_long(int S, int head_dim) { return head_dim == 64 && (S > 256 || (cvb_mha_impl() & 8)); }
-
 int set_smem(const void* fn) {
   CVB_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
   return 0;
@@ -411,11 +373,8 @@ int set_smem(const void* fn) {
 
 }  // namespace
 
-// Return -1 when the shape is left to the shared-memory-resident kernels (head_dim != 64, or S <= 256 without bit 3 of cvb_set_mha_impl),
-// 0 on success, > 0 on error.
-int cvb_mha_fwd_long(const void* QKV, int ldq, int B, int S, int H, int head_dim, float scale, const float* amask, const unsigned char* kpm, void* O,
-                     int ldo, float* LSE, cudaStream_t st) {
-  if (!use_long(S, head_dim)) return -1;
+int cvb_mha_fwd_long(const void* QKV, int ldq, int B, int S, int H, float scale, const float* amask, const unsigned char* kpm, void* O, int ldo,
+                     float* LSE, cudaStream_t st) {
   const int NQT = (S + 127) / 128;
   CUtensorMap tm;
   if (cvb_make_tmap_2d_c64(&tm, QKV, (int64_t)B * S, 3 * H * 64, ldq, 64)) return 1;
@@ -426,9 +385,8 @@ int cvb_mha_fwd_long(const void* QKV, int ldq, int B, int S, int H, int head_dim
   return 0;
 }
 
-int cvb_mha_bwd_long(const void* QKV, int ldq, const void* O, const void* DO, int ldo, const float* LSE, int B, int S, int H, int head_dim, float scale,
+int cvb_mha_bwd_long(const void* QKV, int ldq, const void* O, const void* DO, int ldo, const float* LSE, int B, int S, int H, float scale,
                      const float* amask, const unsigned char* kpm, void* DQKV, int lddq, cudaStream_t st) {
-  if (!use_long(S, head_dim)) return -1;
   const int NT = (S + 127) / 128;
   CUtensorMap tmQKV, tmDO;
   if (cvb_make_tmap_2d_c64(&tmQKV, QKV, (int64_t)B * S, 3 * H * 64, ldq, 64)) return 1;

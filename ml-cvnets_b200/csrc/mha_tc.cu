@@ -1,5 +1,6 @@
-// wgmma / TMA multi-head attention core for head_dim == 64, S <= 256 (ViT-B 197 x 64, CLIP text 77 x 64), sm_90a.
+// wgmma / TMA multi-head attention core for head_dim == 64, S <= 256 (ViT-B 197 x 64), sm_90a.
 // Same contract as mha.cu (cvnets/layers/multi_head_attention.py:187-237): packed projection in, O / LSE out, dQKV in the backward.
+// Key-padding masks only: the router in mha.cu sends heads with an additive mask to the mma.sync kernels.
 //
 // Every operand of a head -- Q, K, V, dO [rows x 64 bf16] -- is ONE TMA box [64 cols x rows] with 128-byte swizzle.  That shared-memory
 // image (128-byte rows, 8-row swizzle atoms of 1 KB) is at the same time
@@ -12,57 +13,20 @@
 // Backward, one CTA per (sample, head): the two warpgroups take alternate 64-key blocks; per (key block, 64-query block)
 //   S^T = K Q^T, dP^T = V dO^T (registers) -> P^T, dS^T -> dV += P^T dO, dK += dS^T Q (register A operands), dQ_q += dS K (dS^T staged
 //   in shared memory, fp32 dQ accumulated in shared memory across the key blocks of both warpgroups)
-#include "common.cuh"
-
-#include <math_constants.h>
-#include <cstdlib>
+#include "mha_wgmma.cuh"
 
 namespace {
 
-constexpr float LOG2E = 1.4426950408889634f;
-constexpr int BOX64 = 64 * 128;  // bytes of a [64 rows x 64 ch] image
-
-__device__ __forceinline__ uint64_t desc_k(uint32_t saddr) { return wgmma_desc(saddr, 16, 1024, WG_SW128); }      // K-major: +32 B per k-step
-__device__ __forceinline__ uint64_t desc_mn(uint32_t saddr) { return wgmma_desc(saddr, BOX64, 1024, WG_SW128); }  // MN-major: +2 KB per k-step
-__device__ __forceinline__ float ex2(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
 // byte offset of the 16-byte chunk `ch` (0..7) of row `row` inside a [rows x 64 ch] SWIZZLE_128B image
 __device__ __forceinline__ uint32_t sw128(int row, int ch) { return static_cast<uint32_t>(row * 128 + ((ch ^ (row & 7)) << 4)); }
-// additive mask term (exp2 domain) of score (q, t), t < S; -inf for padded keys
-__device__ __forceinline__ float mask_add(const float* amask, const uint8_t* kpm, int b, int S, int q, int t) {
-  if (kpm && kpm[(size_t)b * S + t]) return -CUDART_INF_F;
-  if (amask && q < S) return amask[((size_t)b * S + q) * S + t] * LOG2E;
-  return 0.f;
-}
 __device__ __forceinline__ void wg_bar(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); }
-// accumulator columns [16 kk, 16 kk + 16) of an m64n64 fp32 result, scaled, as the bf16 A operand of k-step kk
-__device__ __forceinline__ void to_a_frag(const float* acc, int kk, uint32_t* a) {
-#pragma unroll
-  for (int i = 0; i < 4; ++i) a[i] = pack_bf162(acc[8 * kk + 2 * i], acc[8 * kk + 2 * i + 1]);
-}
-// m64n64 fp32 accumulator * mul -> bf16 rows row0 + r (r < 64, row0 + r < S) of a [.. x 64] global matrix with leading dimension ld
-__device__ __forceinline__ void store_acc(bf16* dst, int ld, const float* acc, float mul, int row0, int S) {
-  const int lane = threadIdx.x & 31, r = ((threadIdx.x & 127) >> 5) * 16 + (lane >> 2);
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const int row = row0 + r + 8 * h;
-    if (row < S) {
-#pragma unroll
-      for (int j = 0; j < 8; ++j)
-        *reinterpret_cast<uint32_t*>(dst + (size_t)row * ld + 8 * j + 2 * (lane & 3)) = pack_bf162(acc[4 * j + 2 * h] * mul, acc[4 * j + 2 * h + 1] * mul);
-    }
-  }
-}
 
 // ------------------------------------------------------------------------------------------------------------- forward
 constexpr int FW_THREADS = 256;
 
 __global__ void __launch_bounds__(FW_THREADS, 1)
     mha_tc_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV, int S, int NCH, int H, int NQT, float scale,
-                      const float* __restrict__ amask, const uint8_t* __restrict__ kpm, bf16* __restrict__ O, int ldo, float* __restrict__ LSE) {
+                      const uint8_t* __restrict__ kpm, bf16* __restrict__ O, int ldo, float* __restrict__ LSE) {
   const int tid = threadIdx.x, lane = tid & 31, wg = tid >> 7;
   int bid = blockIdx.x;
   const int qt = bid % NQT;
@@ -98,7 +62,6 @@ __global__ void __launch_bounds__(FW_THREADS, 1)
   const int rl = ((tid & 127) >> 5) * 16 + (lane >> 2);  // query row (within the warpgroup's 64) of acc[4j + {0,1}]; + 8 for {2,3}
   const int q0 = qt * 128 + wg * 64;
   const float sc2 = scale * LOG2E;
-  const bool masked = (amask != nullptr) || (kpm != nullptr);
   const uint32_t aQ = smem_u32(sQ) + wg * BOX64, aK = smem_u32(sK), aV = smem_u32(sV);
 
   // ---- S = Q K^T, 64-key chunks
@@ -127,7 +90,7 @@ __global__ void __launch_bounds__(FW_THREADS, 1)
         float v = -CUDART_INF_F;
         if (t < S) {
           v = sacc[c][i] * sc2;
-          if (masked) v += mask_add(amask, kpm, b, S, q, t);
+          if (kpm) v += mask_add(nullptr, kpm, b, S, q, t);
         }
         sacc[c][i] = v;
         m[hh] = fmaxf(m[hh], v);
@@ -195,7 +158,7 @@ constexpr int BW_THREADS = 256;
 __global__ void __launch_bounds__(BW_THREADS, 1)
     mha_tc_bwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmDO, const bf16* __restrict__ O,
                       const bf16* __restrict__ DO, int ldo, const float* __restrict__ LSE, int S, int H, int NB, float scale,
-                      const float* __restrict__ amask, const uint8_t* __restrict__ kpm, bf16* __restrict__ DQKV, int lddq) {
+                      const uint8_t* __restrict__ kpm, bf16* __restrict__ DQKV, int lddq) {
   const int tid = threadIdx.x, lane = tid & 31, wg = tid >> 7;
   const int h = blockIdx.x % H, b = blockIdx.x / H;
   const int C = H * 64;
@@ -252,7 +215,6 @@ __global__ void __launch_bounds__(BW_THREADS, 1)
 
   const int rl = ((tid & 127) >> 5) * 16 + (lane >> 2);  // key row (within the block) of acc[4j + {0,1}]; + 8 for {2,3}
   const float sc2 = scale * LOG2E;
-  const bool masked = (amask != nullptr) || (kpm != nullptr);
   const uint32_t aQ = smem_u32(sQ), aK = smem_u32(sK), aV = smem_u32(sV), aDO = smem_u32(sdO), aDS = smem_u32(sdST) + wg * BOX64;
   uint8_t* my_dST = sdST + wg * BOX64;
   bf16* dbase = DQKV + (size_t)b * S * lddq + h * 64;
@@ -277,7 +239,7 @@ __global__ void __launch_bounds__(BW_THREADS, 1)
         float pv = 0.f, dv2 = 0.f;
         if (q < S && t < S) {
           float v = fmaf(st[i], sc2, -sLSE[q]);
-          if (masked) v += mask_add(amask, kpm, b, S, q, t);
+          if (kpm) v += mask_add(nullptr, kpm, b, S, q, t);
           pv = ex2(v);
           dv2 = pv * (dpt[i] - sD[q]);
           if (pv == 0.f) dv2 = 0.f;  // masked keys: exactly zero whatever dP holds
@@ -331,32 +293,9 @@ __global__ void __launch_bounds__(BW_THREADS, 1)
   }
 }
 
-// bit 0: wgmma forward, bit 1: wgmma backward, bit 2: also for heads with an ADDITIVE mask.  Default 3: additive masks (the causal mask of
-// the CLIP text tower, S = 77) stay on the mma.sync kernels, which read the [S, S] mask in coalesced tiles; here every thread gathers
-// single mask values of its score fragment.  bit 3: the streaming kernels of mha_long.cu also for S <= 256 (cross-checks only).
-int g_impl = -1;
-int impl() {
-  if (g_impl < 0) {
-    const char* e = getenv("CVB_MHA_TC");
-    g_impl = e ? atoi(e) : 3;
-  }
-  return g_impl;
-}
-
 }  // namespace
 
-int cvb_mha_impl() { return impl(); }
-
-extern "C" int cvb_set_mha_impl(int mask) {
-  const int old = impl();
-  g_impl = mask & 15;
-  return old;
-}
-
-// Return -1 when the shape is left to the mma.sync kernels (head_dim != 64), 0 on success, > 0 on error.
-int cvb_mha_fwd_tc(const void* QKV, int ldq, int B, int S, int H, int head_dim, float scale, const float* amask, const unsigned char* kpm, void* O,
-                   int ldo, float* LSE, cudaStream_t st) {
-  if (head_dim != 64 || !(impl() & 1) || S > 256 || (amask && !(impl() & 4))) return -1;
+int cvb_mha_fwd_tc(const void* QKV, int ldq, int B, int S, int H, float scale, const unsigned char* kpm, void* O, int ldo, float* LSE, cudaStream_t st) {
   const int NCH = (S + 63) / 64;
   const int NQT = (S + 127) / 128;
   CUtensorMap tmQ, tmKV;
@@ -365,14 +304,13 @@ int cvb_mha_fwd_tc(const void* QKV, int ldq, int B, int S, int H, int head_dim, 
   const size_t smem = (size_t)2 * BOX64 + (size_t)2 * NCH * BOX64 + 1024;
   static bool attr = false;
   if (!attr) { CVB_CUDA(cudaFuncSetAttribute(mha_tc_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024)); attr = true; }
-  CVB_CUDA(cvb_launch(mha_tc_fwd_kernel, B * H * NQT, FW_THREADS, smem, st, tmQ, tmKV, S, NCH, H, NQT, scale, amask, kpm, static_cast<bf16*>(O), ldo, LSE));
+  CVB_CUDA(cvb_launch(mha_tc_fwd_kernel, B * H * NQT, FW_THREADS, smem, st, tmQ, tmKV, S, NCH, H, NQT, scale, kpm, static_cast<bf16*>(O), ldo, LSE));
   CVB_LAUNCH_CHECK();
   return 0;
 }
 
-int cvb_mha_bwd_tc(const void* QKV, int ldq, const void* O, const void* DO, int ldo, const float* LSE, int B, int S, int H, int head_dim, float scale,
-                   const float* amask, const unsigned char* kpm, void* DQKV, int lddq, cudaStream_t st) {
-  if (head_dim != 64 || !(impl() & 2) || S > 256 || (amask && !(impl() & 4))) return -1;
+int cvb_mha_bwd_tc(const void* QKV, int ldq, const void* O, const void* DO, int ldo, const float* LSE, int B, int S, int H, float scale,
+                   const unsigned char* kpm, void* DQKV, int lddq, cudaStream_t st) {
   const int NB = (S + 63) / 64;
   const int R = NB * 64;
   CUtensorMap tmQKV, tmDO;
@@ -383,7 +321,7 @@ int cvb_mha_bwd_tc(const void* QKV, int ldq, const void* O, const void* DO, int 
   static bool attr = false;
   if (!attr) { CVB_CUDA(cudaFuncSetAttribute(mha_tc_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024)); attr = true; }
   CVB_CUDA(cvb_launch(mha_tc_bwd_kernel, B * H, BW_THREADS, smem, st, tmQKV, tmDO, static_cast<const bf16*>(O), static_cast<const bf16*>(DO), ldo, LSE, S,
-                      H, NB, scale, amask, kpm, static_cast<bf16*>(DQKV), lddq));
+                      H, NB, scale, kpm, static_cast<bf16*>(DQKV), lddq));
   CVB_LAUNCH_CHECK();
   return 0;
 }

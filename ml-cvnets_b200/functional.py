@@ -962,18 +962,15 @@ class Concat2Fn(torch.autograd.Function):
 class VitTokensFn(torch.autograd.Function):
     """ViT token assembly (cvnets/models/classification/vit.py:476-507): tokens = cat(cls, patch_embedding + positional_embedding).
     patch: [B, C, nh, nw] channels-last (== token-major [B*N, C]); pos: [1, 1, n_pos, C]; cls: [1, 1, C] or None.  Returns [B, N(+1), C].
-    When the patch count N differs from n_pos (inputs other than 224 x 224), the table is linearly resampled to N rows inside the kernel,
-    as the reference's F.interpolate does (cvnets/layers/positional_embedding.py:90-95)."""
+    The table is linearly resampled to the patch count N inside the kernel, as the reference's F.interpolate does
+    (cvnets/layers/positional_embedding.py:90-95); at N == n_pos (224 x 224 inputs) the resample is the identity."""
 
     @staticmethod
     def forward(ctx, patch, cfg, pos, cls):
         B, C, nh, nw = patch.shape
         N, n_pos = nh * nw, pos.shape[-2]
         p2 = as_2d(to_bf16_cl(patch))
-        if N == n_pos:
-            out = ops.vit_tokens_fwd(p2, pos, cls, B, N, C)
-        else:
-            out = ops.vit_tokens_interp_fwd(p2, pos, cls, B, N, C)
+        out = ops.vit_tokens_interp_fwd(p2, pos, cls, B, N, C)
         ctx.cfg, ctx.dims, ctx.plist, ctx.has_cls = cfg, (B, C, nh, nw, n_pos), cfg.plist, cls is not None
         return out
 
@@ -985,10 +982,7 @@ class VitTokensFn(torch.autograd.Function):
         D = _Dst(ctx.cfg, ctx.plist, g.device, n_pos * C + C + 64, 8, True)
         dpos = D.mat(0, n_pos, C)
         dcls = D.mat(1, 1, C).view(C) if ctx.has_cls else None
-        if N == n_pos:
-            dpatch = ops.vit_tokens_bwd(g, dpos, dcls, B, N, C)
-        else:
-            dpatch = ops.vit_tokens_interp_bwd(g, dpos, dcls, B, N, C)
+        dpatch = ops.vit_tokens_interp_bwd(g, dpos, dcls, B, N, C)
         grads = D.finish()
         return to_4d(dpatch, B, nh, nw), None, grads[0], grads[1] if ctx.has_cls else None
 

@@ -355,21 +355,6 @@ def split2(G: Tensor, C1: int, C2: int) -> Tuple[Tensor, Tensor]:
     return da, db
 
 
-def vit_tokens_fwd(patch: Tensor, pos: Tensor, cls: Optional[Tensor], B: int, N: int, C: int) -> Tensor:
-    S = N + (1 if cls is not None else 0)
-    out = torch.empty((B, S, C), device=patch.device, dtype=torch.bfloat16)
-    L.check(_lib().cvb_vit_tokens_fwd(patch.data_ptr(), pos.data_ptr(), _p(cls), out.data_ptr(), B, N, C, _stream()), "cvb_vit_tokens_fwd")
-    _count()
-    return out
-
-
-def vit_tokens_bwd(dout: Tensor, dpos: Tensor, dcls: Optional[Tensor], B: int, N: int, C: int) -> Tensor:
-    dpatch = torch.empty((B * N, C), device=dout.device, dtype=torch.bfloat16)
-    L.check(_lib().cvb_vit_tokens_bwd(dout.data_ptr(), dpatch.data_ptr(), dpos.data_ptr(), _p(dcls), B, N, C, _stream()), "cvb_vit_tokens_bwd")
-    _count()
-    return dpatch
-
-
 def vit_tokens_interp_fwd(patch: Tensor, pos: Tensor, cls: Optional[Tensor], B: int, N: int, C: int) -> Tensor:
     """Token assembly with the positional table ``pos`` ([.., n_pos, C] fp32) linearly resampled to N rows (F.interpolate, align_corners=False)."""
     S = N + (1 if cls is not None else 0)

@@ -605,28 +605,26 @@ def test_mha_fwd_bwd(ops, B, S, H, c, mask):
 
 
 @pytest.mark.parametrize("B,S,H", [(2, 197, 3), (2, 77, 2), (1, 250, 2)])
-@pytest.mark.parametrize("mask", ["none", "causal", "padding"])
+@pytest.mark.parametrize("mask", ["none", "padding"])
 def test_mha_tc_matches_mma(ops, B, S, H, mask):
-    """head_dim 64 has two implementations: wgmma (mha_tc.cu, the default) and mma.sync (mha.cu).  Same inputs -> same O / LSE / dQKV up to the
-    bf16 rounding of P (the tensor-core operand) and the accumulation order."""
+    """head_dim 64, S <= 256 without an additive mask has two implementations: wgmma (mha_tc.cu, the default) and mma.sync (mha.cu, test
+    mode 1).  Same inputs -> same O / LSE / dQKV up to the bf16 rounding of P (the tensor-core operand) and the accumulation order."""
     from ml_cvnets_b200 import _lib as L
     lib = L.load()
     C = H * 64
     qkv = bf(rnd(B * S, 3 * C, seed=73))
     dO = bf(rnd(B * S, C, seed=74))
-    amask = kpm = None
-    if mask == "causal":
-        amask = torch.full((S, S), float("-inf"), device="cuda").triu(1)[None].repeat(B, 1, 1).contiguous()
+    kpm = None
     if mask == "padding":
         kpm = torch.zeros(B, S, dtype=torch.uint8, device="cuda")
         kpm[:, S - max(1, S // 5):] = 1
     res = {}
     old = lib.cvb_set_mha_impl(0)
     try:
-        for name, m in (("mma", 0), ("tc", 7)):  # 7: wgmma forward + backward, also with an additive mask
+        for name, m in (("mma", 1), ("tc", 0)):
             lib.cvb_set_mha_impl(m)
-            O, LSE = ops.mha_fwd(qkv, B, S, H, 64, 0.125, attn_mask=amask, key_padding_mask=kpm)
-            D = ops.mha_bwd(qkv, O, dO, LSE, B, S, H, 64, 0.125, attn_mask=amask, key_padding_mask=kpm)
+            O, LSE = ops.mha_fwd(qkv, B, S, H, 64, 0.125, key_padding_mask=kpm)
+            D = ops.mha_bwd(qkv, O, dO, LSE, B, S, H, 64, 0.125, key_padding_mask=kpm)
             res[name] = (O.float(), LSE.clone(), D.float())
     finally:
         lib.cvb_set_mha_impl(old)
