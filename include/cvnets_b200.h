@@ -348,6 +348,21 @@ CVB_API int cvb_l2norm_fwd(const void* X, void* Y, float* inv_norm, int M, int C
 CVB_API int cvb_l2norm_bwd(const void* DY, const void* Y, const float* inv_norm, void* DX, int M, int C, cvb_stream_t stream);
 CVB_API int cvb_transpose_bf16(const void* X, void* Y, int R, int C, cvb_stream_t stream);
 CVB_API int cvb_add_bf16_f32(const void* A, const float* B, void* OUT, int64_t n, cvb_stream_t stream);
+/* ---------------------------------------------------------------------------------------------------------------
+ * CLIP zero-shot evaluation (cvnets/text_encoders/transformer.py:428-504, cvnets/models/multi_modal_img_text/clip.py:171-202,
+ * metrics/topk_accuracy.py; csrc/zeroshot.cu)
+ *   class embedding: X = bf16 [R, ldx] projected caption features BEFORE normalisation; perm[c*M + m] = the row of caption m of class c
+ *              (rows outside [0, R) are skipped).  table[k*Cl + c] = normalize(mean_m normalize(X[perm[c*M + m]])), all in fp32, with
+ *              F.normalize's x / max(||x||, 1e-12) and the captions added in order m = 0..M-1.  One writer per class, no atomics:
+ *              bitwise reproducible.  d % 8 == 0, d <= 1024.
+ *   logits / top-k: img = bf16 [B, ldi] L2-normalised image features, table fp32 [d, Cl]; logits fp32 [B, Cl] = scale * img @ table (or
+ *              NULL).  With targets (int64 [B]) and hits (int64 [2]) given, the rank of a row is the number of classes whose logit is
+ *              strictly greater than the target's; hits[0] += (rank < 1), hits[1] += (rank < 5).  A target outside [0, Cl) is a miss.
+ *              Integer adds only: the counts do not depend on the order of the CTAs.  No host sync.
+ * ------------------------------------------------------------------------------------------------------------- */
+CVB_API int cvb_zs_class_embed(const void* X, int ldx, int R, const int* perm, int Cl, int M, int d, float* table, cvb_stream_t stream);
+CVB_API int cvb_zs_logits_topk(const void* img, int ldi, const float* table, int B, int d, int Cl, float scale, const int64_t* targets,
+                               float* logits, int64_t* hits, cvb_stream_t stream);
 /* cudaMemsetAsync(ptr, 0, bytes): the step's ONE workspace clear (a memset node under graph capture, not a kernel) */
 CVB_API int cvb_memset_zero(void* ptr, int64_t bytes, cvb_stream_t stream);
 

@@ -143,6 +143,8 @@ _SIGS = {
     "cvb_l2norm_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "cvb_transpose_bf16": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "cvb_add_bf16_f32": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_void_p]),
+    "cvb_zs_class_embed": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "cvb_zs_logits_topk": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p, c_void_p]),
     "cvb_stem_im2col_mix": (c_int, [c_void_p, c_int64, c_int64, c_int64, c_int64, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "cvb_im2col": (c_int, [c_void_p, c_int, c_int64, c_int64, c_int64, c_int64, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int,
                            c_void_p]),

@@ -187,3 +187,32 @@ class MixingSampler:
         rw, rh = int(r * W), int(r * H)
         x1, y1, x2, y2 = max(r_x - rw, 0), max(r_y - rh, 0), min(r_x + rw, W), min(r_y + rh, H)
         return "cutmix", float(1.0 - (x2 - x1) * (y2 - y1) / (W * H)), (x1, y1, x2, y2)
+
+
+class ZeroShotAccuracy:
+    """Zero-shot top-1 / top-5 accuracy of a CLIP model over an evaluation set (the recipe's ``top1.zero_shot_image_logits``: clip.py:184-202,
+    metrics/topk_accuracy.py).  The class table is built once, from the prompts [B, Cl, M, L], when the metric is created; the model must
+    be in eval mode.  ``update`` scores one image batch and counts its hits on the device (no host sync); ``compute`` syncs once and
+    returns percentages.
+
+        acc = ZeroShotAccuracy(model.eval(), prompts)
+        for images, labels in loader:
+            acc.update(images, labels)
+        acc.compute()                         # {"top1": ..., "top5": ...}
+    """
+
+    def __init__(self, model: torch.nn.Module, class_tokens: torch.Tensor):
+        self.model = model
+        self.table = model.zero_shot_table(class_tokens)
+        self.hits = torch.zeros(2, device=self.table.device, dtype=torch.int64)
+        self.count = 0
+
+    def update(self, images: torch.Tensor, targets: torch.Tensor) -> None:
+        targets = targets.to(device=self.table.device, dtype=torch.int64).contiguous()
+        self.model.zero_shot_logits(images, self.table, targets=targets, hits=self.hits)
+        self.count += int(targets.shape[0])
+
+    def compute(self) -> dict:
+        top1, top5 = self.hits.tolist()
+        n = max(self.count, 1)
+        return {"top1": 100.0 * top1 / n, "top5": 100.0 * top5 / n}

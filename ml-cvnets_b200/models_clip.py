@@ -5,9 +5,15 @@ simple_projection_head.py and loss_fn/multi_modal_img_text/contrastive_loss_clip
     img, txt, logit_scale = model(images, text_tokens)   # L2-normalised features
     loss = clip_contrastive_loss(img, txt, logit_scale)  # all-gather over the process group when distributed
 
+    model.eval()                                         # zero-shot classification (transformer.py:428-504, clip.py:171-202)
+    table = model.zero_shot_table(prompts)               # prompts [1, classes, captions, L] -> fp32 [d, classes]
+    logits = model.zero_shot_logits(images, table)       # 100 * img @ table, fp32 [B, classes]
+    acc = ZeroShotAccuracy(model, prompts)               # engine.py: top-1 / top-5 over an evaluation set, counted on the device
+
 Same attribute names / ``state_dict`` keys as the reference (image_encoder.*, text_encoder.{embedding_layer, positional_embedding,
-transformer.{i}, final_layer_norm, projection_layer}, logit_scale).  Host code only; every kernel is the library's.  Not implemented:
-zero-shot evaluation paths, key_padding_mask with causal masking off, sinusoidal embeddings, dropout > 0 in training.
+transformer.{i}, final_layer_norm, projection_layer}, logit_scale).  Host code only; every kernel is the library's.  3-D and 4-D text
+batches are encoded at each caption's causal prefix (TextTransformer._encode_rows).  Not implemented: key_padding_mask with causal masking
+off (beyond full-length encoding), sinusoidal embeddings, dropout > 0 in training.
 """
 from __future__ import annotations
 
@@ -20,6 +26,7 @@ import torch
 from torch import Tensor, nn
 
 from . import functional as Fn
+from . import ops
 from .layers import Dropout, get_normalization_layer
 from .models_vit import PositionalEmbedding, VisionTransformer, default_vit_opts
 from .modules import TransformerEncoder, _require_cuda
@@ -98,6 +105,8 @@ class TextTransformer(nn.Module):
         self.projection_layer = nn.Parameter(torch.empty(d, projection_dim))
         self.model_dim = d
         self.causal_masking = getattr(opts, "model.text.transformer.causal_masking", False)
+        self.classes_per_split_zero_shot = max(1, int(getattr(opts, "model.text.transformer.classes_per_split_zero_shot", 1)))
+        self.zero_shot_token_budget = 1 << 18  # tokens per tower call when encoding 3-D / 4-D batches: bounds their activation memory
         self.reset_parameters_clip_style()
         self._emb = SimpleNamespace()
         self._proj = _Projection()
@@ -124,17 +133,36 @@ class TextTransformer(nn.Module):
         return self._mask
 
     def forward(self, text_tokens: Tensor, key_padding_mask: Optional[Tensor] = None, *args, **kwargs) -> Tensor:
+        """transformer.py:506-551: [B, L] -> [B, d] features; [B, N, L] (several captions per image) -> [B, N, d]; [B, Cl, M, L] (zero-shot
+        prompts: M captions per class, eval mode only) -> the fp32 [d, Cl] class table of ``forward_zero_shot``."""
         _require_cuda(text_tokens, "TextTransformer")
+        if text_tokens.dim() == 4:
+            return self.forward_zero_shot(text_tokens, key_padding_mask)
+        if text_tokens.dim() == 3:
+            b, n, L = text_tokens.shape
+            kpm = key_padding_mask.reshape(b * n, L) if key_padding_mask is not None else None
+            if torch.is_grad_enabled():  # training on multi-caption batches: full length, the 2-D path's autograd
+                return self.forward(text_tokens.reshape(b * n, L), kpm).view(b, n, -1)
+            feats, where = self._encode_rows(text_tokens.reshape(b * n, L), kpm)
+            return Fn.L2NormFn.apply(feats)[where].view(b, n, -1)
         if text_tokens.dim() != 2:
-            raise NotImplementedError("zero-shot text batches [B, classes, captions, L] are not implemented")
+            raise NotImplementedError(f"text tokens of rank {text_tokens.dim()}: expected [B, L], [B, N, L] or [B, classes, captions, L]")
+        pe = self._checked_pos_embed(text_tokens.shape[-1])
+        return Fn.L2NormFn.apply(self._tower(text_tokens.contiguous(), pe, key_padding_mask))
+
+    def _checked_pos_embed(self, L: int) -> Optional[Tensor]:
         if self.training and self.embedding_dropout.p > 0:
             raise NotImplementedError("embedding dropout > 0 in training mode is not implemented")
         pe = self.positional_embedding.pos_embed.pos_embed if self.positional_embedding is not None else None
-        if pe is not None and pe.shape[2] != text_tokens.shape[1]:
+        if pe is not None and pe.shape[2] != L:
             raise NotImplementedError("interpolated positional embeddings are not implemented (sequence length must equal the context length)")
+        return pe
+
+    def _tower(self, tokens: Tensor, pe: Optional[Tensor], key_padding_mask: Optional[Tensor]) -> Tensor:
+        """transformer.py:354-423 up to the projection: bf16 [b, projection_dim] features of the end-of-text tokens, not yet normalised.
+        ``pe`` holds the first tokens.shape[1] rows of the positional table."""
         emb = self._emb
         emb.ws, emb.plist = getattr(self, "_ws", None), [self.embedding_layer.weight] + ([pe] if pe is not None else [])
-        tokens = text_tokens.contiguous()
         x = Fn.EmbeddingFn.apply(tokens, emb, self.embedding_layer.weight, pe)
         attn_mask = None
         if self.causal_masking:
@@ -144,8 +172,56 @@ class TextTransformer(nn.Module):
             x = layer(x, key_padding_mask=key_padding_mask, attn_mask=attn_mask)
         x = Fn.EotGatherFn.apply(x, tokens)       # LayerNorm is per token: normalising only the gathered token equals norm-then-gather
         x = self.final_layer_norm(x)
-        x = self._proj.apply_to(x, self.projection_layer, self)
-        return Fn.L2NormFn.apply(x)
+        return self._proj.apply_to(x, self.projection_layer, self)
+
+    @torch.no_grad()
+    def _encode_rows(self, tokens: Tensor, key_padding_mask: Optional[Tensor]) -> Tuple[Tensor, Tensor]:
+        """Encodes the rows of a [R, L] token matrix without autograd, in length-bucketed chunks of at most ``zero_shot_token_budget`` tokens.
+
+        With causal masking the end-of-text feature depends only on tokens 0..eot: LayerNorm, the GEMMs and the FFN act per token and
+        attention only looks back.  So each row runs at its own prefix length L' = eot + 1, rounded up to a multiple of 8 (fewer distinct
+        lengths, hence fewer and larger tower calls), on the first L' rows of the positional table and an [L', L'] causal mask.  A chunk
+        holds rows of one L' only, so a row's result does not depend on which other rows share its chunk, nor on the budget.  Without
+        causal masking every row runs at full length (and the key-padding mask, if any, applies).
+
+        Returns (features bf16 [R, projection_dim] before normalisation, in length-sorted order; where: int64 [R], the feature row of token
+        row r)."""
+        R, L = tokens.shape
+        pe = self._checked_pos_embed(L)
+        tokens = tokens.contiguous()
+        if self.causal_masking:
+            lengths = ((tokens.argmax(dim=-1) + 8) // 8 * 8).clamp_(max=L)
+            order = torch.argsort(lengths, stable=True)
+            counts = torch.bincount(lengths, minlength=L + 1).tolist()  # one host sync per table
+            key_padding_mask = None
+        else:
+            order = torch.arange(R, device=tokens.device)
+            counts = [0] * L + [R]
+        where = torch.empty_like(order)
+        where[order] = torch.arange(R, device=tokens.device)
+        feats = torch.empty((R, self.projection_dim), device=tokens.device, dtype=torch.bfloat16)
+        start = 0
+        for Lp, n in enumerate(counts):
+            rows = max(1, self.zero_shot_token_budget // max(Lp, 1))
+            for i in range(start, start + n, rows):
+                idx = order[i:min(i + rows, start + n)]
+                kpm = key_padding_mask[idx].contiguous() if key_padding_mask is not None else None
+                feats[i:i + idx.numel()] = self._tower(tokens[idx, :Lp].contiguous(), pe[:, :, :Lp] if pe is not None else None, kpm)
+            start += n
+        return feats, where
+
+    def forward_zero_shot(self, text_tokens: Tensor, key_padding_mask: Optional[Tensor] = None) -> Tensor:
+        """transformer.py:428-504: the class table of zero-shot classification, fp32 [d, Cl] = transpose(normalize(mean over the M captions
+        of normalize(caption feature))), from the prompts of the first batch element of [B, Cl, M, L] (every element holds the same
+        prompts).  Eval mode only.  The captions are encoded by ``_encode_rows``; ``classes_per_split_zero_shot`` is accepted and, as in
+        the reference, does not change the result (``zero_shot_token_budget`` bounds the memory instead).  The per-caption normalisation,
+        the mean and the final normalisation are one kernel (cvb_zs_class_embed) in fp32."""
+        if self.training:
+            raise NotImplementedError("Zero-shot evaluation is only supported with eval mode")
+        _, Cl, M, L = text_tokens.shape
+        kpm = key_padding_mask[0].reshape(Cl * M, L) if key_padding_mask is not None else None
+        feats, where = self._encode_rows(text_tokens[0].reshape(Cl * M, L), kpm)
+        return ops.zs_class_embed(feats, where.to(torch.int32), Cl, M)
 
 
 class SimpleImageProjectionHead(nn.Module):
@@ -169,9 +245,47 @@ class CLIP(nn.Module):
         self.image_encoder.classifier = SimpleImageProjectionHead(opts, self.image_encoder.embed_dim, proj)
         self.text_encoder = TextTransformer(opts, projection_dim=proj)
         self.logit_scale = nn.Parameter(torch.ones([]) * math.log(1.0 / 0.07))
+        self.cache_text_features_zero_shot = bool(getattr(opts, "model.multi_modal_image_text.clip.cache_text_features_zero_shot", False))
+        self.cached_text_features = None
 
     def forward(self, images: Tensor, text_tokens: Tensor) -> Tuple[Tensor, Tensor, Tensor]:
-        return self.image_encoder(images), self.text_encoder(text_tokens), self.logit_scale
+        """(image features [B, d], text output, raw logit_scale).  The text output is what ``TextTransformer`` returns for the rank of
+        ``text_tokens``: [B, d], [B, N, d], or in eval mode the [d, Cl] zero-shot class table of 4-D prompts."""
+        img = self.image_encoder(images)
+        txt = self.zero_shot_table(text_tokens) if text_tokens.dim() == 4 else self.text_encoder(text_tokens)
+        return img, txt, self.logit_scale
+
+    def zero_shot_table(self, class_tokens: Tensor) -> Tensor:
+        """fp32 [d, Cl] class table of zero-shot prompts [B, Cl, M, L] (eval mode).  With
+        ``model.multi_modal_image_text.clip.cache_text_features_zero_shot`` it is computed once and reused (clip.py:171-178).  Unlike the
+        reference, which never drops that cache, ``train()`` and ``clear_zero_shot_cache()`` drop it: a table kept across further training
+        would score the new weights against the old text tower.  The cache holds zero-shot tables only."""
+        if self.cache_text_features_zero_shot and not self.training:
+            if self.cached_text_features is None:
+                self.cached_text_features = self.text_encoder(class_tokens)
+            return self.cached_text_features
+        return self.text_encoder(class_tokens)
+
+    def clear_zero_shot_cache(self) -> None:
+        self.cached_text_features = None
+
+    def train(self, mode: bool = True):
+        if mode:
+            self.cached_text_features = None
+        return super().train(mode)
+
+    def zero_shot_logits(self, images: Tensor, class_table_or_tokens: Tensor, targets: Optional[Tensor] = None,
+                         hits: Optional[Tensor] = None) -> Tensor:
+        """clip.py:184-202 in eval mode: fp32 zero_shot_image_logits [B, Cl] = 100 * image features @ table (the fixed factor 100, not the
+        logit scale), without autograd.  ``class_table_or_tokens``: an fp32 [d, Cl] table or 4-D prompts (see ``zero_shot_table``).  With
+        ``targets`` (int64 [B]) and ``hits`` (int64 [2] on the device), the batch's top-1 / top-5 hits (metrics/topk_accuracy.py) are added
+        into ``hits`` without a host sync."""
+        if self.training:
+            raise NotImplementedError("Zero-shot evaluation is only supported with eval mode")
+        with torch.no_grad():
+            table = class_table_or_tokens if class_table_or_tokens.dim() == 2 else self.zero_shot_table(class_table_or_tokens)
+            img = self.image_encoder(images)
+            return ops.zs_logits_topk(img, table, 100.0, targets, hits)
 
 
 def clip_contrastive_loss(image_features: Tensor, text_features: Tensor, logit_scale: Tensor, process_group=None, _cfg=None) -> Tensor:

@@ -330,6 +330,44 @@ def add_bf16_f32(A: Optional[Tensor], Bf: Tensor) -> Tensor:
     return out
 
 
+def zs_class_embed(X: Tensor, perm: Tensor, Cl: int, M: int) -> Tensor:
+    """fp32 [d, Cl] class table from the bf16 projected caption features X [R, d] (unnormalised); perm: int32 [Cl * M] row of caption m of
+    class c at c * M + m."""
+    R, d = X.shape
+    if X.dtype != torch.bfloat16 or X.stride(1) != 1:
+        raise ValueError("zs_class_embed: X must be bf16 with unit column stride")
+    if perm.dtype != torch.int32 or perm.numel() != Cl * M or not perm.is_contiguous():
+        raise ValueError(f"zs_class_embed: perm must be a contiguous int32 tensor of Cl * M = {Cl * M} elements")
+    table = torch.empty((d, Cl), device=X.device, dtype=torch.float32)
+    L.check(_lib().cvb_zs_class_embed(X.data_ptr(), X.stride(0), R, perm.data_ptr(), Cl, M, d, table.data_ptr(), _stream()), "cvb_zs_class_embed")
+    _count()
+    return table
+
+
+def zs_logits_topk(img: Tensor, table: Tensor, scale: float = 100.0, targets: Optional[Tensor] = None, hits: Optional[Tensor] = None,
+                   want_logits: bool = True) -> Optional[Tensor]:
+    """fp32 logits [B, Cl] = scale * img @ table (None when ``want_logits`` is False); with ``targets`` (int64 [B]) and ``hits`` (int64 [2]),
+    the top-1 / top-5 hits of the batch are added into ``hits`` on the device."""
+    B, d = img.shape
+    if img.dtype != torch.bfloat16 or img.stride(1) != 1:
+        raise ValueError("zs_logits_topk: img must be bf16 with unit column stride")
+    if table.dtype != torch.float32 or table.dim() != 2 or table.shape[0] != d or not table.is_contiguous():
+        raise ValueError(f"zs_logits_topk: table must be a contiguous fp32 [{d}, classes] tensor, got {tuple(table.shape)} {table.dtype}")
+    if (targets is None) != (hits is None):
+        raise ValueError("zs_logits_topk: targets and hits go together")
+    if targets is not None:
+        if targets.dtype != torch.int64 or targets.shape != (B,) or not targets.is_contiguous():
+            raise ValueError(f"zs_logits_topk: targets must be a contiguous int64 [{B}] tensor")
+        if hits.dtype != torch.int64 or hits.numel() != 2 or not hits.is_contiguous():
+            raise ValueError("zs_logits_topk: hits must be a contiguous int64 [2] tensor")
+    Cl = table.shape[1]
+    logits = torch.empty((B, Cl), device=img.device, dtype=torch.float32) if want_logits else None
+    L.check(_lib().cvb_zs_logits_topk(img.data_ptr(), img.stride(0), table.data_ptr(), B, d, Cl, float(scale), _p(targets), _p(logits), _p(hits),
+                                      _stream()), "cvb_zs_logits_topk")
+    _count()
+    return logits
+
+
 def patch_permute(X: Tensor, B: int, H: int, W: int, ph: int, pw: int, inverse: bool) -> Tensor:
     """MobileViT-v1 unfold (inverse=False: feature-map rows -> token rows [B*P*N, C]) / fold (inverse=True)."""
     out = torch.empty_like(X)
