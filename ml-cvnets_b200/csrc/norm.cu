@@ -566,7 +566,7 @@ __device__ __forceinline__ float act_grad_f(float x, int kind) {
       return cdf + x * 0.3989422804014327f * __expf(-0.5f * x * x);
     }
     case 2: return x > 0.f ? 1.f : 0.f;
-    case 3: return x < -3.0f ? 0.f : (x <= 3.0f ? fmaf(x, 1.0f / 3.0f, 0.5f) : 1.0f);  // torch: hardswish_backward
+    case 3: return x <= -3.0f ? 0.f : (x < 3.0f ? fmaf(x, 1.0f / 3.0f, 0.5f) : 1.0f);  // torch's hardswish_backward: 0 at -3, 1 at 3
     case 4: return (x > -3.0f && x < 3.0f) ? (1.0f / 6.0f) : 0.f;
     default: {
       const float s = 1.0f / (1.0f + __expf(-x));
@@ -985,7 +985,10 @@ extern "C" int cvb_gn_bwd(const void* V, const void* X, const float* mean, const
   const int cap = (6 * cvb_num_sms() + B - 1) / B;
   int rows_per_cta = g1.rows_per_cta;
   if (chunks > cap) { rows_per_cta = ((rows_per_sample + cap - 1) / cap + g1.rpp - 1) / g1.rpp * g1.rpp; chunks = (rows_per_sample + rows_per_cta - 1) / rows_per_cta; }
-  CVB_CUDA(cvb_launch(gn_bwd_stats_kernel, dim3(chunks, B), g1.nthreads, 2 * C * sizeof(double), static_cast<cudaStream_t>(stream),
+  // whole warps: the per-sample sums are warp-shuffle reductions over every lane (cgs * rpp is 240..256 for C = 24, 40, 80, 96, 192, ...);
+  // the threads past cgs * rpp have rr >= rpp and contribute zeros
+  const int nthreads1 = (g1.nthreads + 31) / 32 * 32;
+  CVB_CUDA(cvb_launch(gn_bwd_stats_kernel, dim3(chunks, B), nthreads1, 2 * C * sizeof(double), static_cast<cudaStream_t>(stream),
                       static_cast<const bf16*>(V), static_cast<const bf16*>(X), mean, rstd, gamma, rows_per_sample, C, g1.cgs, g1.rpp, rows_per_cta, dgamma,
                       dbeta, samp_ws, samp_ws + B));
   CVB_LAUNCH_CHECK();

@@ -1,5 +1,7 @@
-"""Kernel-level parity (-m gpu): every C-ABI entry point against a plain PyTorch fp32 restatement of the same op on the
-same (bf16-rounded) inputs.  Tolerances are bf16 output rounding (2^-8 relative) plus fp32 accumulation-order noise."""
+"""Kernel-level parity (-m gpu): C-ABI entry points against a plain PyTorch fp32 restatement of the same op on the
+same (bf16-rounded) inputs.  Tolerances are bf16 output rounding (2^-8 relative) plus fp32 accumulation-order noise.
+test_kernels_edges_gpu.py covers the remaining entry points and the edge shapes / values; test_kernel_coverage_cpu.py checks that
+every export of include/cvnets_b200.h is called by some GPU test."""
 import pytest
 import torch
 
