@@ -584,7 +584,18 @@ extern "C" int cvb_dw_bwd(const cvb_dw_bwd_args* args, cvb_stream_t stream) {
   CVB_CHECK(a.x_mode == CVB_A_RAW || ((a.x_mode == CVB_A_AFF || a.x_mode == CVB_A_AFF_SILU) && a.x_p0 && a.x_p1), "cvb_dw_bwd: bad x_mode %d", a.x_mode);
   if (a.col_sum) CVB_CHECK(a.col_sq != nullptr, "cvb_dw_bwd: col_sq missing");
   CVB_CHECK(a.dilation >= 0 && a.dilation <= 64, "cvb_dw_bwd: bad dilation %d", a.dilation);
-  if (a.dilation > 1) return cvb_dw_bwd_dilated(a, static_cast<cudaStream_t>(stream));
+  if (a.dilation > 1) {
+    // the dilated kernel's per-block dW partials meet in the same fp64 scratch as the walk kernels' (order-independent, so reproducible)
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    double* ws = nullptr;
+    if (cvb_det_alloc(&ws, (size_t)9 * a.C, st)) return 2;
+    cvb_dw_bwd_args b = a;
+    b.dWt = reinterpret_cast<float*>(ws);
+    int rc = cvb_dw_bwd_dilated(b, st);
+    if (rc == 0) rc = cvb_det_add(ws, a.dWt, 9, a.C, a.C, st);
+    const int rf = cvb_det_free(ws, st);
+    return rc ? rc : rf;
+  }
   if (a.stride == 2) CVB_CHECK(a.H % 2 == 0 && a.W % 2 == 0, "cvb_dw_bwd: stride 2 needs even H, W");
   const int s = a.stride;
   const int Ho = (a.H - 1) / s + 1, Wo = (a.W - 1) / s + 1;

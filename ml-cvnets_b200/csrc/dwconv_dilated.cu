@@ -202,7 +202,7 @@ __global__ void __launch_bounds__(DNT) dwd_bwd_kernel(const cvb_dw_bwd_args p, i
         for (int t = 0; t < 9; ++t) {
           float a = 0.f;
           for (int y = 0; y < py; ++y) a += s_red[y * cx + threadIdx.x][t];
-          atomicAdd(p.dWt + (size_t)t * p.C + c + j, a);
+          atomicAdd(reinterpret_cast<double*>(p.dWt) + (size_t)t * p.C + c + j, (double)a);  // fp64 scratch (cvb_dw_bwd)
         }
       }
     }

@@ -403,7 +403,9 @@ int launch_tc(const cvb_gemm_args& a, cudaStream_t st) {
 }
 
 // GroupNorm backward, phase 1 finalize: from A[b,c] = sum_m v, Bx[b,c] = sum_m v*x over the pixels of sample b
-//   dbeta[c] += A;  dgamma[c] += t,  t = rstd_b (Bx - mean_b A) = sum_m v*xhat;   sum g = sum_c gamma_c A;   sum g*xhat = sum_c gamma_c t
+//   dbeta[c] += sum_b A;  dgamma[c] += sum_b t,  t = rstd_b (Bx - mean_b A) = sum_m v*xhat;   sum g = sum_c gamma_c A;   sum g*xhat = sum_c gamma_c t
+// Blocks [0, B) take the per-sample sums, blocks [B, B + ceil(N / 16)) the per-channel ones.  A and t are full fp64 values, so the channel sums
+// add the samples in a fixed order (an fp64 atomic per sample would round differently depending on which block arrives first).
 __global__ void __launch_bounds__(128) gn_bwd_ws_finalize_kernel(const double* __restrict__ ws, const float* __restrict__ mean,
                                                                   const float* __restrict__ rstd, const float* __restrict__ gamma, int B, int N,
                                                                   double* col_sum, double* col_sq, double* samp_sum, double* samp_sq) {
@@ -411,13 +413,34 @@ __global__ void __launch_bounds__(128) gn_bwd_ws_finalize_kernel(const double* _
   pdl_trigger();
   __shared__ double s_red[2][4];
   const int b = blockIdx.x, tid = threadIdx.x;
+  if (b >= B) {  // 16 channels per block, 8 strided sample groups per channel, combined in group order
+    __shared__ double s_col[2][8][16];
+    const int cl = tid & 15, sg = tid >> 4, c = (b - B) * 16 + cl;
+    double sa = 0.0, st = 0.0;
+    if (c < N) {
+#pragma unroll 4
+      for (int s = sg; s < B; s += 8) {
+        const double A = ws[(size_t)s * N + c], Bx = ws[((size_t)B + s) * N + c];
+        sa += A;
+        st += (double)rstd[s] * (Bx - (double)mean[s] * A);
+      }
+    }
+    s_col[0][sg][cl] = sa;
+    s_col[1][sg][cl] = st;
+    __syncthreads();
+    if (sg == 0 && c < N) {
+      for (int g = 1; g < 8; ++g) { sa += s_col[0][g][cl]; st += s_col[1][g][cl]; }
+      col_sum[c] += sa;
+      col_sq[c] += st;
+    }
+    return;
+  }
   const double mu = (double)mean[b], rs = (double)rstd[b];
   double sg = 0.0, sgx = 0.0;
   for (int c = tid; c < N; c += 128) {
     const double A = ws[(size_t)b * N + c], Bx = ws[((size_t)B + b) * N + c];
     const double t = rs * (Bx - mu * A);
     const double gm = gamma ? (double)gamma[c] : 1.0;
-    if (col_sum) { atomicAdd(col_sum + c, A); atomicAdd(col_sq + c, t); }
     sg += gm * A;
     sgx += gm * t;
   }
@@ -439,7 +462,8 @@ int launch_tc_gn_bwd(const cvb_gemm_args& a, cudaStream_t st) {
   int rc = launch_tc<AMODE, TEPI_GN_BWD>(a, st);
   if (rc != 0) return rc;
   const int B = (a.M + a.rows_per_sample - 1) / a.rows_per_sample;
-  CVB_CUDA(cvb_launch(gn_bwd_ws_finalize_kernel, B, 128, 0, st, static_cast<const double*>(a.gn_ws), a.row_mean, a.row_rstd, a.e_p0, B, a.N, a.col_sum,
+  const int col_blocks = a.col_sum ? (a.N + 15) / 16 : 0;
+  CVB_CUDA(cvb_launch(gn_bwd_ws_finalize_kernel, B + col_blocks, 128, 0, st, static_cast<const double*>(a.gn_ws), a.row_mean, a.row_rstd, a.e_p0, B, a.N, a.col_sum,
                       a.col_sq, a.samp_sum, a.samp_sq));
   CVB_LAUNCH_CHECK();
   return 0;
