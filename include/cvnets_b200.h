@@ -121,7 +121,8 @@ CVB_API int cvb_apply_load_mode(const void* A, int lda, const void* A2, int lda2
 
 /* ---------------------------------------------------------------------------------------------------------------
  * Depthwise 3x3 convolution, pad = dilation, stride 1|2, NHWC (ConvLayer2d(groups=C): mobilenetv2.py:194-207,
- * mobilevit_block.py:369-379).  dilation 0 / 1 = dense stencil (TMA walk kernels); dilation > 1 (stride 1 only) = the segmentation
+ * mobilevit_block.py:369-379), and the undilated 5x5 one, pad 2, stride 1|2 (EfficientNet's MBConv blocks: cvnets/modules/efficientnet.py,
+ * config/efficientnet.py).  dilation 0 / 1 = dense stencil (TMA walk kernels); dilation > 1 (stride 1 only) = the segmentation
  * backbones' output_stride 8 / 16 variants (base_image_encoder.py:38-47, mobilevit_v2.py:176-191), a direct-gather kernel.  The producer's BN(+SiLU) is applied on load (x_mode RAW/AFF/AFF_SILU); zero padding
  * is applied AFTER that transform, as in the reference where padding acts on the activated tensor.
  * Output: pre-BN y (bf16) + fp64 per-channel sum / sum of squares of the stored values.
@@ -129,16 +130,17 @@ CVB_API int cvb_apply_load_mode(const void* A, int lda, const void* A2, int lda2
 typedef struct {
   int B, H, W, C, stride;
   const void* X; int x_mode; const float* x_p0; const float* x_p1;
-  const float* Wt;  /* fp32 [9][C] (tap-major), values already rounded to bf16 (autocast semantics) */
+  const float* Wt;  /* fp32 [K*K][C] (tap-major), values already rounded to bf16 (autocast semantics) */
   void* Y;          /* bf16 [B,Ho,Wo,C] */
   double* col_sum; double* col_sq;
   int dilation;     /* 0 or 1: none */
+  int ksize;        /* K: 0 or 3 = 3x3, 5 = 5x5 (pad 2; dilation must be 0 / 1) */
 } cvb_dw_fwd_args;
 CVB_API int cvb_dw_fwd(const cvb_dw_fwd_args* args, cvb_stream_t stream);
 
 /* Backward of the above, fused: dy = load(DZ[,Y2]) (RAW or BNB), dX = conv_transpose(dy) then through the producer's
  * activation (x_mode AFF_SILU: dX *= silu'(p0*x+p1)), statistics col_sum += dX, col_sq += dX*x for the producer's BN
- * backward, and dWt[9][C] += sum dy * load(X)(shifted). */
+ * backward, and dWt[K*K][C] += sum dy * load(X)(shifted).  Stride 2 needs even H and W. */
 typedef struct {
   int B, H, W, C, stride;
   const void* DZ; const void* Y2; int g_mode; const float* g_p0; const float* g_p1; const float* g_p2;
@@ -146,8 +148,9 @@ typedef struct {
   const float* Wt;
   void* DX;         /* bf16 [B,H,W,C] */
   double* col_sum; double* col_sq; /* may be NULL when x_mode == RAW */
-  float* dWt;       /* fp32 [9][C], accumulated (+=) */
+  float* dWt;       /* fp32 [K*K][C], accumulated (+=) */
   int dilation;     /* 0 or 1: none */
+  int ksize;        /* as in cvb_dw_fwd_args */
 } cvb_dw_bwd_args;
 CVB_API int cvb_dw_bwd(const cvb_dw_bwd_args* args, cvb_stream_t stream);
 
@@ -308,6 +311,13 @@ CVB_API int cvb_adamw_step(float* params, const float* grads, float* exp_avg, fl
                    const float* hp, float beta1, float beta2, float eps, float max_norm, float* stats, float* scale, float* step,
                    float growth_factor, float backoff_factor, int growth_interval, float* ema, float ema_momentum, const float* partials,
                    cvb_stream_t stream);
+/* The same step with torch.optim.SGD(momentum, dampening=0, nesterov, weight_decay) in place of AdamW (the SGD recipes: EfficientNet,
+ * MobileNet v1-v3): g' = g*unscale*clip + weight_decay[i]*p;  momentum_buf = momentum*momentum_buf + g' (zero-initialised, which equals
+ * torch's first-step clone);  p -= lr * (g' + momentum*momentum_buf) with nesterov != 0, lr * momentum_buf without.  Same stats / scale /
+ * step / EMA / partials semantics as cvb_adamw_step; cvb_grad_norm must precede it. */
+CVB_API int cvb_sgd_step(float* params, const float* grads, float* momentum_buf, const float* weight_decay, int64_t n, const float* hp, float momentum,
+                         int nesterov, float max_norm, float* stats, float* scale, float* step, float growth_factor, float backoff_factor,
+                         int growth_interval, float* ema, float ema_momentum, const float* partials, cvb_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
  * Classification loss of the step: F.cross_entropy(prediction, target, ignore_index, label_smoothing), mean over the non-ignored

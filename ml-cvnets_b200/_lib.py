@@ -59,7 +59,7 @@ class DwFwdArgs(Structure):
     _fields_ = [
         ("B", c_int), ("H", c_int), ("W", c_int), ("C", c_int), ("stride", c_int),
         ("X", c_void_p), ("x_mode", c_int), ("x_p0", c_void_p), ("x_p1", c_void_p),
-        ("Wt", c_void_p), ("Y", c_void_p), ("col_sum", c_void_p), ("col_sq", c_void_p), ("dilation", c_int),
+        ("Wt", c_void_p), ("Y", c_void_p), ("col_sum", c_void_p), ("col_sq", c_void_p), ("dilation", c_int), ("ksize", c_int),
     ]
 
 
@@ -69,6 +69,7 @@ class DwBwdArgs(Structure):
         ("DZ", c_void_p), ("Y2", c_void_p), ("g_mode", c_int), ("g_p0", c_void_p), ("g_p1", c_void_p), ("g_p2", c_void_p),
         ("X", c_void_p), ("x_mode", c_int), ("x_p0", c_void_p), ("x_p1", c_void_p),
         ("Wt", c_void_p), ("DX", c_void_p), ("col_sum", c_void_p), ("col_sq", c_void_p), ("dWt", c_void_p), ("dilation", c_int),
+        ("ksize", c_int),
     ]
 
 
@@ -132,6 +133,8 @@ _SIGS = {
     "cvb_grad_norm": (c_int, [c_void_p, c_int64, c_void_p, c_float, c_void_p, c_void_p, c_void_p]),
     "cvb_adamw_step": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_float, c_float, c_float, c_float, c_void_p,
                                c_void_p, c_void_p, c_float, c_float, c_int, c_void_p, c_float, c_void_p, c_void_p]),
+    "cvb_sgd_step": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_float, c_int, c_float, c_void_p, c_void_p, c_void_p,
+                             c_float, c_float, c_int, c_void_p, c_float, c_void_p, c_void_p]),
     "cvb_ce_fwd": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "cvb_ce_bwd": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
                            c_void_p, c_void_p, c_void_p, c_void_p]),

@@ -1,10 +1,10 @@
-// Depthwise 3x3 convolution (pad 1, stride 1|2), NHWC bf16, forward and fused backward (sm_90a).
+// Depthwise KxK convolution (K = 3 | 5, pad (K-1)/2, stride 1|2), NHWC bf16, forward and fused backward (sm_90a).
 //
 // HBM-bound stencils whose first implementation was instruction-issue bound (~85 instructions per element).  This version is
 // built around the instruction count:
 //   * a warp spans the CTA's 64 channels (lane = channel pair, one 4-byte bf16x2 access per lane = one conflict-free 128-byte
-//     shared-memory wavefront per warp) and WALKS along a strip of pixels, keeping the 3x3 neighbourhood of the strip's rows in
-//     registers (sliding window: each neighbour is loaded (R+2)/R times instead of 9);
+//     shared-memory wavefront per warp) and WALKS along a strip of pixels, keeping the KxK neighbourhood of the strip's rows in
+//     registers (sliding window: each neighbour is loaded (R+K-1)/R times instead of K*K);
 //   * all arithmetic is fp32 on channel pairs (ffma2 / fmul2 helpers), weights / dW accumulators / BN statistics stay in
 //     registers for the whole batch loop of the CTA;
 //   * backward: for every INPUT pixel p the same neighbourhood dy[p - tap] feeds both products,
@@ -20,8 +20,12 @@ namespace {
 
 constexpr int CB = 64;    // channels per CTA (32 lanes x channel pair)
 constexpr int NT = 256;   // forward: 8 warps, 2 CTAs / SM
-constexpr int NTB = 512;  // backward: 16 warps, 1 CTA / SM
 constexpr int SEG = 8;    // pixels a warp walks per strip (fully unrolled: the window shift is register renaming)
+// backward: 16 warps for 3x3; 5x5 keeps 25 weights + 25 dW accumulators + a 6 x 5 window per lane, which needs the 255-register
+// budget of 8 warps
+template <int K> constexpr int bwd_threads() { return K == 3 ? 512 : 256; }
+// opt-in dynamic shared memory of the backward; with the static part (5x5: 12.5 KB of fp64 dW partials) it must stay within 227 KB per CTA
+template <int K> constexpr int bwd_smem_cap() { return K == 3 ? 216 * 1024 : 200 * 1024; }
 
 // bf16x2 -> two fp32 (exact): two integer-pipe instructions, no conversion unit
 __device__ __forceinline__ float2 up2(uint32_t u) { return make_float2(__uint_as_float(u << 16), __uint_as_float(u & 0xffff0000u)); }
@@ -76,13 +80,14 @@ __device__ __forceinline__ void transform_tile(uint8_t* tile, int TH_, int TW_, 
 }
 
 // ------------------------------------------------------------------------------------------------------------- forward
-// Output tile TH x TW, input tile IH x IW = ((TH-1)S+3) x ((TW-1)S+3) with origin (S*oh0 - 1, S*ow0 - 1).
-//   stride 1: strip = 2 output rows x SEG columns, window 4 x 3;  stride 2: strip = 1 output row x SEG columns, window 3 x 3.
-template <int XMODE, int S>
+// Output tile TH x TW, input tile IH x IW = ((TH-1)S+K) x ((TW-1)S+K) with origin (S*oh0 - P, S*ow0 - P), P = (K-1)/2.
+//   stride 1: strip = 2 output rows x SEG columns, window (K+1) x K;  stride 2: strip = 1 output row x SEG columns, window K x K.
+template <int XMODE, int S, int K>
 __global__ void __launch_bounds__(NT, 2) dw_fwd_kernel(const __grid_constant__ CUtensorMap tmX, const cvb_dw_fwd_args p, int Ho, int Wo, int TH,
                                                        int TW, int tiles_w, int buf_bytes) {
+  constexpr int P = (K - 1) / 2;
   constexpr int R = (S == 1) ? 2 : 1;
-  constexpr int WR = (S == 1) ? 4 : 3;  // window rows
+  constexpr int WR = R + K - 1;  // window rows
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   __shared__ double s_cs[CB], s_cq[CB];  // fp64: the warps' fp32 partials sum exactly, whatever their order
@@ -92,8 +97,8 @@ __global__ void __launch_bounds__(NT, 2) dw_fwd_kernel(const __grid_constant__ C
   const int th_i = blockIdx.x / tiles_w, tw_i = blockIdx.x % tiles_w;
   const int oh0 = th_i * TH, ow0 = tw_i * TW;
   const int c0 = blockIdx.y * CB;
-  const int IH = (TH - 1) * S + 3, IW = (TW - 1) * S + 3;
-  const int h_base = oh0 * S - 1, w_base = ow0 * S - 1;
+  const int IH = (TH - 1) * S + K, IW = (TW - 1) * S + K;
+  const int h_base = oh0 * S - P, w_base = ow0 * S - P;
   const uint32_t tile_bytes = (uint32_t)IH * IW * 128;
   const int n_img = (p.B - (int)blockIdx.z + (int)gridDim.z - 1) / (int)gridDim.z;
 
@@ -119,9 +124,9 @@ __global__ void __launch_bounds__(NT, 2) dw_fwd_kernel(const __grid_constant__ C
   }
   const int cl = c0 + 2 * lane;  // this lane's channel pair
   const bool lane_ok = cl < p.C;
-  float2 wv[9];
+  float2 wv[K * K];
 #pragma unroll
-  for (int t = 0; t < 9; ++t) wv[t] = lane_ok ? make_float2(p.Wt[t * p.C + cl], p.Wt[t * p.C + cl + 1]) : make_float2(0.f, 0.f);
+  for (int t = 0; t < K * K; ++t) wv[t] = lane_ok ? make_float2(p.Wt[t * p.C + cl], p.Wt[t * p.C + cl + 1]) : make_float2(0.f, 0.f);
   float2 cs = make_float2(0.f, 0.f), cq = make_float2(0.f, 0.f);
   const int strips_w = TW / SEG;
   const int n_strips = (TH / R) * strips_w;
@@ -147,25 +152,34 @@ __global__ void __launch_bounds__(NT, 2) dw_fwd_kernel(const __grid_constant__ C
       bf16* yrow[R];
 #pragma unroll
       for (int r = 0; r < R; ++r) yrow[r] = Y + ((size_t)(oh0 + orow + r) * Wo + ow0 + ocol) * p.C;
-      float2 win[WR][3];
+      float2 win[WR][K];  // win[k][c] = input column icol + S*x + c of row irow + k
       if (S == 1) {
 #pragma unroll
-        for (int k = 0; k < WR; ++k) { win[k][1] = lds2(tile, (irow + k) * IW + icol, lane); win[k][2] = lds2(tile, (irow + k) * IW + icol + 1, lane); }
+        for (int k = 0; k < WR; ++k)
+#pragma unroll
+          for (int c = 1; c < K; ++c) win[k][c] = lds2(tile, (irow + k) * IW + icol + c - 1, lane);
       } else {
 #pragma unroll
-        for (int k = 0; k < WR; ++k) win[k][2] = lds2(tile, (irow + k) * IW + icol, lane);
+        for (int k = 0; k < WR; ++k)
+#pragma unroll
+          for (int c = 2; c < K; ++c) win[k][c] = lds2(tile, (irow + k) * IW + icol + c - 2, lane);
       }
 #pragma unroll
       for (int x = 0; x < SEG; ++x) {
         if (S == 1) {
 #pragma unroll
-          for (int k = 0; k < WR; ++k) { win[k][0] = win[k][1]; win[k][1] = win[k][2]; win[k][2] = lds2(tile, (irow + k) * IW + icol + x + 2, lane); }
+          for (int k = 0; k < WR; ++k) {
+#pragma unroll
+            for (int c = 0; c < K - 1; ++c) win[k][c] = win[k][c + 1];
+            win[k][K - 1] = lds2(tile, (irow + k) * IW + icol + x + K - 1, lane);
+          }
         } else {
 #pragma unroll
           for (int k = 0; k < WR; ++k) {
-            win[k][0] = win[k][2];
-            win[k][1] = lds2(tile, (irow + k) * IW + icol + 2 * x + 1, lane);
-            win[k][2] = lds2(tile, (irow + k) * IW + icol + 2 * x + 2, lane);
+#pragma unroll
+            for (int c = 0; c < K - 2; ++c) win[k][c] = win[k][c + 2];
+            win[k][K - 2] = lds2(tile, (irow + k) * IW + icol + 2 * x + K - 2, lane);
+            win[k][K - 1] = lds2(tile, (irow + k) * IW + icol + 2 * x + K - 1, lane);
           }
         }
         const int gw = ow0 + ocol + x;
@@ -173,9 +187,9 @@ __global__ void __launch_bounds__(NT, 2) dw_fwd_kernel(const __grid_constant__ C
         for (int r = 0; r < R; ++r) {
           float2 acc = make_float2(0.f, 0.f);
 #pragma unroll
-          for (int u = 0; u < 3; ++u)
+          for (int u = 0; u < K; ++u)
 #pragma unroll
-            for (int v = 0; v < 3; ++v) acc = ffma2(wv[u * 3 + v], win[r + u][v], acc);
+            for (int v = 0; v < K; ++v) acc = ffma2(wv[u * K + v], win[r + u][v], acc);
           const uint32_t pk = pack_bf162(acc.x, acc.y);
           if (INTERIOR) {
             cs = fadd2(cs, acc);
@@ -220,8 +234,10 @@ __global__ void __launch_bounds__(NT, 2) dw_fwd_kernel(const __grid_constant__ C
 // Per image tile: (dz, x) double-buffered, y2 single-buffered (it is consumed by step 1 only and refilled right after it).
 //   1. dy = c1*dz + c2*y2 + c3 in place (in-bounds pixels only: the zero halo is the transposed conv's padding)
 //   2. one walk over the tile's INPUT pixels: dX, dW, activation backward, BN-backward statistics of the producer.
-// stride 1: strip = 2 input rows x SEG columns, dy window 4 x 3 (halo origin -1).
-// stride 2: strip = 1 OUTPUT row x SEG output columns = 2 x 2SEG input pixels, dy window 2 x 2 (halo +1 on the high side):
+// stride 1: strip = 2 input rows x SEG columns, dy window (K+1) x K (halo origin -P).
+// stride 2: strip = 1 OUTPUT row x SEG output columns = 2 x 2SEG input pixels.  Input pixel (2i+a, 2j+b) receives tap (u, v) from
+//   dy[i + (a+P-u)/2, j + (b+P-v)/2] when a+P-u and b+P-v are even, so the dy rows / columns it needs are i-LO .. i+1 with LO = P/2:
+//   dy window (LO+2) x (LO+2), halo LO on the low side and 1 on the high side.  3x3 (LO = 0):
 //   x(2i,2j)     <- W11 dy[i,j]                      x(2i,2j+1)   <- W10 dy[i,j+1] + W12 dy[i,j]
 //   x(2i+1,2j)   <- W01 dy[i+1,j] + W21 dy[i,j]      x(2i+1,2j+1) <- W00 dy[i+1,j+1] + W02 dy[i+1,j] + W20 dy[i,j+1] + W22 dy[i,j]
 struct PixOut {
@@ -274,24 +290,27 @@ __device__ __forceinline__ void finish_pixel(float2 d, const PixOut& o, float2& 
   if (ok) *reinterpret_cast<uint32_t*>(dst) = pk;
 }
 
-template <int GMODE, int XMODE, int S>
-__global__ void __launch_bounds__(NTB, 1) dw_bwd_kernel(const __grid_constant__ CUtensorMap tmDZ, const __grid_constant__ CUtensorMap tmY2,
-                                                        const __grid_constant__ CUtensorMap tmX, const cvb_dw_bwd_args p, int Ho, int Wo, int TH,
-                                                        int TW, int tiles_w, int g_bytes, int x_bytes) {
+template <int GMODE, int XMODE, int S, int K>
+__global__ void __launch_bounds__(bwd_threads<K>(), 1) dw_bwd_kernel(const __grid_constant__ CUtensorMap tmDZ, const __grid_constant__ CUtensorMap tmY2,
+                                                                     const __grid_constant__ CUtensorMap tmX, const cvb_dw_bwd_args p, int Ho, int Wo,
+                                                                     int TH, int TW, int tiles_w, int g_bytes, int x_bytes) {
   constexpr bool BNB = (GMODE == CVB_A_BNB);
+  constexpr int NTB = bwd_threads<K>();
+  constexpr int P = (K - 1) / 2, LO = P / 2;
+  constexpr int GLO = (S == 1) ? P : LO, GHI = (S == 1) ? P : 1;  // dy halo below / above the tile
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   __shared__ double s_cs[CB], s_cq[CB];  // fp64: the warps' fp32 partials sum exactly, whatever their order
-  __shared__ double s_dw[9][CB];
+  __shared__ double s_dw[K * K][CB];
   __shared__ __align__(16) float s_gp[3 * CB];
   __shared__ __align__(8) uint64_t bar[2], ybar;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int th_i = blockIdx.x / tiles_w, tw_i = blockIdx.x % tiles_w;
   const int oh0 = th_i * TH, ow0 = tw_i * TW;
   const int c0 = blockIdx.y * CB;
-  const int GH = TH + (S == 1 ? 2 : 1), GW = TW + (S == 1 ? 2 : 1);
+  const int GH = TH + GLO + GHI, GW = TW + GLO + GHI;
   const int XH = S * TH, XW = S * TW;  // input tile, no halo
-  const int gh_base = oh0 - (S == 1 ? 1 : 0), gw_base = ow0 - (S == 1 ? 1 : 0);
+  const int gh_base = oh0 - GLO, gw_base = ow0 - GLO;
   const int xh_base = S * oh0, xw_base = S * ow0;
   const int set_bytes = g_bytes + x_bytes;
   uint8_t* sY2 = smem + 2 * set_bytes;
@@ -310,7 +329,7 @@ __global__ void __launch_bounds__(NTB, 1) dw_bwd_kernel(const __grid_constant__ 
     tma_load_4d(sY2, &tmY2, &ybar, c0, gw_base, gh_base, (int)blockIdx.z + i * (int)gridDim.z);
   };
 
-  for (int i = tid; i < 9 * CB; i += NTB) (&s_dw[0][0])[i] = 0.0;
+  for (int i = tid; i < K * K * CB; i += NTB) (&s_dw[0][0])[i] = 0.0;
   if (tid < CB) { s_cs[tid] = 0.0; s_cq[tid] = 0.0; }
   if (tid == 0) {
     mbar_init(&bar[0], 1);
@@ -333,9 +352,9 @@ __global__ void __launch_bounds__(NTB, 1) dw_bwd_kernel(const __grid_constant__ 
   }
   const int cl = c0 + 2 * lane;
   const bool lane_ok = cl < p.C;
-  float2 wv[9], accw[9];
+  float2 wv[K * K], accw[K * K];
 #pragma unroll
-  for (int t = 0; t < 9; ++t) {
+  for (int t = 0; t < K * K; ++t) {
     wv[t] = lane_ok ? make_float2(p.Wt[t * p.C + cl], p.Wt[t * p.C + cl + 1]) : make_float2(0.f, 0.f);
     accw[t] = make_float2(0.f, 0.f);
   }
@@ -401,17 +420,23 @@ __global__ void __launch_bounds__(NTB, 1) dw_bwd_kernel(const __grid_constant__ 
     for (int st = warp; st < n_strips; st += NTB / 32) {
       const int scol = (st % strips_w) * SEG;
       if (S == 1) {
-        const int r0 = (st / strips_w) * 2;  // tile-local input rows r0, r0+1; dy halo rows r0 .. r0+3, halo cols scol .. scol+SEG+1
+        const int r0 = (st / strips_w) * 2;  // tile-local input rows r0, r0+1; dy halo rows r0 .. r0+K, halo cols scol .. scol+SEG+K-2
         bf16* dxrow[2];
 #pragma unroll
         for (int r = 0; r < 2; ++r) dxrow[r] = DX + ((size_t)(oh0 + r0 + r) * p.W + ow0 + scol) * p.C;
-        float2 win[4][3];
+        float2 win[K + 1][K];
 #pragma unroll
-        for (int k = 0; k < 4; ++k) { win[k][1] = lds2(sG, (r0 + k) * GW + scol, lane); win[k][2] = lds2(sG, (r0 + k) * GW + scol + 1, lane); }
+        for (int k = 0; k < K + 1; ++k)
+#pragma unroll
+          for (int c = 1; c < K; ++c) win[k][c] = lds2(sG, (r0 + k) * GW + scol + c - 1, lane);
 #pragma unroll
         for (int x = 0; x < SEG; ++x) {
 #pragma unroll
-          for (int k = 0; k < 4; ++k) { win[k][0] = win[k][1]; win[k][1] = win[k][2]; win[k][2] = lds2(sG, (r0 + k) * GW + scol + x + 2, lane); }
+          for (int k = 0; k < K + 1; ++k) {
+#pragma unroll
+            for (int c = 0; c < K - 1; ++c) win[k][c] = win[k][c + 1];
+            win[k][K - 1] = lds2(sG, (r0 + k) * GW + scol + x + K - 1, lane);
+          }
           const int w = ow0 + scol + x;
 #pragma unroll
           for (int r = 0; r < 2; ++r) {
@@ -419,71 +444,60 @@ __global__ void __launch_bounds__(NTB, 1) dw_bwd_kernel(const __grid_constant__ 
             const bool ok = INTERIOR || ((h < p.H) && (w < p.W) && lane_ok);
             const PixOut o = load_x<XMODE>(sX, (r0 + r) * XW + scol + x, lane, xsc, xsh, ok);
             float2 d = make_float2(0.f, 0.f);
-            // dyn[u][v] = dy[h+1-u][w+1-v] = win[r+2-u][2-v]
+            // dyn[u][v] = dy[h+P-u][w+P-v] = win[r+K-1-u][K-1-v]
 #pragma unroll
-            for (int u = 0; u < 3; ++u)
+            for (int u = 0; u < K; ++u)
 #pragma unroll
-              for (int v = 0; v < 3; ++v) {
-                d = ffma2(wv[u * 3 + v], win[r + 2 - u][2 - v], d);
-                accw[u * 3 + v] = ffma2(o.a, win[r + 2 - u][2 - v], accw[u * 3 + v]);
+              for (int v = 0; v < K; ++v) {
+                d = ffma2(wv[u * K + v], win[r + K - 1 - u][K - 1 - v], d);
+                accw[u * K + v] = ffma2(o.a, win[r + K - 1 - u][K - 1 - v], accw[u * K + v]);
               }
             finish_pixel<XMODE, INTERIOR>(d, o, cs, cq, dxrow[r], ok);
             dxrow[r] += p.C;
           }
         }
       } else {
-        const int i0 = st / strips_w;  // tile-local output row; dy rows i0, i0+1; input rows 2*i0, 2*i0+1
+        constexpr int NW = LO + 2;     // win[k][c] = dy[i - LO + k][j - LO + c]
+        const int i0 = st / strips_w;  // tile-local output row i - oh0; dy tile rows i0 .. i0+LO+1; input rows 2*i0, 2*i0+1
         bf16* dxrow0 = DX + ((size_t)(2 * (oh0 + i0)) * p.W + 2 * (ow0 + scol)) * p.C;
-        float2 win[2][2];
+        float2 win[NW][NW];
 #pragma unroll
-        for (int k = 0; k < 2; ++k) win[k][1] = lds2(sG, (i0 + k) * GW + scol, lane);
+        for (int k = 0; k < NW; ++k)
+#pragma unroll
+          for (int c = 1; c < NW; ++c) win[k][c] = lds2(sG, (i0 + k) * GW + scol + c - 1, lane);
 #pragma unroll
         for (int x = 0; x < SEG; ++x) {
 #pragma unroll
-          for (int k = 0; k < 2; ++k) { win[k][0] = win[k][1]; win[k][1] = lds2(sG, (i0 + k) * GW + scol + x + 1, lane); }
+          for (int k = 0; k < NW; ++k) {
+#pragma unroll
+            for (int c = 0; c < NW - 1; ++c) win[k][c] = win[k][c + 1];
+            win[k][NW - 1] = lds2(sG, (i0 + k) * GW + scol + x + NW - 1, lane);
+          }
           const int hh = 2 * (oh0 + i0), ww = 2 * (ow0 + scol + x);
           const int xp = (2 * i0) * XW + 2 * (scol + x);
           bf16* dx0 = dxrow0 + (size_t)(2 * x) * p.C;
-          bf16* dx1 = dx0 + (size_t)p.W * p.C;
-          const bool ok0 = INTERIOR || hh < p.H, ok1 = INTERIOR || hh + 1 < p.H, okc0 = INTERIOR || ww < p.W, okc1 = INTERIOR || ww + 1 < p.W;
-          {  // (2i, 2j)
-            const bool ok = INTERIOR || (ok0 && okc0 && lane_ok);
-            const PixOut o = load_x<XMODE>(sX, xp, lane, xsc, xsh, ok);
-            float2 d = fmul2(wv[4], win[0][0]);
-            accw[4] = ffma2(o.a, win[0][0], accw[4]);
-            finish_pixel<XMODE, INTERIOR>(d, o, cs, cq, dx0, ok);
-          }
-          {  // (2i, 2j+1)
-            const bool ok = INTERIOR || (ok0 && okc1 && lane_ok);
-            const PixOut o = load_x<XMODE>(sX, xp + 1, lane, xsc, xsh, ok);
-            float2 d = fmul2(wv[3], win[0][1]);
-            d = ffma2(wv[5], win[0][0], d);
-            accw[3] = ffma2(o.a, win[0][1], accw[3]);
-            accw[5] = ffma2(o.a, win[0][0], accw[5]);
-            finish_pixel<XMODE, INTERIOR>(d, o, cs, cq, dx0 + p.C, ok);
-          }
-          {  // (2i+1, 2j)
-            const bool ok = INTERIOR || (ok1 && okc0 && lane_ok);
-            const PixOut o = load_x<XMODE>(sX, xp + XW, lane, xsc, xsh, ok);
-            float2 d = fmul2(wv[1], win[1][0]);
-            d = ffma2(wv[7], win[0][0], d);
-            accw[1] = ffma2(o.a, win[1][0], accw[1]);
-            accw[7] = ffma2(o.a, win[0][0], accw[7]);
-            finish_pixel<XMODE, INTERIOR>(d, o, cs, cq, dx1, ok);
-          }
-          {  // (2i+1, 2j+1)
-            const bool ok = INTERIOR || (ok1 && okc1 && lane_ok);
-            const PixOut o = load_x<XMODE>(sX, xp + XW + 1, lane, xsc, xsh, ok);
-            float2 d = fmul2(wv[0], win[1][1]);
-            d = ffma2(wv[2], win[1][0], d);
-            d = ffma2(wv[6], win[0][1], d);
-            d = ffma2(wv[8], win[0][0], d);
-            accw[0] = ffma2(o.a, win[1][1], accw[0]);
-            accw[2] = ffma2(o.a, win[1][0], accw[2]);
-            accw[6] = ffma2(o.a, win[0][1], accw[6]);
-            accw[8] = ffma2(o.a, win[0][0], accw[8]);
-            finish_pixel<XMODE, INTERIOR>(d, o, cs, cq, dx1 + p.C, ok);
-          }
+#pragma unroll
+          for (int a = 0; a < 2; ++a)
+#pragma unroll
+            for (int b = 0; b < 2; ++b) {  // input pixel (2i+a, 2j+b)
+              const bool ok = INTERIOR || ((hh + a < p.H) && (ww + b < p.W) && lane_ok);
+              const PixOut o = load_x<XMODE>(sX, xp + a * XW + b, lane, xsc, xsh, ok);
+              float2 d = make_float2(0.f, 0.f);
+              bool first = true;  // (resolved at compile time) the first product is a plain multiply
+#pragma unroll
+              for (int u = 0; u < K; ++u) {
+                if ((a + P - u) & 1) continue;
+#pragma unroll
+                for (int v = 0; v < K; ++v) {
+                  if ((b + P - v) & 1) continue;
+                  const float2 g = win[(a + P - u) / 2 + LO][(b + P - v) / 2 + LO];
+                  d = first ? fmul2(wv[u * K + v], g) : ffma2(wv[u * K + v], g, d);
+                  first = false;
+                  accw[u * K + v] = ffma2(o.a, g, accw[u * K + v]);
+                }
+              }
+              finish_pixel<XMODE, INTERIOR>(d, o, cs, cq, dx0 + (size_t)a * p.W * p.C + b * p.C, ok);
+            }
         }
       }
     }
@@ -499,7 +513,7 @@ __global__ void __launch_bounds__(NTB, 1) dw_bwd_kernel(const __grid_constant__ 
   // ---- reductions (once per CTA)
   if (lane_ok) {
 #pragma unroll
-    for (int t = 0; t < 9; ++t) {
+    for (int t = 0; t < K * K; ++t) {
       atomicAdd(&s_dw[t][2 * lane], (double)accw[t].x);
       atomicAdd(&s_dw[t][2 * lane + 1], (double)accw[t].y);
     }
@@ -509,7 +523,7 @@ __global__ void __launch_bounds__(NTB, 1) dw_bwd_kernel(const __grid_constant__ 
     }
   }
   __syncthreads();
-  for (int i = tid; i < 9 * CB; i += NTB) {
+  for (int i = tid; i < K * K * CB; i += NTB) {
     int tp = i / CB, c = i % CB;
     if (c0 + c < p.C) atomicAdd(reinterpret_cast<double*>(p.dWt) + tp * p.C + c0 + c, s_dw[tp][c]);  // fp64 scratch (cvb_dw_bwd)
   }
@@ -535,14 +549,16 @@ extern "C" int cvb_dw_fwd(const cvb_dw_fwd_args* args, cvb_stream_t stream) {
   CVB_CHECK(a.x_mode == CVB_A_RAW || ((a.x_mode == CVB_A_AFF || a.x_mode == CVB_A_AFF_SILU) && a.x_p0 && a.x_p1), "cvb_dw_fwd: bad x_mode %d", a.x_mode);
   if (a.col_sum) CVB_CHECK(a.col_sq != nullptr, "cvb_dw_fwd: col_sq missing");
   CVB_CHECK(a.dilation >= 0 && a.dilation <= 64, "cvb_dw_fwd: bad dilation %d", a.dilation);
+  CVB_CHECK(a.ksize == 0 || a.ksize == 3 || a.ksize == 5, "cvb_dw_fwd: kernel size must be 3 or 5, got %d", a.ksize);
+  CVB_CHECK(a.ksize != 5 || a.dilation <= 1, "cvb_dw_fwd: a dilated 5x5 kernel is not implemented");
   if (a.dilation > 1) return cvb_dw_fwd_dilated(a, static_cast<cudaStream_t>(stream));
-  const int s = a.stride;
+  const int s = a.stride, K = a.ksize == 5 ? 5 : 3;
   const int Ho = (a.H - 1) / s + 1, Wo = (a.W - 1) / s + 1;
-  // two CTAs per SM: two input buffers of <= ~42 KB each
+  // two CTAs per SM: two input buffers of <= ~46 KB each (5x5, stride 1: 8-row tiles keep the 20-column halo'd tile inside that)
   const int TW = (s == 1 && Wo > 8) ? 16 : 8;
-  const int TH = (s == 1) ? (Ho > 8 ? 16 : 8) : 8;
+  const int TH = (s == 1 && K == 3) ? (Ho > 8 ? 16 : 8) : 8;
   const int tiles_h = (Ho + TH - 1) / TH, tiles_w = (Wo + TW - 1) / TW;
-  const int IH = (TH - 1) * s + 3, IW = (TW - 1) * s + 3;
+  const int IH = (TH - 1) * s + K, IW = (TW - 1) * s + K;
   const int buf_bytes = round1k(IH * IW * 128);
   size_t smem = (size_t)2 * buf_bytes + 1024;
   const int cblocks = (a.C + CB - 1) / CB;
@@ -554,21 +570,24 @@ extern "C" int cvb_dw_fwd(const cvb_dw_fwd_args* args, cvb_stream_t stream) {
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   CUtensorMap tmX;
   if (cvb_make_tmap_nhwc(&tmX, a.X, a.B, a.H, a.W, a.C, IH, IW, CB, 0)) return 1;
-#define CVB_DW_FWD(MODE, S)                                                                                               \
+#define CVB_DW_FWD(MODE, S, KS)                                                                                          \
   {                                                                                                                      \
     static bool attr = false;                                                                                            \
-    if (!attr) { CVB_CUDA(cudaFuncSetAttribute(dw_fwd_kernel<MODE, S>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024)); attr = true; } \
-    CVB_CUDA(cvb_launch(dw_fwd_kernel<MODE, S>, grid, NT, smem, st, tmX, a, Ho, Wo, TH, TW, tiles_w, buf_bytes));         \
+    if (!attr) { CVB_CUDA(cudaFuncSetAttribute(dw_fwd_kernel<MODE, S, KS>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024)); attr = true; } \
+    CVB_CUDA(cvb_launch(dw_fwd_kernel<MODE, S, KS>, grid, NT, smem, st, tmX, a, Ho, Wo, TH, TW, tiles_w, buf_bytes));     \
   }
-  if (s == 1) {
-    if (a.x_mode == CVB_A_RAW) CVB_DW_FWD(CVB_A_RAW, 1)
-    else if (a.x_mode == CVB_A_AFF) CVB_DW_FWD(CVB_A_AFF, 1)
-    else CVB_DW_FWD(CVB_A_AFF_SILU, 1)
+#define CVB_DW_FWD_X(S, KS)                                                  \
+  {                                                                          \
+    if (a.x_mode == CVB_A_RAW) CVB_DW_FWD(CVB_A_RAW, S, KS)                  \
+    else if (a.x_mode == CVB_A_AFF) CVB_DW_FWD(CVB_A_AFF, S, KS)             \
+    else CVB_DW_FWD(CVB_A_AFF_SILU, S, KS)                                   \
+  }
+  if (K == 3) {
+    if (s == 1) CVB_DW_FWD_X(1, 3) else CVB_DW_FWD_X(2, 3)
   } else {
-    if (a.x_mode == CVB_A_RAW) CVB_DW_FWD(CVB_A_RAW, 2)
-    else if (a.x_mode == CVB_A_AFF) CVB_DW_FWD(CVB_A_AFF, 2)
-    else CVB_DW_FWD(CVB_A_AFF_SILU, 2)
+    if (s == 1) CVB_DW_FWD_X(1, 5) else CVB_DW_FWD_X(2, 5)
   }
+#undef CVB_DW_FWD_X
 #undef CVB_DW_FWD
   CVB_LAUNCH_CHECK();
   return 0;
@@ -584,6 +603,8 @@ extern "C" int cvb_dw_bwd(const cvb_dw_bwd_args* args, cvb_stream_t stream) {
   CVB_CHECK(a.x_mode == CVB_A_RAW || ((a.x_mode == CVB_A_AFF || a.x_mode == CVB_A_AFF_SILU) && a.x_p0 && a.x_p1), "cvb_dw_bwd: bad x_mode %d", a.x_mode);
   if (a.col_sum) CVB_CHECK(a.col_sq != nullptr, "cvb_dw_bwd: col_sq missing");
   CVB_CHECK(a.dilation >= 0 && a.dilation <= 64, "cvb_dw_bwd: bad dilation %d", a.dilation);
+  CVB_CHECK(a.ksize == 0 || a.ksize == 3 || a.ksize == 5, "cvb_dw_bwd: kernel size must be 3 or 5, got %d", a.ksize);
+  CVB_CHECK(a.ksize != 5 || a.dilation <= 1, "cvb_dw_bwd: a dilated 5x5 kernel is not implemented");
   if (a.dilation > 1) {
     // the dilated kernel's per-block dW partials meet in the same fp64 scratch as the walk kernels' (order-independent, so reproducible)
     cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -597,13 +618,15 @@ extern "C" int cvb_dw_bwd(const cvb_dw_bwd_args* args, cvb_stream_t stream) {
     return rc ? rc : rf;
   }
   if (a.stride == 2) CVB_CHECK(a.H % 2 == 0 && a.W % 2 == 0, "cvb_dw_bwd: stride 2 needs even H, W");
-  const int s = a.stride;
+  const int s = a.stride, K = a.ksize == 5 ? 5 : 3;
   const int Ho = (a.H - 1) / s + 1, Wo = (a.W - 1) / s + 1;
-  // one CTA per SM; stride 1: 16 x 16 input pixels, stride 2: 8 x 16 outputs = 16 x 32 input pixels (small maps: 8-wide tiles)
+  // one CTA per SM; stride 1: 16 x 16 input pixels (5x5: 8 x 16, the 4-pixel halo and the 25-tap dW scratch must fit next to the
+  // double buffers), stride 2: 8 x 16 outputs = 16 x 32 input pixels (small maps: 8-wide tiles)
   const int TW = Wo > 8 ? 16 : 8;
-  const int TH = (s == 1) ? (Ho > 8 ? 16 : 8) : 8;
+  const int TH = (s == 1 && K == 3) ? (Ho > 8 ? 16 : 8) : 8;
   const int tiles_h = (Ho + TH - 1) / TH, tiles_w = (Wo + TW - 1) / TW;
-  const int GH = TH + (s == 1 ? 2 : 1), GW = TW + (s == 1 ? 2 : 1);
+  const int P = (K - 1) / 2, halo = (s == 1) ? 2 * P : P / 2 + 1;
+  const int GH = TH + halo, GW = TW + halo;
   const int XH = s * TH, XW = s * TW;
   const int g_bytes = round1k(GH * GW * 128), x_bytes = round1k(XH * XW * 128);
   const bool bnb = (a.g_mode == CVB_A_BNB);
@@ -623,29 +646,35 @@ extern "C" int cvb_dw_bwd(const cvb_dw_bwd_args* args, cvb_stream_t stream) {
   if (cvb_make_tmap_nhwc(&tmX, a.X, a.B, a.H, a.W, a.C, XH, XW, CB, 0)) return 1;
   // the CTAs' dW partials meet in an fp64 scratch (order-independent), added to dWt afterwards
   double* ws = nullptr;
-  if (cvb_det_alloc(&ws, (size_t)9 * a.C, st)) return 2;
+  if (cvb_det_alloc(&ws, (size_t)K * K * a.C, st)) return 2;
   cvb_dw_bwd_args b = a;
   b.dWt = reinterpret_cast<float*>(ws);
-#define CVB_DW_BWD(GM, XM, S)                                                                                             \
+#define CVB_DW_BWD(GM, XM, S, KS)                                                                                        \
   {                                                                                                                      \
     static bool attr = false;                                                                                            \
-    if (!attr) { CVB_CUDA(cudaFuncSetAttribute(dw_bwd_kernel<GM, XM, S>, cudaFuncAttributeMaxDynamicSharedMemorySize, 216 * 1024)); attr = true; } \
-    CVB_CUDA(cvb_launch(dw_bwd_kernel<GM, XM, S>, grid, NTB, smem, st, tmDZ, tmY2, tmX, b, Ho, Wo, TH, TW, tiles_w, g_bytes, x_bytes));   \
+    if (!attr) { CVB_CUDA(cudaFuncSetAttribute(dw_bwd_kernel<GM, XM, S, KS>, cudaFuncAttributeMaxDynamicSharedMemorySize, bwd_smem_cap<KS>())); attr = true; } \
+    CVB_CUDA(cvb_launch(dw_bwd_kernel<GM, XM, S, KS>, grid, bwd_threads<KS>(), smem, st, tmDZ, tmY2, tmX, b, Ho, Wo, TH, TW, tiles_w, g_bytes,   \
+                        x_bytes));                                                                                       \
   }
-#define CVB_DW_BWD_X(GM, S)                                                   \
+#define CVB_DW_BWD_X(GM, S, KS)                                               \
   {                                                                          \
-    if (a.x_mode == CVB_A_RAW) CVB_DW_BWD(GM, CVB_A_RAW, S)                   \
-    else if (a.x_mode == CVB_A_AFF) CVB_DW_BWD(GM, CVB_A_AFF, S)              \
-    else CVB_DW_BWD(GM, CVB_A_AFF_SILU, S)                                    \
+    if (a.x_mode == CVB_A_RAW) CVB_DW_BWD(GM, CVB_A_RAW, S, KS)               \
+    else if (a.x_mode == CVB_A_AFF) CVB_DW_BWD(GM, CVB_A_AFF, S, KS)          \
+    else CVB_DW_BWD(GM, CVB_A_AFF_SILU, S, KS)                                \
   }
-  if (!bnb) {
-    if (s == 1) CVB_DW_BWD_X(CVB_A_RAW, 1) else CVB_DW_BWD_X(CVB_A_RAW, 2)
+#define CVB_DW_BWD_S(GM, KS)                                                  \
+  {                                                                          \
+    if (s == 1) CVB_DW_BWD_X(GM, 1, KS) else CVB_DW_BWD_X(GM, 2, KS)          \
+  }
+  if (K == 3) {
+    if (!bnb) CVB_DW_BWD_S(CVB_A_RAW, 3) else CVB_DW_BWD_S(CVB_A_BNB, 3)
   } else {
-    if (s == 1) CVB_DW_BWD_X(CVB_A_BNB, 1) else CVB_DW_BWD_X(CVB_A_BNB, 2)
+    if (!bnb) CVB_DW_BWD_S(CVB_A_RAW, 5) else CVB_DW_BWD_S(CVB_A_BNB, 5)
   }
+#undef CVB_DW_BWD_S
 #undef CVB_DW_BWD_X
 #undef CVB_DW_BWD
   CVB_LAUNCH_CHECK();
-  if (cvb_det_add(ws, a.dWt, 9, a.C, a.C, st)) return 2;
+  if (cvb_det_add(ws, a.dWt, K * K, a.C, a.C, st)) return 2;
   return cvb_det_free(ws, st);
 }

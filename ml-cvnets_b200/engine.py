@@ -2,7 +2,7 @@
 
     forward -> cross entropy (label smoothing) -> backward (weight gradients written straight into a flat buffer)
             -> [data parallel: bucketed all-reduce of that buffer over NCCL, overlapped with the rest of the backward]
-            -> GradScaler unscale + inf check + clip_grad_norm_ + AdamW (+ EMA) + GradScaler update   (two launches)
+            -> GradScaler unscale + inf check + clip_grad_norm_ + AdamW or SGD (+ EMA) + GradScaler update   (two launches)
 
 ``TrainStep`` is host code only -- every kernel it launches is one of the library's (include/cvnets_b200.h); there is no ATen kernel
 inside the step (zero-fills are memset nodes, the loss is cvb_ce_*).  Semantics follow the reference: per-GPU BatchNorm statistics
@@ -26,7 +26,7 @@ import torch
 
 from . import functional as Fn
 from . import ops
-from .optim import FlatAdamW
+from .optim import FlatAdamW, FlatSGD
 from .workspace import StepWorkspace
 
 
@@ -45,14 +45,22 @@ class TrainStep:
                  no_decay_bn_filter_bias: bool = True, max_norm: float = 10.0, label_smoothing: float = 0.1, ignore_index: int = -1,
                  ema_momentum: Optional[float] = None, init_scale: float = 65536.0, growth_interval: int = 2000,
                  process_group=None, data_parallel: Optional[bool] = None, n_buckets: int = 3, broadcast_buffers: bool = True,
-                 forward_loss=None):
+                 forward_loss=None, optimizer: str = "adamw", momentum: float = 0.9, nesterov: bool = True):
         """``forward_loss(model, *inputs, cfg) -> loss`` replaces the default ``cross_entropy(model(x), y)`` (e.g. CLIP's contrastive step);
-        ``cfg.scale`` is the device-resident loss scale the loss's backward must multiply by, ``cfg.world / rank / group`` the process group."""
+        ``cfg.scale`` is the device-resident loss scale the loss's backward must multiply by, ``cfg.world / rank / group`` the process group.
+        ``optimizer="sgd"`` swaps AdamW for SGD with ``momentum`` / ``nesterov`` (optim.FlatSGD; ``betas`` / ``eps`` are then unused and
+        ``max_norm`` None / 0 means no clipping)."""
         import torch.distributed as dist
+        if optimizer not in ("adamw", "sgd"):
+            raise ValueError(f"optimizer must be 'adamw' or 'sgd', got {optimizer!r}")
         self.model = model
         self.ws = StepWorkspace(model)
-        self.opt = FlatAdamW(model, self.ws, lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, no_decay_bn_filter_bias=no_decay_bn_filter_bias,
-                             max_norm=max_norm, init_scale=init_scale, growth_interval=growth_interval, ema_momentum=ema_momentum)
+        common = dict(lr=lr, weight_decay=weight_decay, no_decay_bn_filter_bias=no_decay_bn_filter_bias, max_norm=max_norm, init_scale=init_scale,
+                      growth_interval=growth_interval, ema_momentum=ema_momentum)
+        if optimizer == "adamw":
+            self.opt = FlatAdamW(model, self.ws, betas=betas, eps=eps, **common)
+        else:
+            self.opt = FlatSGD(model, self.ws, momentum=momentum, nesterov=nesterov, **common)
         if data_parallel is None:
             data_parallel = dist.is_available() and dist.is_initialized() and dist.get_world_size(process_group) > 1
         self.world = 1

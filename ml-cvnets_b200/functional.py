@@ -606,7 +606,7 @@ class PointwiseConvFn(torch.autograd.Function):
 
 
 class DepthwiseConvFn(torch.autograd.Function):
-    """ConvLayer2d with a depthwise 3x3 kernel (groups = channels, stride 1 | 2, no bias) [-> BatchNorm2d] [-> Swish]."""
+    """ConvLayer2d with a depthwise 3x3 or 5x5 kernel (groups = channels, stride 1 | 2, no bias) [-> BatchNorm2d] [-> Swish]."""
 
     @staticmethod
     def forward(ctx, x, cfg, w, gamma, beta):
@@ -617,12 +617,13 @@ class DepthwiseConvFn(torch.autograd.Function):
         x2 = as_2d(x)
         if cfg.bn is not None:
             st = _fwd_arena(cfg, x.device, 2 * C + 8).f64(2, C)
-            y = ops.dw_fwd(x2, B, H, W, C, s, cfg.prep.get(cfg.i_w), col_stats=st if cfg.bn.batch_stats else None, dilation=cfg.dilation)
+            y = ops.dw_fwd(x2, B, H, W, C, s, cfg.prep.get(cfg.i_w), col_stats=st if cfg.bn.batch_stats else None, dilation=cfg.dilation,
+                           ksize=cfg.k)
             bn = _bn_forward(st, M2, gamma, beta, cfg.bn)
             out = ops.bn_apply(y, bn, act=cfg.act is not None)
             ctx.saved, ctx.ev = (x2, y, bn), (not cfg.bn.batch_stats,)
         else:
-            y = ops.dw_fwd(x2, B, H, W, C, s, cfg.prep.get(cfg.i_w), dilation=cfg.dilation)
+            y = ops.dw_fwd(x2, B, H, W, C, s, cfg.prep.get(cfg.i_w), dilation=cfg.dilation, ksize=cfg.k)
             out = ops.act_fwd(y, cfg.act) if cfg.act is not None else y
             ctx.saved = (x2, y)
         ctx.cfg, ctx.dims, ctx.plist = cfg, (B, C, H, W, Ho, Wo), cfg.plist
@@ -635,7 +636,8 @@ class DepthwiseConvFn(torch.autograd.Function):
         B, C, H, W, Ho, Wo = ctx.dims
         M2 = B * Ho * Wo
         dout = as_2d(to_bf16_cl(gout))
-        D = _Dst(cfg, ctx.plist, dout.device, 9 * C + 64, 2 * C + 16, True)
+        taps = cfg.k * cfg.k
+        D = _Dst(cfg, ctx.plist, dout.device, taps * C + 64, 2 * C + 16, True)
         if cfg.bn is not None:
             x2, y, bn = ctx.saved
             (gamma,) = ctx.saved_tensors
@@ -646,13 +648,14 @@ class DepthwiseConvFn(torch.autograd.Function):
                 dz = dout
             dgb, c = ops.bn_bwd_finalize(sd, M2, gamma, bn, ctx.ev[0], out=D.pair(1, 2))
             D.set_pair(1, 2, dgb)
-            dx, dWt = ops.dw_bwd(dz, x2, B, H, W, C, cfg.stride, cfg.prep.get(cfg.i_w), g_mode=A_BNB, Y2=y, g_p=c, dWt=D.ar.f32(9, C),
-                                 dilation=cfg.dilation)
+            dx, dWt = ops.dw_bwd(dz, x2, B, H, W, C, cfg.stride, cfg.prep.get(cfg.i_w), g_mode=A_BNB, Y2=y, g_p=c, dWt=D.ar.f32(taps, C),
+                                 dilation=cfg.dilation, ksize=cfg.k)
         else:
             x2, y = ctx.saved
             dz = ops.act_bwd(dout, y, cfg.act) if cfg.act is not None else dout
-            dx, dWt = ops.dw_bwd(dz, x2, B, H, W, C, cfg.stride, cfg.prep.get(cfg.i_w), dWt=D.ar.f32(9, C), dilation=cfg.dilation)
-        D.unprep(0, dWt, C, 9, C, 2)
+            dx, dWt = ops.dw_bwd(dz, x2, B, H, W, C, cfg.stride, cfg.prep.get(cfg.i_w), dWt=D.ar.f32(taps, C), dilation=cfg.dilation,
+                                 ksize=cfg.k)
+        D.unprep(0, dWt, C, taps, C, 2)
         grads = D.finish()
         return (to_4d(dx, B, H, W), None, grads[0]) + ((grads[1], grads[2]) if cfg.bn is not None else (None, None))
 
@@ -882,6 +885,24 @@ class DropoutFn(torch.autograd.Function):
         if g.dtype != BF16 or not g.is_contiguous():
             g = g.to(BF16).contiguous()
         return ops.dropout_bwd(g, ctx.p, ctx.key).view(ctx.shape), None
+
+
+class StochasticDepthAddFn(torch.autograd.Function):
+    """``x + StochasticDepth(p, "row")(y)`` on [B, C, H, W] maps (cvnets/modules/efficientnet.py): one hashed per-sample keep factor
+    (0 or 1 / (1 - p)), drawn from a device-resident key and regenerated -- not stored -- in the backward."""
+
+    @staticmethod
+    def forward(ctx, y, x, p):
+        B, C, H, W = y.shape
+        key = ops.rng_next(y.device)
+        ctx.p, ctx.key, ctx.dims = p, key, (B, H, W)
+        return to_4d(ops.dropout_fwd(as_2d(y), as_2d(x), 0.0, key, p_row=p, rows_per_sample=H * W), B, H, W)
+
+    @staticmethod
+    def backward(ctx, gout):
+        B, H, W = ctx.dims
+        g = as_2d(to_bf16_cl(gout))
+        return to_4d(ops.dropout_bwd(g, 0.0, ctx.key, p_row=ctx.p, rows_per_sample=H * W), B, H, W), gout, None
 
 
 class SeScaleFn(torch.autograd.Function):

@@ -88,6 +88,15 @@ class Swish(nn.SiLU):
     def __init__(self, inplace: Optional[bool] = False, *args, **kwargs) -> None:
         super().__init__(inplace=inplace)
 
+    def forward(self, x: Tensor) -> Tensor:
+        """Stand-alone use on a CUDA tensor (the activations of InvertedResidualSE / EfficientNetBlock) is one pass of cvb_act_fwd (bf16 out);
+        inside the fused blocks the module is only a marker."""
+        if not x.is_cuda:
+            return super().forward(x)
+        from . import functional as Fn
+        from . import ops
+        return Fn.ActFn.apply(Fn.to_bf16_cl(x) if x.dim() == 4 else x.to(torch.bfloat16).contiguous(), ops.ACT_SILU)
+
 
 class BatchNorm2d(nn.BatchNorm2d):
     """cvnets/layers/normalization/batch_norm.py:14-49."""
@@ -288,7 +297,7 @@ class ConvLayer2d(BaseLayer):
 
     def forward(self, x: Tensor, residual: Optional[Tensor] = None) -> Tensor:
         """Stand-alone use: the MobileViT stem pattern (3 -> C0, 3x3, stride 2, BN, Swish), any 1x1 conv (+bias) [+BatchNorm] [+Swish/GELU]
-        and the depthwise 3x3 conv [+BatchNorm] [+Swish].  ``residual`` (1x1 only, extension) is added in the GEMM epilogue."""
+        and the depthwise 3x3 / 5x5 conv [+BatchNorm] [+Swish].  ``residual`` (1x1 only, extension) is added in the GEMM epilogue."""
         from types import SimpleNamespace
         from . import functional as Fn
         from . import ops
@@ -311,14 +320,16 @@ class ConvLayer2d(BaseLayer):
         pointwise = (self.groups == 1 and self.dilation == (1, 1) and self.kernel_size[0] == self.kernel_size[1] and self.stride[0] == self.stride[1]
                      and pad is not None and pad[0] == pad[1] and (self.in_channels % 8 == 0 or self.kernel_size[0] > 1))
         dil = self.dilation[0]
-        depthwise = (self.kernel_size == (3, 3) and self.groups == self.in_channels == self.out_channels and self.dilation[0] == self.dilation[1]
-                     and self.stride in ((1, 1), (2, 2)) and (dil == 1 or self.stride == (1, 1)) and conv.bias is None
-                     and tuple(conv.padding) == (dil, dil))
+        # depthwise 3x3 (dilated: stride 1) and undilated 5x5 (EfficientNet)
+        dw_pad = (self.kernel_size[0] - 1) // 2 * dil
+        depthwise = (self.kernel_size in ((3, 3), (5, 5)) and self.groups == self.in_channels == self.out_channels
+                     and self.dilation[0] == self.dilation[1] and self.stride in ((1, 1), (2, 2)) and (dil == 1 or self.stride == (1, 1))
+                     and (dil == 1 or self.kernel_size == (3, 3)) and conv.bias is None and tuple(conv.padding) == (dw_pad, dw_pad))
         if depthwise:
             pointwise = False
         if not (pointwise or depthwise) or self.out_channels % 8 or (depthwise and self.in_channels % 8):
             raise NotImplementedError("stand-alone ConvLayer2d: undilated groups=1 convs with square kernels (out_channels % 8 == 0; in_channels % 8 == 0 "
-                                      "for 1x1) and depthwise 3x3 convs (dilated: stride 1) have kernel paths")
+                                      "for 1x1), depthwise 3x3 convs (dilated: stride 1) and undilated depthwise 5x5 convs have kernel paths")
         if self._stem is None:
             prep = PW()
             k = self.kernel_size[0]

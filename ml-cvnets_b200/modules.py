@@ -167,7 +167,7 @@ class InvertedResidualSE(BaseModule):
     """cvnets/modules/mobilenetv2.py:16-138 (MobileNetv3-style block; SURVEY.md 8f row 4): exp_1x1 (1x1 + BN) -> act -> conv_3x3 (depthwise + BN)
     -> act -> [SqueezeExcitation] -> red_1x1 (1x1 + BN), residual iff stride 1 and Cin == Cout.  Same constructor, child tree and state_dict
     keys (``block.{exp_1x1, act_fn_1, conv_3x3, act_fn_2, se, red_1x1}``; the two act children are ONE module object, as in the reference).
-    Composition of the stand-alone layer kernels; the residual add rides the red_1x1 BatchNorm-apply pass.  Depthwise kernel size 3."""
+    Composition of the stand-alone layer kernels; the residual add rides the red_1x1 BatchNorm-apply pass.  Depthwise kernel size 3 or 5."""
 
     def __init__(self, opts, in_channels: int, out_channels: int, expand_ratio: Union[int, float], dilation: Optional[int] = 1,
                  stride: Optional[int] = 1, use_se: Optional[bool] = False, act_fn_name: Optional[str] = "relu",
@@ -193,8 +193,6 @@ class InvertedResidualSE(BaseModule):
 
     def forward(self, x: Tensor, *args, **kwargs) -> Tensor:
         _require_cuda(x, "InvertedResidualSE")
-        if self.kernel_size != 3:
-            raise NotImplementedError("InvertedResidualSE: depthwise kernel size 3 has a kernel path (5x5 is not implemented)")
         x = Fn.to_bf16_cl(x)
         y = x
         for name, m in self.block._modules.items():  # (named_children() would de-duplicate the shared activation module)
@@ -208,6 +206,32 @@ class InvertedResidualSE(BaseModule):
         return "{}(in_channels={}, out_channels={}, stride={}, exp={}, dilation={}, use_se={}, kernel_size={}, act_fn={})".format(
             self.__class__.__name__, self.in_channels, self.out_channels, self.stride, self.exp, self.dilation, self.use_se, self.kernel_size,
             self.act_fn_name)
+
+
+class EfficientNetBlock(InvertedResidualSE):
+    """cvnets/modules/efficientnet.py: InvertedResidualSE plus a row-mode ``stochastic_depth`` child (torchvision.ops.StochasticDepth) on the
+    block output before the residual add.  Same constructor (``stochastic_depth_prob`` first) and state_dict.  In training with p > 0 the
+    residual add and the per-sample mask run as one pass of the hashed-mask kernel (cvb_dropout_fwd with p_row = p, one sample = Ho*Wo rows)
+    keyed from the device generator, so a captured step draws fresh masks on every replay; otherwise (eval, p = 0) the add rides red_1x1's
+    BatchNorm-apply pass as in InvertedResidualSE."""
+
+    def __init__(self, stochastic_depth_prob: float, *args, **kwargs) -> None:
+        super().__init__(*args, **kwargs)
+        self.stochastic_depth = StochasticDepth(p=stochastic_depth_prob, mode="row")
+
+    def forward(self, x: Tensor, *args, **kwargs) -> Tensor:
+        p = float(self.stochastic_depth.p)
+        if not (self.use_res_connect and self.training and p > 0.0):
+            return super().forward(x)
+        _require_cuda(x, "EfficientNetBlock")
+        x = Fn.to_bf16_cl(x)
+        y = x
+        for m in self.block._modules.values():
+            y = m(y)
+        return Fn.StochasticDepthAddFn.apply(y, x, p)
+
+    def __repr__(self) -> str:
+        return super().__repr__()[:-1] + f", stochastic_depth_prob={self.stochastic_depth.p})"
 
 
 # -------------------------------------------------------------------------------------------------------- LinearAttnFFN

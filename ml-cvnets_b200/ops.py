@@ -207,14 +207,15 @@ def pw_wgrad(G: Tensor, A: Tensor, N: int, K: int, *, g_mode: int = A_RAW, G2: O
 
 # ---------------------------------------------------------------------------------------------------------- depthwise
 def dw_fwd(X: Tensor, B: int, H: int, W: int, C: int, stride: int, Wt: Tensor, *, x_mode: int = A_RAW,
-           x_p: Sequence[Optional[Tensor]] = (None, None), col_stats: Optional[Tensor] = None, dilation: int = 1) -> Tensor:
+           x_p: Sequence[Optional[Tensor]] = (None, None), col_stats: Optional[Tensor] = None, dilation: int = 1, ksize: int = 3) -> Tensor:
+    """Depthwise ksize x ksize conv (ksize 3 or 5, pad (ksize-1)/2 * dilation); ``Wt`` is tap-major fp32 [ksize*ksize, C]."""
     lib = _lib()
     Ho, Wo = (H - 1) // stride + 1, (W - 1) // stride + 1
     Y = torch.empty((B * Ho * Wo, C), device=X.device, dtype=torch.bfloat16)
     a = L.DwFwdArgs()
     a.B, a.H, a.W, a.C, a.stride = B, H, W, C, stride
     a.X, a.x_mode, a.x_p0, a.x_p1 = X.data_ptr(), x_mode, _p(x_p[0]), _p(x_p[1])
-    a.Wt, a.Y, a.dilation = Wt.data_ptr(), Y.data_ptr(), int(dilation)
+    a.Wt, a.Y, a.dilation, a.ksize = Wt.data_ptr(), Y.data_ptr(), int(dilation), int(ksize)
     if col_stats is not None:
         a.col_sum, a.col_sq = col_stats[0].data_ptr(), col_stats[1].data_ptr()
     L.check(lib.cvb_dw_fwd(ctypes.byref(a), _stream()), "cvb_dw_fwd")
@@ -225,18 +226,18 @@ def dw_fwd(X: Tensor, B: int, H: int, W: int, C: int, stride: int, Wt: Tensor, *
 def dw_bwd(DZ: Tensor, X: Tensor, B: int, H: int, W: int, C: int, stride: int, Wt: Tensor, *, g_mode: int = A_RAW,
            Y2: Optional[Tensor] = None, g_p: Sequence[Optional[Tensor]] = (None, None, None), x_mode: int = A_RAW,
            x_p: Sequence[Optional[Tensor]] = (None, None), col_stats: Optional[Tensor] = None,
-           dWt: Optional[Tensor] = None, dilation: int = 1) -> Tuple[Tensor, Tensor]:
-    """Returns (DX bf16 [B*H*W, C], dWt fp32 [9, C]); ``dWt`` if given must be zero-initialised (it is accumulated into)."""
+           dWt: Optional[Tensor] = None, dilation: int = 1, ksize: int = 3) -> Tuple[Tensor, Tensor]:
+    """Returns (DX bf16 [B*H*W, C], dWt fp32 [ksize*ksize, C]); ``dWt`` if given must be zero-initialised (it is accumulated into)."""
     lib = _lib()
     DX = torch.empty((B * H * W, C), device=X.device, dtype=torch.bfloat16)
     if dWt is None:
-        dWt = torch.zeros((9, C), device=X.device, dtype=torch.float32)
+        dWt = torch.zeros((ksize * ksize, C), device=X.device, dtype=torch.float32)
     a = L.DwBwdArgs()
     a.B, a.H, a.W, a.C, a.stride = B, H, W, C, stride
     a.DZ, a.Y2, a.g_mode = DZ.data_ptr(), _p(Y2), g_mode
     a.g_p0, a.g_p1, a.g_p2 = _p(g_p[0]), _p(g_p[1]), _p(g_p[2])
     a.X, a.x_mode, a.x_p0, a.x_p1 = X.data_ptr(), x_mode, _p(x_p[0]), _p(x_p[1])
-    a.Wt, a.DX, a.dWt, a.dilation = Wt.data_ptr(), DX.data_ptr(), dWt.data_ptr(), int(dilation)
+    a.Wt, a.DX, a.dWt, a.dilation, a.ksize = Wt.data_ptr(), DX.data_ptr(), dWt.data_ptr(), int(dilation), int(ksize)
     if col_stats is not None:
         a.col_sum, a.col_sq = col_stats[0].data_ptr(), col_stats[1].data_ptr()
     L.check(lib.cvb_dw_bwd(ctypes.byref(a), _stream()), "cvb_dw_bwd")

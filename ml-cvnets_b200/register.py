@@ -18,6 +18,7 @@ def rebind_modules() -> None:
     from . import modules as ours
     cm.InvertedResidual = ours.InvertedResidual
     cm.InvertedResidualSE = ours.InvertedResidualSE  # mobilenetv3.py / efficientnet.py import it from cvnets.modules
+    cm.EfficientNetBlock = ours.EfficientNetBlock  # models/classification/efficientnet.py
     cm.SqueezeExcitation = ours.SqueezeExcitation
     cm.MobileViTBlockv2 = ours.MobileViTBlockv2
     cm.TransformerEncoder = ours.TransformerEncoder  # used by vit.py:29, mobilevit_block.py (v1), text_encoders/transformer.py:20
@@ -55,16 +56,17 @@ def _make_shell(ours_cls, base_cls, shell_name: str):
 
 
 def register_with_cvnets(name: str = "mobilevit_v2_b200"):
-    """Injection point 2: register this package's assemblers under new model names: ``mobilevit_v2_b200`` (or ``name``), ``mobilevit_b200``, ``vit_b200``.
-    Returns the MobileViTv2 shell class."""
+    """Injection point 2: register this package's assemblers under new model names: ``mobilevit_v2_b200`` (or ``name``), ``mobilevit_b200``, ``vit_b200``,
+    ``efficientnet_b200``.  Returns the MobileViTv2 shell class."""
     from cvnets.models import MODEL_REGISTRY
     from cvnets.models.classification.base_image_encoder import BaseImageEncoder
     from .models import MobileViTv2
+    from .models_effnet import EfficientNet
     from .models_mit import MobileViT
     from .models_vit import VisionTransformer
 
     out = None
-    for reg_name, cls in ((name, MobileViTv2), ("mobilevit_b200", MobileViT), ("vit_b200", VisionTransformer)):
+    for reg_name, cls in ((name, MobileViTv2), ("mobilevit_b200", MobileViT), ("vit_b200", VisionTransformer), ("efficientnet_b200", EfficientNet)):
         key = f"classification:{reg_name}"
         registry = getattr(MODEL_REGISTRY, "registry", {})
         if key in registry:
