@@ -273,8 +273,9 @@ CVB_API int cvb_act_fwd(const void* X, void* Y, int64_t n, int kind, cvb_stream_
 CVB_API int cvb_act_bwd(const void* DY, const void* X, void* DX, int64_t n, int kind, cvb_stream_t stream);
 CVB_API int cvb_ln_stats(const void* X, int ldx, int64_t M, int C, float eps, float* mean, float* rstd, cvb_stream_t stream);
 /* Squeeze-excitation channel scaling (cvnets/modules/squeeze_excitation.py:82-83, used by InvertedResidualSE, cvnets/modules/mobilenetv2.py:16-138):
- * Y[b,p,c] = X[b,p,c] * S[b,c] on a channels-last bf16 map [B, HW, C] with the bf16 scale vector S [B, C] (C % 8 == 0, C <= 2048);
- * backward: DX = DY * S and DS[b,c] += sum_p DY * X (fp32, zero-initialised by the caller). */
+ * Y[b,p,c] = X[b,p,c] * S[b,c] on a channels-last bf16 map [B, HW, C] with the bf16 scale vector S [B, C] (C % 8 == 0);
+ * backward: DX = DY * S and DS[b,c] += sum_p DY * X (fp32, zero-initialised by the caller; the partial sums meet in an fp64 scratch, so DS
+ * is the same bits run to run). */
 CVB_API int cvb_se_scale_fwd(const void* X, const void* S, void* Y, int B, int HW, int C, cvb_stream_t stream);
 CVB_API int cvb_se_scale_bwd(const void* DY, const void* X, const void* S, void* DX, float* DS, int B, int HW, int C, cvb_stream_t stream);
 /* Dropout (cvnets/layers/dropout.py == nn.Dropout) and stochastic depth (torchvision.ops.StochasticDepth(mode="row"), cvnets/modules/transformer.py:97-100)

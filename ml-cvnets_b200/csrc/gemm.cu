@@ -452,8 +452,7 @@ int dispatch_tile(const cvb_gemm_args& a, cudaStream_t st) {
   if (rc == -1 && want128) rc = launch_gemm<64, AMODE, EPI>(a, st, false);
   if (rc == -1 && N > 32) rc = launch_gemm<32, AMODE, EPI>(a, st, false);
   if (rc == -1) rc = launch_gemm<16, AMODE, EPI>(a, st, false);
-  CVB_CHECK(rc != -1, "cvb_pw_gemm: K=%d is too large for the resident weight panel", a.K);
-  return rc;
+  return rc;  // -1: K is too large for the resident weight panel of every N tile
 }
 
 // the (prologue, epilogue) combinations the hot path uses (functional.py) plus STORE / STORE_R for every prologue
@@ -689,7 +688,7 @@ int dispatch_wgrad_a(const cvb_wgrad_args& a, cudaStream_t st) {
 }  // namespace
 
 int cvb_pw_wgrad_tc(const cvb_wgrad_args& a, cudaStream_t st);  // wgrad_tc.cu: wgmma weight-gradient kernel
-int cvb_pw_gemm_tc(const cvb_gemm_args& a, cudaStream_t st);  // gemm_tc.cu: wgmma kernel (all load modes; STORE / residual / SiLU-backward / GroupNorm-backward epilogues)
+int cvb_pw_gemm_tc(const cvb_gemm_args& a, cudaStream_t st, bool any_n);  // gemm_tc.cu: wgmma kernel (all load modes; STORE / residual / SiLU-backward / GroupNorm-backward epilogues)
 static int g_tc_enabled = 1;
 extern "C" int cvb_set_tc_enabled(int on) {
   int old = g_tc_enabled;
@@ -721,22 +720,29 @@ extern "C" int cvb_pw_gemm(const cvb_gemm_args* args, cvb_stream_t stream) {
   if (a.a_mode == CVB_A_BNB)
     CVB_CHECK(a.A2 && a.a_p0 && a.a_p1 && a.a_p2 && a.lda2 % 8 == 0 && cvb_aligned16(a.A2), "cvb_pw_gemm: BNB needs A2 and p0/p1/p2");
   if (g_tc_enabled) {
-    int rc = cvb_pw_gemm_tc(a, st);  // wgmma kernel: STORE / residual / SiLU-backward epilogues, N >= 96
+    int rc = cvb_pw_gemm_tc(a, st, false);  // wgmma kernel: STORE / residual / SiLU-backward epilogues, N >= 96
     if (rc != -1) return rc;
   }
   const int epi = a.e_mode == CVB_E_STORE ? (a.R ? EPI_STORE_R : EPI_STORE) : a.e_mode == CVB_E_SILU ? EPI_SILU
                   : (a.e_mode == CVB_E_SILU_BWD || a.e_mode == CVB_E_LIN_BWD) ? EPI_SILU_BWD : EPI_GN_BWD;
+  int rc;
   switch (a.a_mode) {
-    case CVB_A_RAW: return dispatch_epi<CVB_A_RAW>(a, epi, st);
-    case CVB_A_AFF: CVB_CHECK(a.a_p0 && a.a_p1, "cvb_pw_gemm: AFF needs p0/p1"); return dispatch_epi<CVB_A_AFF>(a, epi, st);
-    case CVB_A_AFF_SILU: CVB_CHECK(a.a_p0 && a.a_p1, "cvb_pw_gemm: AFF_SILU needs p0/p1"); return dispatch_epi<CVB_A_AFF_SILU>(a, epi, st);
-    case CVB_A_SILU: return dispatch_epi<CVB_A_SILU>(a, epi, st);
-    case CVB_A_GN: CVB_CHECK(a.a_p0 && a.a_p1, "cvb_pw_gemm: GN needs gamma/beta"); return dispatch_epi<CVB_A_GN>(a, epi, st);
+    case CVB_A_RAW: rc = dispatch_epi<CVB_A_RAW>(a, epi, st); break;
+    case CVB_A_AFF: CVB_CHECK(a.a_p0 && a.a_p1, "cvb_pw_gemm: AFF needs p0/p1"); rc = dispatch_epi<CVB_A_AFF>(a, epi, st); break;
+    case CVB_A_AFF_SILU: CVB_CHECK(a.a_p0 && a.a_p1, "cvb_pw_gemm: AFF_SILU needs p0/p1"); rc = dispatch_epi<CVB_A_AFF_SILU>(a, epi, st); break;
+    case CVB_A_SILU: rc = dispatch_epi<CVB_A_SILU>(a, epi, st); break;
+    case CVB_A_GN: CVB_CHECK(a.a_p0 && a.a_p1, "cvb_pw_gemm: GN needs gamma/beta"); rc = dispatch_epi<CVB_A_GN>(a, epi, st); break;
     case CVB_A_BNB:
       CVB_CHECK(a.A2 && a.a_p0 && a.a_p1 && a.a_p2 && a.lda2 % 8 == 0 && cvb_aligned16(a.A2), "cvb_pw_gemm: BNB needs A2 and p0/p1/p2");
-      return dispatch_epi<CVB_A_BNB>(a, epi, st);
+      rc = dispatch_epi<CVB_A_BNB>(a, epi, st);
+      break;
     default: cvb_set_error("cvb_pw_gemm: unsupported a_mode %d", a.a_mode); return 1;
   }
+  // a narrow layer whose K does not fit the mma.sync kernel's resident weight panel (the EfficientNet-b6 / b7 squeeze-excitation reduce
+  // convs: K = 3456 / 3840): the wgmma kernel streams the weight k-blocks through its ring
+  if (rc == -1 && g_tc_enabled) rc = cvb_pw_gemm_tc(a, st, true);
+  CVB_CHECK(rc != -1, "cvb_pw_gemm: K=%d is too large for the resident weight panel", a.K);
+  return rc;
 }
 
 extern "C" int cvb_pw_wgrad(const cvb_wgrad_args* args, cvb_stream_t stream) {

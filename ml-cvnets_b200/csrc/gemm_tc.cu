@@ -481,10 +481,11 @@ int dispatch_tc_epi(const cvb_gemm_args& a, cudaStream_t st) {
 }  // namespace
 
 // Returns -1 when the shape / mode is not handled by the wgmma kernel (caller uses the mma.sync kernel), 0 on success, > 0 on error.
-int cvb_pw_gemm_tc(const cvb_gemm_args& a, cudaStream_t st) {
+// any_n: take narrow / ragged N too (the mma.sync kernel cannot hold this K).
+int cvb_pw_gemm_tc(const cvb_gemm_args& a, cudaStream_t st, bool any_n) {
   // a CTA computes 128 output channels: narrow layers would idle most of them -> mma.sync kernel
   static const int min_n = [] { const char* e = getenv("CVB_TC_MIN_N"); return e ? atoi(e) : 96; }();  // diagnostics: route narrower layers here
-  if (a.N < min_n || (a.N >= 96 && a.N % 128 != 0 && a.N % 128 < 64 && a.N < 256)) return -1;  // narrow / ragged N would leave most of a 128-channel tile idle
+  if (!any_n && (a.N < min_n || (a.N >= 96 && a.N % 128 != 0 && a.N % 128 < 64 && a.N < 256))) return -1;  // narrow / ragged N would leave most of a 128-channel tile idle
   switch (a.a_mode) {
     case CVB_A_RAW: return dispatch_tc_epi<CVB_A_RAW>(a, st);
     case CVB_A_AFF: return dispatch_tc_epi<CVB_A_AFF>(a, st);

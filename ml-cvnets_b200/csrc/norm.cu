@@ -136,6 +136,8 @@ int cvb_make_tmap_2d_c64(CUtensorMap* map, const void* base, int64_t rows, int c
 namespace {
 
 constexpr int NT = 256;
+// channels one CTA of a per-channel reduction covers (one 8-channel group per thread); wider maps add a grid dimension of channel chunks
+constexpr int CH_CHUNK = 8 * NT;
 
 // row-block geometry shared by the per-channel reduction kernels
 struct RowGeom { int cgs, rpp, nthreads, rows_per_cta, ctas; };
@@ -330,20 +332,23 @@ __global__ void __launch_bounds__(1024) apply_load_mode_rows_kernel(const bf16* 
 // mode 0: BN backward reduce: dz = dout (act 0) or dout*silu'(sc*y+sh) (act 1); s0 += dz, s1 += dz*y; optional DZ store.
 __global__ void __launch_bounds__(NT) bn_bwd_reduce_kernel(const bf16* __restrict__ DOUT, const bf16* __restrict__ Y, const float* __restrict__ scale,
                                                            const float* __restrict__ shift, int act, bf16* __restrict__ DZ, double* s0, double* s1,
-                                                           int64_t M, int C, int cgs, int rpp, int rows_per_cta) {
+                                                           int64_t M, int C, int rows_per_cta) {
   pdl_wait();
   pdl_trigger();
-  extern __shared__ double sdred[];  // fp64: the threads' fp32 partials add exactly, whatever the order; [2][C]
+  extern __shared__ double sdred[];  // fp64: the threads' fp32 partials add exactly, whatever the order; [2][nc]
   const int tid = threadIdx.x;
-  for (int i = tid; i < 2 * C; i += blockDim.x) sdred[i] = 0.0;
+  // grid: (row blocks, channel chunks); thread = (8-channel group of the chunk, row lane)
+  const int c0 = blockIdx.y * CH_CHUNK, nc = min(C - c0, CH_CHUNK), cgs = nc / 8, rpp = blockDim.x / cgs;
+  for (int i = tid; i < 2 * nc; i += blockDim.x) sdred[i] = 0.0;
   __syncthreads();
   const int cg = tid % cgs, rr = tid / cgs;
-  const int c = cg * 8;
+  const int c = c0 + cg * 8;
   float sc[8], sh[8], a0[8], a1[8];
 #pragma unroll
   for (int j = 0; j < 8; ++j) { sc[j] = act ? scale[c + j] : 1.f; sh[j] = act ? shift[c + j] : 0.f; a0[j] = 0.f; a1[j] = 0.f; }
   int64_t r_begin = (int64_t)blockIdx.x * rows_per_cta, r_end = r_begin + rows_per_cta;
   if (r_end > M) r_end = M;
+  if (rr >= rpp) r_end = r_begin;  // the threads past cgs * rpp of a narrower last chunk
   for (int64_t r = r_begin + rr; r < r_end; r += rpp) {
     float d[8], y[8];
     unpack8(ldg16_stream(DOUT + r * C + c), d);
@@ -356,10 +361,12 @@ __global__ void __launch_bounds__(NT) bn_bwd_reduce_kernel(const bf16* __restric
     }
     if (DZ) stg16(DZ + r * C + c, pack8(d));
   }
+  if (rr < rpp) {
 #pragma unroll
-  for (int j = 0; j < 8; ++j) { atomicAdd(&sdred[c + j], (double)a0[j]); atomicAdd(&sdred[C + c + j], (double)a1[j]); }
+    for (int j = 0; j < 8; ++j) { atomicAdd(&sdred[cg * 8 + j], (double)a0[j]); atomicAdd(&sdred[nc + cg * 8 + j], (double)a1[j]); }
+  }
   __syncthreads();
-  for (int i = tid; i < C; i += blockDim.x) { atomicAdd(s0 + i, sdred[i]); atomicAdd(s1 + i, sdred[C + i]); }
+  for (int i = tid; i < nc; i += blockDim.x) { atomicAdd(s0 + c0 + i, sdred[i]); atomicAdd(s1 + c0 + i, sdred[nc + i]); }
 }
 
 // column sums of a bf16 / fp32 [M, ld] matrix into fp32
@@ -677,27 +684,29 @@ __global__ void __launch_bounds__(NT) gn_bwd_apply_kernel(const bf16* __restrict
 __global__ void __launch_bounds__(NT) pool_fwd_kernel(const bf16* __restrict__ X, int HW, int C, bf16* __restrict__ OUT) {
   pdl_wait();
   pdl_trigger();
-  // grid: (C/8 chunks rounded to blocks of 32 lanes..., B); thread = (chunk, row group)
-  extern __shared__ double sdred[];  // fp64: the threads' fp32 partials add exactly, whatever the order; [C]
+  // grid: (B, channel chunks); thread = (8-channel group of the chunk, row lane)
+  extern __shared__ double sdred[];  // fp64: the threads' fp32 partials add exactly, whatever the order; [nc]
   const int b = blockIdx.x;
-  const int cgs = C / 8;
+  const int c0 = blockIdx.y * CH_CHUNK, nc = min(C - c0, CH_CHUNK), cgs = nc / 8;
   const int tid = threadIdx.x;
-  for (int i = tid; i < C; i += blockDim.x) sdred[i] = 0.0;
+  for (int i = tid; i < nc; i += blockDim.x) sdred[i] = 0.0;
   __syncthreads();
   const int cg = tid % cgs, rr = tid / cgs, rpp = blockDim.x / cgs;
-  float a[8];
+  if (rr < rpp) {  // the threads past cgs * rpp of a narrower last chunk have no rows
+    float a[8];
 #pragma unroll
-  for (int j = 0; j < 8; ++j) a[j] = 0.f;
-  for (int r = rr; r < HW; r += rpp) {
-    float f[8];
-    unpack8(ldg16(X + ((int64_t)b * HW + r) * C + cg * 8), f);
+    for (int j = 0; j < 8; ++j) a[j] = 0.f;
+    for (int r = rr; r < HW; r += rpp) {
+      float f[8];
+      unpack8(ldg16(X + ((int64_t)b * HW + r) * C + c0 + cg * 8), f);
 #pragma unroll
-    for (int j = 0; j < 8; ++j) a[j] += f[j];
+      for (int j = 0; j < 8; ++j) a[j] += f[j];
+    }
+#pragma unroll
+    for (int j = 0; j < 8; ++j) atomicAdd(&sdred[cg * 8 + j], (double)a[j]);
   }
-#pragma unroll
-  for (int j = 0; j < 8; ++j) atomicAdd(&sdred[cg * 8 + j], (double)a[j]);
   __syncthreads();
-  for (int i = tid; i < C; i += blockDim.x) OUT[(int64_t)b * C + i] = __float2bfloat16_rn((float)sdred[i] / (float)HW);
+  for (int i = tid; i < nc; i += blockDim.x) OUT[(int64_t)b * C + c0 + i] = __float2bfloat16_rn((float)sdred[i] / (float)HW);
 }
 
 __global__ void __launch_bounds__(NT) pool_bwd_kernel(const bf16* __restrict__ DOUT, int HW, int C, bf16* __restrict__ DX, int64_t nvec) {
@@ -894,12 +903,13 @@ extern "C" int cvb_apply_load_mode(const void* A, int lda, const void* A2, int l
 
 extern "C" int cvb_bn_bwd_reduce(const void* DOUT, const void* Y, const float* scale, const float* shift, int act, void* DZ, double* sum_dz,
                                  double* sum_dzy, int64_t M, int C, cvb_stream_t stream) {
-  CVB_CHECK(DOUT && Y && sum_dz && sum_dzy && M > 0 && C > 0 && C % 8 == 0 && C <= 2048, "cvb_bn_bwd_reduce: bad arguments");
+  CVB_CHECK(DOUT && Y && sum_dz && sum_dzy && M > 0 && C > 0 && C % 8 == 0, "cvb_bn_bwd_reduce: bad arguments");
   if (act) CVB_CHECK(scale && shift, "cvb_bn_bwd_reduce: act needs scale/shift");
-  RowGeom g = row_geom(M, C);
-  CVB_CUDA(cvb_launch(bn_bwd_reduce_kernel, g.ctas, g.nthreads, 2 * C * sizeof(double), static_cast<cudaStream_t>(stream), 
-      static_cast<const bf16*>(DOUT), static_cast<const bf16*>(Y), scale, shift, act, static_cast<bf16*>(DZ), sum_dz, sum_dzy, M, C, g.cgs, g.rpp,
-      g.rows_per_cta));
+  const int nc = C < CH_CHUNK ? C : CH_CHUNK;
+  RowGeom g = row_geom(M, nc);
+  CVB_CUDA(cvb_launch(bn_bwd_reduce_kernel, dim3(g.ctas, (C + CH_CHUNK - 1) / CH_CHUNK), g.nthreads, 2 * nc * sizeof(double),
+      static_cast<cudaStream_t>(stream), static_cast<const bf16*>(DOUT), static_cast<const bf16*>(Y), scale, shift, act, static_cast<bf16*>(DZ), sum_dz,
+      sum_dzy, M, C, g.rows_per_cta));
   CVB_LAUNCH_CHECK();
   return 0;
 }
@@ -1002,10 +1012,12 @@ extern "C" int cvb_gn_bwd(const void* V, const void* X, const float* mean, const
 }
 
 extern "C" int cvb_global_pool_fwd(const void* X, int B, int HW, int C, void* OUT, cvb_stream_t stream) {
-  CVB_CHECK(X && OUT && B > 0 && HW > 0 && C > 0 && C % 8 == 0 && C <= 2048, "cvb_global_pool_fwd: bad arguments");
-  int cgs = C / 8;
+  CVB_CHECK(X && OUT && B > 0 && HW > 0 && C > 0 && C % 8 == 0, "cvb_global_pool_fwd: bad arguments");
+  const int nc = C < CH_CHUNK ? C : CH_CHUNK;
+  int cgs = nc / 8;
   int rpp = NT / cgs; if (rpp < 1) rpp = 1;
-  CVB_CUDA(cvb_launch(pool_fwd_kernel, B, cgs * rpp, C * sizeof(double), static_cast<cudaStream_t>(stream), static_cast<const bf16*>(X), HW, C, static_cast<bf16*>(OUT)));
+  CVB_CUDA(cvb_launch(pool_fwd_kernel, dim3(B, (C + CH_CHUNK - 1) / CH_CHUNK), cgs * rpp, nc * sizeof(double), static_cast<cudaStream_t>(stream),
+                      static_cast<const bf16*>(X), HW, C, static_cast<bf16*>(OUT)));
   CVB_LAUNCH_CHECK();
   return 0;
 }

@@ -34,7 +34,6 @@ F64 = torch.float64
 NONDETERMINISTIC = {
     "cvb_ln_bwd": "dgamma / dbeta of the ViT / CLIP LayerNorm backward are fp32 atomics of per-CTA partials",
     "cvb_mha_bwd": "the register-resident (S <= 256) attention backward sums dQ with shared-memory float atomics",
-    "cvb_se_scale_bwd": "the squeeze-excitation scale gradient DS is an fp32 atomic sum over pixel blocks",
     "cvb_embedding_bwd": "token-embedding gradients add repeated token ids with fp32 atomics",
     "cvb_ce_bwd": "the CLIP logit-scale gradient dlogit_scale is an fp32 atomic sum over rows (dlogits themselves have one writer)",
     "cvb_col_sum": "fp32 atomic column sums; no training step calls it",
