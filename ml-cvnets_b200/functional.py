@@ -10,7 +10,6 @@ Reference semantics restated per function; citations are relative to the referen
 from __future__ import annotations
 
 from types import SimpleNamespace
-from typing import List
 
 import torch
 
@@ -54,16 +53,6 @@ def _bn_forward(stats, count, gamma, beta, c):
     return ops.bn_eval_scale_shift(gamma, beta, c.running_mean, c.running_var, c.eps)
 
 
-def _zeros64(device, *sizes: int) -> List[torch.Tensor]:
-    """One memset for all fp64 [2, n] accumulators of a pass."""
-    buf = torch.zeros(2 * sum(sizes), device=device, dtype=torch.float64)
-    out, o = [], 0
-    for n in sizes:
-        out.append(buf[o:o + 2 * n].view(2, n))
-        o += 2 * n
-    return out
-
-
 class LazyBN:
     """A module output handed to the NEXT hot-path module still PRE-BatchNorm (DESIGN.md "lazy module boundaries").
 
@@ -90,12 +79,17 @@ def _ws_of(cfg, params):
     return ws if all(ws.has(p) for p in params) else None
 
 
-def _fwd_arena(cfg, device, n64: int) -> Arena:
+def _arena(cfg, kind: str, ws, device) -> Arena:
+    """Scratch of one forward ("fwd") or backward ("bwd") of the module behind ``cfg``, sized by what its earlier calls carved (the
+    record ``cfg.arena_<kind>``): a slice of the step arena when ``ws`` is given, else zeroed per call."""
+    rec = vars(cfg).setdefault("arena_" + kind, [0, 0])
+    return ws.arena((id(cfg), kind), rec) if ws is not None else Arena(rec, device)
+
+
+def _fwd_arena(cfg, device) -> Arena:
     """fp64 statistics accumulators of one forward: one memset per module, or a slice of the step arena (no launch at all)."""
     ws = getattr(cfg, "ws", None)
-    if ws is not None and ws.active:
-        return ws.arena((id(cfg), "fwd"), 0, n64)
-    return Arena(device, 0, n64)
+    return _arena(cfg, "fwd", ws if ws is not None and ws.active else None, device)
 
 
 class _Dst:
@@ -105,11 +99,11 @@ class _Dst:
     function returns ``None`` for the parameters (no AccumulateGrad kernels, no gather for the optimizer / all-reduce).  Otherwise: fresh
     slices of a per-call arena, returned to autograd as usual (what a plain ``loss.backward()`` on the drop-in modules gets)."""
 
-    def __init__(self, cfg, params, device, n32: int, n64: int, use_ws: bool):
+    def __init__(self, cfg, params, device, use_ws: bool):
         self.params = list(params)
         self.ws = _ws_of(cfg, self.params) if use_ws else None
         self.key = (id(cfg), "bwd")
-        self.ar = self.ws.arena(self.key, n32, n64) if self.ws is not None else Arena(device, n32, n64)
+        self.ar = _arena(cfg, "bwd", self.ws, device)
         self.grads = [None] * len(self.params)
         self.late = []
 
@@ -170,7 +164,7 @@ class StemFn(torch.autograd.Function):
         ws = getattr(cfg, "ws", None)
         A0 = ops.stem_im2col(xin, mix=ws.mix if (ws is not None and ws.active) else None)  # batch mixing rides in the gather (TrainStep.set_mix)
         Ws = cfg.prep.get(cfg.i_w)
-        st = _fwd_arena(cfg, x.device, 2 * C0 + 8).f64(2, C0)
+        st = _fwd_arena(cfg, x.device).f64(2, C0)
         y = ops.pw_gemm(A0, Ws, C0, col_stats=st if cfg.bn.batch_stats else None)
         bn = _bn_forward(st, M, gamma, beta, cfg.bn)
         ctx.lz_out = cfg.last_lazy = LazyBN(bn, True) if cfg.lazy_out else None
@@ -188,7 +182,7 @@ class StemFn(torch.autograd.Function):
         A0, y, bn = ctx.saved
         (gamma,) = ctx.saved_tensors
         g2 = as_2d(to_bf16_cl(gout))
-        D = _Dst(cfg, ctx.plist, g2.device, C0 * 32 + 64, 2 * C0 + 16, True)
+        D = _Dst(cfg, ctx.plist, g2.device, True)
         if ctx.lz_out is not None:  # the consumer already went through the activation and took the BatchNorm-backward sums
             assert ctx.lz_out.stats is not None, "lazy module output was consumed by a module that does not know the protocol"
             dz, sd = g2, ctx.lz_out.stats
@@ -215,7 +209,7 @@ class InvertedResidualFn(torch.autograd.Function):
         M, M2 = B * H * W, B * Ho * Wo
         x2 = as_2d(x)
         P = cfg.prep
-        fa = _fwd_arena(cfg, x.device, 2 * (2 * hid + cout) + 16)
+        fa = _fwd_arena(cfg, x.device)
         st1, st2, st3 = fa.f64(2, hid), fa.f64(2, hid), fa.f64(2, cout)
         bs = [c.batch_stats for c in cfg.bn]  # per layer: individual BatchNorms may be frozen (base_model.py:139-165)
         lz = ctx.lz_in = cfg.lazy_in
@@ -252,7 +246,7 @@ class InvertedResidualFn(torch.autograd.Function):
         ev = ctx.ev
         dout = as_2d(to_bf16_cl(gout))
         # parameter order: (w1, g1, b1, wd, g2, b2, w3, g3, b3)
-        D = _Dst(cfg, ctx.plist, dout.device, cout * hid + hid * Cin + 9 * hid + 64, 2 * (cout + 2 * hid + Cin) + 16, True)
+        D = _Dst(cfg, ctx.plist, dout.device, True)
         ar = D.ar
         sd3, sd2, sd1 = ar.f64(2, cout), ar.f64(2, hid), ar.f64(2, hid)
         # red_1x1 + BN3 (no activation): dz3 = dout
@@ -305,7 +299,7 @@ class MobileViTBlockv2Fn(torch.autograd.Function):
         wd0, g0, b0, wl = params[:4]
         gL, bL, wp, gp, bp = params[4 + 12 * n:]
         bs = [c.batch_stats for c in cfg.bn]
-        fa = _fwd_arena(cfg, x.device, 4 * C + (2 * n + 1) * (2 * B + 2) + 16)
+        fa = _fwd_arena(cfg, x.device)
         st0, stp = fa.f64(2, C), fa.f64(2, C)
         samp = [fa.f64(2, B) for _ in range(2 * n + 1)]
         gcount = HW * d
@@ -360,9 +354,7 @@ class MobileViTBlockv2Fn(torch.autograd.Function):
         dev = x2.device
         gcount = HW * d
         dout = as_2d(to_bf16_cl(gout))
-        n32 = sum(int(q.numel()) for q in params) + n * 8 * d + 16 * len(params) + 9 * C + 2 * (2 * d + 8) * n + 64
-        n64 = 6 * C + (n + 1) * (2 * d + 2 * B + 2 * d) + n * (2 * ffn + 2 * d + 2 * B + 2 * d) + 64 + (2 * n + 1) * (2 * B * d + 2)
-        D = _Dst(cfg, ctx.plist, dev, n32, n64, True)
+        D = _Dst(cfg, ctx.plist, dev, True)
         ar = D.ar
         sdp, sd0 = ar.f64(2, C), ar.f64(2, C)
         # ---- conv_proj (GN -> 1x1 -> BN, no act)
@@ -464,7 +456,7 @@ class PoolLinearFn(torch.autograd.Function):
         else:
             g = torch.zeros((B, npad), device=pooled.device, dtype=BF16)
             g[:, :ncls] = gout
-        D = _Dst(cfg, ctx.plist, pooled.device, npad * C + npad + 64, 8, npad == ncls)
+        D = _Dst(cfg, ctx.plist, pooled.device, npad == ncls)
         if npad == ncls:
             dW, db = D.mat(0, npad, C), D.mat(1, 1, npad).view(npad)
             ops.pw_wgrad_side(g, pooled, npad, C, dW=dW, dbias=db)
@@ -529,7 +521,7 @@ class PointwiseConvFn(torch.autograd.Function):
         R = as_2d(residual) if residual is not None else None
         ob = None
         if cfg.bn is not None:
-            st = _fwd_arena(cfg, x.device, 2 * cout + 8).f64(2, cout)
+            st = _fwd_arena(cfg, x.device).f64(2, cout)
             y = ops.pw_gemm(x2, P.get(cfg.i_w), cout, bias=bias, col_stats=st if cfg.bn.batch_stats else None)
             bn = _bn_forward(st, M, gamma, beta, cfg.bn)
             if cfg.act in (None, ops.ACT_SILU):
@@ -563,7 +555,7 @@ class PointwiseConvFn(torch.autograd.Function):
         dout = as_2d(to_bf16_cl(gout))
         x2 = ctx.saved[0]
         Kc = x2.shape[1]
-        D = _Dst(cfg, ctx.plist, dout.device, cout * Kc + cout + 64, 2 * cout + 16, True)
+        D = _Dst(cfg, ctx.plist, dout.device, True)
         has_bias = cfg.has_bias
         db = D.mat(1, 1, cout).view(cout) if has_bias else None
         dW = D.ar.f32(cout, Kc) if dense else D.mat(0, cout, Cin)
@@ -616,7 +608,7 @@ class DepthwiseConvFn(torch.autograd.Function):
         M2 = B * Ho * Wo
         x2 = as_2d(x)
         if cfg.bn is not None:
-            st = _fwd_arena(cfg, x.device, 2 * C + 8).f64(2, C)
+            st = _fwd_arena(cfg, x.device).f64(2, C)
             y = ops.dw_fwd(x2, B, H, W, C, s, cfg.prep.get(cfg.i_w), col_stats=st if cfg.bn.batch_stats else None, dilation=cfg.dilation,
                            ksize=cfg.k)
             bn = _bn_forward(st, M2, gamma, beta, cfg.bn)
@@ -637,7 +629,7 @@ class DepthwiseConvFn(torch.autograd.Function):
         M2 = B * Ho * Wo
         dout = as_2d(to_bf16_cl(gout))
         taps = cfg.k * cfg.k
-        D = _Dst(cfg, ctx.plist, dout.device, taps * C + 64, 2 * C + 16, True)
+        D = _Dst(cfg, ctx.plist, dout.device, True)
         if cfg.bn is not None:
             x2, y, bn = ctx.saved
             (gamma,) = ctx.saved_tensors
@@ -669,7 +661,7 @@ class GroupNorm1Fn(torch.autograd.Function):
         B, C, H, W = x.shape
         rps = H * W
         x2 = as_2d(x)
-        st = _fwd_arena(cfg, x.device, 2 * B + 8).f64(2, B)
+        st = _fwd_arena(cfg, x.device).f64(2, B)
         ops.gn_stats(x2, B, rps, st)
         gn = ops.gn_finalize(st, rps * C, cfg.eps)
         out = ops.apply_load_mode(x2, ops.A_GN, C, a_p=(gamma, beta, None), row_stats=(gn[0], gn[1]), rows_per_sample=rps)
@@ -684,7 +676,7 @@ class GroupNorm1Fn(torch.autograd.Function):
         x2, gn = ctx.saved
         (gamma,) = ctx.saved_tensors
         dout = as_2d(to_bf16_cl(gout))
-        D = _Dst(cfg, ctx.plist, dout.device, 64, 2 * C + 2 * B + 16, True)
+        D = _Dst(cfg, ctx.plist, dout.device, True)
         dgb, wsp = D.ar.f64(2, C), D.ar.f64(2, B)
         dx = ops.gn_bwd(dout, x2, gn, gamma, float(H * W * C), B, H * W, dgb[0], dgb[1], wsp)
         D.late64(0, dgb[0])
@@ -718,7 +710,7 @@ class LayerNormFn(torch.autograd.Function):
         dy = gout.reshape(-1, C)
         if dy.dtype != BF16 or not dy.is_contiguous():
             dy = dy.to(BF16).contiguous()
-        D = _Dst(cfg, ctx.plist, dy.device, 64, 2 * C + 16, True)
+        D = _Dst(cfg, ctx.plist, dy.device, True)
         cs = D.ar.f64(2, C)
         dx = ops.ln_bwd(dy, x2, ln, gamma, cs)
         D.late64(0, cs[1])
@@ -760,7 +752,7 @@ class LinearSelfAttentionFn(torch.autograd.Function):
         Pw = cfg.prep
         x2, qkv, xp2, qkp, O, S, CTX = ctx.saved
         dy = as_2d(to_bf16_cl(gout))
-        D = _Dst(cfg, ctx.plist, dy.device, (2 * d + 8) * (d + 1) + d * d + d + 64, 16, True)
+        D = _Dst(cfg, ctx.plist, dy.device, True)
         ar = D.ar
         ops.pw_wgrad_side(dy, O, d, d, dW=D.mat(2, d, d), dbias=D.mat(3, 1, d).view(d))
         dO = ops.pw_gemm(dy, Pw.get(cfg.i_wot), d, K=d)
@@ -811,7 +803,7 @@ class LinearFn(torch.autograd.Function):
         elif g.dtype != BF16 or not g.is_contiguous():
             g = g.to(BF16).contiguous()
         has_b = len(ctx.plist) > 1
-        D = _Dst(cfg, ctx.plist, g.device, npad * cin + npad + 64, 8, npad == cout)
+        D = _Dst(cfg, ctx.plist, g.device, npad == cout)
         if npad == cout:
             ops.pw_wgrad_side(g, x2, npad, cin, dW=D.mat(0, npad, cin), dbias=D.mat(1, 1, npad).view(npad) if has_b else None)
         else:
@@ -1000,7 +992,7 @@ class VitTokensFn(torch.autograd.Function):
         B, C, nh, nw, n_pos = ctx.dims
         N = nh * nw
         g = gout if (gout.dtype == BF16 and gout.is_contiguous()) else gout.to(BF16).contiguous()
-        D = _Dst(ctx.cfg, ctx.plist, g.device, n_pos * C + C + 64, 8, True)
+        D = _Dst(ctx.cfg, ctx.plist, g.device, True)
         dpos = D.mat(0, n_pos, C)
         dcls = D.mat(1, 1, C).view(C) if ctx.has_cls else None
         dpatch = ops.vit_tokens_interp_bwd(g, dpos, dcls, B, N, C)
@@ -1025,7 +1017,7 @@ class EmbeddingFn(torch.autograd.Function):
         V, C = ctx.shape
         B, S = ctx.tokens.shape
         g = g if (g.dtype == BF16 and g.is_contiguous()) else g.to(BF16).contiguous()
-        D = _Dst(ctx.cfg, ctx.plist, g.device, V * C + S * C + 64, 8, True)
+        D = _Dst(ctx.cfg, ctx.plist, g.device, True)
         dtable = D.mat(0, V, C)
         dpos = D.mat(1, S, C) if ctx.has_pos else None
         ops.embedding_bwd(g, ctx.tokens, dtable, dpos)
@@ -1066,7 +1058,7 @@ class ProjectionFn(torch.autograd.Function):
         din, dout = ctx.shape
         (x2,) = ctx.saved
         g = g if (g.dtype == BF16 and g.is_contiguous()) else g.to(BF16).contiguous()
-        D = _Dst(ctx.cfg, ctx.plist, g.device, din * dout + 64, 8, True)
+        D = _Dst(ctx.cfg, ctx.plist, g.device, True)
         ops.pw_wgrad_side(x2, g, din, dout, dW=D.mat(0, din, dout))
         dx = ops.pw_gemm(g, ctx.cfg.prep.get(ctx.cfg.i_p), din, K=dout)
         ops.join_side()
@@ -1135,7 +1127,7 @@ class ClipLossFn(torch.autograd.Function):
         N, d, G = ctx.dims
         img, txt, I_all, T_all, Li, Lt, labels, lse_i, nv_i, lse_t, nv_t, p = ctx.saved
         g = (gout.float() * 0.5).contiguous()
-        D = _Dst(cfg, ctx.plist, img.device, 64, 8, True)
+        D = _Dst(cfg, ctx.plist, img.device, True)
         dp = D.mat(0, 1, 1)
         scale = getattr(cfg, "scale", None)
         dLi = ops.ce_bwd(Li, G, labels, -1, 0.0, lse_i, nv_i, g, scale, G, logit_scale=p, dlogit_scale=dp)
@@ -1237,7 +1229,7 @@ class TransformerEncoderFn(torch.autograd.Function):
         drop = getattr(cfg, "drop", None)  # (p, p_ffn, p_row) in training with dropout / stochastic depth > 0 (transformer.py:97-100, 139-156)
         keys = None
         if drop is None:
-            samp = _fwd_arena(cfg, x.device, 2 * M + 8).f64(2, M)
+            samp = _fwd_arena(cfg, x.device).f64(2, M)
             X1 = ops.pw_gemm(O, P.get(cfg.i_wo), C, bias=bo, R=x2, samp_stats=samp, rows_per_sample=1)
             ln2 = ops.gn_finalize(samp, C, cfg.eps)
             if keep_n:
@@ -1288,7 +1280,7 @@ class TransformerEncoderFn(torch.autograd.Function):
         dev = x2.device
         dY = gout.reshape(M, C).to(BF16).contiguous()
         # parameter order: (g1, b1, wqkv, bqkv, wo, bo, g2, b2, w1, bb1, w2, bb2)
-        D = _Dst(cfg, ctx.plist, dev, 4 * C * C + 2 * C * ffn + 8 * C + ffn + 64, 8 * C + 2 * ffn + 64, True)
+        D = _Dst(cfg, ctx.plist, dev, True)
         ar = D.ar
         vec = lambda i, n: D.mat(i, 1, n).view(n)  # noqa: E731
         # ---- FFN

@@ -15,6 +15,7 @@ Anything that does not know about the workspace still works: autograd accumulate
 from __future__ import annotations
 
 import ctypes
+import math
 from typing import Dict, List, Optional, Sequence, Tuple
 
 import torch
@@ -25,40 +26,46 @@ ALIGN = 8  # every parameter starts at a multiple of 8 floats (32 B): the weight
 
 
 class Arena:
-    """Zero-initialised fp32 / fp64 scratch handed out in slices (accumulators, kernel-layout gradients).  Fresh per call unless carved
-    out of a StepWorkspace (then it is zeroed by the step's single memset)."""
+    """Zero-initialised fp32 / fp64 scratch handed out in carves (accumulators, kernel-layout gradients), each 16-byte aligned.
 
-    def __init__(self, device=None, n32: int = 0, n64: int = 0, b32: Optional[torch.Tensor] = None, b64: Optional[torch.Tensor] = None):
-        self.b32 = torch.zeros(n32, device=device, dtype=torch.float32) if b32 is None else b32
-        self.b64 = torch.zeros(n64, device=device, dtype=torch.float64) if b64 is None else b64
-        self.o32 = self.o64 = 0
+    ``rec`` is the record ``[n32, n64]`` of one arena key: the most that earlier calls with that key carved.  The arena is one zeroed buffer
+    per dtype of that size -- fresh per call, or a slice of a StepWorkspace zeroed by the step's single memset.  A carve that does not fit
+    (no record yet, or a larger shape than before) gets a zeroed tensor of its own and raises the record, so the next call fits."""
+
+    def __init__(self, rec: List[int], device=None, b32: Optional[torch.Tensor] = None, b64: Optional[torch.Tensor] = None):
+        self.rec = rec
+        self.b32 = torch.zeros(rec[0], device=device, dtype=torch.float32) if b32 is None else b32
+        self.b64 = torch.zeros(rec[1], device=device, dtype=torch.float64) if b64 is None else b64
+        self.used = [0, 0]  # elements carved so far, fp32 and fp64
         self.c32 = None
 
     def f32(self, *shape: int) -> torch.Tensor:
-        n = 1
-        for d in shape:
-            n *= d
-        v = self.b32[self.o32:self.o32 + n].view(*shape)
-        self.o32 += (n + 3) // 4 * 4
-        assert self.o32 <= self.b32.numel(), "fp32 arena exhausted"
-        return v
+        return self._carve(0, self.b32, shape, 4)
 
     def f64(self, *shape: int) -> torch.Tensor:
-        n = 1
-        for d in shape:
-            n *= d
-        v = self.b64[self.o64:self.o64 + n].view(*shape)
-        self.o64 += (n + 1) // 2 * 2
-        assert self.o64 <= self.b64.numel(), "fp64 arena exhausted"
-        return v
+        return self._carve(1, self.b64, shape, 2)
+
+    def _carve(self, i: int, buf: torch.Tensor, shape, align: int) -> torch.Tensor:
+        n, o = math.prod(shape), self.used[i]
+        self.used[i] = end = o + (n + align - 1) // align * align
+        self.rec[i] = max(self.rec[i], end)
+        v = buf[o:o + n] if end <= buf.numel() else self._own(end - o, buf)[:n]
+        return v.view(*shape)
+
+    @staticmethod
+    def _own(n: int, like: torch.Tensor) -> torch.Tensor:
+        """The tensor of a carve that does not fit the buffer."""
+        return torch.zeros(n, device=like.device, dtype=like.dtype)
 
     def cast(self):
-        """fp64 statistics -> fp32 (ONE conversion kernel); call after the last kernel that accumulates into them."""
+        """fp64 statistics -> fp32 (ONE conversion kernel for the buffer); call after the last kernel that accumulates into them."""
         self.c32 = self.b64.float()
 
     def as_f32(self, v64: torch.Tensor) -> torch.Tensor:
-        o = v64.storage_offset() - self.b64.storage_offset()
-        return self.c32[o:o + v64.numel()].view(v64.shape)
+        o = (v64.data_ptr() - self.b64.data_ptr()) // 8
+        if 0 <= o < self.b64.numel():
+            return self.c32[o:o + v64.numel()].view(v64.shape)
+        return v64.float()  # a carve of its own
 
 
 class StepWorkspace:
@@ -88,8 +95,7 @@ class StepWorkspace:
         # step follows per-iteration changes (engine.TrainStep.set_mix)
         self.mix = torch.zeros(6, device=dev, dtype=torch.float32)
         self.mix[1] = 1.0
-        self._plan: Dict[tuple, Tuple[int, int, int, int]] = {}
-        self._requests: Dict[tuple, Tuple[int, int]] = {}
+        self._plan: Dict[tuple, Tuple[List[int], int, int, int, int]] = {}  # arena key -> (record, o32, n32, o64, n64) of its slice
         self._used = set()
         self._buf32 = self._buf64 = None
         self._cast_tables: Dict[tuple, Tuple[torch.Tensor, int, int]] = {}
@@ -126,28 +132,23 @@ class StepWorkspace:
         return id(p) in self._gviews
 
     # ----------------------------------------------------------------------------------------------------------------- arena
-    def arena(self, key: tuple, n32: int, n64: int) -> Arena:
-        """Scratch for one forward / backward of one module.  Planned (persistent, zeroed by begin_step) from the second step on."""
-        n32, n64 = (n32 + 7) // 8 * 8, (n64 + 3) // 4 * 4
-        if not self.active:
-            return Arena(self.device, n32, n64)
-        plan = self._plan.get(key)
-        if plan is None or key in self._used or plan[1] != n32 or plan[3] != n64:
-            if plan is None:
-                self._requests[key] = (n32, n64)
-            return Arena(self.device, n32, n64)
+    def arena(self, key: tuple, rec: List[int]) -> Arena:
+        """Scratch for one forward / backward of one module (``rec``: the key's record, see Arena): its slice of the step arena, planned
+        from the records and zeroed by begin_step.  Until the slice is planned, or when a call outgrows it, the call's carves are tensors of
+        their own and the next begin_step re-plans."""
+        plan = self._plan.setdefault(key, (rec, 0, 0, 0, 0))
+        if self._buf32 is None or key in self._used:
+            return Arena(rec, self.device)
         self._used.add(key)
-        o32, _, o64, _ = plan
-        return Arena(b32=self._buf32[o32:o32 + n32], b64=self._buf64[o64:o64 + n64])
+        _, o32, n32, o64, n64 = plan
+        return Arena(rec, b32=self._buf32[o32:o32 + n32], b64=self._buf64[o64:o64 + n64])
 
     def _replan(self):
-        for k, v in self._requests.items():
-            self._plan.setdefault(k, (0, v[0], 0, v[1]))
-        self._requests.clear()
         o32 = o64 = 0
         new = {}
-        for k, (_, n32, _, n64) in self._plan.items():
-            new[k] = (o32, n32, o64, n64)
+        for k, (rec, *_) in self._plan.items():
+            n32, n64 = (rec[0] + 7) // 8 * 8, (rec[1] + 3) // 4 * 4  # 32-byte aligned slices
+            new[k] = (rec, o32, n32, o64, n64)
             o32 += n32
             o64 += n64
         self._plan = new
@@ -157,7 +158,8 @@ class StepWorkspace:
 
     def begin_step(self):
         """Zero the gradient buffer and the arena (two memset nodes), reset the per-step bookkeeping."""
-        if self._requests:
+        outgrown = any(r[0] > n32 or r[1] > n64 for r, _, n32, _, n64 in self._plan.values())
+        if self._plan and (self._buf32 is None or outgrown):
             if torch.cuda.is_current_stream_capturing():
                 raise RuntimeError("StepWorkspace: run at least two eager steps before capturing the step in a CUDA graph")
             self._replan()
