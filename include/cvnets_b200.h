@@ -289,6 +289,45 @@ CVB_API int cvb_dropout_fwd(const void* V, const void* R, void* Y, int64_t M, in
                     cvb_stream_t stream);
 CVB_API int cvb_dropout_bwd(const void* DY, void* DV, int64_t M, int C, int rows_per_sample, float p, float p_row, const void* key, cvb_stream_t stream);
 
+/* RangeAugment (cvnets/neural_augmentor/neural_aug.py DistributionNeuralAugmentor, loss_fn/neural_augmentation.py) on fp32 NCHW images [B, 3, H, W]
+ * in [0, 1], contiguous.  `mix` (NULL = off) is the batch-mixing record of cvb_stem_im2col_mix, applied on the fly: the augmentor sees the mixed image.
+ * Every augmentation is affine per (sample, channel), so the chain is x_aug = clip(A x_mix + Bc + C eps, 0, 1) with coef[b, c] = (A, Bc, C).
+ * Draws are hashes of the 64-bit key at `key` (cvb_rng_next), recomputed by every kernel that needs them:
+ *   cvb_na_plan     draw table tab[4 + 3 B]: tab[0..2] augmentation (0 brightness, 1 contrast, 2 noise) at each position of a uniformly random
+ *                   order of the enabled ones (bit k of `enabled`; -1 past them), tab[3] their count, tab[4 + k B + b] = u ~ U[0, 1) if sample b is
+ *                   one of the max(1, B / 2) distinct samples drawn for augmentation k, else -1.  B <= 4096.
+ *   cvb_na_noise    the N(0, 1) field eps [B, 3, H, W] the other kernels recompute (for tests).
+ *   cvb_na_stats    per-plane means of x_mix and eps (fp64 [B * 3] each; eps only when need_eps).
+ *   cvb_na_compose  coef fp32 [B * 3, 3] from the table, the means and the sampler parameters raw[6] = (_low, _high) of brightness, contrast,
+ *                   noise (device fp32 scalars; NULL pairs = disabled): low / high = sigmoid(raw) (max - min) + min with the reference's bounds.
+ *   cvb_na_apply    Y = x_aug (fp32 NCHW) and sq[b * 3 + c] = sum (x_aug - x_mix)^2 (fp64).
+ *   cvb_na_bwd_reduce  red[b * 3 + c] = (sum g x_mix, sum g, sum g eps) of g = [0 <= pre-clip <= 1] (DY + 2 g_sq (x_aug - x_mix)) (DY or g_sq NULL = 0).
+ *   cvb_na_param_grad  grads[j] = d loss / d raw[j] (fp32 scalars, overwritten) from red: the chain rule through the composition, the draws, the
+ *                   contrast means and the sigmoid bounds.
+ *   cvb_na_loss_fwd loss = w_na * L_na + w_ce * *ce (the composite loss; ce may be NULL = 0), L_na = alpha / 65025 * mean_b smooth_l1(mse_b -
+ *                   target[min(step, T - 1)]), mse_b = 65025 * sum_c sq[b, c] / (3 H W); parts (may be NULL) = (*ce, L_na).
+ *   cvb_na_loss_bwd g_sq[b * 3 + c] = d loss / d sq[b, c], times *grad_out and *grad_scale (either may be NULL = 1); g_ce (may be NULL) =
+ *                   *grad_out * w_ce, the gradient handed to the cross entropy (whose backward applies the loss scale).
+ * All sums are fp64 in a fixed order: the same bits run to run. */
+CVB_API int cvb_na_plan(const void* key, int B, int enabled, float* tab, cvb_stream_t stream);
+CVB_API int cvb_na_noise(const void* key, int B, int H, int W, float* eps, cvb_stream_t stream);
+CVB_API int cvb_na_stats(const float* X, const float* mix, const void* key, int B, int H, int W, int need_eps, double* mu_x, double* mu_e, cvb_stream_t stream);
+CVB_API int cvb_na_compose(const float* tab, const double* mu_x, const double* mu_e, const float* const* raw, int B, float* coef, cvb_stream_t stream);
+CVB_API int cvb_na_apply(const float* X, const float* mix, const void* key, const float* coef, int B, int H, int W, int need_eps, float* Y, double* sq,
+                 cvb_stream_t stream);
+CVB_API int cvb_na_bwd_reduce(const float* DY, const double* g_sq, const float* X, const float* mix, const void* key, const float* coef, int B, int H, int W,
+                      int need_eps, double* red, cvb_stream_t stream);
+CVB_API int cvb_na_param_grad(const float* tab, const double* mu_x, const double* mu_e, const double* red, const float* const* raw, int B,
+                      float* const* grads, cvb_stream_t stream);
+CVB_API int cvb_na_loss_fwd(const double* sq, int B, int H, int W, const float* target, int T, const int64_t* step, float alpha, float w_na, const float* ce,
+                    float w_ce, float* loss, float* parts, cvb_stream_t stream);
+CVB_API int cvb_na_loss_bwd(const double* sq, int B, int H, int W, const float* target, int T, const int64_t* step, float alpha, float w_na,
+                    const float* grad_out, const float* grad_scale, double* g_sq, float* g_ce, float w_ce, cvb_stream_t stream);
+/* Input gradient of the stem conv (3 -> C0, 3x3, stride 2, pad 1): dX fp32 NCHW [B, 3, 2 Ho, 2 Wo] = conv_transpose(dy, W) with
+ * dy = bf16(p0 dz + p1 y + p2) (CVB_A_BNB on the bf16 [B*Ho*Wo, C0] dz / y, coef fp32 [3, C0]) and the prepared bf16 weight [C0, 32]
+ * (columns ci*9 + u*3 + v).  C0 a multiple of 8, <= 64. */
+CVB_API int cvb_stem_dgrad(const void* dz, const void* y, const float* coef, const void* w, int B, int Ho, int Wo, int C0, float* dX, cvb_stream_t stream);
+
 /* ---------------------------------------------------------------------------------------------------------------
  * Per-step tail of the training loop (engine/training_engine.py:289-312) on FLAT fp32 buffers of n elements: GradScaler unscale +
  * inf check, clip_grad_norm_, AdamW, GradScaler update -- two launches, all state on the device (CUDA-graph friendly).

@@ -164,6 +164,18 @@ _SIGS = {
     "cvb_col_sum": (c_int, [c_void_p, c_int, c_int, c_int64, c_int, c_void_p, c_void_p]),
     "cvb_prep_weights": (c_int, [c_void_p, c_int, c_int, c_void_p]),
     "cvb_unprep_grad": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    "cvb_na_plan": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p]),
+    "cvb_na_noise": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "cvb_na_stats": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "cvb_na_compose": (c_int, [c_void_p, c_void_p, c_void_p, POINTER(c_void_p), c_int, c_void_p, c_void_p]),
+    "cvb_na_apply": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "cvb_na_bwd_reduce": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "cvb_na_param_grad": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_void_p), c_int, POINTER(c_void_p), c_void_p]),
+    "cvb_na_loss_fwd": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_float, c_float, c_void_p, c_float, c_void_p, c_void_p,
+                                c_void_p]),
+    "cvb_na_loss_bwd": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_float, c_float, c_void_p, c_void_p, c_void_p, c_void_p,
+                                c_float, c_void_p]),
+    "cvb_stem_dgrad": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
 }
 
 EXPORTS = tuple(_SIGS.keys())

@@ -9,7 +9,7 @@ import sys
 from concurrent.futures import ThreadPoolExecutor
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-SOURCES = ["gemm.cu", "gemm_tc.cu", "wgrad_tc.cu", "dwconv.cu", "dwconv_dilated.cu", "norm.cu", "linattn.cu", "mha.cu", "mha_tc.cu", "mha_long.cu", "optim.cu", "loss.cu", "conv.cu", "clip.cu", "zeroshot.cu", "se.cu", "dropout.cu"]
+SOURCES = ["gemm.cu", "gemm_tc.cu", "wgrad_tc.cu", "dwconv.cu", "dwconv_dilated.cu", "norm.cu", "linattn.cu", "mha.cu", "mha_tc.cu", "mha_long.cu", "optim.cu", "loss.cu", "conv.cu", "clip.cu", "zeroshot.cu", "se.cu", "dropout.cu", "neural_aug.cu"]
 LIB = os.path.join(HERE, "libcvnets_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]

@@ -45,11 +45,14 @@ class TrainStep:
                  no_decay_bn_filter_bias: bool = True, max_norm: float = 10.0, label_smoothing: float = 0.1, ignore_index: int = -1,
                  ema_momentum: Optional[float] = None, init_scale: float = 65536.0, growth_interval: int = 2000,
                  process_group=None, data_parallel: Optional[bool] = None, n_buckets: int = 3, broadcast_buffers: bool = True,
-                 forward_loss=None, optimizer: str = "adamw", momentum: float = 0.9, nesterov: bool = True):
+                 forward_loss=None, optimizer: str = "adamw", momentum: float = 0.9, nesterov: bool = True,
+                 aug_loss: Optional["NeuralAugmentationLoss"] = None, ce_weight: float = 1.0):
         """``forward_loss(model, *inputs, cfg) -> loss`` replaces the default ``cross_entropy(model(x), y)`` (e.g. CLIP's contrastive step);
         ``cfg.scale`` is the device-resident loss scale the loss's backward must multiply by, ``cfg.world / rank / group`` the process group.
         ``optimizer="sgd"`` swaps AdamW for SGD with ``momentum`` / ``nesterov`` (optim.FlatSGD; ``betas`` / ``eps`` are then unused and
-        ``max_norm`` None / 0 means no clipping)."""
+        ``max_norm`` None / 0 means no clipping).  A model with a RangeAugment augmentor returns ``{"augmented_tensor", "logits"}``; the cross
+        entropy reads ``logits``, and with ``aug_loss`` the step minimises ``ce_weight * CE + aug_loss.weight * L_na`` (the RangeAugment recipes'
+        composite_loss); ``loss_parts`` (device fp32 [2]) then holds (CE, L_na) of the last step."""
         import torch.distributed as dist
         if optimizer not in ("adamw", "sgd"):
             raise ValueError(f"optimizer must be 'adamw' or 'sgd', got {optimizer!r}")
@@ -77,6 +80,10 @@ class TrainStep:
                                         mix=self.ws.mix)
         self._mix_host = torch.tensor([0.0, 1.0, 0.0, 0.0, 0.0, 0.0]).pin_memory()
         self.forward_loss = forward_loss
+        if aug_loss is None and ce_weight != 1.0:
+            raise ValueError("ce_weight weighs the cross entropy against aug_loss; without aug_loss the loss is the cross entropy")
+        self.aug_loss, self.ce_weight = aug_loss, float(ce_weight)
+        self.loss_parts = torch.zeros(2, device=self.ws.device, dtype=torch.float32) if aug_loss is not None else None
         self.loss_cfg.group = process_group
         self.loss_cfg.world, self.loss_cfg.rank = self.world, (dist.get_rank(process_group) if data_parallel else 0)
         self._one = torch.ones((), device=self.ws.device, dtype=torch.float32)
@@ -87,6 +94,13 @@ class TrainStep:
     # ---- scheduler / checkpoint hooks
     def set_lr(self, lr: float) -> None:
         self.opt.set_lr(lr)
+
+    def set_epoch(self, epoch: int) -> None:
+        """Curriculum position of ``aug_loss`` for the NEXT steps (the epoch, or the iteration when the scheduler is iteration based); a device
+        scalar, so a captured step follows it."""
+        if self.aug_loss is None:
+            raise RuntimeError("set_epoch: this TrainStep has no aug_loss")
+        self.aug_loss.set_epoch(epoch)
 
     def set_mix(self, kind: Optional[str] = None, lam: float = 1.0, box=(0, 0, 0, 0)) -> None:
         """Batch mixing for the NEXT steps (SURVEY.md 8f row 3; reference: apply_mixing_transforms, engine/training_engine.py:236-238).
@@ -116,7 +130,16 @@ class TrainStep:
         try:
             if self.forward_loss is None:
                 x, y = inputs
-                loss = cross_entropy(self.model(x), y, _cfg=self.loss_cfg)
+                out = self.model(x)
+                if isinstance(out, dict):  # a model with a RangeAugment augmentor (base_image_encoder.py:282-298)
+                    loss = cross_entropy(out["logits"], y, _cfg=self.loss_cfg)
+                    if self.aug_loss is not None:
+                        loss = self.aug_loss.composite(out["augmented_tensor"], loss, self.ce_weight, self.loss_cfg.scale, self.loss_parts)
+                elif self.aug_loss is not None:
+                    raise ValueError("TrainStep(aug_loss=...) needs a model with a RangeAugment augmentor (model.learn_augmentation.mode: "
+                                     "distribution); this model returned plain logits")
+                else:
+                    loss = cross_entropy(out, y, _cfg=self.loss_cfg)
             else:
                 loss = self.forward_loss(self.model, *inputs, self.loss_cfg)
             torch.autograd.backward(loss, grad_tensors=self._one)
@@ -167,6 +190,79 @@ class TrainStep:
     @property
     def static_inputs(self):
         return None if self._static is None else self._static[:-1]
+
+
+def linear_curriculum(start: float, end: float, period: int) -> torch.Tensor:
+    """loss_fn/neural_augmentation.py:linear_curriculum: period + 1 points from start to end."""
+    return torch.linspace(start=start, end=end, steps=period + 1, dtype=torch.float)
+
+
+def cosine_curriculum(start: float, end: float, period: int) -> torch.Tensor:
+    """loss_fn/neural_augmentation.py:cosine_curriculum."""
+    import math
+    return torch.tensor([end + 0.5 * (start - end) * (1 + math.cos(math.pi * i / (period + 1))) for i in range(period + 1)], dtype=torch.float)
+
+
+def psnr_to_mse(psnr: float) -> float:
+    """PSNR = 20 log10(255) - 10 log10(MSE) (neural_augmentation.py:69)."""
+    import math
+    return 10.0 ** ((20.0 * math.log10(255.0) - psnr) / 10.0)
+
+
+class NeuralAugmentationLoss:
+    """The RangeAugment loss with the PSNR metric (loss_fn/neural_augmentation.py:NeuralAugmentation): a smooth-L1 loss between each augmented
+    image's MSE against its (mixed) input, in 0..255 units, and a target MSE, times alpha / 65025.  ``target_value`` is a PSNR or a
+    (start, end) pair followed over ``period`` (= scheduler.max_epochs, or max_iterations when iteration based) steps by the ``linear`` or
+    ``cosine`` curriculum; past the end the last entry holds.  The table and the position (``set_epoch``) live on the device.  ``weight`` is
+    the term's weight in the composite loss.  The loss reads the squared errors the augmentor kernels computed (``augmented_tensor`` must come
+    from ``DistributionNeuralAugmentor``)."""
+
+    def __init__(self, target_value=(40, 10), curriculum_method: str = "cosine", alpha: float = 100.0, period: Optional[int] = None,
+                 weight: float = 1.0):
+        if isinstance(target_value, (int, float)):
+            self.table = torch.tensor([psnr_to_mse(float(target_value))], dtype=torch.float)
+        elif isinstance(target_value, (list, tuple)) and len(target_value) == 2:
+            if period is None:
+                raise ValueError("a (start, end) target needs period (scheduler.max_epochs or scheduler.max_iterations)")
+            fn = {"linear": linear_curriculum, "cosine": cosine_curriculum}.get(curriculum_method)
+            if fn is None:
+                raise NotImplementedError(f"curriculum_method {curriculum_method!r}: 'linear' or 'cosine'")
+            self.table = fn(start=psnr_to_mse(float(target_value[0])), end=psnr_to_mse(float(target_value[1])), period=int(period))
+        else:
+            raise NotImplementedError(f"target_value {target_value!r}: a PSNR or a (start, end) pair")
+        self.alpha, self.weight = float(alpha), float(weight)
+        self.epoch = 0
+        self._target = self._step = None
+
+    def _device(self, device):
+        if self._target is None or self._target.device != device:
+            self._target = self.table.to(device)
+            self._step = torch.tensor([self.epoch], dtype=torch.int64, device=device)
+        return self._target, self._step
+
+    def set_epoch(self, epoch: int) -> None:
+        self.epoch = int(epoch)
+        if self._step is not None:
+            # a fresh pinned buffer per call: the copy queued by an earlier call may not have run yet and must still read its own value
+            # (the host allocator keeps the buffer until the copy is done)
+            self._step.copy_(torch.tensor([self.epoch], dtype=torch.int64).pin_memory(), non_blocking=True)
+
+    def _apply(self, x_aug: torch.Tensor, ce, w_na: float, ce_weight: float, scale, parts):
+        sq = getattr(x_aug, "_cvb_sq", None)
+        if sq is None:
+            raise ValueError("NeuralAugmentationLoss needs the augmented_tensor of a DistributionNeuralAugmentor (model output in training mode)")
+        target, step = self._device(sq.device)
+        cfg = SimpleNamespace(target=target, step=step, alpha=self.alpha, w_na=w_na, w_ce=float(ce_weight), H=x_aug.shape[2], W=x_aug.shape[3],
+                              scale=scale, parts=parts)
+        return Fn.NeuralAugLossFn.apply(sq, ce, cfg)
+
+    def __call__(self, input_sample, prediction) -> torch.Tensor:
+        """L_na of ``prediction["augmented_tensor"]`` (the reference's call signature; the input is the image the augmentor was given)."""
+        return self._apply(prediction["augmented_tensor"], None, 1.0, 1.0, None, None)
+
+    def composite(self, x_aug: torch.Tensor, ce: torch.Tensor, ce_weight: float = 1.0, scale=None, parts=None) -> torch.Tensor:
+        """ce_weight * ce + weight * L_na in one launch; ``parts`` (device fp32 [2]) receives (ce, L_na)."""
+        return self._apply(x_aug, ce, self.weight, ce_weight, scale, parts)
 
 
 class MixingSampler:

@@ -162,7 +162,9 @@ class StemFn(torch.autograd.Function):
         M = B * Ho * Wo
         xin = x if x.dtype == torch.float32 else x.float()
         ws = getattr(cfg, "ws", None)
-        A0 = ops.stem_im2col(xin, mix=ws.mix if (ws is not None and ws.active) else None)  # batch mixing rides in the gather (TrainStep.set_mix)
+        # batch mixing rides in the gather (TrainStep.set_mix), unless the input is the augmentor's output, which is already mixed
+        mix = ws.mix if (ws is not None and ws.active and not getattr(x, "_cvb_premixed", False)) else None
+        A0 = ops.stem_im2col(xin, mix=mix)
         Ws = cfg.prep.get(cfg.i_w)
         st = _fwd_arena(cfg, x.device).f64(2, C0)
         y = ops.pw_gemm(A0, Ws, C0, col_stats=st if cfg.bn.batch_stats else None)
@@ -170,7 +172,7 @@ class StemFn(torch.autograd.Function):
         ctx.lz_out = cfg.last_lazy = LazyBN(bn, True) if cfg.lazy_out else None
         out = y if cfg.lazy_out else ops.bn_apply(y, bn, act=True)
         ctx.cfg, ctx.dims, ctx.ev = cfg, (B, Ho, Wo, C0, M), (not cfg.bn.batch_stats,)
-        ctx.saved = (A0, y, bn)
+        ctx.saved = (A0, y, bn, Ws)
         ctx.plist = cfg.plist
         ctx.save_for_backward(gamma)
         return to_4d(out, B, Ho, Wo)
@@ -179,7 +181,7 @@ class StemFn(torch.autograd.Function):
     def backward(ctx, gout):
         cfg = ctx.cfg
         B, Ho, Wo, C0, M = ctx.dims
-        A0, y, bn = ctx.saved
+        A0, y, bn, Ws = ctx.saved
         (gamma,) = ctx.saved_tensors
         g2 = as_2d(to_bf16_cl(gout))
         D = _Dst(cfg, ctx.plist, g2.device, True)
@@ -193,8 +195,86 @@ class StemFn(torch.autograd.Function):
         D.set_pair(1, 2, dgb)
         dW = ops.pw_wgrad_side(dz, A0, C0, 32, g_mode=A_BNB, G2=y, g_p=coef, dW=D.ar.f32(C0, 32))
         D.unprep(0, dW, C0, 27, 32, 0, side=True)
+        # the image's gradient exists only when something upstream learns (the RangeAugment sampler parameters)
+        dx = ops.stem_dgrad(dz, y, coef, Ws, B, Ho, Wo) if ctx.needs_input_grad[0] else None
         ops.join_side()
+        return (dx, None) + D.finish()
+
+
+# ==================================================================================================================
+# RangeAugment (cvnets/neural_augmentor/neural_aug.py:214-236 with DistributionNeuralAugmentor's UniformSamplers) and its loss
+# (loss_fn/neural_augmentation.py:178-218).  Kernels and draw layout: csrc/neural_aug.cu.
+# ==================================================================================================================
+class NeuralAugmentFn(torch.autograd.Function):
+    """(x, cfg, *raw) -> (x_aug fp32 [B, 3, H, W], sq fp64 [B, 3] = per-(sample, channel) sum of (x_aug - x_mix)^2).
+
+    ``raw`` are the enabled samplers' (_low, _high) parameters in brightness, contrast, noise order; ``cfg.enabled`` says which.  Inside
+    TrainStep the image is first mixed as ``ws.mix`` says (on the fly, in every kernel that reads it), so the augmentor, the stem and the
+    PSNR loss all see the mixed image, as the reference's training_engine.py:236-238 does."""
+
+    @staticmethod
+    def forward(ctx, x, cfg, *raw):
+        B, C, H, W = x.shape
+        if C != 3:
+            raise NotImplementedError(f"RangeAugment: {C}-channel input (the kernels take RGB images)")
+        x = x.float().contiguous()
+        ws = _ws_of(cfg, raw)
+        mix = ws.mix if ws is not None else None
+        key = ops.rng_next(x.device)
+        full = [None] * 6
+        it = iter(raw)
+        for k in range(3):
+            if cfg.enabled >> k & 1:
+                full[2 * k], full[2 * k + 1] = next(it), next(it)
+        fa = _fwd_arena(cfg, x.device)
+        tab, mu, coef, sq = fa.f32(4 + 3 * B), fa.f64(2, 3 * B), fa.f32(3 * B, 3), fa.f64(B, 3)
+        need_eps = bool(cfg.enabled & 4)
+        ops.na_plan(key, B, cfg.enabled, tab)
+        ops.na_stats(x, mix, key, need_eps, mu)
+        ops.na_compose(tab, mu, full, B, coef)
+        y = ops.na_apply(x, mix, key, coef, need_eps, sq)
+        ctx.cfg, ctx.saved = cfg, (x, mix, key, tab, mu, coef, full, need_eps)
+        ctx.plist = list(raw)
+        ctx.set_materialize_grads(False)  # an output without a gradient arrives as None (no zero tensor is filled); the kernel skips its term
+        return y, sq
+
+    @staticmethod
+    def backward(ctx, g_y, g_sq):
+        x, mix, key, tab, mu, coef, full, need_eps = ctx.saved
+        B = x.shape[0]
+        D = _Dst(ctx.cfg, ctx.plist, x.device, True)
+        red = D.ar.f64(3 * B, 3)
+        ops.na_bwd_reduce(None if g_y is None else g_y.float().contiguous(), None if g_sq is None else g_sq.contiguous(), x, mix, key, coef, need_eps,
+                          red)
+        dests, i = [None] * 6, 0
+        for j in range(6):
+            if full[j] is not None:
+                dests[j] = D.mat(i, 1, 1)
+                i += 1
+        ops.na_param_grad(tab, mu, red, full, B, dests)
         return (None, None) + D.finish()
+
+
+class NeuralAugLossFn(torch.autograd.Function):
+    """(sq fp64 [B, 3], ce 0-dim or None) -> w_na * L_na + w_ce * ce, L_na = alpha / 65025 * mean_b smooth_l1(mse_b - target[step]) (0-dim
+    fp32; loss_fn/composite_loss.py with loss_fn/neural_augmentation.py).  ``cfg``: target (device fp32 table), step (device int64 [1]), alpha,
+    w_na, w_ce, H, W, scale (device loss scale or None), parts (device fp32 [2] for (ce, L_na), or None)."""
+
+    @staticmethod
+    def forward(ctx, sq, ce, cfg):
+        loss = torch.empty((), device=sq.device, dtype=torch.float32)
+        ops.na_loss_fwd(sq, cfg.H, cfg.W, cfg.target, cfg.step, cfg.alpha, loss, w_na=cfg.w_na, ce=ce, w_ce=cfg.w_ce, parts=cfg.parts)
+        ctx.cfg, ctx.has_ce = cfg, ce is not None
+        ctx.save_for_backward(sq)
+        return loss
+
+    @staticmethod
+    def backward(ctx, g):
+        (sq,) = ctx.saved_tensors
+        c = ctx.cfg
+        g_ce = torch.empty((), device=sq.device, dtype=torch.float32) if ctx.has_ce else None
+        g_sq = ops.na_loss_bwd(sq, c.H, c.W, c.target, c.step, c.alpha, g.contiguous(), c.scale, w_na=c.w_na, g_ce=g_ce, w_ce=c.w_ce)
+        return g_sq, g_ce, None
 
 
 # ==================================================================================================================

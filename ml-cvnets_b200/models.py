@@ -8,7 +8,7 @@ from __future__ import annotations
 
 import argparse
 from types import SimpleNamespace
-from typing import Dict, List, Optional, Tuple
+from typing import Dict, List, Optional, Tuple, Union
 
 import torch
 from torch import Tensor, nn
@@ -16,6 +16,7 @@ from torch import Tensor, nn
 from . import functional as Fn
 from .layers import ConvLayer2d, GlobalPool, Identity, LinearLayer, norm_layers_tuple
 from .modules import InvertedResidual, MobileViTBlockv2, _require_cuda, make_divisible
+from .neural_aug import augmented_forward, build_neural_augmentor
 from .ops import PreparedWeights as PW
 
 
@@ -80,6 +81,7 @@ class MobileViTv2(nn.Module):
         self.output_stride = output_stride
         self.model_conf_dict = dict()
         c0 = cfg["layer0"]["out_channels"]
+        self.neural_augmentor = build_neural_augmentor(opts)  # before conv_1: its parameters come first (base_image_encoder.py:50)
         self.conv_1 = ConvLayer2d(opts=opts, in_channels=cfg["layer0"]["img_channels"], out_channels=c0, kernel_size=3, stride=2,
                                   use_norm=True, use_act=True)
         self.model_conf_dict["conv1"] = {"in": 3, "out": c0}
@@ -242,6 +244,8 @@ class MobileViTv2(nn.Module):
         self._head.prep.prepare(force=self.training)
         return Fn.PoolLinearFn.apply(Fn.to_bf16_cl(x), self._head, lin.weight, lin.bias)
 
-    def forward(self, x: Tensor, *args, **kwargs) -> Tensor:
+    def forward(self, x: Tensor, *args, **kwargs) -> Union[Tensor, Dict[str, Optional[Tensor]]]:
         _require_cuda(x, "MobileViTv2")
+        if self.neural_augmentor is not None:
+            return augmented_forward(self, x)
         return self.forward_classifier(x)

@@ -9,12 +9,13 @@ from __future__ import annotations
 
 import argparse
 import math
-from typing import Dict, List, Optional, Tuple
+from typing import Dict, List, Optional, Tuple, Union
 
 from torch import Tensor, nn
 
 from .layers import ConvLayer2d, Dropout, GlobalPool, LinearLayer, norm_layers_tuple
 from .modules import EfficientNetBlock, _require_cuda, make_divisible
+from .neural_aug import augmented_forward, build_neural_augmentor
 
 # mode: (width_mult, depth_mult, train_resolution)
 _COMPOUND_SCALING = {"b0": (1.0, 1.0, 224), "b1": (1.0, 1.1, 240), "b2": (1.1, 1.2, 260), "b3": (1.2, 1.4, 300), "b4": (1.4, 1.8, 380),
@@ -67,6 +68,7 @@ class EfficientNet(nn.Module):
         cfg = get_effnet_configuration(opts)
         self.opts, self.dilation = opts, 1
         c = cfg["layer_1"][0][3]
+        self.neural_augmentor = build_neural_augmentor(opts)  # before conv_1: its parameters come first (base_image_encoder.py:50)
         self.conv_1 = ConvLayer2d(opts=opts, in_channels=3, out_channels=c, kernel_size=3, stride=2, use_norm=True, use_act=True)
         prev = 0
         for name in LAYERS:
@@ -141,9 +143,14 @@ class EfficientNet(nn.Module):
                 out["out_l5_exp"] = self.conv_1x1_exp(x)
         return out
 
-    def forward(self, x: Tensor, *args, **kwargs) -> Tensor:
+    def forward_classifier(self, x: Tensor, *args, **kwargs) -> Tensor:
         _require_cuda(x, "EfficientNet")
         x = self.classifier.global_pool(self.extract_features(x))
         if hasattr(self.classifier, "classifier_dropout"):
             x = self.classifier.classifier_dropout(x)
         return self.classifier.classifier_fc(x)
+
+    def forward(self, x: Tensor, *args, **kwargs) -> Union[Tensor, Dict[str, Optional[Tensor]]]:
+        if self.neural_augmentor is not None:
+            return augmented_forward(self, x)
+        return self.forward_classifier(x)

@@ -5,12 +5,13 @@ conv_1, layer_1 .. layer_5, conv_1x1_exp, classifier.{global_pool, [dropout,] fc
 from __future__ import annotations
 
 import argparse
-from typing import Dict, Optional, Tuple
+from typing import Dict, Optional, Tuple, Union
 
 from torch import Tensor, nn
 
 from .layers import ConvLayer2d, Dropout, GlobalPool, LinearLayer, norm_layers_tuple
 from .modules import InvertedResidual, MobileViTBlock, _require_cuda
+from .neural_aug import augmented_forward, build_neural_augmentor
 
 
 def default_mit_opts(mode: str = "xx_small", n_classes: int = 1000, **extra) -> argparse.Namespace:
@@ -60,6 +61,7 @@ class MobileViT(nn.Module):
         classifier_dropout = getattr(opts, "model.classification.classifier_dropout", 0.0)
         cfg = get_mit_configuration(opts)
         self.opts, self.dilation = opts, 1
+        self.neural_augmentor = build_neural_augmentor(opts)  # before conv_1: its parameters come first (base_image_encoder.py:50)
         self.conv_1 = ConvLayer2d(opts=opts, in_channels=3, out_channels=16, kernel_size=3, stride=2, use_norm=True, use_act=True)
         c = 16
         for li in range(1, 6):
@@ -124,7 +126,12 @@ class MobileViT(nn.Module):
             x = getattr(self, f"layer_{li}")(x)
         return self.conv_1x1_exp(x)
 
-    def forward(self, x: Tensor, *args, **kwargs) -> Tensor:
+    def forward(self, x: Tensor, *args, **kwargs) -> Union[Tensor, Dict[str, Optional[Tensor]]]:
+        if self.neural_augmentor is not None:
+            return augmented_forward(self, x)
+        return self.forward_classifier(x)
+
+    def forward_classifier(self, x: Tensor, *args, **kwargs) -> Tensor:
         _require_cuda(x, "MobileViT")
         x = self.extract_features(x)
         x = self.classifier.global_pool(x)

@@ -680,6 +680,94 @@ def dropout_bwd(DY: Tensor, p: float, key: Tensor, p_row: float = 0.0, rows_per_
     return DV
 
 
+# ----------------------------------------------------------------------------------------------------- RangeAugment
+def _ptr6(ts: Sequence[Optional[Tensor]]):
+    return (ctypes.c_void_p * 6)(*[_p(t) for t in ts])
+
+
+def na_plan(key: Tensor, B: int, enabled: int, tab: Tensor) -> Tensor:
+    """Draw table fp32 [4 + 3 B] of one step (see cvb_na_plan); ``enabled`` bit k = brightness / contrast / noise."""
+    L.check(_lib().cvb_na_plan(key.data_ptr(), B, int(enabled), tab.data_ptr(), _stream()), "cvb_na_plan")
+    _count()
+    return tab
+
+
+def na_noise(key: Tensor, B: int, H: int, W: int) -> Tensor:
+    """The N(0, 1) field fp32 [B, 3, H, W] that the RangeAugment kernels recompute from ``key``."""
+    eps = torch.empty((B, 3, H, W), device=key.device, dtype=torch.float32)
+    L.check(_lib().cvb_na_noise(key.data_ptr(), B, H, W, eps.data_ptr(), _stream()), "cvb_na_noise")
+    _count()
+    return eps
+
+
+def na_stats(x: Tensor, mix: Optional[Tensor], key: Tensor, need_eps: bool, mu: Tensor) -> Tensor:
+    """Per-plane means of the mixed image and of eps into fp64 ``mu`` [2, B * 3]."""
+    B, _, H, W = x.shape
+    L.check(_lib().cvb_na_stats(x.data_ptr(), _p(mix), key.data_ptr(), B, H, W, int(need_eps), mu[0].data_ptr(), mu[1].data_ptr(), _stream()),
+            "cvb_na_stats")
+    _count()
+    return mu
+
+
+def na_compose(tab: Tensor, mu: Tensor, raw: Sequence[Optional[Tensor]], B: int, coef: Tensor) -> Tensor:
+    """coef fp32 [B * 3, 3] = (A, Bc, C) per plane; ``raw`` = (_low, _high) x (brightness, contrast, noise), None where disabled."""
+    L.check(_lib().cvb_na_compose(tab.data_ptr(), mu[0].data_ptr(), mu[1].data_ptr(), _ptr6(raw), B, coef.data_ptr(), _stream()), "cvb_na_compose")
+    _count()
+    return coef
+
+
+def na_apply(x: Tensor, mix: Optional[Tensor], key: Tensor, coef: Tensor, need_eps: bool, sq: Tensor) -> Tensor:
+    """x_aug fp32 [B, 3, H, W]; writes the per-plane squared errors into fp64 ``sq`` [B, 3]."""
+    B, _, H, W = x.shape
+    Y = torch.empty_like(x)
+    L.check(_lib().cvb_na_apply(x.data_ptr(), _p(mix), key.data_ptr(), coef.data_ptr(), B, H, W, int(need_eps), Y.data_ptr(), sq.data_ptr(), _stream()),
+            "cvb_na_apply")
+    _count()
+    return Y
+
+
+def na_bwd_reduce(dY: Optional[Tensor], g_sq: Optional[Tensor], x: Tensor, mix: Optional[Tensor], key: Tensor, coef: Tensor, need_eps: bool,
+                  red: Tensor) -> Tensor:
+    B, _, H, W = x.shape
+    L.check(_lib().cvb_na_bwd_reduce(_p(dY), _p(g_sq), x.data_ptr(), _p(mix), key.data_ptr(), coef.data_ptr(), B, H, W, int(need_eps), red.data_ptr(),
+                                     _stream()), "cvb_na_bwd_reduce")
+    _count()
+    return red
+
+
+def na_param_grad(tab: Tensor, mu: Tensor, red: Tensor, raw: Sequence[Optional[Tensor]], B: int, grads: Sequence[Optional[Tensor]]):
+    L.check(_lib().cvb_na_param_grad(tab.data_ptr(), mu[0].data_ptr(), mu[1].data_ptr(), red.data_ptr(), _ptr6(raw), B, _ptr6(grads), _stream()),
+            "cvb_na_param_grad")
+    _count()
+
+
+def na_loss_fwd(sq: Tensor, H: int, W: int, target: Tensor, step: Tensor, alpha: float, loss: Tensor, w_na: float = 1.0, ce: Optional[Tensor] = None,
+                w_ce: float = 1.0, parts: Optional[Tensor] = None) -> Tensor:
+    """loss (0-dim fp32) = w_na * L_na(sq) + w_ce * ce; ``parts`` fp32 [2] receives (ce, L_na)."""
+    L.check(_lib().cvb_na_loss_fwd(sq.data_ptr(), sq.shape[0], H, W, target.data_ptr(), target.numel(), step.data_ptr(), float(alpha), float(w_na), _p(ce),
+                                   float(w_ce), loss.data_ptr(), _p(parts), _stream()), "cvb_na_loss_fwd")
+    _count()
+    return loss
+
+
+def na_loss_bwd(sq: Tensor, H: int, W: int, target: Tensor, step: Tensor, alpha: float, grad_out: Optional[Tensor], grad_scale: Optional[Tensor],
+                w_na: float = 1.0, g_ce: Optional[Tensor] = None, w_ce: float = 1.0) -> Tensor:
+    g_sq = torch.empty_like(sq)
+    L.check(_lib().cvb_na_loss_bwd(sq.data_ptr(), sq.shape[0], H, W, target.data_ptr(), target.numel(), step.data_ptr(), float(alpha), float(w_na),
+                                   _p(grad_out), _p(grad_scale), g_sq.data_ptr(), _p(g_ce), float(w_ce), _stream()), "cvb_na_loss_bwd")
+    _count()
+    return g_sq
+
+
+def stem_dgrad(dz: Tensor, y: Tensor, coef: Tensor, Ws: Tensor, B: int, Ho: int, Wo: int) -> Tensor:
+    """Stem input gradient fp32 [B, 3, 2 Ho, 2 Wo] from dz / y bf16 [B*Ho*Wo, C0], the BatchNorm-backward coef [3, C0] and the prepared weight."""
+    C0 = dz.shape[1]
+    dX = torch.empty((B, 3, 2 * Ho, 2 * Wo), device=dz.device, dtype=torch.float32)
+    L.check(_lib().cvb_stem_dgrad(dz.data_ptr(), y.data_ptr(), coef.data_ptr(), Ws.data_ptr(), B, Ho, Wo, C0, dX.data_ptr(), _stream()), "cvb_stem_dgrad")
+    _count()
+    return dX
+
+
 def ln_stats(X: Tensor, eps: float) -> Tensor:
     """per-token LayerNorm statistics of a bf16 [M, C] matrix -> fp32 [2, M] (mean, rstd)."""
     lib = _lib()
