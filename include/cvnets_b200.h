@@ -265,10 +265,17 @@ CVB_API int cvb_set_mha_impl(int mode);
  * dgamma[c] += sum_m V*xhat, dbeta[c] += sum_m V, col_sum[c] += sum_m DX (optional: bias gradient of the producer).  C <= 1024. */
 CVB_API int cvb_ln_bwd(const void* V, const void* X, const float* mean, const float* rstd, const float* gamma, const void* DRES, void* DX,
                int64_t M, int C, double* dgamma, double* dbeta, double* col_sum, cvb_stream_t stream);
-/* element-wise activation passes over contiguous bf16 tensors of n elements (n % 8 == 0): Y = act(X);  DX = DY * act'(X).
- * kind 0 = SiLU (cvnets/layers/activation/swish.py), 1 = GELU (cvnets/layers/activation/gelu.py: nn.GELU, erf form), 2 = ReLU, 3 = Hardswish,
- * 4 = Hardsigmoid, 5 = Sigmoid (cvnets/layers/activation/{relu,hard_swish,hard_sigmoid,sigmoid}.py).  Used by the TransformerEncoder FFN
- * (cvnets/modules/transformer.py:86-95) when the activation is not the GEMM-fused SiLU, and by InvertedResidualSE / SqueezeExcitation. */
+/* element-wise activation passes over contiguous bf16 tensors of n elements (n % 8 == 0): Y = act(X);  DX = DY * act'(X), act = kind.
+ * Used by the TransformerEncoder FFN (cvnets/modules/transformer.py:86-95) when the activation is not the GEMM-fused SiLU, and by
+ * InvertedResidualSE / SqueezeExcitation. */
+enum {
+  CVB_ACT_SILU = 0,     /* cvnets/layers/activation/swish.py                      */
+  CVB_ACT_GELU,         /* cvnets/layers/activation/gelu.py: nn.GELU, erf form    */
+  CVB_ACT_RELU,         /* cvnets/layers/activation/relu.py                       */
+  CVB_ACT_HARDSWISH,    /* cvnets/layers/activation/hard_swish.py: x*relu6(x+3)/6 */
+  CVB_ACT_HARDSIGMOID,  /* cvnets/layers/activation/hard_sigmoid.py: relu6(x+3)/6 */
+  CVB_ACT_SIGMOID       /* cvnets/layers/activation/sigmoid.py                    */
+};
 CVB_API int cvb_act_fwd(const void* X, void* Y, int64_t n, int kind, cvb_stream_t stream);
 CVB_API int cvb_act_bwd(const void* DY, const void* X, void* DX, int64_t n, int kind, cvb_stream_t stream);
 CVB_API int cvb_ln_stats(const void* X, int ldx, int64_t M, int C, float eps, float* mean, float* rstd, cvb_stream_t stream);
@@ -424,23 +431,32 @@ CVB_API int cvb_global_pool_bwd(const void* DOUT, int B, int HW, int C, void* DX
 /* fp32 [N] += column sums of a bf16 (or fp32) [M, ld] matrix */
 CVB_API int cvb_col_sum(const void* X, int x_fp32, int ld, int64_t M, int N, float* out, cvb_stream_t stream);
 
-/* Batched weight preparation: one launch converts every fp32 parameter the step needs into the kernel layouts.
- * kind 0: dst[r*ldd + c] = bf16(src[perm(r)*cols + c])           (row-major [rows, cols] -> bf16 [rows, ldd], zero padded)
- * kind 1: dst[c*ldd + r] = bf16(src[perm(r)*cols + c])           (transposed:          -> bf16 [cols, ldd])
- * kind 2: dst_f32[c*rows + r] = float(bf16(src[r*cols + c]))     (depthwise / stem: [C, taps] -> fp32 [taps, C], bf16-rounded)
- * kind 3: dst_f32[perm^-1 ...]: dst_f32[r] = src[perm(r)]        (fp32 vector gather, e.g. permuted bias; cols = 1)
- * kind 4: dst[r*ldd + (t*Cin + ci)] = bf16(src[r*cols + ci*taps + t])   (dense conv weight [Cout, Cin, k, k] -> patch-matrix order; rot = taps = k*k)
- * kind 5: the same, transposed: dst[(t*Cin + ci)*ldd + r]
- * perm(r) = (r + rot) % rows for r < rows (rot = 1 moves the reference's leading query row of qkv_proj to the end; kinds 0, 1, 3). */
+/* Layout kinds of cvb_prep_weights (fp32 parameter -> kernel layout) and of cvb_unprep_grad (fp32 gradient in a kernel layout -> the
+ * parameter's layout; ROWMAJOR, TAPMAJOR_F32, VECTOR_F32 and PATCH only).  perm(r) = (r + rot) % rows for r < rows (rot = 1 moves the
+ * reference's leading query row of qkv_proj to the end; ROWMAJOR, TRANSPOSED, VECTOR_F32). */
+enum {
+  CVB_PREP_ROWMAJOR = 0,  /* prep:   dst[r*ldd + c] = bf16(src[perm(r)*cols + c])   (row-major [rows, cols] -> bf16 [rows, ldd], zero padded)
+                             unprep: dst[perm(r)*cols + c] = src[r*lds + c]                                                        */
+  CVB_PREP_TRANSPOSED,    /* prep:   dst[c*ldd + r] = bf16(src[perm(r)*cols + c])   (transposed: -> bf16 [cols, ldd])              */
+  CVB_PREP_TAPMAJOR_F32,  /* prep:   dst_f32[c*rows + r] = float(bf16(src[r*cols + c]))   (depthwise / stem: [C, taps] -> fp32 [taps, C],
+                                     bf16-rounded)
+                             unprep: tap-major [taps, C] -> [C, taps]                                                              */
+  CVB_PREP_VECTOR_F32,    /* prep:   dst_f32[r] = src[perm(r)]   (fp32 vector gather, e.g. permuted bias; cols = 1)
+                             unprep: dst[perm(r)] = src[r]                                                                         */
+  CVB_PREP_PATCH,         /* prep:   dst[r*ldd + (t*Cin + ci)] = bf16(src[r*cols + ci*taps + t])   (dense conv weight [Cout, Cin, k, k] ->
+                                     patch-matrix order; rot = taps = k*k)
+                             unprep: dst[r*cols + ci*taps + t] = src[r*lds + t*Cin + ci], rot = taps (dense-conv weight gradients)  */
+  CVB_PREP_PATCH_T        /* prep:   the same, transposed: dst[(t*Cin + ci)*ldd + r]                                                */
+};
+
+/* Batched weight preparation: one launch converts every fp32 parameter the step needs into the kernel layouts. */
 typedef struct {
   const float* src; void* dst; int rows, cols, ldd, dst_rows; int kind; int rot;
 } cvb_prep_desc;
 CVB_API int cvb_prep_weights(const cvb_prep_desc* descs_device, int n_desc, int max_elems, cvb_stream_t stream);
 
-/* fp32 gradient scatter-back for permuted layouts: dst[perm(r)*cols + c] = src[r*lds + c] (kind 0) or
- * dst[c*?]..: kind 2 (tap-major [taps, C] -> [C, taps]).  Used for qkv / depthwise / stem weight gradients. */
+/* fp32 gradient scatter-back for permuted layouts (qkv / depthwise / stem / dense-conv weight gradients). */
 CVB_API int cvb_unprep_grad(const float* src, float* dst, int rows, int cols, int lds, int kind, int rot, cvb_stream_t stream);
-/* (kind 4: dst[r*cols + ci*taps + t] = src[r*lds + t*Cin + ci], rot = taps: the inverse of prep kind 4 for dense-conv weight gradients) */
 
 /* ---------------------------------------------------------------------------------------------------------------
  * Dense (groups = 1) k x k convolution = im2col + cvb_pw_gemm (ConvLayer2d at cvnets/models/classification/vit.py:90-121 -- the ViT / CLIP

@@ -552,29 +552,28 @@ __global__ void __launch_bounds__(NT) ln_bwd_kernel(const bf16* __restrict__ V, 
 }
 
 // stand-alone activation passes for the transformer FFN when the activation is not SiLU (GELU of the ViT / CLIP recipes; the
-// SiLU FFN keeps the activation fused into the GEMM load / epilogue modes).  kind: 0 = SiLU, 1 = GELU (erf form, nn.GELU default),
-// 2 = ReLU, 3 = Hardswish x*relu6(x+3)/6, 4 = Hardsigmoid relu6(x+3)/6 (cvnets/layers/activation/{relu,hard_swish,hard_sigmoid}.py: the
-// MobileNetv3-style InvertedResidualSE block, cvnets/modules/mobilenetv2.py:16-138), 5 = Sigmoid
+// SiLU FFN keeps the activation fused into the GEMM load / epilogue modes; Hardswish / Hardsigmoid: the MobileNetv3-style InvertedResidualSE
+// block, cvnets/modules/mobilenetv2.py:16-138).  kind: CVB_ACT_*; the default branch is CVB_ACT_SIGMOID.
 __device__ __forceinline__ float act_fwd_f(float x, int kind) {
   switch (kind) {
-    case 0: return silu_f(x);
-    case 1: return 0.5f * x * (1.0f + erff(x * 0.70710678118654752f));
-    case 2: return fmaxf(x, 0.f);
-    case 3: return x * fminf(fmaxf(x + 3.0f, 0.f), 6.0f) * (1.0f / 6.0f);
-    case 4: return fminf(fmaxf(x + 3.0f, 0.f), 6.0f) * (1.0f / 6.0f);
+    case CVB_ACT_SILU: return silu_f(x);
+    case CVB_ACT_GELU: return 0.5f * x * (1.0f + erff(x * 0.70710678118654752f));
+    case CVB_ACT_RELU: return fmaxf(x, 0.f);
+    case CVB_ACT_HARDSWISH: return x * fminf(fmaxf(x + 3.0f, 0.f), 6.0f) * (1.0f / 6.0f);
+    case CVB_ACT_HARDSIGMOID: return fminf(fmaxf(x + 3.0f, 0.f), 6.0f) * (1.0f / 6.0f);
     default: return 1.0f / (1.0f + __expf(-x));
   }
 }
 __device__ __forceinline__ float act_grad_f(float x, int kind) {
   switch (kind) {
-    case 0: return silu_grad_f(x);
-    case 1: {
+    case CVB_ACT_SILU: return silu_grad_f(x);
+    case CVB_ACT_GELU: {
       const float cdf = 0.5f * (1.0f + erff(x * 0.70710678118654752f));
       return cdf + x * 0.3989422804014327f * __expf(-0.5f * x * x);
     }
-    case 2: return x > 0.f ? 1.f : 0.f;
-    case 3: return x <= -3.0f ? 0.f : (x < 3.0f ? fmaf(x, 1.0f / 3.0f, 0.5f) : 1.0f);  // torch's hardswish_backward: 0 at -3, 1 at 3
-    case 4: return (x > -3.0f && x < 3.0f) ? (1.0f / 6.0f) : 0.f;
+    case CVB_ACT_RELU: return x > 0.f ? 1.f : 0.f;
+    case CVB_ACT_HARDSWISH: return x <= -3.0f ? 0.f : (x < 3.0f ? fmaf(x, 1.0f / 3.0f, 0.5f) : 1.0f);  // torch's hardswish_backward: 0 at -3, 1 at 3
+    case CVB_ACT_HARDSIGMOID: return (x > -3.0f && x < 3.0f) ? (1.0f / 6.0f) : 0.f;
     default: {
       const float s = 1.0f / (1.0f + __expf(-x));
       return s * (1.0f - s);
@@ -778,28 +777,29 @@ __global__ void __launch_bounds__(NT) prep_weights_kernel(const cvb_prep_desc* _
   pdl_wait();
   pdl_trigger();
   const cvb_prep_desc d = descs[blockIdx.y];
-  const int64_t total = (d.kind == 2) ? (int64_t)d.rows * d.cols : (d.kind == 3 ? (int64_t)d.dst_rows : (int64_t)d.dst_rows * d.ldd);
+  const int64_t total = (d.kind == CVB_PREP_TAPMAJOR_F32) ? (int64_t)d.rows * d.cols
+                        : (d.kind == CVB_PREP_VECTOR_F32 ? (int64_t)d.dst_rows : (int64_t)d.dst_rows * d.ldd);
   for (int64_t i = (int64_t)blockIdx.x * NT + threadIdx.x; i < total; i += (int64_t)gridDim.x * NT) {
-    if (d.kind == 0) {
+    if (d.kind == CVB_PREP_ROWMAJOR) {
       int r = (int)(i / d.ldd), c = (int)(i % d.ldd);
       float v = (r < d.rows && c < d.cols) ? d.src[(int64_t)perm_row(r, d.rows, d.rot) * d.cols + c] : 0.f;
       static_cast<bf16*>(d.dst)[i] = __float2bfloat16_rn(v);
-    } else if (d.kind == 1) {
+    } else if (d.kind == CVB_PREP_TRANSPOSED) {
       int c = (int)(i / d.ldd), r = (int)(i % d.ldd);
       float v = (r < d.rows && c < d.cols) ? d.src[(int64_t)perm_row(r, d.rows, d.rot) * d.cols + c] : 0.f;
       static_cast<bf16*>(d.dst)[i] = __float2bfloat16_rn(v);
-    } else if (d.kind == 2) {
+    } else if (d.kind == CVB_PREP_TAPMAJOR_F32) {
       int tap = (int)(i / d.rows), ch = (int)(i % d.rows);
       static_cast<float*>(d.dst)[i] = bf16_round(d.src[(int64_t)ch * d.cols + tap]);
-    } else if (d.kind == 4 || d.kind == 5) {
+    } else if (d.kind == CVB_PREP_PATCH || d.kind == CVB_PREP_PATCH_T) {
       // dense conv weight [rows = Cout][cols = Cin * taps] in (ci, tap) order -> patch-matrix order (tap, ci); rot = taps.
-      // kind 4: row-major [dst_rows, ldd];  kind 5: transposed [cols, ldd >= rows]
-      const int r = (d.kind == 4) ? (int)(i / d.ldd) : (int)(i % d.ldd), c = (d.kind == 4) ? (int)(i % d.ldd) : (int)(i / d.ldd);
+      // PATCH: row-major [dst_rows, ldd];  PATCH_T: transposed [cols, ldd >= rows]
+      const int r = (d.kind == CVB_PREP_PATCH) ? (int)(i / d.ldd) : (int)(i % d.ldd), c = (d.kind == CVB_PREP_PATCH) ? (int)(i % d.ldd) : (int)(i / d.ldd);
       const int cin = d.cols / d.rot;
       float v = 0.f;
       if (r < d.rows && c < d.cols) v = d.src[(int64_t)r * d.cols + (c % cin) * d.rot + c / cin];
       static_cast<bf16*>(d.dst)[i] = __float2bfloat16_rn(v);
-    } else {
+    } else {  // CVB_PREP_VECTOR_F32
       int r = (int)i;
       static_cast<float*>(d.dst)[i] = (r < d.rows) ? d.src[perm_row(r, d.rows, d.rot)] : 0.f;
     }
@@ -812,17 +812,17 @@ __global__ void __launch_bounds__(NT) unprep_grad_kernel(const float* __restrict
   pdl_trigger();
   const int64_t total = (int64_t)rows * cols;
   for (int64_t i = (int64_t)blockIdx.x * NT + threadIdx.x; i < total; i += (int64_t)gridDim.x * NT) {
-    if (kind == 0) {
+    if (kind == CVB_PREP_ROWMAJOR) {
       int r = (int)(i / cols), c = (int)(i % cols);
       dst[(int64_t)perm_row(r, rows, rot) * cols + c] = src[(int64_t)r * lds + c];
-    } else if (kind == 2) {  // src [taps=cols][C=rows] -> dst [C][taps]
+    } else if (kind == CVB_PREP_TAPMAJOR_F32) {  // src [taps=cols][C=rows] -> dst [C][taps]
       int ch = (int)(i / cols), tap = (int)(i % cols);
       dst[i] = src[(int64_t)tap * rows + ch];
-    } else if (kind == 4) {  // src [rows][(tap, ci)] (leading dim lds) -> dst [rows][(ci, tap)], rot = taps
+    } else if (kind == CVB_PREP_PATCH) {  // src [rows][(tap, ci)] (leading dim lds) -> dst [rows][(ci, tap)], rot = taps
       int r = (int)(i / cols), c = (int)(i % cols);
       const int cin = cols / rot;
       dst[(int64_t)r * cols + (c % cin) * rot + c / cin] = src[(int64_t)r * lds + c];
-    } else {
+    } else {  // CVB_PREP_VECTOR_F32
       dst[perm_row((int)i, rows, rot)] = src[i];
     }
   }
@@ -949,13 +949,15 @@ extern "C" int cvb_ln_bwd(const void* V, const void* X, const float* mean, const
 }
 
 extern "C" int cvb_act_fwd(const void* X, void* Y, int64_t n, int kind, cvb_stream_t stream) {
-  CVB_CHECK(X && Y && n > 0 && n % 8 == 0 && cvb_aligned16(X) && cvb_aligned16(Y) && kind >= 0 && kind <= 5, "cvb_act_fwd: bad arguments");
+  CVB_CHECK(X && Y && n > 0 && n % 8 == 0 && cvb_aligned16(X) && cvb_aligned16(Y) && kind >= CVB_ACT_SILU && kind <= CVB_ACT_SIGMOID,
+            "cvb_act_fwd: bad arguments");
   CVB_CUDA(cvb_launch(act_fwd_kernel, grid_for(n / 8), NT, 0, static_cast<cudaStream_t>(stream), static_cast<const bf16*>(X), static_cast<bf16*>(Y), n / 8, kind));
   CVB_LAUNCH_CHECK();
   return 0;
 }
 extern "C" int cvb_act_bwd(const void* DY, const void* X, void* DX, int64_t n, int kind, cvb_stream_t stream) {
-  CVB_CHECK(DY && X && DX && n > 0 && n % 8 == 0 && cvb_aligned16(DY) && cvb_aligned16(X) && cvb_aligned16(DX) && kind >= 0 && kind <= 5,
+  CVB_CHECK(DY && X && DX && n > 0 && n % 8 == 0 && cvb_aligned16(DY) && cvb_aligned16(X) && cvb_aligned16(DX) && kind >= CVB_ACT_SILU &&
+                kind <= CVB_ACT_SIGMOID,
             "cvb_act_bwd: bad arguments");
   CVB_CUDA(cvb_launch(act_bwd_kernel, grid_for(n / 8), NT, 0, static_cast<cudaStream_t>(stream), static_cast<const bf16*>(DY), static_cast<const bf16*>(X),
                       static_cast<bf16*>(DX), n / 8, kind));

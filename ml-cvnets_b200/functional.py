@@ -16,6 +16,7 @@ import torch
 from . import ops
 from .workspace import Arena
 from .ops import A_AFF, A_AFF_SILU, A_BNB, A_GN, A_RAW, A_SILU, E_GN_BWD, E_SILU_BWD, E_STORE
+from .ops import PreparedWeights as PW
 
 BF16 = torch.bfloat16
 
@@ -127,7 +128,7 @@ class _Dst:
 
     def unprep(self, i: int, src, rows: int, cols: int, lds: int, kind: int, rot: int = 0, side: bool = False):
         """kernel-layout gradient (rotated / padded / tap-major) -> the parameter's own layout."""
-        out = self.ws.gview(self.params[i]).view((rows, cols) if kind != 3 else (rows,)) if self.ws is not None else None
+        out = self.ws.gview(self.params[i]).view((rows, cols) if kind != PW.KIND_VECTOR_F32 else (rows,)) if self.ws is not None else None
         g = ops.unprep_grad(src, rows, cols, lds, kind, rot=rot, side=side, out=out)
         if self.ws is None:
             self.grads[i] = g.view(self.params[i].shape)
@@ -194,7 +195,7 @@ class StemFn(torch.autograd.Function):
         dgb, coef = ops.bn_bwd_finalize(sd, M, gamma, bn, eval_mode=ctx.ev[0], out=D.pair(1, 2))
         D.set_pair(1, 2, dgb)
         dW = ops.pw_wgrad_side(dz, A0, C0, 32, g_mode=A_BNB, G2=y, g_p=coef, dW=D.ar.f32(C0, 32))
-        D.unprep(0, dW, C0, 27, 32, 0, side=True)
+        D.unprep(0, dW, C0, 27, 32, PW.KIND_ROWMAJOR, side=True)
         # the image's gradient exists only when something upstream learns (the RangeAugment sampler parameters)
         dx = ops.stem_dgrad(dz, y, coef, Ws, B, Ho, Wo) if ctx.needs_input_grad[0] else None
         ops.join_side()
@@ -345,7 +346,7 @@ class InvertedResidualFn(torch.autograd.Function):
         D.set_pair(4, 5, dgb2)
         dz1, dWt = ops.dw_bwd(dz2, y1, B, H, W, hid, s, P.get(cfg.i_wd), g_mode=A_BNB, Y2=y2, g_p=c2, x_mode=A_AFF_SILU,
                               x_p=(bn1[2], bn1[3]), col_stats=sd1, dWt=ar.f32(9, hid), dilation=cfg.dilation)
-        D.unprep(3, dWt, hid, 9, hid, 2)
+        D.unprep(3, dWt, hid, 9, hid, PW.KIND_TAPMAJOR_F32)
         # exp_1x1 + BN1
         dgb1, c1 = ops.bn_bwd_finalize(sd1, M, g1, bn1, ev[0], out=D.pair(1, 2))
         D.set_pair(1, 2, dgb1)
@@ -481,8 +482,8 @@ class MobileViTBlockv2Fn(torch.autograd.Function):
             dqkv = ops.linattn_bwd(qkv, dO, S, CTX, B, H, W, d, dbias=dbq)
             dWq = ops.pw_wgrad_side(dqkv, X, 2 * d + 8, d, a_mode=A_GN, a_p=(ga, ba), row_stats=(gnA[0], gnA[1]), rows_per_sample=HW,
                                     dW=ar.f32(2 * d + 8, d))
-            D.unprep(o + 2, dWq, 2 * d + 1, d, d, 0, rot=1, side=True)
-            D.unprep(o + 3, dbq, 2 * d + 1, 1, 1, 3, rot=1)
+            D.unprep(o + 2, dWq, 2 * d + 1, d, d, PW.KIND_ROWMAJOR, rot=1, side=True)
+            D.unprep(o + 3, dbq, 2 * d + 1, 1, 1, PW.KIND_VECTOR_F32, rot=1)
             csa, ssa, bsum = ar.f64(2, d), ar.f64(2, B), ar.f64(d)
             gA = ops.pw_gemm(dqkv, P.get(ix.wqkvt), d, K=2 * d + 8, e_mode=E_GN_BWD, Y=X, e_p=(ga, None), row_stats=(gnA[0], gnA[1]),
                              rows_per_sample=HW, col_stats=csa, samp_stats=ssa, gn_ws=ar.f64(2, B, d))
@@ -503,7 +504,7 @@ class MobileViTBlockv2Fn(torch.autograd.Function):
         else:
             dx, dWt = ops.dw_bwd(dz0, x2, B, H, W, C, 1, P.get(cfg.i_wd0), g_mode=A_BNB, Y2=y0, g_p=c0, x_mode=A_RAW, dWt=ar.f32(9, C),
                                  dilation=cfg.dilation)
-        D.unprep(0, dWt, C, 9, C, 2)
+        D.unprep(0, dWt, C, 9, C, PW.KIND_TAPMAJOR_F32)
         ops.join_side()
         return (to_4d(dx, B, H, W), None) + D.finish()
 
@@ -663,7 +664,7 @@ class PointwiseConvFn(torch.autograd.Function):
                 dA = ops.pw_gemm(dh, P.get(cfg.i_wt), Kc, K=cout)
             ops.pw_wgrad_side(dh, x2, cout, Kc, dW=dW, dbias=db)
         if dense:
-            D.unprep(0, dW, cout, cfg.k * cfg.k * Cin, Kc, 4, rot=cfg.k * cfg.k, side=True)
+            D.unprep(0, dW, cout, cfg.k * cfg.k * Cin, Kc, PW.KIND_PATCH, rot=cfg.k * cfg.k, side=True)
         ops.join_side()
         dx = None
         if need_dx:
@@ -727,7 +728,7 @@ class DepthwiseConvFn(torch.autograd.Function):
             dz = ops.act_bwd(dout, y, cfg.act) if cfg.act is not None else dout
             dx, dWt = ops.dw_bwd(dz, x2, B, H, W, C, cfg.stride, cfg.prep.get(cfg.i_w), dWt=D.ar.f32(taps, C), dilation=cfg.dilation,
                                  ksize=cfg.k)
-        D.unprep(0, dWt, C, taps, C, 2)
+        D.unprep(0, dWt, C, taps, C, PW.KIND_TAPMAJOR_F32)
         grads = D.finish()
         return (to_4d(dx, B, H, W), None, grads[0]) + ((grads[1], grads[2]) if cfg.bn is not None else (None, None))
 
@@ -849,8 +850,8 @@ class LinearSelfAttentionFn(torch.autograd.Function):
             ops.pw_wgrad_side(dqkv, x2, 2 * d + 8, d, dW=dWq)
             dx = ops.pw_gemm(dqkv, Pw.get(cfg.i_wqkvt), d, K=2 * d + 8)
             dxp = to_4d(ops.pw_gemm(dqkp, Pw.get(cfg.i_wqkvt), d, K=2 * d + 8), B, Pp, Mp)
-        D.unprep(0, dWq, 2 * d + 1, d, d, 0, rot=1, side=True)
-        D.unprep(1, dbq, 2 * d + 1, 1, 1, 3, rot=1)
+        D.unprep(0, dWq, 2 * d + 1, d, d, PW.KIND_ROWMAJOR, rot=1, side=True)
+        D.unprep(1, dbq, 2 * d + 1, 1, 1, PW.KIND_VECTOR_F32, rot=1)
         ops.join_side()
         return (to_4d(dx, B, Pp, N), None, dxp, gout if ctx.has_res else None) + D.finish()
 

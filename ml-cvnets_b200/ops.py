@@ -13,7 +13,9 @@ from typing import Optional, Sequence, Tuple
 import torch
 
 from . import _lib as L
-from ._lib import (A_AFF, A_AFF_SILU, A_BNB, A_GN, A_RAW, A_SILU, E_GN_BWD, E_LIN_BWD, E_SILU, E_SILU_BWD, E_STORE)  # noqa: F401
+from ._lib import (A_AFF, A_AFF_SILU, A_BNB, A_GN, A_RAW, A_SILU, E_GN_BWD, E_LIN_BWD, E_SILU, E_SILU_BWD, E_STORE,  # noqa: F401
+                   ACT_GELU, ACT_HARDSIGMOID, ACT_HARDSWISH, ACT_RELU, ACT_SIGMOID, ACT_SILU,
+                   cvb_dw_bwd_args, cvb_dw_fwd_args, cvb_gemm_args, cvb_prep_desc, cvb_wgrad_args)
 
 Tensor = torch.Tensor
 launch_count = 0  # number of kernels launched through this module (bench.py reports it as gpu_launches)
@@ -129,7 +131,7 @@ def pw_gemm(A: Tensor, W: Tensor, N: int, *, K: Optional[int] = None, a_mode: in
             row_stats = None
     if out is None:
         out = torch.empty((M, N), device=A.device, dtype=torch.bfloat16)
-    a = L.GemmArgs()
+    a = cvb_gemm_args()
     a.M, a.N, a.K = M, N, K
     a.A, a.lda = A.data_ptr(), A.stride(0)
     if A2 is not None:
@@ -154,7 +156,7 @@ def pw_gemm(A: Tensor, W: Tensor, N: int, *, K: Optional[int] = None, a_mode: in
         a.samp_sum, a.samp_sq = samp_stats[0].data_ptr(), samp_stats[1].data_ptr()
     if gn_ws is not None:
         a.gn_ws = gn_ws.data_ptr()
-    L.check(lib.cvb_pw_gemm(ctypes.byref(a), _stream()), "cvb_pw_gemm")
+    lib.cvb_pw_gemm(ctypes.byref(a), _stream())
     _count()
     return out
 
@@ -165,9 +167,9 @@ def apply_load_mode(A: Tensor, mode: int, K: int, *, A2: Optional[Tensor] = None
     M = A.shape[0]
     out = torch.empty((M, K), device=A.device, dtype=torch.bfloat16)
     p2 = a_p[2] if len(a_p) > 2 else None
-    L.check(lib.cvb_apply_load_mode(A.data_ptr(), A.stride(0), _p(A2), A2.stride(0) if A2 is not None else 0, mode, _p(a_p[0]), _p(a_p[1]), _p(p2),
-                                    _p(row_stats[0]) if row_stats is not None else None, _p(row_stats[1]) if row_stats is not None else None,
-                                    rows_per_sample, out.data_ptr(), out.stride(0), M, K, _stream()), "cvb_apply_load_mode")
+    lib.cvb_apply_load_mode(A.data_ptr(), A.stride(0), _p(A2), A2.stride(0) if A2 is not None else 0, mode, _p(a_p[0]), _p(a_p[1]), _p(p2),
+                            _p(row_stats[0]) if row_stats is not None else None, _p(row_stats[1]) if row_stats is not None else None,
+                            rows_per_sample, out.data_ptr(), out.stride(0), M, K, _stream())
     _count()
     return out
 
@@ -185,7 +187,7 @@ def pw_wgrad(G: Tensor, A: Tensor, N: int, K: int, *, g_mode: int = A_RAW, G2: O
         if a_mode != A_RAW and K >= WIDE_K and N >= WIDE_N_WGRAD:
             A = apply_load_mode(A, a_mode, K, a_p=a_p, row_stats=row_stats, rows_per_sample=rows_per_sample)  # on the stream of the weight gradient
             a_mode, a_p, row_stats = A_RAW, (None, None), None
-        a = L.WgradArgs()
+        a = cvb_wgrad_args()
         a.M, a.N, a.K = G.shape[0], N, K
         a.G, a.ldg, a.g_mode = G.data_ptr(), G.stride(0), g_mode
         if G2 is not None:
@@ -198,7 +200,7 @@ def pw_wgrad(G: Tensor, A: Tensor, N: int, K: int, *, g_mode: int = A_RAW, G2: O
         a.rows_per_sample = rows_per_sample
         a.dW, a.lddw = dW.data_ptr(), dW.stride(0)
         a.dbias = _p(dbias)
-        L.check(lib.cvb_pw_wgrad(ctypes.byref(a), _stream()), "cvb_pw_wgrad")
+        lib.cvb_pw_wgrad(ctypes.byref(a), _stream())
         if side:
             _hold(G, G2, A, A0, dW, dbias)
     _count()
@@ -212,13 +214,13 @@ def dw_fwd(X: Tensor, B: int, H: int, W: int, C: int, stride: int, Wt: Tensor, *
     lib = _lib()
     Ho, Wo = (H - 1) // stride + 1, (W - 1) // stride + 1
     Y = torch.empty((B * Ho * Wo, C), device=X.device, dtype=torch.bfloat16)
-    a = L.DwFwdArgs()
+    a = cvb_dw_fwd_args()
     a.B, a.H, a.W, a.C, a.stride = B, H, W, C, stride
     a.X, a.x_mode, a.x_p0, a.x_p1 = X.data_ptr(), x_mode, _p(x_p[0]), _p(x_p[1])
     a.Wt, a.Y, a.dilation, a.ksize = Wt.data_ptr(), Y.data_ptr(), int(dilation), int(ksize)
     if col_stats is not None:
         a.col_sum, a.col_sq = col_stats[0].data_ptr(), col_stats[1].data_ptr()
-    L.check(lib.cvb_dw_fwd(ctypes.byref(a), _stream()), "cvb_dw_fwd")
+    lib.cvb_dw_fwd(ctypes.byref(a), _stream())
     _count()
     return Y
 
@@ -232,7 +234,7 @@ def dw_bwd(DZ: Tensor, X: Tensor, B: int, H: int, W: int, C: int, stride: int, W
     DX = torch.empty((B * H * W, C), device=X.device, dtype=torch.bfloat16)
     if dWt is None:
         dWt = torch.zeros((ksize * ksize, C), device=X.device, dtype=torch.float32)
-    a = L.DwBwdArgs()
+    a = cvb_dw_bwd_args()
     a.B, a.H, a.W, a.C, a.stride = B, H, W, C, stride
     a.DZ, a.Y2, a.g_mode = DZ.data_ptr(), _p(Y2), g_mode
     a.g_p0, a.g_p1, a.g_p2 = _p(g_p[0]), _p(g_p[1]), _p(g_p[2])
@@ -240,7 +242,7 @@ def dw_bwd(DZ: Tensor, X: Tensor, B: int, H: int, W: int, C: int, stride: int, W
     a.Wt, a.DX, a.dWt, a.dilation, a.ksize = Wt.data_ptr(), DX.data_ptr(), dWt.data_ptr(), int(dilation), int(ksize)
     if col_stats is not None:
         a.col_sum, a.col_sq = col_stats[0].data_ptr(), col_stats[1].data_ptr()
-    L.check(lib.cvb_dw_bwd(ctypes.byref(a), _stream()), "cvb_dw_bwd")
+    lib.cvb_dw_bwd(ctypes.byref(a), _stream())
     _count()
     return DX, dWt
 
@@ -253,8 +255,7 @@ def im2col(x: Tensor, k: int, stride: int, pad: int, lda: Optional[int] = None) 
     A = torch.empty((B * Ho * Wo, lda), device=x.device, dtype=torch.bfloat16)
     assert x.dtype in (torch.float32, torch.bfloat16)
     sn, sc, sh, sw = x.stride()
-    L.check(_lib().cvb_im2col(x.data_ptr(), int(x.dtype == torch.float32), sn, sc, sh, sw, B, Cin, H, W, k, stride, pad, A.data_ptr(), lda, _stream()),
-            "cvb_im2col")
+    _lib().cvb_im2col(x.data_ptr(), int(x.dtype == torch.float32), sn, sc, sh, sw, B, Cin, H, W, k, stride, pad, A.data_ptr(), lda, _stream())
     _count()
     return A, Ho, Wo
 
@@ -262,7 +263,7 @@ def im2col(x: Tensor, k: int, stride: int, pad: int, lda: Optional[int] = None) 
 def col2im(dA: Tensor, B: int, Cin: int, H: int, W: int, k: int, stride: int, pad: int) -> Tensor:
     """adjoint of im2col for channels-last bf16: returns dX as the [B*H*W, Cin] matrix."""
     dX = torch.empty((B * H * W, Cin), device=dA.device, dtype=torch.bfloat16)
-    L.check(_lib().cvb_col2im(dA.data_ptr(), dA.stride(0), B, Cin, H, W, k, stride, pad, dX.data_ptr(), _stream()), "cvb_col2im")
+    _lib().cvb_col2im(dA.data_ptr(), dA.stride(0), B, Cin, H, W, k, stride, pad, dX.data_ptr(), _stream())
     _count()
     return dX
 
@@ -271,7 +272,7 @@ def embedding_fwd(tokens: Tensor, table: Tensor, pos: Optional[Tensor]) -> Tenso
     B, S = tokens.shape
     V, C = table.shape
     out = torch.empty((B, S, C), device=table.device, dtype=torch.bfloat16)
-    L.check(_lib().cvb_embedding_fwd(tokens.data_ptr(), table.data_ptr(), _p(pos), out.data_ptr(), B, S, C, V, _stream()), "cvb_embedding_fwd")
+    _lib().cvb_embedding_fwd(tokens.data_ptr(), table.data_ptr(), _p(pos), out.data_ptr(), B, S, C, V, _stream())
     _count()
     return out
 
@@ -279,7 +280,7 @@ def embedding_fwd(tokens: Tensor, table: Tensor, pos: Optional[Tensor]) -> Tenso
 def embedding_bwd(dout: Tensor, tokens: Tensor, dtable: Tensor, dpos: Optional[Tensor]) -> None:
     B, S = tokens.shape
     V, C = dtable.shape
-    L.check(_lib().cvb_embedding_bwd(dout.data_ptr(), tokens.data_ptr(), dtable.data_ptr(), _p(dpos), B, S, C, V, _stream()), "cvb_embedding_bwd")
+    _lib().cvb_embedding_bwd(dout.data_ptr(), tokens.data_ptr(), dtable.data_ptr(), _p(dpos), B, S, C, V, _stream())
     _count()
 
 
@@ -287,14 +288,14 @@ def eot_gather_fwd(X: Tensor, tokens: Tensor):
     B, S, C = X.shape
     out = torch.empty((B, C), device=X.device, dtype=torch.bfloat16)
     idx = torch.empty((B,), device=X.device, dtype=torch.int32)
-    L.check(_lib().cvb_eot_gather_fwd(X.data_ptr(), tokens.data_ptr(), B, S, C, out.data_ptr(), idx.data_ptr(), _stream()), "cvb_eot_gather_fwd")
+    _lib().cvb_eot_gather_fwd(X.data_ptr(), tokens.data_ptr(), B, S, C, out.data_ptr(), idx.data_ptr(), _stream())
     _count()
     return out, idx
 
 
 def eot_gather_bwd(dout: Tensor, idx: Tensor, B: int, S: int, C: int) -> Tensor:
     dX = torch.empty((B, S, C), device=dout.device, dtype=torch.bfloat16)
-    L.check(_lib().cvb_eot_gather_bwd(dout.data_ptr(), idx.data_ptr(), B, S, C, dX.data_ptr(), _stream()), "cvb_eot_gather_bwd")
+    _lib().cvb_eot_gather_bwd(dout.data_ptr(), idx.data_ptr(), B, S, C, dX.data_ptr(), _stream())
     _count()
     return dX
 
@@ -303,7 +304,7 @@ def l2norm_fwd(X: Tensor, eps: float = 1e-12):
     M, C = X.shape
     Y = torch.empty_like(X)
     inv = torch.empty((M,), device=X.device, dtype=torch.float32)
-    L.check(_lib().cvb_l2norm_fwd(X.data_ptr(), Y.data_ptr(), inv.data_ptr(), M, C, float(eps), _stream()), "cvb_l2norm_fwd")
+    _lib().cvb_l2norm_fwd(X.data_ptr(), Y.data_ptr(), inv.data_ptr(), M, C, float(eps), _stream())
     _count()
     return Y, inv
 
@@ -311,7 +312,7 @@ def l2norm_fwd(X: Tensor, eps: float = 1e-12):
 def l2norm_bwd(DY: Tensor, Y: Tensor, inv: Tensor) -> Tensor:
     M, C = Y.shape
     DX = torch.empty_like(Y)
-    L.check(_lib().cvb_l2norm_bwd(DY.data_ptr(), Y.data_ptr(), inv.data_ptr(), DX.data_ptr(), M, C, _stream()), "cvb_l2norm_bwd")
+    _lib().cvb_l2norm_bwd(DY.data_ptr(), Y.data_ptr(), inv.data_ptr(), DX.data_ptr(), M, C, _stream())
     _count()
     return DX
 
@@ -319,14 +320,14 @@ def l2norm_bwd(DY: Tensor, Y: Tensor, inv: Tensor) -> Tensor:
 def transpose_bf16(X: Tensor) -> Tensor:
     R, C = X.shape
     Y = torch.empty((C, R), device=X.device, dtype=torch.bfloat16)
-    L.check(_lib().cvb_transpose_bf16(X.data_ptr(), Y.data_ptr(), R, C, _stream()), "cvb_transpose_bf16")
+    _lib().cvb_transpose_bf16(X.data_ptr(), Y.data_ptr(), R, C, _stream())
     _count()
     return Y
 
 
 def add_bf16_f32(A: Optional[Tensor], Bf: Tensor) -> Tensor:
     out = torch.empty(Bf.shape, device=Bf.device, dtype=torch.bfloat16)
-    L.check(_lib().cvb_add_bf16_f32(_p(A), Bf.data_ptr(), out.data_ptr(), Bf.numel(), _stream()), "cvb_add_bf16_f32")
+    _lib().cvb_add_bf16_f32(_p(A), Bf.data_ptr(), out.data_ptr(), Bf.numel(), _stream())
     _count()
     return out
 
@@ -340,7 +341,7 @@ def zs_class_embed(X: Tensor, perm: Tensor, Cl: int, M: int) -> Tensor:
     if perm.dtype != torch.int32 or perm.numel() != Cl * M or not perm.is_contiguous():
         raise ValueError(f"zs_class_embed: perm must be a contiguous int32 tensor of Cl * M = {Cl * M} elements")
     table = torch.empty((d, Cl), device=X.device, dtype=torch.float32)
-    L.check(_lib().cvb_zs_class_embed(X.data_ptr(), X.stride(0), R, perm.data_ptr(), Cl, M, d, table.data_ptr(), _stream()), "cvb_zs_class_embed")
+    _lib().cvb_zs_class_embed(X.data_ptr(), X.stride(0), R, perm.data_ptr(), Cl, M, d, table.data_ptr(), _stream())
     _count()
     return table
 
@@ -363,8 +364,8 @@ def zs_logits_topk(img: Tensor, table: Tensor, scale: float = 100.0, targets: Op
             raise ValueError("zs_logits_topk: hits must be a contiguous int64 [2] tensor")
     Cl = table.shape[1]
     logits = torch.empty((B, Cl), device=img.device, dtype=torch.float32) if want_logits else None
-    L.check(_lib().cvb_zs_logits_topk(img.data_ptr(), img.stride(0), table.data_ptr(), B, d, Cl, float(scale), _p(targets), _p(logits), _p(hits),
-                                      _stream()), "cvb_zs_logits_topk")
+    _lib().cvb_zs_logits_topk(img.data_ptr(), img.stride(0), table.data_ptr(), B, d, Cl, float(scale), _p(targets), _p(logits), _p(hits),
+                              _stream())
     _count()
     return logits
 
@@ -372,7 +373,7 @@ def zs_logits_topk(img: Tensor, table: Tensor, scale: float = 100.0, targets: Op
 def patch_permute(X: Tensor, B: int, H: int, W: int, ph: int, pw: int, inverse: bool) -> Tensor:
     """MobileViT-v1 unfold (inverse=False: feature-map rows -> token rows [B*P*N, C]) / fold (inverse=True)."""
     out = torch.empty_like(X)
-    L.check(_lib().cvb_patch_permute(X.data_ptr(), out.data_ptr(), B, H, W, X.shape[1], ph, pw, int(inverse), _stream()), "cvb_patch_permute")
+    _lib().cvb_patch_permute(X.data_ptr(), out.data_ptr(), B, H, W, X.shape[1], ph, pw, int(inverse), _stream())
     _count()
     return out
 
@@ -380,7 +381,7 @@ def patch_permute(X: Tensor, B: int, H: int, W: int, ph: int, pw: int, inverse: 
 def concat2(A: Tensor, Bt: Tensor) -> Tensor:
     M, C1, C2 = A.shape[0], A.shape[1], Bt.shape[1]
     out = torch.empty((M, C1 + C2), device=A.device, dtype=torch.bfloat16)
-    L.check(_lib().cvb_concat2(A.data_ptr(), Bt.data_ptr(), C1, C2, M, out.data_ptr(), _stream()), "cvb_concat2")
+    _lib().cvb_concat2(A.data_ptr(), Bt.data_ptr(), C1, C2, M, out.data_ptr(), _stream())
     _count()
     return out
 
@@ -389,7 +390,7 @@ def split2(G: Tensor, C1: int, C2: int) -> Tuple[Tensor, Tensor]:
     M = G.shape[0]
     da = torch.empty((M, C1), device=G.device, dtype=torch.bfloat16)
     db = torch.empty((M, C2), device=G.device, dtype=torch.bfloat16)
-    L.check(_lib().cvb_split2(G.data_ptr(), C1, C2, M, da.data_ptr(), db.data_ptr(), _stream()), "cvb_split2")
+    _lib().cvb_split2(G.data_ptr(), C1, C2, M, da.data_ptr(), db.data_ptr(), _stream())
     _count()
     return da, db
 
@@ -398,8 +399,7 @@ def vit_tokens_interp_fwd(patch: Tensor, pos: Tensor, cls: Optional[Tensor], B: 
     """Token assembly with the positional table ``pos`` ([.., n_pos, C] fp32) linearly resampled to N rows (F.interpolate, align_corners=False)."""
     S = N + (1 if cls is not None else 0)
     out = torch.empty((B, S, C), device=patch.device, dtype=torch.bfloat16)
-    L.check(_lib().cvb_vit_tokens_interp_fwd(patch.data_ptr(), pos.data_ptr(), pos.shape[-2], _p(cls), out.data_ptr(), B, N, C, _stream()),
-            "cvb_vit_tokens_interp_fwd")
+    _lib().cvb_vit_tokens_interp_fwd(patch.data_ptr(), pos.data_ptr(), pos.shape[-2], _p(cls), out.data_ptr(), B, N, C, _stream())
     _count()
     return out
 
@@ -407,8 +407,7 @@ def vit_tokens_interp_fwd(patch: Tensor, pos: Tensor, cls: Optional[Tensor], B: 
 def vit_tokens_interp_bwd(dout: Tensor, dpos: Tensor, dcls: Optional[Tensor], B: int, N: int, C: int) -> Tensor:
     """Adjoint of vit_tokens_interp_fwd: returns dpatch, adds into dpos ([n_pos, C] fp32) and dcls."""
     dpatch = torch.empty((B * N, C), device=dout.device, dtype=torch.bfloat16)
-    L.check(_lib().cvb_vit_tokens_interp_bwd(dout.data_ptr(), dpatch.data_ptr(), dpos.data_ptr(), dpos.shape[-2], _p(dcls), B, N, C, _stream()),
-            "cvb_vit_tokens_interp_bwd")
+    _lib().cvb_vit_tokens_interp_bwd(dout.data_ptr(), dpatch.data_ptr(), dpos.data_ptr(), dpos.shape[-2], _p(dcls), B, N, C, _stream())
     _count()
     return dpatch
 
@@ -420,7 +419,7 @@ def stem_im2col(x: Tensor, mix: Optional[Tensor] = None) -> Tensor:
     assert C == 3 and x.dtype == torch.float32
     A = torch.empty((B * (H // 2) * (W // 2), 32), device=x.device, dtype=torch.bfloat16)
     sn, sc, sh, sw = x.stride()
-    L.check(lib.cvb_stem_im2col_mix(x.data_ptr(), sn, sc, sh, sw, B, H, W, A.data_ptr(), _p(mix), _stream()), "cvb_stem_im2col")
+    lib.cvb_stem_im2col_mix(x.data_ptr(), sn, sc, sh, sw, B, H, W, A.data_ptr(), _p(mix), _stream())
     _count()
     return A
 
@@ -432,9 +431,9 @@ def bn_finalize(stats: Tensor, count: float, gamma: Tensor, beta: Tensor, eps: f
     lib = _lib()
     C = stats.shape[1]
     out = torch.empty((4, C), device=stats.device, dtype=torch.float32)
-    L.check(lib.cvb_bn_finalize(stats[0].data_ptr(), stats[1].data_ptr(), float(count), _p(gamma), _p(beta), eps, momentum,
-                                _p(running_mean), _p(running_var), _p(nbt), out[0].data_ptr(), out[1].data_ptr(), out[2].data_ptr(),
-                                out[3].data_ptr(), C, _stream()), "cvb_bn_finalize")
+    lib.cvb_bn_finalize(stats[0].data_ptr(), stats[1].data_ptr(), float(count), _p(gamma), _p(beta), eps, momentum,
+                        _p(running_mean), _p(running_var), _p(nbt), out[0].data_ptr(), out[1].data_ptr(), out[2].data_ptr(),
+                        out[3].data_ptr(), C, _stream())
     _count()
     return out
 
@@ -443,8 +442,8 @@ def bn_eval_scale_shift(gamma: Tensor, beta: Tensor, running_mean: Tensor, runni
     lib = _lib()
     C = running_mean.shape[0]
     out = torch.empty((4, C), device=running_mean.device, dtype=torch.float32)
-    L.check(lib.cvb_bn_eval_scale_shift(_p(gamma), _p(beta), running_mean.data_ptr(), running_var.data_ptr(), eps, out[0].data_ptr(),
-                                        out[1].data_ptr(), out[2].data_ptr(), out[3].data_ptr(), C, _stream()), "cvb_bn_eval_scale_shift")
+    lib.cvb_bn_eval_scale_shift(_p(gamma), _p(beta), running_mean.data_ptr(), running_var.data_ptr(), eps, out[0].data_ptr(),
+                                out[1].data_ptr(), out[2].data_ptr(), out[3].data_ptr(), C, _stream())
     _count()
     return out
 
@@ -457,9 +456,9 @@ def bn_bwd_finalize(stats: Tensor, count: float, gamma: Tensor, bn: Tensor, eval
     C = stats.shape[1]
     dgb = torch.empty((2, C), device=stats.device, dtype=torch.float32) if out is None else out
     coef = torch.empty((3, C), device=stats.device, dtype=torch.float32)
-    L.check(lib.cvb_bn_bwd_finalize(stats[0].data_ptr(), stats[1].data_ptr(), float(count), _p(gamma), bn[0].data_ptr(), bn[1].data_ptr(),
-                                    int(eval_mode), dgb[0].data_ptr(), dgb[1].data_ptr(), coef[0].data_ptr(), coef[1].data_ptr(),
-                                    coef[2].data_ptr(), C, _stream()), "cvb_bn_bwd_finalize")
+    lib.cvb_bn_bwd_finalize(stats[0].data_ptr(), stats[1].data_ptr(), float(count), _p(gamma), bn[0].data_ptr(), bn[1].data_ptr(),
+                            int(eval_mode), dgb[0].data_ptr(), dgb[1].data_ptr(), coef[0].data_ptr(), coef[1].data_ptr(),
+                            coef[2].data_ptr(), C, _stream())
     _count()
     return dgb, coef
 
@@ -468,7 +467,7 @@ def bn_apply(Y: Tensor, bn: Tensor, act: bool, R: Optional[Tensor] = None) -> Te
     lib = _lib()
     M, C = Y.shape
     out = torch.empty_like(Y)
-    L.check(lib.cvb_bn_apply(Y.data_ptr(), bn[2].data_ptr(), bn[3].data_ptr(), int(act), _p(R), out.data_ptr(), M, C, _stream()), "cvb_bn_apply")
+    lib.cvb_bn_apply(Y.data_ptr(), bn[2].data_ptr(), bn[3].data_ptr(), int(act), _p(R), out.data_ptr(), M, C, _stream())
     _count()
     return out
 
@@ -477,8 +476,8 @@ def bn_bwd_reduce(DOUT: Tensor, Y: Tensor, stats: Tensor, bn: Optional[Tensor] =
     lib = _lib()
     M, C = Y.shape
     DZ = torch.empty_like(Y) if store_dz else None
-    L.check(lib.cvb_bn_bwd_reduce(DOUT.data_ptr(), Y.data_ptr(), _p(bn[2]) if act else None, _p(bn[3]) if act else None, int(act), _p(DZ),
-                                  stats[0].data_ptr(), stats[1].data_ptr(), M, C, _stream()), "cvb_bn_bwd_reduce")
+    lib.cvb_bn_bwd_reduce(DOUT.data_ptr(), Y.data_ptr(), _p(bn[2]) if act else None, _p(bn[3]) if act else None, int(act), _p(DZ),
+                          stats[0].data_ptr(), stats[1].data_ptr(), M, C, _stream())
     _count()
     return DZ
 
@@ -488,16 +487,14 @@ def gn_finalize(stats: Tensor, count: float, eps: float) -> Tensor:
     lib = _lib()
     B = stats.shape[1]
     out = torch.empty((2, B), device=stats.device, dtype=torch.float32)
-    L.check(lib.cvb_gn_finalize(stats[0].data_ptr(), stats[1].data_ptr(), float(count), eps, out[0].data_ptr(), out[1].data_ptr(), B, _stream()),
-            "cvb_gn_finalize")
+    lib.cvb_gn_finalize(stats[0].data_ptr(), stats[1].data_ptr(), float(count), eps, out[0].data_ptr(), out[1].data_ptr(), B, _stream())
     _count()
     return out
 
 
 def gn_stats(X: Tensor, B: int, rows_per_sample: int, stats: Tensor):
     lib = _lib()
-    L.check(lib.cvb_gn_stats(X.data_ptr(), X.stride(0), B, rows_per_sample, X.shape[1], stats[0].data_ptr(), stats[1].data_ptr(), _stream()),
-            "cvb_gn_stats")
+    lib.cvb_gn_stats(X.data_ptr(), X.stride(0), B, rows_per_sample, X.shape[1], stats[0].data_ptr(), stats[1].data_ptr(), _stream())
     _count()
 
 
@@ -505,8 +502,8 @@ def gn_bwd_apply(G: Tensor, X: Tensor, gn: Tensor, sstats: Tensor, count: float,
                  DRES: Optional[Tensor] = None, col_sum: Optional[Tensor] = None) -> Tensor:
     lib = _lib()
     DX = torch.empty_like(G)
-    L.check(lib.cvb_gn_bwd_apply(G.data_ptr(), X.data_ptr(), gn[0].data_ptr(), gn[1].data_ptr(), sstats[0].data_ptr(), sstats[1].data_ptr(),
-                                 float(count), _p(DRES), DX.data_ptr(), B, rows_per_sample, G.shape[1], _p(col_sum), _stream()), "cvb_gn_bwd_apply")
+    lib.cvb_gn_bwd_apply(G.data_ptr(), X.data_ptr(), gn[0].data_ptr(), gn[1].data_ptr(), sstats[0].data_ptr(), sstats[1].data_ptr(),
+                         float(count), _p(DRES), DX.data_ptr(), B, rows_per_sample, G.shape[1], _p(col_sum), _stream())
     _count()
     return DX
 
@@ -520,8 +517,7 @@ def linattn_fwd(QKV: Tensor, B: int, H: int, W: int, d: int, patch: int = 2):
     O = torch.empty((M, d), device=QKV.device, dtype=torch.bfloat16)
     S = torch.empty((B, Pp, N), device=QKV.device, dtype=torch.float32)
     CTX = torch.empty((B, Pp, d), device=QKV.device, dtype=torch.float32)
-    L.check(lib.cvb_linattn_fwd(QKV.data_ptr(), QKV.stride(0), B, H, W, d, patch, O.data_ptr(), O.stride(0), S.data_ptr(), CTX.data_ptr(), _stream()),
-            "cvb_linattn_fwd")
+    lib.cvb_linattn_fwd(QKV.data_ptr(), QKV.stride(0), B, H, W, d, patch, O.data_ptr(), O.stride(0), S.data_ptr(), CTX.data_ptr(), _stream())
     _count()
     return O, S, CTX
 
@@ -530,8 +526,8 @@ def linattn_bwd(QKV: Tensor, DO: Tensor, S: Tensor, CTX: Tensor, B: int, H: int,
                 patch: int = 2) -> Tensor:
     lib = _lib()
     DQKV = torch.empty_like(QKV)
-    L.check(lib.cvb_linattn_bwd(QKV.data_ptr(), QKV.stride(0), DO.data_ptr(), DO.stride(0), S.data_ptr(), CTX.data_ptr(), B, H, W, d, patch,
-                                DQKV.data_ptr(), _p(dbias), _stream()), "cvb_linattn_bwd")
+    lib.cvb_linattn_bwd(QKV.data_ptr(), QKV.stride(0), DO.data_ptr(), DO.stride(0), S.data_ptr(), CTX.data_ptr(), B, H, W, d, patch,
+                        DQKV.data_ptr(), _p(dbias), _stream())
     _count()
     return DQKV
 
@@ -541,8 +537,8 @@ def linattn_cross_fwd(QKP: Tensor, QKVX: Tensor, B: int, Pp: int, Mp: int, N: in
     O = torch.empty((B * Pp * N, d), device=QKP.device, dtype=torch.bfloat16)
     S = torch.empty((B, Pp, Mp), device=QKP.device, dtype=torch.float32)
     CTX = torch.empty((B, Pp, d), device=QKP.device, dtype=torch.float32)
-    L.check(_lib().cvb_linattn_cross_fwd(QKP.data_ptr(), QKP.stride(0), B, Pp, Mp, d, QKVX.data_ptr(), QKVX.stride(0), N, O.data_ptr(), O.stride(0),
-                                         S.data_ptr(), CTX.data_ptr(), _stream()), "cvb_linattn_cross_fwd")
+    _lib().cvb_linattn_cross_fwd(QKP.data_ptr(), QKP.stride(0), B, Pp, Mp, d, QKVX.data_ptr(), QKVX.stride(0), N, O.data_ptr(), O.stride(0),
+                                 S.data_ptr(), CTX.data_ptr(), _stream())
     _count()
     return O, S, CTX
 
@@ -550,9 +546,8 @@ def linattn_cross_fwd(QKP: Tensor, QKVX: Tensor, B: int, Pp: int, Mp: int, N: in
 def linattn_cross_bwd(QKP: Tensor, QKVX: Tensor, DO: Tensor, S: Tensor, CTX: Tensor, B: int, Pp: int, Mp: int, N: int, d: int,
                       dbias: Optional[Tensor] = None):
     DQKP, DQKVX = torch.zeros_like(QKP), torch.zeros_like(QKVX)  # the kernel writes k/q columns of the first, v columns of the second
-    L.check(_lib().cvb_linattn_cross_bwd(QKP.data_ptr(), QKP.stride(0), QKVX.data_ptr(), QKVX.stride(0), DO.data_ptr(), DO.stride(0), S.data_ptr(),
-                                         CTX.data_ptr(), B, Pp, Mp, N, d, DQKP.data_ptr(), DQKVX.data_ptr(), _p(dbias), _stream()),
-            "cvb_linattn_cross_bwd")
+    _lib().cvb_linattn_cross_bwd(QKP.data_ptr(), QKP.stride(0), QKVX.data_ptr(), QKVX.stride(0), DO.data_ptr(), DO.stride(0), S.data_ptr(),
+                                 CTX.data_ptr(), B, Pp, Mp, N, d, DQKP.data_ptr(), DQKVX.data_ptr(), _p(dbias), _stream())
     _count()
     return DQKP, DQKVX
 
@@ -561,8 +556,8 @@ def gn_bwd(V: Tensor, X: Tensor, gn: Tensor, gamma: Tensor, count: float, B: int
            DRES: Optional[Tensor] = None) -> Tensor:
     """Stand-alone GroupNorm(1, C) backward (two launches); dgamma/dbeta fp64 [C] accumulators, samp_ws zeroed fp64 [2, B]."""
     DX = torch.empty_like(V)
-    L.check(_lib().cvb_gn_bwd(V.data_ptr(), X.data_ptr(), gn[0].data_ptr(), gn[1].data_ptr(), gamma.data_ptr(), float(count), _p(DRES), DX.data_ptr(), B,
-                              rows_per_sample, V.shape[1], dgamma.data_ptr(), dbeta.data_ptr(), samp_ws.data_ptr(), _stream()), "cvb_gn_bwd")
+    _lib().cvb_gn_bwd(V.data_ptr(), X.data_ptr(), gn[0].data_ptr(), gn[1].data_ptr(), gamma.data_ptr(), float(count), _p(DRES), DX.data_ptr(), B,
+                      rows_per_sample, V.shape[1], dgamma.data_ptr(), dbeta.data_ptr(), samp_ws.data_ptr(), _stream())
     _count(2)
     return DX
 
@@ -573,8 +568,8 @@ def mha_fwd(QKV: Tensor, B: int, S: int, H: int, head_dim: int, scale: float, at
     lib = _lib()
     O = torch.empty((B * S, H * head_dim), device=QKV.device, dtype=torch.bfloat16)
     LSE = torch.empty((B, H, S), device=QKV.device, dtype=torch.float32)
-    L.check(lib.cvb_mha_fwd(QKV.data_ptr(), QKV.stride(0), B, S, H, head_dim, float(scale), _p(attn_mask), _p(key_padding_mask), O.data_ptr(),
-                            O.stride(0), LSE.data_ptr(), _stream()), "cvb_mha_fwd")
+    lib.cvb_mha_fwd(QKV.data_ptr(), QKV.stride(0), B, S, H, head_dim, float(scale), _p(attn_mask), _p(key_padding_mask), O.data_ptr(),
+                    O.stride(0), LSE.data_ptr(), _stream())
     _count()
     return O, LSE
 
@@ -583,8 +578,8 @@ def mha_bwd(QKV: Tensor, O: Tensor, DO: Tensor, LSE: Tensor, B: int, S: int, H: 
             attn_mask: Optional[Tensor] = None, key_padding_mask: Optional[Tensor] = None) -> Tensor:
     lib = _lib()
     DQKV = torch.empty_like(QKV)
-    L.check(lib.cvb_mha_bwd(QKV.data_ptr(), QKV.stride(0), O.data_ptr(), DO.data_ptr(), O.stride(0), LSE.data_ptr(), B, S, H, head_dim, float(scale),
-                            _p(attn_mask), _p(key_padding_mask), DQKV.data_ptr(), DQKV.stride(0), _stream()), "cvb_mha_bwd")
+    lib.cvb_mha_bwd(QKV.data_ptr(), QKV.stride(0), O.data_ptr(), DO.data_ptr(), O.stride(0), LSE.data_ptr(), B, S, H, head_dim, float(scale),
+                    _p(attn_mask), _p(key_padding_mask), DQKV.data_ptr(), DQKV.stride(0), _stream())
     _count()
     return DQKV
 
@@ -594,25 +589,22 @@ def ln_bwd(V: Tensor, X: Tensor, ln: Tensor, gamma: Tensor, col_stats: Tensor, D
     """One-pass LayerNorm backward; ``col_stats`` fp64 [2, C] receives (dbeta, dgamma) like the GN_BWD epilogue's col_stats."""
     M, C = V.shape
     DX = torch.empty_like(V)
-    L.check(_lib().cvb_ln_bwd(V.data_ptr(), X.data_ptr(), ln[0].data_ptr(), ln[1].data_ptr(), gamma.data_ptr(), _p(DRES), DX.data_ptr(), M, C,
-                              col_stats[1].data_ptr(), col_stats[0].data_ptr(), _p(col_sum), _stream()), "cvb_ln_bwd")
+    _lib().cvb_ln_bwd(V.data_ptr(), X.data_ptr(), ln[0].data_ptr(), ln[1].data_ptr(), gamma.data_ptr(), _p(DRES), DX.data_ptr(), M, C,
+                      col_stats[1].data_ptr(), col_stats[0].data_ptr(), _p(col_sum), _stream())
     _count()
     return DX
 
 
-ACT_SILU, ACT_GELU, ACT_RELU, ACT_HARDSWISH, ACT_HARDSIGMOID, ACT_SIGMOID = 0, 1, 2, 3, 4, 5
-
-
 def act_fwd(X: Tensor, kind: int) -> Tensor:
     Y = torch.empty_like(X)
-    L.check(_lib().cvb_act_fwd(X.data_ptr(), Y.data_ptr(), X.numel(), kind, _stream()), "cvb_act_fwd")
+    _lib().cvb_act_fwd(X.data_ptr(), Y.data_ptr(), X.numel(), kind, _stream())
     _count()
     return Y
 
 
 def act_bwd(DY: Tensor, X: Tensor, kind: int) -> Tensor:
     DX = torch.empty_like(DY)
-    L.check(_lib().cvb_act_bwd(DY.data_ptr(), X.data_ptr(), DX.data_ptr(), X.numel(), kind, _stream()), "cvb_act_bwd")
+    _lib().cvb_act_bwd(DY.data_ptr(), X.data_ptr(), DX.data_ptr(), X.numel(), kind, _stream())
     _count()
     return DX
 
@@ -620,7 +612,7 @@ def act_bwd(DY: Tensor, X: Tensor, kind: int) -> Tensor:
 def se_scale_fwd(X: Tensor, S: Tensor, B: int, HW: int) -> Tensor:
     """Y[b,p,c] = X[b,p,c] * S[b,c]: X bf16 [B*HW, C] channels-last rows, S bf16 [B, C] (squeeze_excitation.py:82-83)."""
     Y = torch.empty_like(X)
-    L.check(_lib().cvb_se_scale_fwd(X.data_ptr(), S.data_ptr(), Y.data_ptr(), B, HW, X.shape[1], _stream()), "cvb_se_scale_fwd")
+    _lib().cvb_se_scale_fwd(X.data_ptr(), S.data_ptr(), Y.data_ptr(), B, HW, X.shape[1], _stream())
     _count()
     return Y
 
@@ -629,7 +621,7 @@ def se_scale_bwd(DY: Tensor, X: Tensor, S: Tensor, B: int, HW: int):
     """DX = DY * S (bf16) and DS[b,c] = sum_p DY * X (fp32 [B, C])."""
     DX = torch.empty_like(DY)
     DS = torch.zeros((B, X.shape[1]), device=X.device, dtype=torch.float32)
-    L.check(_lib().cvb_se_scale_bwd(DY.data_ptr(), X.data_ptr(), S.data_ptr(), DX.data_ptr(), DS.data_ptr(), B, HW, X.shape[1], _stream()), "cvb_se_scale_bwd")
+    _lib().cvb_se_scale_bwd(DY.data_ptr(), X.data_ptr(), S.data_ptr(), DX.data_ptr(), DS.data_ptr(), B, HW, X.shape[1], _stream())
     _count()
     return DX, DS
 
@@ -656,7 +648,7 @@ def rng_next(device) -> Tensor:
     if dev not in _RNG:
         rng_seed(device=dev)
     key = torch.empty(1, device=dev, dtype=torch.int64)
-    L.check(_lib().cvb_rng_next(_RNG[dev].data_ptr(), key.data_ptr(), _stream()), "cvb_rng_next")
+    _lib().cvb_rng_next(_RNG[dev].data_ptr(), key.data_ptr(), _stream())
     _count()
     return key
 
@@ -665,8 +657,7 @@ def dropout_fwd(V: Tensor, R: Optional[Tensor], p: float, key: Tensor, p_row: fl
     """Y = R + V * mask / (1 - p) [* per-sample stochastic-depth factor] on bf16 [M, C] (see cvb_dropout_fwd)."""
     M, C = V.shape
     Y = torch.empty_like(V)
-    L.check(_lib().cvb_dropout_fwd(V.data_ptr(), _p(R), Y.data_ptr(), M, C, rows_per_sample, float(p), float(p_row), key.data_ptr(), _stream()),
-            "cvb_dropout_fwd")
+    _lib().cvb_dropout_fwd(V.data_ptr(), _p(R), Y.data_ptr(), M, C, rows_per_sample, float(p), float(p_row), key.data_ptr(), _stream())
     _count()
     return Y
 
@@ -674,8 +665,7 @@ def dropout_fwd(V: Tensor, R: Optional[Tensor], p: float, key: Tensor, p_row: fl
 def dropout_bwd(DY: Tensor, p: float, key: Tensor, p_row: float = 0.0, rows_per_sample: int = 0) -> Tensor:
     M, C = DY.shape
     DV = torch.empty_like(DY)
-    L.check(_lib().cvb_dropout_bwd(DY.data_ptr(), DV.data_ptr(), M, C, rows_per_sample, float(p), float(p_row), key.data_ptr(), _stream()),
-            "cvb_dropout_bwd")
+    _lib().cvb_dropout_bwd(DY.data_ptr(), DV.data_ptr(), M, C, rows_per_sample, float(p), float(p_row), key.data_ptr(), _stream())
     _count()
     return DV
 
@@ -687,7 +677,7 @@ def _ptr6(ts: Sequence[Optional[Tensor]]):
 
 def na_plan(key: Tensor, B: int, enabled: int, tab: Tensor) -> Tensor:
     """Draw table fp32 [4 + 3 B] of one step (see cvb_na_plan); ``enabled`` bit k = brightness / contrast / noise."""
-    L.check(_lib().cvb_na_plan(key.data_ptr(), B, int(enabled), tab.data_ptr(), _stream()), "cvb_na_plan")
+    _lib().cvb_na_plan(key.data_ptr(), B, int(enabled), tab.data_ptr(), _stream())
     _count()
     return tab
 
@@ -695,7 +685,7 @@ def na_plan(key: Tensor, B: int, enabled: int, tab: Tensor) -> Tensor:
 def na_noise(key: Tensor, B: int, H: int, W: int) -> Tensor:
     """The N(0, 1) field fp32 [B, 3, H, W] that the RangeAugment kernels recompute from ``key``."""
     eps = torch.empty((B, 3, H, W), device=key.device, dtype=torch.float32)
-    L.check(_lib().cvb_na_noise(key.data_ptr(), B, H, W, eps.data_ptr(), _stream()), "cvb_na_noise")
+    _lib().cvb_na_noise(key.data_ptr(), B, H, W, eps.data_ptr(), _stream())
     _count()
     return eps
 
@@ -703,15 +693,14 @@ def na_noise(key: Tensor, B: int, H: int, W: int) -> Tensor:
 def na_stats(x: Tensor, mix: Optional[Tensor], key: Tensor, need_eps: bool, mu: Tensor) -> Tensor:
     """Per-plane means of the mixed image and of eps into fp64 ``mu`` [2, B * 3]."""
     B, _, H, W = x.shape
-    L.check(_lib().cvb_na_stats(x.data_ptr(), _p(mix), key.data_ptr(), B, H, W, int(need_eps), mu[0].data_ptr(), mu[1].data_ptr(), _stream()),
-            "cvb_na_stats")
+    _lib().cvb_na_stats(x.data_ptr(), _p(mix), key.data_ptr(), B, H, W, int(need_eps), mu[0].data_ptr(), mu[1].data_ptr(), _stream())
     _count()
     return mu
 
 
 def na_compose(tab: Tensor, mu: Tensor, raw: Sequence[Optional[Tensor]], B: int, coef: Tensor) -> Tensor:
     """coef fp32 [B * 3, 3] = (A, Bc, C) per plane; ``raw`` = (_low, _high) x (brightness, contrast, noise), None where disabled."""
-    L.check(_lib().cvb_na_compose(tab.data_ptr(), mu[0].data_ptr(), mu[1].data_ptr(), _ptr6(raw), B, coef.data_ptr(), _stream()), "cvb_na_compose")
+    _lib().cvb_na_compose(tab.data_ptr(), mu[0].data_ptr(), mu[1].data_ptr(), _ptr6(raw), B, coef.data_ptr(), _stream())
     _count()
     return coef
 
@@ -720,8 +709,7 @@ def na_apply(x: Tensor, mix: Optional[Tensor], key: Tensor, coef: Tensor, need_e
     """x_aug fp32 [B, 3, H, W]; writes the per-plane squared errors into fp64 ``sq`` [B, 3]."""
     B, _, H, W = x.shape
     Y = torch.empty_like(x)
-    L.check(_lib().cvb_na_apply(x.data_ptr(), _p(mix), key.data_ptr(), coef.data_ptr(), B, H, W, int(need_eps), Y.data_ptr(), sq.data_ptr(), _stream()),
-            "cvb_na_apply")
+    _lib().cvb_na_apply(x.data_ptr(), _p(mix), key.data_ptr(), coef.data_ptr(), B, H, W, int(need_eps), Y.data_ptr(), sq.data_ptr(), _stream())
     _count()
     return Y
 
@@ -729,23 +717,22 @@ def na_apply(x: Tensor, mix: Optional[Tensor], key: Tensor, coef: Tensor, need_e
 def na_bwd_reduce(dY: Optional[Tensor], g_sq: Optional[Tensor], x: Tensor, mix: Optional[Tensor], key: Tensor, coef: Tensor, need_eps: bool,
                   red: Tensor) -> Tensor:
     B, _, H, W = x.shape
-    L.check(_lib().cvb_na_bwd_reduce(_p(dY), _p(g_sq), x.data_ptr(), _p(mix), key.data_ptr(), coef.data_ptr(), B, H, W, int(need_eps), red.data_ptr(),
-                                     _stream()), "cvb_na_bwd_reduce")
+    _lib().cvb_na_bwd_reduce(_p(dY), _p(g_sq), x.data_ptr(), _p(mix), key.data_ptr(), coef.data_ptr(), B, H, W, int(need_eps), red.data_ptr(),
+                             _stream())
     _count()
     return red
 
 
 def na_param_grad(tab: Tensor, mu: Tensor, red: Tensor, raw: Sequence[Optional[Tensor]], B: int, grads: Sequence[Optional[Tensor]]):
-    L.check(_lib().cvb_na_param_grad(tab.data_ptr(), mu[0].data_ptr(), mu[1].data_ptr(), red.data_ptr(), _ptr6(raw), B, _ptr6(grads), _stream()),
-            "cvb_na_param_grad")
+    _lib().cvb_na_param_grad(tab.data_ptr(), mu[0].data_ptr(), mu[1].data_ptr(), red.data_ptr(), _ptr6(raw), B, _ptr6(grads), _stream())
     _count()
 
 
 def na_loss_fwd(sq: Tensor, H: int, W: int, target: Tensor, step: Tensor, alpha: float, loss: Tensor, w_na: float = 1.0, ce: Optional[Tensor] = None,
                 w_ce: float = 1.0, parts: Optional[Tensor] = None) -> Tensor:
     """loss (0-dim fp32) = w_na * L_na(sq) + w_ce * ce; ``parts`` fp32 [2] receives (ce, L_na)."""
-    L.check(_lib().cvb_na_loss_fwd(sq.data_ptr(), sq.shape[0], H, W, target.data_ptr(), target.numel(), step.data_ptr(), float(alpha), float(w_na), _p(ce),
-                                   float(w_ce), loss.data_ptr(), _p(parts), _stream()), "cvb_na_loss_fwd")
+    _lib().cvb_na_loss_fwd(sq.data_ptr(), sq.shape[0], H, W, target.data_ptr(), target.numel(), step.data_ptr(), float(alpha), float(w_na), _p(ce),
+                           float(w_ce), loss.data_ptr(), _p(parts), _stream())
     _count()
     return loss
 
@@ -753,8 +740,8 @@ def na_loss_fwd(sq: Tensor, H: int, W: int, target: Tensor, step: Tensor, alpha:
 def na_loss_bwd(sq: Tensor, H: int, W: int, target: Tensor, step: Tensor, alpha: float, grad_out: Optional[Tensor], grad_scale: Optional[Tensor],
                 w_na: float = 1.0, g_ce: Optional[Tensor] = None, w_ce: float = 1.0) -> Tensor:
     g_sq = torch.empty_like(sq)
-    L.check(_lib().cvb_na_loss_bwd(sq.data_ptr(), sq.shape[0], H, W, target.data_ptr(), target.numel(), step.data_ptr(), float(alpha), float(w_na),
-                                   _p(grad_out), _p(grad_scale), g_sq.data_ptr(), _p(g_ce), float(w_ce), _stream()), "cvb_na_loss_bwd")
+    _lib().cvb_na_loss_bwd(sq.data_ptr(), sq.shape[0], H, W, target.data_ptr(), target.numel(), step.data_ptr(), float(alpha), float(w_na),
+                           _p(grad_out), _p(grad_scale), g_sq.data_ptr(), _p(g_ce), float(w_ce), _stream())
     _count()
     return g_sq
 
@@ -763,7 +750,7 @@ def stem_dgrad(dz: Tensor, y: Tensor, coef: Tensor, Ws: Tensor, B: int, Ho: int,
     """Stem input gradient fp32 [B, 3, 2 Ho, 2 Wo] from dz / y bf16 [B*Ho*Wo, C0], the BatchNorm-backward coef [3, C0] and the prepared weight."""
     C0 = dz.shape[1]
     dX = torch.empty((B, 3, 2 * Ho, 2 * Wo), device=dz.device, dtype=torch.float32)
-    L.check(_lib().cvb_stem_dgrad(dz.data_ptr(), y.data_ptr(), coef.data_ptr(), Ws.data_ptr(), B, Ho, Wo, C0, dX.data_ptr(), _stream()), "cvb_stem_dgrad")
+    _lib().cvb_stem_dgrad(dz.data_ptr(), y.data_ptr(), coef.data_ptr(), Ws.data_ptr(), B, Ho, Wo, C0, dX.data_ptr(), _stream())
     _count()
     return dX
 
@@ -773,7 +760,7 @@ def ln_stats(X: Tensor, eps: float) -> Tensor:
     lib = _lib()
     M, C = X.shape
     out = torch.empty((2, M), device=X.device, dtype=torch.float32)
-    L.check(lib.cvb_ln_stats(X.data_ptr(), X.stride(0), M, C, float(eps), out[0].data_ptr(), out[1].data_ptr(), _stream()), "cvb_ln_stats")
+    lib.cvb_ln_stats(X.data_ptr(), X.stride(0), M, C, float(eps), out[0].data_ptr(), out[1].data_ptr(), _stream())
     _count()
     return out
 
@@ -783,7 +770,7 @@ def global_pool_fwd(X: Tensor, B: int, HW: int) -> Tensor:
     lib = _lib()
     C = X.shape[1]
     out = torch.empty((B, C), device=X.device, dtype=torch.bfloat16)
-    L.check(lib.cvb_global_pool_fwd(X.data_ptr(), B, HW, C, out.data_ptr(), _stream()), "cvb_global_pool_fwd")
+    lib.cvb_global_pool_fwd(X.data_ptr(), B, HW, C, out.data_ptr(), _stream())
     _count()
     return out
 
@@ -792,7 +779,7 @@ def global_pool_bwd(DOUT: Tensor, B: int, HW: int) -> Tensor:
     lib = _lib()
     C = DOUT.shape[1]
     DX = torch.empty((B * HW, C), device=DOUT.device, dtype=torch.bfloat16)
-    L.check(lib.cvb_global_pool_bwd(DOUT.data_ptr(), B, HW, C, DX.data_ptr(), _stream()), "cvb_global_pool_bwd")
+    lib.cvb_global_pool_bwd(DOUT.data_ptr(), B, HW, C, DX.data_ptr(), _stream())
     _count()
     return DX
 
@@ -802,7 +789,7 @@ def col_sum(X: Tensor, N: Optional[int] = None, out: Optional[Tensor] = None) ->
     N = X.shape[1] if N is None else N
     if out is None:
         out = torch.zeros((N,), device=X.device, dtype=torch.float32)
-    L.check(lib.cvb_col_sum(X.data_ptr(), int(X.dtype == torch.float32), X.stride(0), X.shape[0], N, out.data_ptr(), _stream()), "cvb_col_sum")
+    lib.cvb_col_sum(X.data_ptr(), int(X.dtype == torch.float32), X.stride(0), X.shape[0], N, out.data_ptr(), _stream())
     _count()
     return out
 
@@ -813,8 +800,8 @@ def ce_fwd(logits: Tensor, C: int, target: Tensor, ignore_index: int, smoothing:
     B = logits.shape[0]
     lse = torch.empty(B, device=logits.device, dtype=torch.float32)
     out = torch.empty(2, device=logits.device, dtype=torch.float32)
-    L.check(_lib().cvb_ce_fwd(logits.data_ptr(), logits.stride(0), B, C, target.data_ptr(), int(ignore_index), float(smoothing), lse.data_ptr(),
-                              out[0:1].data_ptr(), out[1:2].data_ptr(), _p(mix), _p(logit_scale), _stream()), "cvb_ce_fwd")
+    _lib().cvb_ce_fwd(logits.data_ptr(), logits.stride(0), B, C, target.data_ptr(), int(ignore_index), float(smoothing), lse.data_ptr(),
+                      out[0:1].data_ptr(), out[1:2].data_ptr(), _p(mix), _p(logit_scale), _stream())
     _count()
     return out[0:1], lse, out[1:2]
 
@@ -824,9 +811,8 @@ def ce_bwd(logits: Tensor, C: int, target: Tensor, ignore_index: int, smoothing:
            dlogit_scale: Optional[Tensor] = None) -> Tensor:
     B = logits.shape[0]
     d = torch.empty((B, ldd), device=logits.device, dtype=torch.bfloat16)
-    L.check(_lib().cvb_ce_bwd(logits.data_ptr(), logits.stride(0), B, C, target.data_ptr(), int(ignore_index), float(smoothing), lse.data_ptr(),
-                              n_valid.data_ptr(), _p(gout), _p(gscale), d.data_ptr(), ldd, _p(mix), _p(logit_scale), _p(dlogit_scale), _stream()),
-            "cvb_ce_bwd")
+    _lib().cvb_ce_bwd(logits.data_ptr(), logits.stride(0), B, C, target.data_ptr(), int(ignore_index), float(smoothing), lse.data_ptr(),
+                      n_valid.data_ptr(), _p(gout), _p(gscale), d.data_ptr(), ldd, _p(mix), _p(logit_scale), _p(dlogit_scale), _stream())
     _count()
     return d
 
@@ -838,10 +824,10 @@ def pw_wgrad_side(G: Tensor, A: Tensor, N: int, K: int, **kw) -> Tensor:
 
 def unprep_grad(src: Tensor, rows: int, cols: int, lds: int, kind: int, rot: int = 0, side: bool = False, out: Optional[Tensor] = None) -> Tensor:
     lib = _lib()
-    dst = torch.empty((rows, cols) if kind != 3 else (rows,), device=src.device, dtype=torch.float32) if out is None else out
-    assert dst.is_contiguous() and dst.numel() == rows * (cols if kind != 3 else 1)
+    dst = torch.empty((rows, cols) if kind != PreparedWeights.KIND_VECTOR_F32 else (rows,), device=src.device, dtype=torch.float32) if out is None else out
+    assert dst.is_contiguous() and dst.numel() == rows * (cols if kind != PreparedWeights.KIND_VECTOR_F32 else 1)
     with _SideCtx(side):
-        L.check(lib.cvb_unprep_grad(src.data_ptr(), dst.data_ptr(), rows, cols, lds, kind, rot, _stream()), "cvb_unprep_grad")
+        lib.cvb_unprep_grad(src.data_ptr(), dst.data_ptr(), rows, cols, lds, kind, rot, _stream())
         if side:
             _hold(src, dst)
     _count()
@@ -864,8 +850,9 @@ class PreparedWeights:
     new, SURVEY.md 8b); these buffers are a cache keyed on the parameters' ``_version`` and storage address.
     """
 
-    KIND_ROWMAJOR, KIND_TRANSPOSED, KIND_TAPMAJOR_F32, KIND_VECTOR_F32 = 0, 1, 2, 3
-    KIND_PATCH, KIND_PATCH_T = 4, 5  # dense conv weight [Cout, Cin, k, k] -> [Cout, (tap, ci)] / its transpose (rot = taps = k*k)
+    # the layout kinds of cvb_prep_weights / cvb_unprep_grad (CVB_PREP_* in the header)
+    KIND_ROWMAJOR, KIND_TRANSPOSED, KIND_TAPMAJOR_F32 = L.PREP_ROWMAJOR, L.PREP_TRANSPOSED, L.PREP_TAPMAJOR_F32
+    KIND_VECTOR_F32, KIND_PATCH, KIND_PATCH_T = L.PREP_VECTOR_F32, L.PREP_PATCH, L.PREP_PATCH_T
 
     def __init__(self):
         self._entries = []  # (param, dst, rows, cols, ldd, dst_rows, kind, rot)
@@ -916,10 +903,10 @@ class PreparedWeights:
         if self._table is None or key != self._key:
             if self._entries[0][1] is None or self._entries[0][1].device != device:
                 self._alloc(device)
-            descs = (L.PrepDesc * len(self._entries))()
+            descs = (cvb_prep_desc * len(self._entries))()
             for i, (param, dst, rows, cols, ldd, dst_rows, kind, rot) in enumerate(self._entries):
                 assert param.dtype == torch.float32 and param.is_contiguous(), "parameters must be contiguous fp32"
-                descs[i] = L.PrepDesc(param.data_ptr(), dst.data_ptr(), rows, cols, ldd, dst_rows, kind, rot)
+                descs[i] = cvb_prep_desc(param.data_ptr(), dst.data_ptr(), rows, cols, ldd, dst_rows, kind, rot)
             raw = torch.frombuffer(bytearray(bytes(descs)), dtype=torch.uint8)
             self._table = raw.to(device)
             self._key = key
@@ -929,7 +916,7 @@ class PreparedWeights:
         # refresh was not a training-mode one (a training forward refreshes BEFORE that step's optimizer update)
         if not force and versions == self._versions and not self._forced_last:
             return
-        L.check(_lib().cvb_prep_weights(self._table.data_ptr(), len(self._entries), int(self._max_elems), _stream()), "cvb_prep_weights")
+        _lib().cvb_prep_weights(self._table.data_ptr(), len(self._entries), int(self._max_elems), _stream())
         _count()
         self._versions = versions
         self._forced_last = bool(force)

@@ -17,7 +17,6 @@ from typing import Dict, Optional
 
 import torch
 
-from . import _lib as L
 from .ops import _count, _lib, _stream, invalidate_prepared_weights
 from .workspace import StepWorkspace
 
@@ -75,8 +74,8 @@ class _FlatStep:
         lr_now = self.param_groups[0]["lr"]
         if lr_now != float(self._hp_host[0]) and not torch.cuda.is_current_stream_capturing():
             self.set_lr(lr_now)
-        L.check(_lib().cvb_grad_norm(self.flat_g.data_ptr(), self.n, self.scale.data_ptr(), float(grad_div), self.stats.data_ptr(),
-                                     self.partials.data_ptr(), _stream()), "cvb_grad_norm")
+        _lib().cvb_grad_norm(self.flat_g.data_ptr(), self.n, self.scale.data_ptr(), float(grad_div), self.stats.data_ptr(),
+                             self.partials.data_ptr(), _stream())
         _count()
         self._update()
         _count()
@@ -130,8 +129,8 @@ class FlatAdamW(_FlatStep):
 
     def _update(self) -> None:
         b1, b2, eps = self.consts
-        L.check(_lib().cvb_adamw_step(self.flat_p.data_ptr(), self.flat_g.data_ptr(), self.exp_avg.data_ptr(), self.exp_avg_sq.data_ptr(),
-                                      self.wd.data_ptr(), self.n, self.hp.data_ptr(), b1, b2, eps, self.max_norm, *self._tail_args()), "cvb_adamw_step")
+        _lib().cvb_adamw_step(self.flat_p.data_ptr(), self.flat_g.data_ptr(), self.exp_avg.data_ptr(), self.exp_avg_sq.data_ptr(),
+                              self.wd.data_ptr(), self.n, self.hp.data_ptr(), b1, b2, eps, self.max_norm, *self._tail_args())
 
 
 class FlatSGD(_FlatStep):
@@ -150,5 +149,5 @@ class FlatSGD(_FlatStep):
         self.momentum, self.nesterov = float(momentum), bool(nesterov)
 
     def _update(self) -> None:
-        L.check(_lib().cvb_sgd_step(self.flat_p.data_ptr(), self.flat_g.data_ptr(), self.momentum_buffer.data_ptr(), self.wd.data_ptr(), self.n,
-                                    self.hp.data_ptr(), self.momentum, int(self.nesterov), self.max_norm, *self._tail_args()), "cvb_sgd_step")
+        _lib().cvb_sgd_step(self.flat_p.data_ptr(), self.flat_g.data_ptr(), self.momentum_buffer.data_ptr(), self.wd.data_ptr(), self.n,
+                            self.hp.data_ptr(), self.momentum, int(self.nesterov), self.max_norm, *self._tail_args())

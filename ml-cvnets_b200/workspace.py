@@ -166,10 +166,10 @@ class StepWorkspace:
         self._used.clear()
         lib = L.load()
         st = torch.cuda.current_stream().cuda_stream
-        L.check(lib.cvb_memset_zero(self.flat_g.data_ptr(), self.flat_g.numel() * 4, st), "cvb_memset_zero")
+        lib.cvb_memset_zero(self.flat_g.data_ptr(), self.flat_g.numel() * 4, st)
         if self._buf32 is not None:
-            L.check(lib.cvb_memset_zero(self._buf32.data_ptr(), self._buf32.numel() * 4, st), "cvb_memset_zero")
-            L.check(lib.cvb_memset_zero(self._buf64.data_ptr(), self._buf64.numel() * 8, st), "cvb_memset_zero")
+            lib.cvb_memset_zero(self._buf32.data_ptr(), self._buf32.numel() * 4, st)
+            lib.cvb_memset_zero(self._buf64.data_ptr(), self._buf64.numel() * 8, st)
         self._units_done = 0
         self._works = []
         self._reset_bucket_state()
@@ -185,17 +185,17 @@ class StepWorkspace:
         if cached is None or cached[3] != sig:
             if torch.cuda.is_current_stream_capturing():
                 raise RuntimeError("StepWorkspace: descriptor table missing during capture (run two eager warm-up steps first)")
-            descs = (L.CastDesc * len(pairs))()
+            descs = (L.cvb_cast_desc * len(pairs))()
             mx = 1
             for i, (s, d) in enumerate(pairs):
                 assert s.dtype == torch.float64 and d.dtype == torch.float32 and s.numel() == d.numel() and s.is_contiguous() and d.is_contiguous()
-                descs[i] = L.CastDesc(s.data_ptr(), d.data_ptr(), s.numel(), 0)
+                descs[i] = L.cvb_cast_desc(s.data_ptr(), d.data_ptr(), s.numel(), 0)
                 mx = max(mx, s.numel())
             table = torch.frombuffer(bytearray(bytes(descs)), dtype=torch.uint8).to(self.device)
             cached = (table, len(pairs), mx, sig)
             self._cast_tables[key] = cached
         from . import ops
-        L.check(L.load().cvb_cast_f64_f32(cached[0].data_ptr(), cached[1], cached[2], torch.cuda.current_stream().cuda_stream), "cvb_cast_f64_f32")
+        L.load().cvb_cast_f64_f32(cached[0].data_ptr(), cached[1], cached[2], torch.cuda.current_stream().cuda_stream)
         ops._count()
 
     # ---------------------------------------------------------------------------------------------- data-parallel gradient exchange

@@ -338,9 +338,9 @@ def test_sgd_step_vs_torch(pkg):
     assert torch.equal(opt.flat_p, twin.flat_p) and torch.equal(opt.momentum_buffer, twin.momentum_buffer) and torch.equal(opt.ema, twin.ema)
 
 
-def test_sgd_step_kernel_export_checks(pkg):
+def test_sgd_step_kernel_raises_on_nesterov_without_momentum(pkg):
     from ml_cvnets_b200 import _lib as L
     lib = L.load()
     # Nesterov without momentum is rejected (torch.optim.SGD raises for it too)
-    rc = lib.cvb_sgd_step(None, None, None, None, 0, None, 0.0, 1, 0.0, None, None, None, 2.0, 0.5, 2000, None, 0.0, None, None)
-    assert rc != 0
+    with pytest.raises(L.CvbError, match="cvb_sgd_step failed"):
+        lib.cvb_sgd_step(None, None, None, None, 0, None, 0.0, 1, 0.0, None, None, None, 2.0, 0.5, 2000, None, 0.0, None, None)

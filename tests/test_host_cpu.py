@@ -33,26 +33,61 @@ def test_library_exports_every_declared_symbol():
     assert declared <= exported
 
 
-def test_struct_layouts_match_header():
-    """ctypes mirrors of the argument structs must list the header's fields in order."""
+def test_struct_layouts_match_c_compiler(tmp_path):
+    """The C compiler's sizeof / offsetof of every argument struct, and sizeof of every scalar parameter type, equal the derived ctypes
+    types': same field types and layout, not just the same names."""
+    import ctypes
     from ml_cvnets_b200 import _lib
-    hdr = open(os.path.join(REPO, "include", "cvnets_b200.h")).read()
+    structs = {n: t for n, t in vars(_lib).items() if isinstance(t, type) and issubclass(t, ctypes.Structure) and t is not ctypes.Structure}
+    assert set(structs) == {"cvb_gemm_args", "cvb_wgrad_args", "cvb_dw_fwd_args", "cvb_dw_bwd_args", "cvb_prep_desc", "cvb_cast_desc"}
+    want = {}
+    for name, cls in structs.items():
+        want[f"sizeof({name})"] = ctypes.sizeof(cls)
+        want.update({f"offsetof({name}, {f})": getattr(cls, f).offset for f, _ in cls._fields_})
+    scalars = dict(_lib._SCALARS, **{"void*": ctypes.c_void_p, "const char*": ctypes.c_char_p})
+    want.update({f"sizeof({t})": ctypes.sizeof(c) for t, c in scalars.items()})
+    probe = tmp_path / "probe.c"
+    probe.write_text('#include <stddef.h>\n#include <stdio.h>\n#include "cvnets_b200.h"\nint main(void) {\n'
+                     + "".join(f'  printf("%s %zu\\n", "{k}", {k});\n' for k in want) + "  return 0;\n}\n")
+    subprocess.run(["cc", "-std=c99", "-Wall", "-Werror", "-I", os.path.dirname(_lib.HEADER), str(probe), "-o", str(tmp_path / "probe")],
+                   check=True)
+    out = subprocess.run([str(tmp_path / "probe")], capture_output=True, text=True, check=True).stdout
+    got = {k: int(v) for k, v in (line.rsplit(" ", 1) for line in out.splitlines())}
+    assert got == want
 
-    def fields(struct_name):
-        body = dict((n, b) for b, n in re.findall(r"typedef struct \{([^}]*)\} (\w+);", hdr))[struct_name]
-        body = re.sub(r"/\*.*?\*/", "", body, flags=re.S)
-        names = []
-        for decl in body.split(";"):
-            decl = decl.strip()
-            if not decl:
-                continue
-            for part in decl.split(","):
-                names.append(re.findall(r"[A-Za-z_][A-Za-z0-9_]*", part)[-1])
-        return names
 
-    for cname, cls in (("cvb_gemm_args", _lib.GemmArgs), ("cvb_wgrad_args", _lib.WgradArgs), ("cvb_dw_fwd_args", _lib.DwFwdArgs),
-                       ("cvb_dw_bwd_args", _lib.DwBwdArgs), ("cvb_prep_desc", _lib.PrepDesc)):
-        assert fields(cname) == [f[0] for f in cls._fields_], cname
+def test_derived_signatures():
+    """Spot checks of the header -> ctypes mapping: int64_t, double, struct pointers, device descriptor tables, pointer arrays, const char*."""
+    import ctypes
+    from ml_cvnets_b200 import _lib
+    sigs = _lib._PROTOTYPES
+    assert sigs["cvb_stem_im2col"][1][1:5] == [ctypes.c_int64] * 4 and sigs["cvb_stem_im2col"][1][5] is ctypes.c_int
+    assert sigs["cvb_bn_finalize"][1][2] is ctypes.c_double and sigs["cvb_bn_finalize"][1][5] is ctypes.c_float
+    assert sigs["cvb_na_compose"][1][3] is ctypes.POINTER(ctypes.c_void_p)
+    assert sigs["cvb_na_param_grad"][1][4] is sigs["cvb_na_param_grad"][1][6] is ctypes.POINTER(ctypes.c_void_p)
+    assert sigs["cvb_pw_gemm"] == (ctypes.c_int, [ctypes.POINTER(_lib.cvb_gemm_args), ctypes.c_void_p])
+    assert sigs["cvb_prep_weights"][1][0] is ctypes.c_void_p  # descs_device: an address in device memory
+    assert sigs["cvb_last_error"] == (ctypes.c_char_p, [])
+    assert (_lib.ABI_VERSION, _lib.A_BNB, _lib.E_LIN_BWD, _lib.ACT_SIGMOID, _lib.PREP_PATCH_T) == (11, 5, 4, 5, 5)
+
+
+def test_header_parser_rejects_unknown_input(tmp_path):
+    from ml_cvnets_b200 import _lib
+    hdr = open(_lib.HEADER).read()
+    proto = "CVB_API int cvb_act_fwd(const void* X, void* Y, int64_t n, int kind, cvb_stream_t stream);"
+    assert proto in hdr
+    for bad in (hdr.replace(proto, proto.replace("int64_t n", "long n")), hdr.replace(proto, proto + "\nstatic int cvb_counter;")):
+        (tmp_path / "h.h").write_text(bad)
+        with pytest.raises(_lib.CvbError, match="unrecognised"):
+            _lib._parse(str(tmp_path / "h.h"))
+
+
+def test_failed_status_raises_with_the_library_message():
+    import __graft_entry__ as ge
+    ge.build()
+    from ml_cvnets_b200 import _lib
+    with pytest.raises(_lib.CvbError, match=r"^cvb_act_fwd failed \(rc=1\): cvb_act_fwd: bad arguments$"):
+        _lib.load().cvb_act_fwd(None, None, 8, _lib.ACT_GELU, None)  # argument validation fails before any CUDA call
 
 
 def test_state_dict_contract_and_signatures(golden_dir):

@@ -657,14 +657,13 @@ class _Tail:
         self.max_norm, self.gi = float(max_norm), int(growth_interval)
 
     def step(self, grads, grad_div):
-        from ml_cvnets_b200 import _lib as L
         st = torch.cuda.current_stream().cuda_stream
-        L.check(self.lib.cvb_grad_norm(grads.data_ptr(), self.n, self.scale.data_ptr(), float(grad_div), self.stats.data_ptr(),
-                                       self.partials.data_ptr(), st), "cvb_grad_norm")
-        L.check(self.lib.cvb_adamw_step(self.p.data_ptr(), grads.data_ptr(), self.m.data_ptr(), self.v.data_ptr(), self.wd.data_ptr(), self.n,
-                                        self.hp.data_ptr(), 0.9, 0.999, 1e-8, self.max_norm, self.stats.data_ptr(), self.scale.data_ptr(),
-                                        self.step_count.data_ptr(), 2.0, 0.5, self.gi, self.ema.data_ptr() if self.ema is not None else None,
-                                        self.ema_m, self.partials.data_ptr(), st), "cvb_adamw_step")
+        self.lib.cvb_grad_norm(grads.data_ptr(), self.n, self.scale.data_ptr(), float(grad_div), self.stats.data_ptr(),
+                               self.partials.data_ptr(), st)
+        self.lib.cvb_adamw_step(self.p.data_ptr(), grads.data_ptr(), self.m.data_ptr(), self.v.data_ptr(), self.wd.data_ptr(), self.n,
+                                self.hp.data_ptr(), 0.9, 0.999, 1e-8, self.max_norm, self.stats.data_ptr(), self.scale.data_ptr(),
+                                self.step_count.data_ptr(), 2.0, 0.5, self.gi, self.ema.data_ptr() if self.ema is not None else None,
+                                self.ema_m, self.partials.data_ptr(), st)
 
     def state(self):
         out = [self.p, self.m, self.v, self.stats, self.scale, self.step_count, self.partials]
@@ -748,7 +747,7 @@ def _check_tail(tail, ref, what):
         assert e <= 2e-6 + 1e-5 * float(ref.ema.abs().max()), f"{what}: EMA max abs diff {e}"
 
 
-def test_grad_norm_adamw_past_grid_caps(ops, sms):
+def test_grad_norm_adamw_step_past_grid_caps(ops, sms):
     """per-element weight decay, grad_div 4 (DDP's world size), EMA on, clipping active; then a step with inf in the last block's range and one
     with NaN in the n % 4 tail, each skipped with the scale backed off and the EMA still updated; then a normal step.  Twice, bitwise."""
     from ml_cvnets_b200 import _lib as L
@@ -793,7 +792,7 @@ def test_grad_norm_adamw_past_grid_caps(ops, sms):
     assert float(tail.step_count) == 2.0 and float(tail.scale[0]) == 65536.0 * 0.25
 
 
-def test_adamw_scale_growth_without_clipping(ops, sms):
+def test_adamw_step_scale_growth_without_clipping(ops, sms):
     """growth_interval 2: the loss scale doubles after every second finite step; max_norm 0 turns clipping off (large gradients untouched)"""
     from ml_cvnets_b200 import _lib as L
     lib = L.load()
