@@ -39,6 +39,19 @@ __device__ float block_reduce_max(float v, float* ws) {
   return t;
 }
 
+// Rows whose 16-byte loads a thread issues together.  Every loop over a thread's rows n = grp, grp + ngrp, ... keeps that ascending order, so
+// the fp32 chains it accumulates do not depend on the batching; the first batch of each pass is loaded before the barrier that precedes it.
+constexpr int LA_U = 4;
+
+__device__ __forceinline__ void load_rows(uint4 (&v)[LA_U], const bf16* base, int ld, int col, int b, int p, int n0, int step, int N, int H, int W,
+                                          int unf) {
+#pragma unroll
+  for (int u = 0; u < LA_U; ++u) {
+    const int n = n0 + u * step;
+    if (n < N) v[u] = ldg16(base + pix_index(b, p, n, H, W, unf) * ld + col);
+  }
+}
+
 // dynamic smem: s[N] | ctx[d] | partials[ngrp][d]
 // Cross-attention (linear_attention.py:163-207): query/key come from QKV (N rows per (b, p), the "previous" tensor), the values and the
 // output live in VX / O with Nv rows per (b, p); self-attention passes VX = QKV, Nv = N.
@@ -51,10 +64,17 @@ __global__ void __launch_bounds__(NT) linattn_fwd_kernel(const bf16* __restrict_
   __shared__ float ws[NT / 32];
   const int N = unf ? W : (H >> 1) * (W >> 1);
   const int P = unf ? H : 4;
+  const int Wv = (VX == QKV) ? W : Nv;  // cross-attention is unfolded-only: row (b, p, n) of a [B, P, Nv, *] matrix
   float* s_s = sm;
   float* s_ctx = sm + N;
   const int b = blockIdx.x / P, p = blockIdx.x % P;
   const int tid = threadIdx.x;
+  const int cgs = d >> 3;
+  const int cg = tid % cgs, grp = tid / cgs, ngrp = blockDim.x / cgs;
+  const int n_first = grp < ngrp ? grp : N;  // threads beyond cgs*ngrp only take part in the block-wide steps
+  const int nv_first = grp < ngrp ? grp : Nv;
+  uint4 kb[LA_U];
+  load_rows(kb, QKV, ldq, cg * 8, b, p, n_first, ngrp, N, H, W, unf);
 
   // softmax over the N patches of the query channel (column 2d)
   float lmax = -INFINITY;
@@ -71,7 +91,6 @@ __global__ void __launch_bounds__(NT) linattn_fwd_kernel(const bf16* __restrict_
     lsum += e;
   }
   const float inv = 1.f / block_reduce_sum(lsum, ws);
-  for (int i = tid; i < d; i += blockDim.x) s_ctx[i] = 0.f;
   for (int n = tid; n < N; n += blockDim.x) {
     float sv = s_s[n] * inv;
     s_s[n] = sv;
@@ -80,19 +99,24 @@ __global__ void __launch_bounds__(NT) linattn_fwd_kernel(const bf16* __restrict_
   __syncthreads();
 
   // ctx[c] = sum_n key[n,c] * s[n]
-  const int cgs = d >> 3;
-  const int cg = tid % cgs, grp = tid / cgs, ngrp = blockDim.x / cgs;
-  const int n_first = grp < ngrp ? grp : N;  // threads beyond cgs*ngrp only take part in the block-wide steps
   float acc[8];
 #pragma unroll
   for (int j = 0; j < 8; ++j) acc[j] = 0.f;
-  for (int n = n_first; n < N; n += ngrp) {
-    float k[8];
-    unpack8(ldg16(QKV + pix_index(b, p, n, H, W, unf) * ldq + cg * 8), k);
-    const float sv = s_s[n];
+  for (int n0 = n_first; n0 < N; n0 += LA_U * ngrp) {
+    if (n0 != n_first) load_rows(kb, QKV, ldq, cg * 8, b, p, n0, ngrp, N, H, W, unf);
 #pragma unroll
-    for (int j = 0; j < 8; ++j) acc[j] = fmaf(k[j], sv, acc[j]);
+    for (int u = 0; u < LA_U; ++u) {
+      const int n = n0 + u * ngrp;
+      if (n >= N) break;
+      float k[8];
+      unpack8(kb[u], k);
+      const float sv = s_s[n];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) acc[j] = fmaf(k[j], sv, acc[j]);
+    }
   }
+  uint4 vb[LA_U];
+  load_rows(vb, VX, ldvx, d + cg * 8, b, p, nv_first, ngrp, Nv, H, Wv, unf);
   // deterministic cross-group reduction (fixed order): partials -> smem [ngrp][d] -> ordered sum
   float* s_part = s_ctx + d;
   if (grp < ngrp) {
@@ -111,18 +135,34 @@ __global__ void __launch_bounds__(NT) linattn_fwd_kernel(const bf16* __restrict_
 #pragma unroll
   for (int j = 0; j < 8; ++j) ctx[j] = s_ctx[cg * 8 + j];
   // O = relu(value) * ctx
-  const int Wv = (VX == QKV) ? W : Nv;  // cross-attention is unfolded-only: row (b, p, n) of a [B, P, Nv, *] matrix
-  for (int n = (grp < ngrp ? grp : Nv); n < Nv; n += ngrp) {
-    const int64_t m = pix_index(b, p, n, H, Wv, unf);
-    float v[8];
-    unpack8(ldg16(VX + m * ldvx + d + cg * 8), v);
+  for (int n0 = nv_first; n0 < Nv; n0 += LA_U * ngrp) {
+    if (n0 != nv_first) load_rows(vb, VX, ldvx, d + cg * 8, b, p, n0, ngrp, Nv, H, Wv, unf);
 #pragma unroll
-    for (int j = 0; j < 8; ++j) v[j] = fmaxf(v[j], 0.f) * ctx[j];
-    stg16(O + m * ldo + cg * 8, pack8(v));
+    for (int u = 0; u < LA_U; ++u) {
+      const int n = n0 + u * ngrp;
+      if (n >= Nv) break;
+      float v[8];
+      unpack8(vb[u], v);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) v[j] = fmaxf(v[j], 0.f) * ctx[j];
+      stg16(O + pix_index(b, p, n, H, Wv, unf) * ldo + cg * 8, pack8(v));
+    }
   }
 }
 
-// dynamic smem: s[N] | ds[N] | ctx[d] | dctx[d] | dbk[d] | dbv[d]
+// The channel groups of one row n are the cgs consecutive threads grp * cgs .. grp * cgs + cgs - 1; they span at most la_pieces(cgs) warps.
+__host__ __device__ inline int la_pieces(int cgs) {
+  int q = 1;
+  for (int g = 0; g < NT / cgs; ++g) {
+    const int w = (g * cgs + cgs - 1) / 32 - (g * cgs) / 32 + 1;
+    q = w > q ? w : q;
+  }
+  return q;
+}
+
+// dynamic smem: dsp[npc][N] | dctx[d] | dbk[d] | dbv[d] (fp64) | part[2][ngrp][d] | s[N] | ctx[d] (fp32)
+// Every sum that several threads contribute to is fp64 and fixed-order: the warp pieces of a row's ds by shuffles, the cross-group partials of
+// dctx, dbv and dbk through part[].
 __global__ void __launch_bounds__(NT) linattn_bwd_kernel(const bf16* __restrict__ QKV, int ldq, const bf16* __restrict__ DO, int ldo,
                                                          const float* __restrict__ S, const float* __restrict__ CTX, int H, int W, int d,
                                                          bf16* __restrict__ DQKV, double* __restrict__ dbias, int unf, const bf16* __restrict__ VX,
@@ -134,73 +174,133 @@ __global__ void __launch_bounds__(NT) linattn_bwd_kernel(const bf16* __restrict_
   const int N = unf ? W : (H >> 1) * (W >> 1);
   const int P = unf ? H : 4;
   const int Wv = (VX == QKV) ? W : Nv;
-  // the sums the warps contribute to are fp64: their fp32 partials add exactly, whatever the order
-  double* s_ds = smd;
-  double* s_dctx = s_ds + N;
+  const int cgs = d >> 3;
+  const int npc = la_pieces(cgs);
+  const int ngrp = blockDim.x / cgs;
+  double* s_dsp = smd;
+  double* s_dctx = s_dsp + (size_t)npc * N;
   double* s_dbk = s_dctx + d;
   double* s_dbv = s_dbk + d;
-  float* s_s = reinterpret_cast<float*>(s_dbv + d);
+  float* s_part = reinterpret_cast<float*>(s_dbv + d);
+  float* s_s = s_part + 2 * ngrp * d;
   float* s_ctx = s_s + N;
   const int b = blockIdx.x / P, p = blockIdx.x % P;
   const int tid = threadIdx.x;
-  for (int n = tid; n < N; n += blockDim.x) { s_s[n] = S[((int64_t)b * P + p) * N + n]; s_ds[n] = 0.0; }
-  for (int i = tid; i < d; i += blockDim.x) { s_ctx[i] = CTX[((int64_t)b * P + p) * d + i]; s_dctx[i] = 0.0; s_dbk[i] = 0.0; s_dbv[i] = 0.0; }
+  const int cg = tid % cgs, grp = tid / cgs;
+  const int n_first = grp < ngrp ? grp : N;
+  const int nv_first = grp < ngrp ? grp : Nv;
+  uint4 vb[LA_U], gb[LA_U];
+  load_rows(vb, VX, ldvx, d + cg * 8, b, p, nv_first, ngrp, Nv, H, Wv, unf);
+  load_rows(gb, DO, ldo, cg * 8, b, p, nv_first, ngrp, Nv, H, Wv, unf);
+  for (int n = tid; n < N; n += blockDim.x) s_s[n] = S[((int64_t)b * P + p) * N + n];
+  for (int i = tid; i < npc * N; i += blockDim.x) s_dsp[i] = 0.0;
+  for (int i = tid; i < d; i += blockDim.x) s_ctx[i] = CTX[((int64_t)b * P + p) * d + i];
   __syncthreads();
 
-  const int cgs = d >> 3;
-  const int cg = tid % cgs, grp = tid / cgs, ngrp = blockDim.x / cgs;
-  const int n_first = grp < ngrp ? grp : N;
   // pass 1: dctx[c] = sum_n dO*relu(V);  dV = dO * ctx * 1[V>0]
   {
     float ctx[8], acc[8], dbv[8];
 #pragma unroll
     for (int j = 0; j < 8; ++j) { ctx[j] = s_ctx[cg * 8 + j]; acc[j] = 0.f; dbv[j] = 0.f; }
-    for (int n = (grp < ngrp ? grp : Nv); n < Nv; n += ngrp) {
-      const int64_t m = pix_index(b, p, n, H, Wv, unf);
-      float v[8], g[8];
-      unpack8(ldg16(VX + m * ldvx + d + cg * 8), v);
-      unpack8(ldg16(DO + m * ldo + cg * 8), g);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const bool pos = v[j] > 0.f;
-        acc[j] = fmaf(g[j], pos ? v[j] : 0.f, acc[j]);
-        g[j] = pos ? bf16_round(g[j] * ctx[j]) : 0.f;
-        dbv[j] += g[j];
+    for (int n0 = nv_first; n0 < Nv; n0 += LA_U * ngrp) {
+      if (n0 != nv_first) {
+        load_rows(vb, VX, ldvx, d + cg * 8, b, p, n0, ngrp, Nv, H, Wv, unf);
+        load_rows(gb, DO, ldo, cg * 8, b, p, n0, ngrp, Nv, H, Wv, unf);
       }
-      stg16(DVX + m * ldvx + d + cg * 8, pack8(g));
+#pragma unroll
+      for (int u = 0; u < LA_U; ++u) {
+        const int n = n0 + u * ngrp;
+        if (n >= Nv) break;
+        float v[8], g[8];
+        unpack8(vb[u], v);
+        unpack8(gb[u], g);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const bool pos = v[j] > 0.f;
+          acc[j] = fmaf(g[j], pos ? v[j] : 0.f, acc[j]);
+          g[j] = pos ? bf16_round(g[j] * ctx[j]) : 0.f;
+          dbv[j] += g[j];
+        }
+        stg16(DVX + pix_index(b, p, n, H, Wv, unf) * ldvx + d + cg * 8, pack8(g));
+      }
     }
     if (grp < ngrp) {
 #pragma unroll
-      for (int j = 0; j < 8; ++j) { atomicAdd(&s_dctx[cg * 8 + j], (double)acc[j]); atomicAdd(&s_dbv[cg * 8 + j], (double)dbv[j]); }
+      for (int j = 0; j < 8; ++j) { s_part[grp * d + cg * 8 + j] = acc[j]; s_part[(ngrp + grp) * d + cg * 8 + j] = dbv[j]; }
     }
   }
+  uint4 kb[LA_U];
+  load_rows(kb, QKV, ldq, cg * 8, b, p, n_first, ngrp, N, H, W, unf);
   __syncthreads();
-  // pass 2: ds[n] = sum_c dctx[c]*K[n,c];  dK = dctx * s[n]
+  for (int i = tid; i < d; i += blockDim.x) {
+    double t = 0.0, tv = 0.0;
+    for (int gq = 0; gq < ngrp; ++gq) { t += (double)s_part[gq * d + i]; tv += (double)s_part[(ngrp + gq) * d + i]; }
+    s_dctx[i] = t;
+    s_dbv[i] = tv;
+  }
+  __syncthreads();
+  // pass 2: ds[n] = sum_c dctx[c]*K[n,c];  dK = dctx * s[n].  The trip count is the same for every thread (the row reductions are warp
+  // shuffles); a thread's row n = grp + k * ngrp is real when grp < ngrp and n < N.
   {
+    const int lane = tid & 31, warp = tid >> 5;
+    // this thread's row occupies lanes [seg_lo, seg_hi] of the warp; threads without a row form one-lane segments
+    const int seg_lo = grp < ngrp ? max(grp * cgs - warp * 32, 0) : lane;
+    const int seg_hi = grp < ngrp ? min(grp * cgs + cgs - 1 - warp * 32, 31) : lane;
+    const int piece = warp - (grp * cgs) / 32;
     float dctx[8], dbk[8];
 #pragma unroll
     for (int j = 0; j < 8; ++j) { dctx[j] = (float)s_dctx[cg * 8 + j]; dbk[j] = 0.f; }
-    for (int n = n_first; n < N; n += ngrp) {
-      const int64_t m = pix_index(b, p, n, H, W, unf);
-      float k[8], dk[8];
-      unpack8(ldg16(QKV + m * ldq + cg * 8), k);
-      const float sv = s_s[n];
-      float part = 0.f;
+    const int steps = (N + ngrp - 1) / ngrp;
+    for (int k0 = 0; k0 < steps; k0 += LA_U) {
+      const int n0 = grp + k0 * ngrp;
+      if (k0 != 0) load_rows(kb, QKV, ldq, cg * 8, b, p, grp < ngrp ? n0 : N, ngrp, N, H, W, unf);
 #pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        part = fmaf(dctx[j], k[j], part);
-        dk[j] = bf16_round(dctx[j] * sv);
-        dbk[j] += dk[j];
+      for (int u = 0; u < LA_U; ++u) {
+        if (k0 + u >= steps) break;
+        const int n = n0 + u * ngrp;
+        const bool real = grp < ngrp && n < N;
+        double part = 0.0;
+        if (real) {
+          float k[8], dk[8];
+          unpack8(kb[u], k);
+          const float sv = s_s[n];
+          float pf = 0.f;
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            pf = fmaf(dctx[j], k[j], pf);
+            dk[j] = bf16_round(dctx[j] * sv);
+            dbk[j] += dk[j];
+          }
+          part = (double)pf;
+          stg16(DQKV + pix_index(b, p, n, H, W, unf) * ldq + cg * 8, pack8(dk));
+        }
+        for (int o = 1; o < 32 && o < cgs; o <<= 1) {
+          const double t = __shfl_down_sync(0xffffffffu, part, o);
+          if (lane + o <= seg_hi) part += t;
+        }
+        if (real && lane == seg_lo) s_dsp[piece * N + n] = part;
       }
-      atomicAdd(&s_ds[n], (double)part);
-      stg16(DQKV + m * ldq + cg * 8, pack8(dk));
     }
     if (grp < ngrp) {
 #pragma unroll
-      for (int j = 0; j < 8; ++j) atomicAdd(&s_dbk[cg * 8 + j], (double)dbk[j]);
+      for (int j = 0; j < 8; ++j) s_part[grp * d + cg * 8 + j] = dbk[j];
     }
   }
   __syncthreads();
+  for (int n = tid; n < N; n += blockDim.x) {
+    double t = 0.0;
+    for (int q = 0; q < npc; ++q) t += s_dsp[q * N + n];
+    s_dsp[n] = t;  // slot q = 0 of row n: read only by this thread
+  }
+  if (dbias) {
+    for (int i = tid; i < d; i += blockDim.x) {
+      double t = 0.0;
+      for (int gq = 0; gq < ngrp; ++gq) t += (double)s_part[gq * d + i];
+      s_dbk[i] = t;
+    }
+  }
+  __syncthreads();
+  const double* s_ds = s_dsp;
   // dq = s * (ds - sum_n ds*s); written with the zero pad of the last 16-byte chunk
   float ldot = 0.f;
   for (int n = tid; n < N; n += blockDim.x) ldot += (float)s_ds[n] * s_s[n];
@@ -274,7 +374,8 @@ static int linattn_bwd_impl(const void* QKV, int ldq, const void* DO, int ldo, c
   CVB_CHECK(VX == QKV || patch == 0, "cvb_linattn_bwd: cross-attention needs the unfolded layout (patch = 0)");
   CVB_CHECK(DVX && ldvx % 8 == 0 && ldvx >= 2 * d && Nv > 0, "cvb_linattn_bwd: bad value tensor");
   const int nthreads = NT;
-  size_t smem = (size_t)(N + 3 * d) * sizeof(double) + (size_t)(N + d) * sizeof(float);
+  const int cgs = d / 8;
+  size_t smem = (size_t)(la_pieces(cgs) * N + 3 * d) * sizeof(double) + (size_t)(2 * (NT / cgs) * d + N + d) * sizeof(float);
   CVB_CHECK(smem <= 200 * 1024, "cvb_linattn_bwd: N=%d too large", N);
   static bool attr = false;
   if (!attr) { CVB_CUDA(cudaFuncSetAttribute(linattn_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); attr = true; }

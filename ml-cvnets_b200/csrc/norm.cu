@@ -632,6 +632,11 @@ __global__ void __launch_bounds__(NT) ln_stats_kernel(const bf16* __restrict__ X
   }
 }
 
+// Row-block geometry (row_geom): thread = (8-channel group cg, row lane rr) walks rows r_begin + rr, + rpp, ... of its CTA's run.  That walk
+// fixes the fp32 chain of each column partial; the loads of GNB_U consecutive steps are issued before any of them is used, so a thread has
+// up to 3 * GNB_U 16-byte loads in flight.  b is constant over most of a run of rows: the per-sample terms are recomputed only where a thread's
+// rows cross into the next sample.
+constexpr int GNB_U = 2;
 __global__ void __launch_bounds__(NT) gn_bwd_apply_kernel(const bf16* __restrict__ G, const bf16* __restrict__ X, const float* __restrict__ mean,
                                                           const float* __restrict__ rstd, const double* __restrict__ sg, const double* __restrict__ sgx,
                                                           double count, const bf16* __restrict__ DRES, bf16* __restrict__ DX, int64_t M,
@@ -639,43 +644,68 @@ __global__ void __launch_bounds__(NT) gn_bwd_apply_kernel(const bf16* __restrict
                                                           const float* __restrict__ gamma) {
   pdl_wait();
   pdl_trigger();
-  extern __shared__ double sdred[];  // fp64: the threads' fp32 partials add exactly, whatever the order; [C]
+  extern __shared__ float spart[];  // [rpp][C]: the threads' fp32 column partials, added in fp64 in a fixed order
   const int tid = threadIdx.x;
-  if (col_sum) { for (int i = tid; i < C; i += blockDim.x) sdred[i] = 0.0; __syncthreads(); }
   const int cg = tid % cgs, rr = tid / cgs;
   const int c = cg * 8;
   float a0[8], gm[8];
 #pragma unroll
   for (int j = 0; j < 8; ++j) { a0[j] = 0.f; gm[j] = gamma ? gamma[c + j] : 1.0f; }
-  int64_t r_begin = (int64_t)blockIdx.x * rows_per_cta, r_end = r_begin + rows_per_cta;
-  if (r_end > M) r_end = M;
-  for (int64_t r = r_begin + rr; r < r_end; r += rpp) {
-    const int b = (int)(r / rows_per_sample);
-    const float mu = mean[b], rs = rstd[b];
-    const float m1 = (float)(sg[b] / count), m2 = (float)(sgx[b] / count);
-    float g[8], x[8];
-    unpack8(ldg16_stream(G + r * C + c), g);
-    unpack8(ldg16_stream(X + r * C + c), x);
+  const int64_t r_begin = (int64_t)blockIdx.x * rows_per_cta;
+  const int64_t r_end = r_begin + rows_per_cta < M ? r_begin + rows_per_cta : M;
+  int64_t r = r_begin + rr;
+  int b = (int)(r / rows_per_sample);
+  int64_t b_end = (int64_t)(b + 1) * rows_per_sample;  // first row of sample b + 1
+  float mu = 0.f, rs = 0.f, m1 = 0.f, m2 = 0.f;
+  if (r < r_end) { mu = mean[b]; rs = rstd[b]; m1 = (float)(sg[b] / count); m2 = (float)(sgx[b] / count); }
+  for (; r < r_end; r += GNB_U * rpp) {
+    uint4 gv[GNB_U], xv[GNB_U], dv[GNB_U];
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      float xh = (x[j] - mu) * rs;
-      g[j] = rs * (g[j] * gm[j] - m1 - xh * m2);
-    }
-    if (DRES) {
-      float d[8];
-      unpack8(ldg16_stream(DRES + r * C + c), d);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) g[j] += d[j];
+    for (int u = 0; u < GNB_U; ++u) {
+      const int64_t ru = r + (int64_t)u * rpp;
+      if (ru < r_end) {
+        gv[u] = ldg16_stream(G + ru * C + c);
+        xv[u] = ldg16_stream(X + ru * C + c);
+        if (DRES) dv[u] = ldg16_stream(DRES + ru * C + c);
+      }
     }
 #pragma unroll
-    for (int j = 0; j < 8; ++j) a0[j] += g[j];  // column sums (bias gradients) from the unrounded fp32 values
-    stg16(DX + r * C + c, pack8(g));
+    for (int u = 0; u < GNB_U; ++u) {
+      const int64_t ru = r + (int64_t)u * rpp;
+      if (ru >= r_end) break;
+      if (ru >= b_end) {
+        do { ++b; b_end += rows_per_sample; } while (ru >= b_end);
+        mu = mean[b]; rs = rstd[b]; m1 = (float)(sg[b] / count); m2 = (float)(sgx[b] / count);
+      }
+      float g[8], x[8];
+      unpack8(gv[u], g);
+      unpack8(xv[u], x);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        float xh = (x[j] - mu) * rs;
+        g[j] = rs * (g[j] * gm[j] - m1 - xh * m2);
+      }
+      if (DRES) {
+        float d[8];
+        unpack8(dv[u], d);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) g[j] += d[j];
+      }
+#pragma unroll
+      for (int j = 0; j < 8; ++j) a0[j] += g[j];  // column sums (bias gradients) from the unrounded fp32 values
+      stg16(DX + ru * C + c, pack8(g));
+    }
   }
   if (col_sum) {
-#pragma unroll
-    for (int j = 0; j < 8; ++j) atomicAdd(&sdred[c + j], (double)a0[j]);
+    float4* dst = reinterpret_cast<float4*>(spart + rr * C + c);
+    dst[0] = make_float4(a0[0], a0[1], a0[2], a0[3]);
+    dst[1] = make_float4(a0[4], a0[5], a0[6], a0[7]);
     __syncthreads();
-    for (int i = tid; i < C; i += blockDim.x) atomicAdd(col_sum + i, sdred[i]);
+    for (int i = tid; i < C; i += blockDim.x) {
+      double t = 0.0;
+      for (int q = 0; q < rpp; ++q) t += (double)spart[q * C + i];
+      atomicAdd(col_sum + i, t);
+    }
   }
 }
 
@@ -980,7 +1010,7 @@ extern "C" int cvb_gn_bwd_apply(const void* G, const void* X, const float* mean,
             "cvb_gn_bwd_apply: bad arguments");
   int64_t M = (int64_t)B * rows_per_sample;
   RowGeom g = row_geom(M, C);
-  CVB_CUDA(cvb_launch(gn_bwd_apply_kernel, g.ctas, g.nthreads, C * sizeof(double), static_cast<cudaStream_t>(stream), 
+  CVB_CUDA(cvb_launch(gn_bwd_apply_kernel, g.ctas, g.nthreads, col_sum ? g.rpp * C * sizeof(float) : 0, static_cast<cudaStream_t>(stream),
       static_cast<const bf16*>(G), static_cast<const bf16*>(X), mean, rstd, sg, sgx, count, static_cast<const bf16*>(DRES), static_cast<bf16*>(DX), M,
       rows_per_sample, C, col_sum, g.cgs, g.rpp, g.rows_per_cta, static_cast<const float*>(nullptr)));
   CVB_LAUNCH_CHECK();
@@ -1005,7 +1035,7 @@ extern "C" int cvb_gn_bwd(const void* V, const void* X, const float* mean, const
                       dbeta, samp_ws, samp_ws + B));
   CVB_LAUNCH_CHECK();
   RowGeom g = row_geom(M, C);
-  CVB_CUDA(cvb_launch(gn_bwd_apply_kernel, g.ctas, g.nthreads, C * sizeof(double), static_cast<cudaStream_t>(stream), static_cast<const bf16*>(V),
+  CVB_CUDA(cvb_launch(gn_bwd_apply_kernel, g.ctas, g.nthreads, 0, static_cast<cudaStream_t>(stream), static_cast<const bf16*>(V),
                       static_cast<const bf16*>(X), mean, rstd, static_cast<const double*>(samp_ws), static_cast<const double*>(samp_ws + B), count,
                       static_cast<const bf16*>(DRES), static_cast<bf16*>(DX), M, rows_per_sample, C, static_cast<double*>(nullptr), g.cgs, g.rpp,
                       g.rows_per_cta, gamma));

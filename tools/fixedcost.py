@@ -37,6 +37,19 @@ for pdl in (True, False):
         assert 0 == (lib.cvb_bn_finalize(s2[0].data_ptr(), s2[1].data_ptr(), 1000.0, bn.weight.data_ptr(), bn.bias.data_ptr(), 1e-5, 0.1, 0, 0, 0,
                                       outs[0].data_ptr(), outs[1].data_ptr(), outs[2].data_ptr(), outs[3].data_ptr(), C, torch.cuda.current_stream().cuda_stream))
     print(f"bn_finalize (1 tiny CTA x2)                     {graph_time(fin):8.2f} us/launch")
+    # the MobileViTv2 attention units' non-GEMM kernels: one sample (fixed cost) and the B = 128 bench batch, back to back in a graph
+    for (H, d) in [(32, 128), (16, 192), (8, 256)]:
+        for Bq in (1, 128):
+            M = Bq * H * H
+            qkv = torch.randn(M, 2 * d + 8, device=dev).to(BF); dO = torch.randn(M, d, device=dev).to(BF); dbq = torch.zeros(2 * d + 8, device=dev)
+            _, S, CTX = ops.linattn_fwd(qkv, Bq, H, H, d)
+            G = torch.randn(M, d, device=dev).to(BF); X = torch.randn(M, d, device=dev).to(BF)
+            gn = torch.stack([vec(Bq, 0.1), vec(Bq, 0.1, 1.0)]); ss = torch.randn(2, Bq, device=dev, dtype=torch.float64)
+            col = torch.zeros(d, device=dev, dtype=torch.float64)
+            uf = graph_time(lambda: ops.linattn_fwd(qkv, Bq, H, H, d))
+            ub = graph_time(lambda: ops.linattn_bwd(qkv, dO, S, CTX, Bq, H, H, d, dbias=dbq))
+            ug = graph_time(lambda: ops.gn_bwd_apply(G, X, gn, ss, float(H * H * d), Bq, H * H, DRES=dO, col_sum=col))
+            print(f"B={Bq:3d} @{H}^2 d={d}: linattn_fwd {uf:8.2f}  linattn_bwd+dbias {ub:8.2f}  gn_bwd_apply+DRES+col_sum {ug:8.2f} us/launch")
     for tc in (True, False):
         ops.set_tc_enabled(tc)
         for (N, K, mode) in [(192, 192, A_RAW), (256, 128, A_RAW), (192, 384, A_SILU)]:

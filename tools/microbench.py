@@ -18,8 +18,28 @@ def t(fn, reps=reps):
     e.record(); torch.cuda.synchronize()
     return s.elapsed_time(e) / reps
 
+def tg(fn, n=20, reps=5):
+    """Per-launch time of n back-to-back launches captured in one CUDA graph: no host-side launch cost, which dominates an eager loop of
+    the small attention-stage kernels."""
+    s = torch.cuda.Stream()
+    with torch.cuda.stream(s):
+        fn(); fn()
+    torch.cuda.synchronize()
+    g = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(g):
+        for _ in range(n): fn()
+    g.replay(); torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(reps): g.replay()
+    e1.record(); torch.cuda.synchronize()
+    return e0.elapsed_time(e1) / (reps * n)
+
+HBM_PEAK = 3.35e12  # H100 SXM data sheet, bytes/s
+
 def report(name, ms, nbytes):
-    print(f"{name:60s} {ms*1e3:9.1f} us  {nbytes/ms/1e6:8.1f} GB/s ({nbytes/1e6:.0f} MB algorithmic)", flush=True)
+    print(f"{name:60s} {ms*1e3:9.1f} us  {nbytes/ms/1e6:8.1f} GB/s  {nbytes/(ms*1e-3)/HBM_PEAK:5.2f} of HBM peak ({nbytes/1e6:.1f} MB algorithmic)",
+          flush=True)
 
 B = 128
 def vec(n, s=1.0, o=0.0): return torch.randn(n, device=dev) * s + o
@@ -79,3 +99,26 @@ if which in ("all", "dw", "prof"):
         gp = (vec(C, 0.2, 1.0), vec(C, 0.1), vec(C, 0.1))
         ms = t(lambda: ops.dw_bwd(DZ, X, B, H, H, C, s, Wt, g_mode=A_BNB, Y2=Y2, g_p=gp, x_mode=A_AFF_SILU, x_p=p, col_stats=col))
         report(name + " bwd", ms, 2.0 * C * B * (2 * H * H + 2 * Ho * Ho))
+
+# the MobileViTv2 attention units' memory-bound kernels at the three transformer stages (feature map H x H, d channels), timed as graph
+# replays; the 8^2 operands (13-25 MB) fit in the 50 MB L2, so their rates there are L2-assisted
+if which in ("all", "attn"):
+    for (H, d) in [(32, 128), (16, 192), (8, 256)]:
+        M, ld = B * H * H, 2 * d + 8
+        qkv = torch.randn(M, ld, device=dev).to(BF)
+        O, S, CTX = ops.linattn_fwd(qkv, B, H, H, d)
+        # reads key, value and the query column, writes O and the fp32 softmax S
+        ms = tg(lambda: ops.linattn_fwd(qkv, B, H, H, d))
+        report(f"linattn_fwd @{H}^2 d={d}", ms, M * (2.0 * 2 * d + 2 + 2 * d + 4))
+        dO = torch.randn(M, d, device=dev).to(BF)
+        dbq = torch.zeros(ld, device=dev)
+        # reads value, dO, key, the query column and S; writes dV, dK and the 8-column dq chunk
+        ms = tg(lambda: ops.linattn_bwd(qkv, dO, S, CTX, B, H, H, d, dbias=dbq))
+        report(f"linattn_bwd @{H}^2 d={d} +dbias", ms, M * (2.0 * 5 * d + 2 + 4 + 16))
+        G = torch.randn(M, d, device=dev).to(BF); X = torch.randn(M, d, device=dev).to(BF); R = torch.randn(M, d, device=dev).to(BF)
+        gn = torch.stack([vec(B, 0.1), vec(B, 0.1, 1.0)]); ss = torch.randn(2, B, device=dev, dtype=torch.float64) * 100
+        col = torch.zeros(d, device=dev, dtype=torch.float64)
+        for (res, cs) in [(None, col), (R, col), (R, None), (None, None)]:
+            ms = tg(lambda: ops.gn_bwd_apply(G, X, gn, ss, float(H * H * d), B, H * H, DRES=res, col_sum=cs))
+            report(f"gn_bwd_apply @{H}^2 C={d} {'+DRES' if res is not None else '-DRES'} {'+col_sum' if cs is not None else '-col_sum'}", ms,
+                   2.0 * M * d * (3 + (res is not None)))
