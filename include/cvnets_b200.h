@@ -334,6 +334,12 @@ CVB_API int cvb_na_loss_bwd(const double* sq, int B, int H, int W, const float* 
  * dy = bf16(p0 dz + p1 y + p2) (CVB_A_BNB on the bf16 [B*Ho*Wo, C0] dz / y, coef fp32 [3, C0]) and the prepared bf16 weight [C0, 32]
  * (columns ci*9 + u*3 + v).  C0 a multiple of 8, <= 64. */
 CVB_API int cvb_stem_dgrad(const void* dz, const void* y, const float* coef, const void* w, int B, int Ho, int Wo, int C0, float* dX, cvb_stream_t stream);
+/* Input gradient of the ViT / CLIP conv stem's first conv (3 -> C0, 4x4, stride 4, pad 1; vit.py:90-121): dX fp32 NCHW [B, 3, 4 Ho, 4 Wo] =
+ * conv_transpose(dy, W) with dy = bf16(p0 dz + p1 y + p2) (CVB_A_BNB on the bf16 [B*Ho*Wo, C0] dz / y, coef fp32 [3, C0]) and the prepared
+ * bf16 weight [C0, 48] (CVB_PREP_PATCH: columns (u*4 + v)*3 + ci).  Every element of dX is written, the last image row and column (which
+ * lie in no window) with 0; no atomics, bitwise reproducible.  C0 a multiple of 16, <= 320; dz, y, coef, dX 16-byte aligned. */
+CVB_API int cvb_patch_stem_dgrad(const void* dz, const void* y, const float* coef, const void* w, int B, int Ho, int Wo, int C0, float* dX,
+                                 cvb_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
  * Per-step tail of the training loop (engine/training_engine.py:289-312) on FLAT fp32 buffers of n elements: GradScaler unscale +

@@ -449,6 +449,135 @@ __global__ void __launch_bounds__(NA_NT) stem_dgrad_kernel(const bf16* __restric
   }
 }
 
+// ViT / CLIP conv-stem input gradient (3 -> C0, k = stride = 4, pad 1): dX[b, ci, 4i-1+u, 4j-1+v] = sum over co of dy[b, i, j, co] W[co, (4u+v)*3 + ci],
+// dy = bf16(p0 dz + p1 y + p2).  Stride = kernel, so the windows never overlap and every dX element has exactly one writer (no atomics, no
+// memset, bitwise reproducible).  The padding shifts the windows by one pixel: window i covers rows 4i-1 .. 4i+2, so image row / column -1 is
+// padding and H-1 / W-1 lie in no window (gradient 0).  The aligned float4 dX[.., 4q .. 4q+3] therefore holds columns v = 1..3 of patch q and
+// v = 0 of patch q+1.  A warp owns 15 consecutive patches of one patch row and also computes the 16th (the right neighbour; zero past the
+// row's end, which yields the W-1 column), stages the [16 x 48] result in shared memory and writes each image row as float4s, neighbouring
+// patches on neighbouring lanes.  The [16 x C0] x [C0 x 48] product runs on mma.sync m16n8k16 with the weight resident in shared memory; the
+// reduction order over channels is permuted so that each lane reads 8 consecutive channels (16 bytes) of its two rows per 32-channel step.
+constexpr int PS_NT = 384;
+constexpr int PS_WARPS = PS_NT / 32;
+constexpr int PS_OWN = 15;    // patches a warp writes; it computes PS_OWN + 1
+constexpr int PS_LDS = 56;    // staging row stride (floats): conflict-free float2 stores of the accumulator fragments
+constexpr int PS_MAX_C0 = 320;
+
+__host__ __device__ constexpr int ps_ldw(int C0) { return C0 + ((32 - C0 % 64) + 64) % 64; }  // weight row stride (bf16) = 32 mod 64
+__host__ __device__ constexpr size_t ps_smem(int C0) {
+  return (size_t)48 * ps_ldw(C0) * 2 + (size_t)3 * C0 * 4 + (size_t)PS_WARPS * 16 * PS_LDS * 4;
+}
+
+// n bf16 BatchNorm-backward values of one row (n = 8 or 4): channels c .. c+n-1, zero for a row past the patch row's end
+template <int N>
+__device__ __forceinline__ void ps_bnb(const uint32_t* z, const uint32_t* y, const float* cs, int C0, int c, bool valid, uint32_t* d) {
+#pragma unroll
+  for (int q = 0; q < N / 2; ++q) {
+    const float2 zz = unpack_bf162(z[q]), yy = unpack_bf162(y[q]);
+    const int k = c + 2 * q;
+    const float lo = fmaf(cs[k], zz.x, fmaf(cs[C0 + k], yy.x, cs[2 * C0 + k]));
+    const float hi = fmaf(cs[k + 1], zz.y, fmaf(cs[C0 + k + 1], yy.y, cs[2 * C0 + k + 1]));
+    d[q] = valid ? pack_bf162(lo, hi) : 0u;
+  }
+}
+
+__global__ void __launch_bounds__(PS_NT) patch_stem_dgrad_kernel(const bf16* __restrict__ DZ, const bf16* __restrict__ Yp, const float* __restrict__ coef,
+                                                                 const bf16* __restrict__ Wp, int B, int Ho, int Wo, int C0, float* __restrict__ DX) {
+  extern __shared__ __align__(16) unsigned char ps_raw[];
+  const int ldw = ps_ldw(C0);
+  bf16* sW = reinterpret_cast<bf16*>(ps_raw);                          // [48][ldw]: column n of the prepared [C0, 48] weight, channels contiguous
+  float* cs = reinterpret_cast<float*>(ps_raw + (size_t)48 * ldw * 2);  // [3][C0]
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, tq = lane & 3;
+  float* stg = cs + 3 * C0 + warp * 16 * PS_LDS;                        // [16][PS_LDS] per warp
+  pdl_wait();
+  pdl_trigger();
+  for (int t = threadIdx.x; t < 48 * C0; t += PS_NT) sW[(t % 48) * ldw + t / 48] = Wp[t];
+  for (int t = threadIdx.x; t < 3 * C0; t += PS_NT) cs[t] = coef[t];
+  __syncthreads();
+  const int H = 4 * Ho, W = 4 * Wo;
+  const int nchunk = (Wo + PS_OWN - 1) / PS_OWN;
+  const int64_t tiles = (int64_t)B * Ho * nchunk;
+  const int nfull = C0 / 32;
+  const bool tail = (C0 % 32) != 0;
+  for (int64_t t = (int64_t)blockIdx.x * PS_WARPS + warp; t < tiles; t += (int64_t)gridDim.x * PS_WARPS) {
+    const int64_t prow = t / nchunk;  // b * Ho + i
+    const int j0 = (int)(t % nchunk) * PS_OWN;
+    const bool v_lo = j0 + g < Wo, v_hi = j0 + g + 8 < Wo;
+    const bf16* zlo = DZ + (prow * Wo + j0 + g) * C0;
+    const bf16* ylo = Yp + (prow * Wo + j0 + g) * C0;
+    const bf16* zhi = zlo + 8 * (int64_t)C0;
+    const bf16* yhi = ylo + 8 * (int64_t)C0;
+    float acc[6][4];
+#pragma unroll
+    for (int nt = 0; nt < 6; ++nt) acc[nt][0] = acc[nt][1] = acc[nt][2] = acc[nt][3] = 0.f;
+    const uint4 zero4 = make_uint4(0, 0, 0, 0);
+    uint4 nz0 = zero4, ny0 = zero4, nz1 = zero4, ny1 = zero4;
+    if (nfull > 0) {
+      const int c = 8 * tq;
+      if (v_lo) nz0 = ldg16_stream(zlo + c), ny0 = ldg16_stream(ylo + c);
+      if (v_hi) nz1 = ldg16_stream(zhi + c), ny1 = ldg16_stream(yhi + c);
+    }
+    for (int s = 0; s < nfull; ++s) {
+      const uint4 z0 = nz0, y0 = ny0, z1 = nz1, y1 = ny1;
+      if (s + 1 < nfull) {  // the next 32 channels are in flight while these go through the tensor cores
+        const int c = 32 * (s + 1) + 8 * tq;
+        if (v_lo) nz0 = ldg16_stream(zlo + c), ny0 = ldg16_stream(ylo + c);
+        if (v_hi) nz1 = ldg16_stream(zhi + c), ny1 = ldg16_stream(yhi + c);
+      }
+      const int c = 32 * s + 8 * tq;
+      uint32_t dl[4], dh[4];
+      ps_bnb<8>(&z0.x, &y0.x, cs, C0, c, v_lo, dl);
+      ps_bnb<8>(&z1.x, &y1.x, cs, C0, c, v_hi, dh);
+      const uint32_t a0[4] = {dl[0], dh[0], dl[1], dh[1]};  // channels c+0..3: k-step 2s
+      const uint32_t a1[4] = {dl[2], dh[2], dl[3], dh[3]};  // channels c+4..7: k-step 2s+1
+#pragma unroll
+      for (int nt = 0; nt < 6; ++nt) {
+        const uint4 w = *reinterpret_cast<const uint4*>(sW + (8 * nt + g) * ldw + c);
+        mma_bf16_16816(acc[nt], a0, w.x, w.y);
+        mma_bf16_16816(acc[nt], a1, w.z, w.w);
+      }
+    }
+    if (tail) {  // C0 = 32 nfull + 16: one k-step, 4 channels (8 bytes) per lane and row
+      const int c = 32 * nfull + 4 * tq;
+      uint2 z0 = make_uint2(0, 0), y0 = z0, z1 = z0, y1 = z0;
+      if (v_lo) z0 = __ldg(reinterpret_cast<const uint2*>(zlo + c)), y0 = __ldg(reinterpret_cast<const uint2*>(ylo + c));
+      if (v_hi) z1 = __ldg(reinterpret_cast<const uint2*>(zhi + c)), y1 = __ldg(reinterpret_cast<const uint2*>(yhi + c));
+      uint32_t dl[2], dh[2];
+      ps_bnb<4>(&z0.x, &y0.x, cs, C0, c, v_lo, dl);
+      ps_bnb<4>(&z1.x, &y1.x, cs, C0, c, v_hi, dh);
+      const uint32_t a[4] = {dl[0], dh[0], dl[1], dh[1]};
+#pragma unroll
+      for (int nt = 0; nt < 6; ++nt) {
+        const uint2 w = *reinterpret_cast<const uint2*>(sW + (8 * nt + g) * ldw + c);
+        mma_bf16_16816(acc[nt], a, w.x, w.y);
+      }
+    }
+#pragma unroll
+    for (int nt = 0; nt < 6; ++nt) {
+      *reinterpret_cast<float2*>(stg + g * PS_LDS + 8 * nt + 2 * tq) = make_float2(acc[nt][0], acc[nt][1]);
+      *reinterpret_cast<float2*>(stg + (g + 8) * PS_LDS + 8 * nt + 2 * tq) = make_float2(acc[nt][2], acc[nt][3]);
+    }
+    __syncwarp();
+    const int qo = lane & 15, half = lane >> 4;
+    const int b = (int)(prow / Ho), i = (int)(prow % Ho);
+    if (qo < PS_OWN && j0 + qo < Wo) {
+      const float* p = stg + qo * PS_LDS;
+      float* base = DX + (int64_t)b * 3 * H * W + 4 * (j0 + qo);
+#pragma unroll
+      for (int it = 0; it < 6; ++it) {
+        const int combo = 2 * it + half, u = combo / 3, ci = combo % 3;
+        const int r = 4 * i - 1 + u;
+        if (r >= 0)
+          *reinterpret_cast<float4*>(base + ((int64_t)ci * H + r) * W) =
+              make_float4(p[(4 * u + 1) * 3 + ci], p[(4 * u + 2) * 3 + ci], p[(4 * u + 3) * 3 + ci], p[PS_LDS + (4 * u) * 3 + ci]);
+      }
+      if (i == Ho - 1)  // image row H-1 lies in no window
+        for (int ci = half; ci < 3; ci += 2) *reinterpret_cast<float4*>(base + ((int64_t)ci * H + H - 1) * W) = make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+    __syncwarp();
+  }
+}
+
 int grid_for(int64_t items) {
   int64_t g = (items + NA_NT - 1) / NA_NT;
   const int64_t cap = 8 * (int64_t)cvb_num_sms();
@@ -555,6 +684,25 @@ extern "C" int cvb_stem_dgrad(const void* dz, const void* y, const float* coef, 
             "cvb_stem_dgrad: bad arguments (C0 a multiple of 8 up to 64)");
   CVB_CHECK(cvb_aligned16(dz) && cvb_aligned16(y) && (reinterpret_cast<uintptr_t>(dX) & 7) == 0, "cvb_stem_dgrad: misaligned operand");
   CVB_CUDA(cvb_launch(stem_dgrad_kernel, grid_for((int64_t)B * Ho * Wo), NA_NT, 0, static_cast<cudaStream_t>(stream), static_cast<const bf16*>(dz),
+                      static_cast<const bf16*>(y), coef, static_cast<const bf16*>(w), B, Ho, Wo, C0, dX));
+  CVB_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int cvb_patch_stem_dgrad(const void* dz, const void* y, const float* coef, const void* w, int B, int Ho, int Wo, int C0, float* dX,
+                                    cvb_stream_t stream) {
+  CVB_CHECK(dz && y && coef && w && dX && B > 0 && Ho > 0 && Wo > 0 && C0 >= 16 && C0 <= PS_MAX_C0 && C0 % 16 == 0,
+            "cvb_patch_stem_dgrad: bad arguments (C0 a multiple of 16 up to %d)", PS_MAX_C0);
+  CVB_CHECK(cvb_aligned16(dz) && cvb_aligned16(y) && cvb_aligned16(dX) && cvb_aligned16(coef), "cvb_patch_stem_dgrad: misaligned operand");
+  static bool attr = false;
+  if (!attr) {
+    CVB_CUDA(cudaFuncSetAttribute(patch_stem_dgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ps_smem(PS_MAX_C0)));
+    attr = true;
+  }
+  const int64_t tiles = (int64_t)B * Ho * ((Wo + PS_OWN - 1) / PS_OWN);
+  const int64_t want = (tiles + PS_WARPS - 1) / PS_WARPS;
+  const int grid = (int)(want < cvb_num_sms() ? want : cvb_num_sms());  // persistent: at most one CTA per SM
+  CVB_CUDA(cvb_launch(patch_stem_dgrad_kernel, grid, PS_NT, ps_smem(C0), static_cast<cudaStream_t>(stream), static_cast<const bf16*>(dz),
                       static_cast<const bf16*>(y), coef, static_cast<const bf16*>(w), B, Ho, Wo, C0, dX));
   CVB_LAUNCH_CHECK();
   return 0;

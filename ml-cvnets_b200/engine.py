@@ -52,7 +52,10 @@ class TrainStep:
         ``optimizer="sgd"`` swaps AdamW for SGD with ``momentum`` / ``nesterov`` (optim.FlatSGD; ``betas`` / ``eps`` are then unused and
         ``max_norm`` None / 0 means no clipping).  A model with a RangeAugment augmentor returns ``{"augmented_tensor", "logits"}``; the cross
         entropy reads ``logits``, and with ``aug_loss`` the step minimises ``ce_weight * CE + aug_loss.weight * L_na`` (the RangeAugment recipes'
-        composite_loss); ``loss_parts`` (device fp32 [2]) then holds (CE, L_na) of the last step."""
+        composite_loss); ``loss_parts`` (device fp32 [2]) then holds (CE, L_na) of the last step.  A ``forward_loss`` of such a model returns
+        ``(loss, augmented_tensor)``; with ``aug_loss`` the step then minimises ``ce_weight * loss + aug_loss.weight * L_na`` and ``loss_parts``
+        holds (loss, L_na).  ``loss`` must apply ``cfg.scale`` in its backward, as the built-in losses do; the composite hands it its weighted
+        gradient unscaled (the CLIP recipe's step: INTEGRATION.md)."""
         import torch.distributed as dist
         if optimizer not in ("adamw", "sgd"):
             raise ValueError(f"optimizer must be 'adamw' or 'sgd', got {optimizer!r}")
@@ -142,6 +145,12 @@ class TrainStep:
                     loss = cross_entropy(out, y, _cfg=self.loss_cfg)
             else:
                 loss = self.forward_loss(self.model, *inputs, self.loss_cfg)
+                if isinstance(loss, tuple):  # (loss, augmented_tensor): a model with a RangeAugment augmentor, e.g. CLIP
+                    if self.aug_loss is None:
+                        raise ValueError("forward_loss returned (loss, augmented_tensor) but this TrainStep has no aug_loss: pass "
+                                         "aug_loss=NeuralAugmentationLoss(...) or return the loss alone")
+                    loss, x_aug = loss
+                    loss = self.aug_loss.composite(x_aug, loss, self.ce_weight, self.loss_cfg.scale, self.loss_parts)
             torch.autograd.backward(loss, grad_tensors=self._one)
         finally:
             ws.active = False

@@ -623,6 +623,7 @@ class PointwiseConvFn(torch.autograd.Function):
             out = ops.pw_gemm(x2, P.get(cfg.i_w), cout, bias=bias, R=R)
             ctx.saved = (x2,)
         ctx.cfg, ctx.dims, ctx.plist, ctx.has_res = cfg, (B, Cin, H, W, Ho, Wo), cfg.plist, residual is not None
+        ctx.x_fp32_nchw = x.dtype == torch.float32 and x.is_contiguous()
         ctx.save_for_backward(gamma) if gamma is not None else None
         return to_4d(out, B, Ho, Wo)
 
@@ -641,7 +642,11 @@ class PointwiseConvFn(torch.autograd.Function):
         db = D.mat(1, 1, cout).view(cout) if has_bias else None
         dW = D.ar.f32(cout, Kc) if dense else D.mat(0, cout, Cin)
         need_dx = ctx.needs_input_grad[0]
-        dA = None
+        dA = dx = None
+        # the ViT / CLIP image stem (fp32 3-channel image, 4x4 stride-4 pad-1 windows): its image gradient, which the RangeAugment augmentor
+        # reads, comes straight from (dz, y) as fp32 NCHW (cvb_patch_stem_dgrad) instead of a GEMM, col2im and a conversion
+        patch_stem = (need_dx and cfg.bn is not None and ctx.x_fp32_nchw and Cin == 3 and cfg.k == 4 and cfg.stride == 4 and cfg.pad == 1
+                      and H % 4 == 0 and W % 4 == 0 and cout % 16 == 0 and cout <= 320)
         if cfg.bn is not None:
             _, y, bn, ob = ctx.saved
             (gamma,) = ctx.saved_tensors
@@ -655,7 +660,9 @@ class PointwiseConvFn(torch.autograd.Function):
             gi, bi = (2, 3) if has_bias else (1, 2)
             dgb, c = ops.bn_bwd_finalize(sd, M, gamma, bn, ctx.ev[0], out=D.pair(gi, bi))
             D.set_pair(gi, bi, dgb)
-            if need_dx:
+            if patch_stem:
+                dx = ops.patch_stem_dgrad(dz, y, c, P.get(cfg.i_w), B, Ho, Wo)
+            elif need_dx:
                 dA = ops.pw_gemm(dz, P.get(cfg.i_wt), Kc, K=cout, a_mode=A_BNB, A2=y, a_p=c)
             ops.pw_wgrad_side(dz, x2, cout, Kc, g_mode=A_BNB, G2=y, g_p=c, dW=dW, dbias=db)
         else:
@@ -666,8 +673,7 @@ class PointwiseConvFn(torch.autograd.Function):
         if dense:
             D.unprep(0, dW, cout, cfg.k * cfg.k * Cin, Kc, PW.KIND_PATCH, rot=cfg.k * cfg.k, side=True)
         ops.join_side()
-        dx = None
-        if need_dx:
+        if dA is not None:
             dx = to_4d(ops.col2im(dA, B, Cin, H, W, cfg.k, cfg.stride, cfg.pad) if dense else dA, B, H, W)
         grads = D.finish()
         full = [grads[0], None, None, None]

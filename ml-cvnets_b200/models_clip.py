@@ -4,6 +4,7 @@ simple_projection_head.py and loss_fn/multi_modal_img_text/contrastive_loss_clip
     model = CLIP(default_clip_opts())                    # ViT-B/16 image tower + 12-layer text transformer, projection 512
     img, txt, logit_scale = model(images, text_tokens)   # L2-normalised features
     loss = clip_contrastive_loss(img, txt, logit_scale)  # all-gather over the process group when distributed
+    # with model.learn_augmentation.mode = distribution (RangeAugment): model(images, text_tokens) -> (img, txt, logit_scale, augmented_tensor)
 
     model.eval()                                         # zero-shot classification (transformer.py:428-504, clip.py:171-202)
     table = model.zero_shot_table(prompts)               # prompts [1, classes, captions, L] -> fp32 [d, classes]
@@ -241,18 +242,30 @@ class CLIP(nn.Module):
     def __init__(self, opts, *args, **kwargs) -> None:
         super().__init__()
         proj = getattr(opts, "model.multi_modal_image_text.clip.projection_dim", 256)
-        self.image_encoder = VisionTransformer(opts)
+        self.image_encoder = VisionTransformer(opts)  # builds image_encoder.neural_augmentor from model.learn_augmentation.* (clip.py:219-223)
         self.image_encoder.classifier = SimpleImageProjectionHead(opts, self.image_encoder.embed_dim, proj)
         self.text_encoder = TextTransformer(opts, projection_dim=proj)
         self.logit_scale = nn.Parameter(torch.ones([]) * math.log(1.0 / 0.07))
         self.cache_text_features_zero_shot = bool(getattr(opts, "model.multi_modal_image_text.clip.cache_text_features_zero_shot", False))
         self.cached_text_features = None
 
-    def forward(self, images: Tensor, text_tokens: Tensor) -> Tuple[Tensor, Tensor, Tensor]:
-        """(image features [B, d], text output, raw logit_scale).  The text output is what ``TextTransformer`` returns for the rank of
-        ``text_tokens``: [B, d], [B, N, d], or in eval mode the [d, Cl] zero-shot class table of 4-D prompts."""
-        img = self.image_encoder(images)
+    def encode_images(self, images: Tensor) -> Tuple[Tensor, Optional[Tensor]]:
+        """(image features, augmented_tensor): the image tower returns the reference's dict when it has a RangeAugment augmentor
+        (clip.py:152-161); augmented_tensor is None without one and in eval mode."""
+        out = self.image_encoder(images)
+        if isinstance(out, dict):
+            return out["logits"], out["augmented_tensor"]
+        return out, None
+
+    def forward(self, images: Tensor, text_tokens: Tensor):
+        """(image features [B, d], text output, raw logit_scale), and with a RangeAugment augmentor (``model.learn_augmentation.mode:
+        distribution``) a fourth entry, the augmented image (None in eval mode) that ``engine.NeuralAugmentationLoss`` reads.  The text output
+        is what ``TextTransformer`` returns for the rank of ``text_tokens``: [B, d], [B, N, d], or in eval mode the [d, Cl] zero-shot class
+        table of 4-D prompts."""
+        img, x_aug = self.encode_images(images)
         txt = self.zero_shot_table(text_tokens) if text_tokens.dim() == 4 else self.text_encoder(text_tokens)
+        if self.image_encoder.neural_augmentor is not None:
+            return img, txt, self.logit_scale, x_aug
         return img, txt, self.logit_scale
 
     def zero_shot_table(self, class_tokens: Tensor) -> Tensor:
@@ -284,7 +297,7 @@ class CLIP(nn.Module):
             raise NotImplementedError("Zero-shot evaluation is only supported with eval mode")
         with torch.no_grad():
             table = class_table_or_tokens if class_table_or_tokens.dim() == 2 else self.zero_shot_table(class_table_or_tokens)
-            img = self.image_encoder(images)
+            img, _ = self.encode_images(images)
             return ops.zs_logits_topk(img, table, 100.0, targets, hits)
 
 

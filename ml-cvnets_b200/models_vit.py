@@ -14,7 +14,7 @@ from __future__ import annotations
 
 import argparse
 from types import SimpleNamespace
-from typing import Dict, List, Optional, Tuple
+from typing import Dict, List, Optional, Tuple, Union
 
 import numpy as np
 import torch
@@ -24,6 +24,7 @@ from . import functional as Fn
 from . import ops
 from .layers import ConvLayer2d, Dropout, LinearLayer, get_normalization_layer, norm_layers_tuple
 from .modules import TransformerEncoder, _require_cuda
+from .neural_aug import augmented_forward, build_neural_augmentor
 
 
 def default_vit_opts(mode: str = "base", n_classes: int = 1000, **extra) -> argparse.Namespace:
@@ -85,6 +86,7 @@ class VisionTransformer(nn.Module):
         cfg = get_vit_configuration(opts)
         d, ffn, n_layers, heads, norm_layer = cfg["embed_dim"], cfg["ffn_dim"], cfg["n_transformer_layers"], cfg["n_attn_heads"], cfg["norm_layer"]
         self.opts = opts
+        self.neural_augmentor = build_neural_augmentor(opts)  # before patch_emb: its parameters come first (base_image_encoder.py:50)
         stem_dim = max(32, d // 4)
         self.patch_emb = nn.Sequential(
             ConvLayer2d(opts=opts, in_channels=3, out_channels=stem_dim, kernel_size=4, stride=4, bias=False, use_norm=True, use_act=True),
@@ -165,6 +167,13 @@ class VisionTransformer(nn.Module):
             raise NotImplementedError("no_cls_token (mean over tokens) is not implemented")
         return self.post_transformer_norm(x)
 
-    def forward(self, x: Tensor, *args, **kwargs) -> Tensor:
+    def forward_classifier(self, x: Tensor, *args, **kwargs) -> Tensor:
         _require_cuda(x, "VisionTransformer")
         return self.classifier(self.extract_features(x))
+
+    def forward(self, x: Tensor, *args, **kwargs) -> Union[Tensor, Dict[str, Optional[Tensor]]]:
+        """Logits; with a RangeAugment augmentor the reference's {"augmented_tensor", "logits"} (vit.py:592-610), augmented_tensor None in
+        eval mode."""
+        if self.neural_augmentor is not None:
+            return augmented_forward(self, x)
+        return self.forward_classifier(x)

@@ -755,6 +755,18 @@ def stem_dgrad(dz: Tensor, y: Tensor, coef: Tensor, Ws: Tensor, B: int, Ho: int,
     return dX
 
 
+def patch_stem_dgrad(dz: Tensor, y: Tensor, coef: Tensor, Wp: Tensor, B: int, Ho: int, Wo: int) -> Tensor:
+    """Input gradient of the ViT conv stem's 4x4 stride-4 pad-1 conv, fp32 NCHW [B, 3, 4 Ho, 4 Wo], from dz / y bf16 [B*Ho*Wo, C0], the
+    BatchNorm-backward coef [3, C0] and the prepared patch-order weight [C0, 48]."""
+    C0 = dz.shape[1]
+    if not (dz.is_contiguous() and y.is_contiguous() and coef.is_contiguous() and tuple(Wp.shape) == (C0, 48) and Wp.is_contiguous()):
+        raise ValueError("patch_stem_dgrad: dz / y [B*Ho*Wo, C0], coef [3, C0] and the weight [C0, 48] must be contiguous")
+    dX = torch.empty((B, 3, 4 * Ho, 4 * Wo), device=dz.device, dtype=torch.float32)
+    _lib().cvb_patch_stem_dgrad(dz.data_ptr(), y.data_ptr(), coef.data_ptr(), Wp.data_ptr(), B, Ho, Wo, C0, dX.data_ptr(), _stream())
+    _count()
+    return dX
+
+
 def ln_stats(X: Tensor, eps: float) -> Tensor:
     """per-token LayerNorm statistics of a bf16 [M, C] matrix -> fp32 [2, M] (mean, rstd)."""
     lib = _lib()

@@ -85,7 +85,7 @@ def main():
     targets = torch.randint(0, CLASSES, (B,), device="cuda", generator=g)
     hits = torch.zeros(2, device="cuda", dtype=torch.int64)
     with torch.no_grad():
-        img = model.image_encoder(images)
+        img, _ = model.encode_images(images)
     for _ in range(3):
         model.zero_shot_logits(images, truncated, targets=targets, hits=hits)
         ops.zs_logits_topk(img, truncated, 100.0, targets, hits)

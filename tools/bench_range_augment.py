@@ -1,16 +1,24 @@
-"""RangeAugment cost on the EfficientNet-B0 recipe (examples/range_augment/classification/efficientnet_b0.yaml): 224^2, B = 256, SGD (momentum 0.9,
-Nesterov, weight decay 4e-5), EMA 0.0005, label smoothing 0.1, mixup every step.
+"""RangeAugment cost on the recipes' training step, 224^2:
+  * efficientnet_b0 (default; examples/range_augment/classification/efficientnet_b0.yaml): B = 256, SGD (momentum 0.9, Nesterov, weight decay
+    4e-5), EMA 0.0005, label smoothing 0.1, mixup every step;
+  * vit_b16 (examples/range_augment/clip_finetune_imagenet/clip_vit_base.yaml, the ViT-B/16 image tower on ImageNet): B = 64, AdamW (weight
+    decay 0.2), clip 1.0, label smoothing 0.1, mixup every step;
+  * clip_b16 (examples/range_augment/clip/clip_vit_base.yaml): CLIP ViT-B/16, B = 256 synthetic image-text pairs, AdamW (weight decay 0.2),
+    clip 1.0, contrastive loss.
+  The NA loss is the recipes' PSNR loss, target (40, 20) on the cosine curriculum.
 
-    python tools/bench_range_augment.py OUTDIR [--steps 10] [--rounds 3] [--batch 256]
+    python tools/bench_range_augment.py OUTDIR [--model efficientnet_b0|vit_b16|clip_b16] [--steps 10] [--rounds 3] [--batch B]
 
 Writes OUTDIR/range_augment.json and prints it:
   * the card (name, power limit, SM clocks) read by nvidia-smi in the same run;
   * the captured TrainStep with and without RangeAugment (+ the NA loss), the two timed in alternating rounds (CUDA events over --steps
     replays each);
   * the new kernels alone at the step's shapes (CUDA events), achieved bytes/s against 3.35 TB/s, bytes = the tensors each must read and
-    write once (the image is read once per pass, twice under mixup);
-  * eager PyTorch on the same GPU: the tests/efficientnet_ref.py network under bf16 autocast with and without the restated reference augmentor
-    and its PSNR loss (tests/range_augment_ref.py, torch's own random draws), forward + backward, alternated; and the augmentor + loss alone.
+    write once (the image is read once per pass, twice under mixup); the stem input gradient is cvb_stem_dgrad (3x3 stem, C0 = 32) for
+    EfficientNet and cvb_patch_stem_dgrad (4x4 stride-4 stem, C0 = 192) for the ViT models;
+  * EfficientNet only: eager PyTorch on the same GPU, the tests/efficientnet_ref.py network under bf16 autocast with and without the restated
+    reference augmentor and its PSNR loss (tests/range_augment_ref.py, torch's own random draws), forward + backward, alternated; and the
+    augmentor + loss alone.
 """
 import argparse
 import json
@@ -49,21 +57,41 @@ def timed(fn, n):
     return e0.elapsed_time(e1) / n
 
 
-def make_step(m, B, res, augment):
-    from ml_cvnets_b200.models_effnet import default_effnet_opts
+def make_step(m, B, res, augment, model_name="efficientnet_b0"):
     torch.manual_seed(0)
-    model = m.EfficientNet(default_effnet_opts("b0", n_classes=1000, **(AUG if augment else {}))).cuda().train()
-    na = m.NeuralAugmentationLoss(target_value=(40, 10), curriculum_method="cosine", period=400) if augment else None
-    step = m.TrainStep(model, optimizer="sgd", lr=0.1, weight_decay=4e-5, momentum=0.9, nesterov=True, label_smoothing=0.1, ema_momentum=0.0005,
-                       max_norm=None, aug_loss=na)
-    step.set_mix("mixup", 0.7)
+    opts = AUG if augment else {}
     x = torch.rand(B, 3, res, res, device="cuda")
     y = torch.randint(0, 1000, (B,), device="cuda")
+    if model_name == "efficientnet_b0":
+        from ml_cvnets_b200.models_effnet import default_effnet_opts
+        model = m.EfficientNet(default_effnet_opts("b0", n_classes=1000, **opts)).cuda().train()
+        na = m.NeuralAugmentationLoss(target_value=(40, 10), curriculum_method="cosine", period=400) if augment else None
+        step = m.TrainStep(model, optimizer="sgd", lr=0.1, weight_decay=4e-5, momentum=0.9, nesterov=True, label_smoothing=0.1, ema_momentum=0.0005,
+                           max_norm=None, aug_loss=na)
+        step.set_mix("mixup", 0.7)
+    elif model_name == "vit_b16":
+        model = m.VisionTransformer(m.default_vit_opts("base", n_classes=1000, **opts)).cuda().train()
+        na = m.NeuralAugmentationLoss(target_value=(40, 20), curriculum_method="cosine", period=10) if augment else None
+        step = m.TrainStep(model, lr=1e-5, weight_decay=0.2, max_norm=1.0, label_smoothing=0.1, aug_loss=na)
+        step.set_mix("mixup", 0.7)
+    else:
+        model = m.CLIP(m.default_clip_opts("base", **opts)).cuda().train()
+        na = m.NeuralAugmentationLoss(target_value=(40, 20), curriculum_method="cosine", period=12) if augment else None
+
+        def clip_loss(mod, im, tok, cfg):
+            out = mod(im, tok)
+            loss = m.clip_contrastive_loss(*out[:3], _cfg=cfg)
+            return (loss, out[3]) if augment else loss
+
+        step = m.TrainStep(model, lr=5e-4, weight_decay=0.2, max_norm=1.0, aug_loss=na, forward_loss=clip_loss)
+        gen = torch.Generator(device="cuda").manual_seed(1234)
+        y = torch.randint(1, 49406, (B, 77), device="cuda", generator=gen)
+        y[torch.arange(B, device="cuda"), torch.randint(1, 77, (B,), device="cuda", generator=gen)] = 49407
     step.capture(x, y)
     return step, x, y
 
 
-def kernels(m, B, H, W):
+def kernels(m, B, H, W, patch_stem=False):
     ops = m.ops
     x = torch.rand(B, 3, H, W, device="cuda")
     mix = torch.tensor([1.0, 0.7, 0, 0, 0, 0], device="cuda")
@@ -79,18 +107,21 @@ def kernels(m, B, H, W):
     ops.na_compose(tab, mu, raw, B, coef)
     y = ops.na_apply(x, mix, key, coef, True, sq)
     img = x.numel() * 4
-    C0, Ho, Wo = 32, H // 2, W // 2
+    C0, Ho, Wo = (192, H // 4, W // 4) if patch_stem else (32, H // 2, W // 2)
     dz = torch.randn(B * Ho * Wo, C0, device="cuda").to(torch.bfloat16)
     yb = torch.randn(B * Ho * Wo, C0, device="cuda").to(torch.bfloat16)
     cf = torch.randn(3, C0, device="cuda")
-    Ws = torch.randn(C0, 32, device="cuda").to(torch.bfloat16)
+    Ws = torch.randn(C0, 48 if patch_stem else 32, device="cuda").to(torch.bfloat16)
     runs = {
         "na_stats": (lambda: ops.na_stats(x, mix, key, True, mu), 2 * img),
         "na_apply": (lambda: ops.na_apply(x, mix, key, coef, True, sq), 3 * img),
         "na_bwd_reduce": (lambda: ops.na_bwd_reduce(y, None, x, mix, key, coef, True, red), 3 * img),
-        "stem_dgrad": (lambda: ops.stem_dgrad(dz, yb, cf, Ws, B, Ho, Wo), 2 * dz.numel() * 2 + img),
-        "na_plan": (lambda: ops.na_plan(key, B, 7, tab), tab.numel() * 4),
     }
+    if patch_stem:
+        runs["patch_stem_dgrad"] = (lambda: ops.patch_stem_dgrad(dz, yb, cf, Ws, B, Ho, Wo), 2 * dz.numel() * 2 + img)
+    else:
+        runs["stem_dgrad"] = (lambda: ops.stem_dgrad(dz, yb, cf, Ws, B, Ho, Wo), 2 * dz.numel() * 2 + img)
+    runs["na_plan"] = (lambda: ops.na_plan(key, B, 7, tab), tab.numel() * 4)
     out = {}
     for name, (fn, nbytes) in runs.items():
         for _ in range(3):
@@ -162,16 +193,19 @@ def main():
     ap.add_argument("outdir")
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--rounds", type=int, default=3)
-    ap.add_argument("--batch", type=int, default=256)
+    ap.add_argument("--model", choices=("efficientnet_b0", "vit_b16", "clip_b16"), default="efficientnet_b0")
+    ap.add_argument("--batch", type=int, default=None, help="default: the recipe's per-GPU batch (256; 64 for vit_b16)")
     ap.add_argument("--res", type=int, default=224)
     a = ap.parse_args()
+    if a.batch is None:
+        a.batch = 64 if a.model == "vit_b16" else 256
     if not torch.cuda.is_available():
         raise SystemExit("bench_range_augment.py needs a CUDA device")
     import ml_cvnets_b200 as m
     os.makedirs(a.outdir, exist_ok=True)
-    res = {"card": card(), "batch": a.batch, "res": a.res}
-    plain = make_step(m, a.batch, a.res, False)
-    aug = make_step(m, a.batch, a.res, True)
+    res = {"card": card(), "model": a.model, "batch": a.batch, "res": a.res}
+    plain = make_step(m, a.batch, a.res, False, a.model)
+    aug = make_step(m, a.batch, a.res, True, a.model)
     times = {"without": [], "with": []}
     for _ in range(a.rounds):
         for name, (step, x, y) in (("without", plain), ("with", aug)):
@@ -182,10 +216,12 @@ def main():
     res["launches_per_step"] = {"without": plain[0].launches_per_step, "with": aug[0].launches_per_step}
     del plain, aug
     torch.cuda.empty_cache()
-    res["kernels"] = kernels(m, a.batch, a.res, a.res)
-    res["eager_pytorch_reference"] = eager_reference(a.batch, a.res, a.res, a.steps, a.rounds)
+    res["kernels"] = kernels(m, a.batch, a.res, a.res, patch_stem=a.model != "efficientnet_b0")
+    if a.model == "efficientnet_b0":
+        res["eager_pytorch_reference"] = eager_reference(a.batch, a.res, a.res, a.steps, a.rounds)
     res["card_after"] = card()
-    with open(os.path.join(a.outdir, "range_augment.json"), "w") as f:
+    name = "range_augment.json" if a.model == "efficientnet_b0" else f"range_augment_{a.model}.json"
+    with open(os.path.join(a.outdir, name), "w") as f:
         json.dump(res, f, indent=1)
     print(json.dumps(res))
 
