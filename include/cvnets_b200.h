@@ -31,7 +31,7 @@ typedef void* cvb_stream_t; /* cudaStream_t */
 #define CVB_API
 #endif
 
-#define CVB_ABI_VERSION 11
+#define CVB_ABI_VERSION 12
 
 /* operand "load modes": the normalisation / activation of the PRODUCER layer is applied while the CONSUMER loads it
  * (training-mode BatchNorm cannot be fused into its own conv: SURVEY.md section 7 "hard parts"). */
@@ -114,7 +114,8 @@ typedef struct {
 CVB_API int cvb_pw_wgrad(const cvb_wgrad_args* args, cvb_stream_t stream);
 
 /* OUT[m,k] = load(A[,A2])[m,k] (bf16): materialises one of the operand load modes above.  Used for WIDE layers (K >= 384 with
- * several N tiles, all late-stage and L2-resident) where applying the prologue once is cheaper than once per N tile. */
+ * several N tiles, all late-stage and L2-resident) where applying the prologue once is cheaper than once per N tile.
+ * K <= 8192, M < 2^31. */
 CVB_API int cvb_apply_load_mode(const void* A, int lda, const void* A2, int lda2, int mode, const float* p0, const float* p1, const float* p2,
                                 const float* row_mean, const float* row_rstd, int rows_per_sample, void* OUT, int ldo, int64_t M, int K,
                                 cvb_stream_t stream);
@@ -159,16 +160,14 @@ CVB_API int cvb_dw_bwd(const cvb_dw_bwd_args* args, cvb_stream_t stream);
  * A[(b,oh,ow), ci*9+u*3+v] = bf16(X[b,ci,2oh+u-1,2ow+v-1]) (zero padded; columns 27..31 are zero), fp32 image in with
  * arbitrary element strides (NCHW or channels_last).  The 32-column bf16 patch matrix costs 64 B/pixel (the stem's
  * output alone is 64 B/pixel at C0=32) and lets forward, BN statistics and dW reuse the GEMM kernels.
- * ------------------------------------------------------------------------------------------------------------- */
-CVB_API int cvb_stem_im2col(const float* X, int64_t sxn, int64_t sxc, int64_t sxh, int64_t sxw, int B, int H, int W, void* A,
-                    cvb_stream_t stream);
-/* The same gather with the reference's batch-mixing input transforms folded in (SURVEY.md 8f row 3: engine/training_engine.py:236-238,
+ * The gather folds in the reference's batch-mixing input transforms (SURVEY.md 8f row 3: engine/training_engine.py:236-238,
  * data/transforms/image_torch.py:99-137 RandomMixup, :290-342 RandomCutmix).  mix: DEVICE float[6] = {mode, lambda, x1, y1, x2, y2} or NULL;
  * every sample pairs with its predecessor in the batch (image.roll(1, 0)): mode 1 (mixup) x = lambda*x + (1-lambda)*x_prev in fp32;
- * mode 2 (cutmix) rows [y1,y2) x columns [x1,x2) come from x_prev; mode 0 = off.  The matching target distribution
- * lambda*onehot(y[b]) + (1-lambda)*onehot(y[b-1]) is what cvb_ce_fwd / cvb_ce_bwd use when given the same `mix`. */
-CVB_API int cvb_stem_im2col_mix(const float* X, int64_t sxn, int64_t sxc, int64_t sxh, int64_t sxw, int B, int H, int W, void* A, const float* mix,
-                        cvb_stream_t stream);
+ * mode 2 (cutmix) rows [y1,y2) x columns [x1,x2) come from x_prev; mode 0 or NULL = off.  The matching target distribution
+ * lambda*onehot(y[b]) + (1-lambda)*onehot(y[b-1]) is what cvb_ce_fwd / cvb_ce_bwd use when given the same `mix`.
+ * ------------------------------------------------------------------------------------------------------------- */
+CVB_API int cvb_stem_im2col(const float* X, int64_t sxn, int64_t sxc, int64_t sxh, int64_t sxw, int B, int H, int W, void* A, const float* mix,
+                    cvb_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
  * BatchNorm2d bookkeeping (cvnets/layers/normalization/batch_norm.py:14-49; math SURVEY App. A1)
@@ -297,7 +296,7 @@ CVB_API int cvb_dropout_fwd(const void* V, const void* R, void* Y, int64_t M, in
 CVB_API int cvb_dropout_bwd(const void* DY, void* DV, int64_t M, int C, int rows_per_sample, float p, float p_row, const void* key, cvb_stream_t stream);
 
 /* RangeAugment (cvnets/neural_augmentor/neural_aug.py DistributionNeuralAugmentor, loss_fn/neural_augmentation.py) on fp32 NCHW images [B, 3, H, W]
- * in [0, 1], contiguous.  `mix` (NULL = off) is the batch-mixing record of cvb_stem_im2col_mix, applied on the fly: the augmentor sees the mixed image.
+ * in [0, 1], contiguous.  `mix` (NULL = off) is the batch-mixing record of cvb_stem_im2col, applied on the fly: the augmentor sees the mixed image.
  * Every augmentation is affine per (sample, channel), so the chain is x_aug = clip(A x_mix + Bc + C eps, 0, 1) with coef[b, c] = (A, Bc, C).
  * Draws are hashes of the 64-bit key at `key` (cvb_rng_next), recomputed by every kernel that needs them:
  *   cvb_na_plan     draw table tab[4 + 3 B]: tab[0..2] augmentation (0 brightness, 1 contrast, 2 noise) at each position of a uniformly random
@@ -383,7 +382,7 @@ CVB_API int cvb_sgd_step(float* params, const float* grads, float* momentum_buf,
  * gradient w.r.t. the raw similarities and accumulates d loss / d logit_scale into dlogit_scale (fp32, atomically; 0 where the clamp is active).
  * ------------------------------------------------------------------------------------------------------------- */
 CVB_API int cvb_ce_fwd(const void* logits, int ld, int B, int C, const int64_t* target, int ignore_index, float label_smoothing, float* lse,
-               float* loss, float* n_valid, const float* mix /* see cvb_stem_im2col_mix; NULL = plain targets */, const float* logit_scale,
+               float* loss, float* n_valid, const float* mix /* see cvb_stem_im2col; NULL = plain targets */, const float* logit_scale,
                cvb_stream_t stream);
 CVB_API int cvb_ce_bwd(const void* logits, int ld, int B, int C, const int64_t* target, int ignore_index, float label_smoothing, const float* lse,
                const float* n_valid, const float* grad_out, const float* grad_scale, void* dlogits, int ldd, const float* mix,
@@ -430,12 +429,10 @@ CVB_API int cvb_zs_logits_topk(const void* img, int ldi, const float* table, int
 CVB_API int cvb_memset_zero(void* ptr, int64_t bytes, cvb_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
- * GlobalPool(mean) (cvnets/layers/global_pool.py:60-71) and small utilities
+ * GlobalPool(mean) (cvnets/layers/global_pool.py:60-71)
  * ------------------------------------------------------------------------------------------------------------- */
 CVB_API int cvb_global_pool_fwd(const void* X, int B, int HW, int C, void* OUT, cvb_stream_t stream);  /* bf16 -> bf16 [B,C] */
 CVB_API int cvb_global_pool_bwd(const void* DOUT, int B, int HW, int C, void* DX, cvb_stream_t stream); /* broadcast / HW */
-/* fp32 [N] += column sums of a bf16 (or fp32) [M, ld] matrix */
-CVB_API int cvb_col_sum(const void* X, int x_fp32, int ld, int64_t M, int N, float* out, cvb_stream_t stream);
 
 /* Layout kinds of cvb_prep_weights (fp32 parameter -> kernel layout) and of cvb_unprep_grad (fp32 gradient in a kernel layout -> the
  * parameter's layout; ROWMAJOR, TAPMAJOR_F32, VECTOR_F32 and PATCH only).  perm(r) = (r + rot) % rows for r < rows (rot = 1 moves the

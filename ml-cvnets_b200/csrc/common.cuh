@@ -48,30 +48,16 @@ int cvb_det_free(double* scratch, cudaStream_t st);
 // ---------------------------------------------------------------------------------------------- small device helpers
 // SiLU through ONE special-function op: sigmoid(z) = 0.5 + 0.5 tanh(z/2) with tanh.approx.f32 (MUFU.TANH, max abs error 2^-11), instead of
 // ex2 + rcp (two MUFU ops at 16 / clk / SM: the SiLU of a large activation tensor would be bound by the MUFU pipe).  The
-// absolute error of silu is <= |z| * 2.5e-4 -- below bf16 resolution of every value that is not itself negligible.  -DCVB_SILU_EXP=1
-// restores the exp formulation (A/B and accuracy checks).
-#ifndef CVB_SILU_EXP
-#define CVB_SILU_EXP 0
-#endif
+// absolute error of silu is <= |z| * 2.5e-4 -- below bf16 resolution of every value that is not itself negligible.
 __device__ __forceinline__ float tanh_approx_f(float x) {
   float y;
   asm("tanh.approx.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-__device__ __forceinline__ float sigmoid_f(float z) {
-#if CVB_SILU_EXP
-  return 1.0f / (1.0f + __expf(-z));
-#else
-  return fmaf(0.5f, tanh_approx_f(0.5f * z), 0.5f);
-#endif
-}
+__device__ __forceinline__ float sigmoid_f(float z) { return fmaf(0.5f, tanh_approx_f(0.5f * z), 0.5f); }
 __device__ __forceinline__ float silu_f(float z) {
-#if CVB_SILU_EXP
-  return z / (1.0f + __expf(-z));
-#else
   const float h = 0.5f * z;
   return fmaf(h, tanh_approx_f(h), h);
-#endif
 }
 // d/dz [z*sigmoid(z)] = s*(1 + z*(1-s))
 __device__ __forceinline__ float silu_grad_f(float z) {

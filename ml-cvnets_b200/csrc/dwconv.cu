@@ -46,12 +46,10 @@ __device__ __forceinline__ void transform_tile(uint8_t* tile, int TH_, int TW_, 
   *reinterpret_cast<float4*>(sc + 4) = *reinterpret_cast<const float4*>(s_par + pch * 8 + 4);
   *reinterpret_cast<float4*>(sh) = *reinterpret_cast<const float4*>(s_par + CB + pch * 8);
   *reinterpret_cast<float4*>(sh + 4) = *reinterpret_cast<const float4*>(s_par + CB + pch * 8 + 4);
-#if !CVB_SILU_EXP
   if (XMODE == CVB_A_AFF_SILU) {  // silu(z) = h + h * tanh(h), h = z / 2: fold the 1/2 into the affine parameters
 #pragma unroll
     for (int j = 0; j < 8; ++j) { sc[j] *= 0.5f; sh[j] *= 0.5f; }
   }
-#endif
   for (int ih = warp; ih < TH_; ih += NTHR / 32) {
     const int h = h_base + ih;
     if (h < 0 || h >= H) continue;
@@ -65,13 +63,7 @@ __device__ __forceinline__ void transform_tile(uint8_t* tile, int TH_, int TW_, 
 #pragma unroll
       for (int j = 0; j < 4; ++j) {  // fp32 channel pairs: 2 ffma2 + 2 MUFU per channel pair
         float2 z = ffma2(make_float2(sc[2 * j], sc[2 * j + 1]), up2(rw[j]), make_float2(sh[2 * j], sh[2 * j + 1]));
-        if (XMODE == CVB_A_AFF_SILU) {
-#if CVB_SILU_EXP
-          z = make_float2(silu_f(z.x), silu_f(z.y));
-#else
-          z = ffma2(z, make_float2(tanh_approx_f(z.x), tanh_approx_f(z.y)), z);
-#endif
-        }
+        if (XMODE == CVB_A_AFF_SILU) z = ffma2(z, make_float2(tanh_approx_f(z.x), tanh_approx_f(z.y)), z);
         ow[j] = pack_bf162(z.x, z.y);
       }
       *ptr = make_uint4(ow[0], ow[1], ow[2], ow[3]);

@@ -51,7 +51,7 @@ __device__ __forceinline__ Mix load_mix(const float* mix) {
   }
   return m;
 }
-// x_mix of plane (b, c) at pixel i: the rule of cvb_stem_im2col_mix (image.roll(1, 0) partner, fp32)
+// x_mix of plane (b, c) at pixel i: the rule of cvb_stem_im2col (image.roll(1, 0) partner, fp32)
 __device__ __forceinline__ float mixed(const float* __restrict__ X, const Mix& m, int B, int b, int c, int H, int W, int i) {
   const int64_t HW = (int64_t)H * W;
   float v = __ldg(X + ((int64_t)b * 3 + c) * HW + i);

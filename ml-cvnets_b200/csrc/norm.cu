@@ -256,38 +256,8 @@ __global__ void __launch_bounds__(NT) bn_apply_kernel(const bf16* __restrict__ Y
 }
 
 // ------------------------------------------------------------------------------------------------ elementwise: operand load modes
-// OUT[m, k] = load(A[, A2])[m, k]: materialises a prologue once for WIDE layers (many N tiles would each repeat it in the GEMM)
-__global__ void __launch_bounds__(NT) apply_load_mode_kernel(const bf16* __restrict__ A, const bf16* __restrict__ A2, int mode,
-                                                             const float* __restrict__ p0, const float* __restrict__ p1,
-                                                             const float* __restrict__ p2, const float* __restrict__ row_mean,
-                                                             const float* __restrict__ row_rstd, int rps, bf16* __restrict__ OUT, int64_t nvec,
-                                                             int cgs, int lda, int lda2, int ldo) {
-  pdl_wait();
-  pdl_trigger();
-  for (int64_t v = (int64_t)blockIdx.x * NT + threadIdx.x; v < nvec; v += (int64_t)gridDim.x * NT) {
-    const int64_t m = v / cgs;
-    const int c = (int)(v % cgs) * 8;
-    float f[8];
-    unpack8(ldg16_stream(A + m * lda + c), f);
-    if (mode == CVB_A_BNB) {
-      float y[8];
-      unpack8(ldg16_stream(A2 + m * lda2 + c), y);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) f[j] = fmaf(__ldg(p0 + c + j), f[j], fmaf(__ldg(p1 + c + j), y[j], __ldg(p2 + c + j)));
-    } else if (mode == CVB_A_GN) {
-      const int b = (int)(m / rps);
-      const float mu = __ldg(row_mean + b), rs = __ldg(row_rstd + b);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) f[j] = fmaf((f[j] - mu) * rs, __ldg(p0 + c + j), __ldg(p1 + c + j));
-    } else {
-#pragma unroll
-      for (int j = 0; j < 8; ++j) f[j] = apply_mode(mode, f[j], (mode == CVB_A_SILU) ? 1.f : __ldg(p0 + c + j), (mode == CVB_A_SILU) ? 0.f : __ldg(p1 + c + j));
-    }
-    stg16(OUT + m * ldo + c, pack8(f));
-  }
-}
-
-// Same operation, row-block geometry (row_geom): thread = (8-channel group, row lane); its per-channel parameters live in registers.
+// OUT[m, k] = load(A[, A2])[m, k]: materialises a prologue once for WIDE layers (many N tiles would each repeat it in the GEMM).
+// Row-block geometry (row_geom): thread = (8-channel group, row lane); its per-channel parameters live in registers.
 __global__ void __launch_bounds__(1024) apply_load_mode_rows_kernel(const bf16* __restrict__ A, const bf16* __restrict__ A2, int mode,
                                                                     const float* __restrict__ p0, const float* __restrict__ p1,
                                                                     const float* __restrict__ p2, const float* __restrict__ row_mean,
@@ -367,26 +337,6 @@ __global__ void __launch_bounds__(NT) bn_bwd_reduce_kernel(const bf16* __restric
   }
   __syncthreads();
   for (int i = tid; i < nc; i += blockDim.x) { atomicAdd(s0 + c0 + i, sdred[i]); atomicAdd(s1 + c0 + i, sdred[nc + i]); }
-}
-
-// column sums of a bf16 / fp32 [M, ld] matrix into fp32
-__global__ void __launch_bounds__(NT) col_sum_kernel(const void* __restrict__ X, int x_fp32, int ld, int64_t M, int N, float* out, int rows_per_cta) {
-  pdl_wait();
-  pdl_trigger();
-  // thread per column (strided), rows looped: N is small (<= 1024) and M small for the fp32 use (classifier)
-  int64_t r_begin = (int64_t)blockIdx.y * rows_per_cta, r_end = r_begin + rows_per_cta;
-  if (r_end > M) r_end = M;
-  int n = blockIdx.x * NT + threadIdx.x;
-  if (n >= N) return;
-  float acc = 0.f;
-  if (x_fp32) {
-    const float* x = static_cast<const float*>(X);
-    for (int64_t r = r_begin; r < r_end; ++r) acc += x[r * ld + n];
-  } else {
-    const bf16* x = static_cast<const bf16*>(X);
-    for (int64_t r = r_begin; r < r_end; ++r) acc += __bfloat162float(x[r * ld + n]);
-  }
-  atomicAdd(out + n, acc);
 }
 
 // per-sample sum / sumsq
@@ -909,24 +859,15 @@ extern "C" int cvb_apply_load_mode(const void* A, int lda, const void* A2, int l
                                    const float* row_mean, const float* row_rstd, int rows_per_sample, void* OUT, int ldo, int64_t M, int K,
                                    cvb_stream_t stream) {
   CVB_CHECK(A && OUT && M > 0 && K > 0 && K % 8 == 0 && lda % 8 == 0 && ldo % 8 == 0, "cvb_apply_load_mode: bad arguments");
+  CVB_CHECK(K <= 8192 && M < (int64_t)1 << 31, "cvb_apply_load_mode: K = %d, M = %lld (at most 8192 channels and 2^31 - 1 rows)", K, (long long)M);
   CVB_CHECK(mode >= CVB_A_AFF && mode <= CVB_A_BNB, "cvb_apply_load_mode: mode %d", mode);
   if (mode == CVB_A_BNB) CVB_CHECK(A2 && p0 && p1 && p2 && lda2 % 8 == 0, "cvb_apply_load_mode: BNB needs A2 and p0/p1/p2");
   if (mode == CVB_A_GN) CVB_CHECK(row_mean && row_rstd && rows_per_sample > 0 && p0 && p1, "cvb_apply_load_mode: GN needs statistics");
   if (mode == CVB_A_AFF || mode == CVB_A_AFF_SILU) CVB_CHECK(p0 && p1, "cvb_apply_load_mode: AFF needs p0/p1");
-  int64_t nvec = M * (K / 8);
-  if (K / 8 <= 1024 && M < (int64_t)1 << 31) {
-    // row-block form: a thread keeps one 8-channel group (its parameters stay in registers) and walks rows -- no per-vector 64-bit division, no
-    // per-element parameter loads (the grid-stride form below ran the ViT-B LayerNorm pre-pass at 1.9 TB/s)
-    RowGeom g = row_geom(M, K);
-    CVB_CUDA(cvb_launch(apply_load_mode_rows_kernel, g.ctas, g.nthreads, 0, static_cast<cudaStream_t>(stream), static_cast<const bf16*>(A),
-                        static_cast<const bf16*>(A2), mode, p0, p1, p2, row_mean, row_rstd, rows_per_sample > 0 ? rows_per_sample : 1,
-                        static_cast<bf16*>(OUT), (int)M, g.cgs, g.rpp, g.rows_per_cta, lda, lda2, ldo));
-    CVB_LAUNCH_CHECK();
-    return 0;
-  }
-  CVB_CUDA(cvb_launch(apply_load_mode_kernel, grid_for(nvec), NT, 0, static_cast<cudaStream_t>(stream), 
-      static_cast<const bf16*>(A), static_cast<const bf16*>(A2), mode, p0, p1, p2, row_mean, row_rstd, rows_per_sample > 0 ? rows_per_sample : 1,
-      static_cast<bf16*>(OUT), nvec, K / 8, lda, lda2, ldo));
+  RowGeom g = row_geom(M, K);
+  CVB_CUDA(cvb_launch(apply_load_mode_rows_kernel, g.ctas, g.nthreads, 0, static_cast<cudaStream_t>(stream), static_cast<const bf16*>(A),
+                      static_cast<const bf16*>(A2), mode, p0, p1, p2, row_mean, row_rstd, rows_per_sample > 0 ? rows_per_sample : 1,
+                      static_cast<bf16*>(OUT), (int)M, g.cgs, g.rpp, g.rows_per_cta, lda, lda2, ldo));
   CVB_LAUNCH_CHECK();
   return 0;
 }
@@ -1062,27 +1003,14 @@ extern "C" int cvb_global_pool_bwd(const void* DOUT, int B, int HW, int C, void*
   return 0;
 }
 
-extern "C" int cvb_col_sum(const void* X, int x_fp32, int ld, int64_t M, int N, float* out, cvb_stream_t stream) {
-  CVB_CHECK(X && out && M > 0 && N > 0 && ld >= N, "cvb_col_sum: bad arguments");
-  int rows_per_cta = 256;
-  dim3 grid((N + NT - 1) / NT, (unsigned)((M + rows_per_cta - 1) / rows_per_cta));
-  CVB_CUDA(cvb_launch(col_sum_kernel, grid, NT, 0, static_cast<cudaStream_t>(stream), X, x_fp32, ld, M, N, out, rows_per_cta));
-  CVB_LAUNCH_CHECK();
-  return 0;
-}
-
-extern "C" int cvb_stem_im2col_mix(const float* X, int64_t sxn, int64_t sxc, int64_t sxh, int64_t sxw, int B, int H, int W, void* A, const float* mix,
-                                   cvb_stream_t stream) {
+extern "C" int cvb_stem_im2col(const float* X, int64_t sxn, int64_t sxc, int64_t sxh, int64_t sxw, int B, int H, int W, void* A, const float* mix,
+                               cvb_stream_t stream) {
   CVB_CHECK(X && A && B > 0 && H > 0 && W > 0 && H % 2 == 0 && W % 2 == 0, "cvb_stem_im2col: bad arguments (H, W must be even)");
   int64_t total = (int64_t)B * (H / 2) * (W / 2) * 4;
   CVB_CUDA(cvb_launch(stem_im2col_kernel, grid_for(total), NT, 0, static_cast<cudaStream_t>(stream), X, sxn, sxc, sxh, sxw, B, H, W, static_cast<bf16*>(A),
                       mix));
   CVB_LAUNCH_CHECK();
   return 0;
-}
-
-extern "C" int cvb_stem_im2col(const float* X, int64_t sxn, int64_t sxc, int64_t sxh, int64_t sxw, int B, int H, int W, void* A, cvb_stream_t stream) {
-  return cvb_stem_im2col_mix(X, sxn, sxc, sxh, sxw, B, H, W, A, nullptr, stream);
 }
 
 extern "C" int cvb_prep_weights(const cvb_prep_desc* descs_device, int n_desc, int max_elems, cvb_stream_t stream) {

@@ -1305,7 +1305,7 @@ class TransformerEncoderFn(torch.autograd.Function):
         # wide layers (ViT / CLIP: K = 768 under 18-24 N tiles): the LayerNorm prologue is applied ONCE by a pre-pass (ops.WIDE_K / WIDE_N policy, which
         # pw_gemm would apply internally) and the normalised tokens are KEPT for the weight gradient of the same projection, which would otherwise
         # re-normalise them (one extra pass over the tokens per weight-gradient block)
-        keep_n = ops.KEEP_NORMALISED and C >= ops.WIDE_K and 3 * C >= ops.WIDE_N_WGRAD and ffn >= ops.WIDE_N_WGRAD
+        keep_n = C >= ops.WIDE_K and 3 * C >= ops.WIDE_N_WGRAD and ffn >= ops.WIDE_N_WGRAD
         xn1 = xn2 = None
         if keep_n:
             xn1 = ops.apply_load_mode(x2, A_GN, C, a_p=(g1, b1), row_stats=(ln1[0], ln1[1]), rows_per_sample=1)

@@ -7,7 +7,6 @@ every wrapper launches on ``torch.cuda.current_stream()`` and never synchronises
 from __future__ import annotations
 
 import ctypes
-import os
 from typing import Optional, Sequence, Tuple
 
 import torch
@@ -37,8 +36,9 @@ def _lib():
 # Weight-gradient GEMMs are off the critical path of the backward pass (their results are only needed by the optimizer), so the
 # autograd functions issue them on a second stream: `side=True` forks from the current stream (everything enqueued so far is a
 # dependency), and `join_side()` at the end of each backward makes the current stream wait for them.  Under CUDA-graph capture this
-# becomes a parallel branch of the graph whose CTAs fill the tails of the main-branch kernels.  CVB_WGRAD_STREAM=0 disables it.
-_SIDE = {"on": os.environ.get("CVB_WGRAD_STREAM", "1") != "0", "streams": {}, "dirty": False, "held": []}
+# becomes a parallel branch of the graph whose CTAs fill the tails of the main-branch kernels.  "on" is a testing hook: the reproducibility
+# tests also run the step with every weight gradient on the current stream.
+_SIDE = {"on": True, "streams": {}, "dirty": False, "held": []}
 
 
 class _SideCtx:
@@ -102,15 +102,13 @@ def set_pdl_enabled(on: bool) -> bool:
 # --------------------------------------------------------------------------------------------------------------- GEMM
 # wide-layer policy: when the prologue would be re-applied by MANY N tiles (ViT / CLIP: K = 768 / 3072 under 18-24 N tiles) it is applied once
 # by a pre-pass instead.  With 8 transform warps the in-kernel prologue won on every MobileViTv2 layer (same-box A/B: 12.47 -> 12.23 ms per
-# step without the pre-pass), so the policy now needs N >= WIDE_N as well.  CVB_WIDE_K=100000 disables the pre-pass (diagnostics).
-WIDE_K = int(os.environ.get("CVB_WIDE_K", "384"))
-WIDE_N = int(os.environ.get("CVB_WIDE_N", "1024"))
+# step without the pre-pass), so the policy now needs N >= WIDE_N as well.
+WIDE_K = 384
+WIDE_N = 1024
 # weight gradients: every 128-row block of dW (N / 128 CTAs per K block) re-applies the prologue to the SAME activation operand inside its transform
 # warps.  For the LayerNorm-fused weight gradients of the ViT-B qkv_proj / ffn.1 (N = 2304 / 3072, 18 / 24 blocks) that repeated prologue costs
 # far more than one pre-pass -> one pre-pass, then the RAW kernel.
-WIDE_N_WGRAD = int(os.environ.get("CVB_WIDE_N_WGRAD", "1536"))
-# TransformerEncoderFn keeps the pre-pass output of its two LayerNorm-fused projections for their weight gradients (2 x [tokens, C] bf16 per layer)
-KEEP_NORMALISED = int(os.environ.get("CVB_KEEP_NORMALISED", "1")) != 0
+WIDE_N_WGRAD = 1536
 
 
 def pw_gemm(A: Tensor, W: Tensor, N: int, *, K: Optional[int] = None, a_mode: int = A_RAW, A2: Optional[Tensor] = None,
@@ -419,7 +417,7 @@ def stem_im2col(x: Tensor, mix: Optional[Tensor] = None) -> Tensor:
     assert C == 3 and x.dtype == torch.float32
     A = torch.empty((B * (H // 2) * (W // 2), 32), device=x.device, dtype=torch.bfloat16)
     sn, sc, sh, sw = x.stride()
-    lib.cvb_stem_im2col_mix(x.data_ptr(), sn, sc, sh, sw, B, H, W, A.data_ptr(), _p(mix), _stream())
+    lib.cvb_stem_im2col(x.data_ptr(), sn, sc, sh, sw, B, H, W, A.data_ptr(), _p(mix), _stream())
     _count()
     return A
 
@@ -794,16 +792,6 @@ def global_pool_bwd(DOUT: Tensor, B: int, HW: int) -> Tensor:
     lib.cvb_global_pool_bwd(DOUT.data_ptr(), B, HW, C, DX.data_ptr(), _stream())
     _count()
     return DX
-
-
-def col_sum(X: Tensor, N: Optional[int] = None, out: Optional[Tensor] = None) -> Tensor:
-    lib = _lib()
-    N = X.shape[1] if N is None else N
-    if out is None:
-        out = torch.zeros((N,), device=X.device, dtype=torch.float32)
-    lib.cvb_col_sum(X.data_ptr(), int(X.dtype == torch.float32), X.stride(0), X.shape[0], N, out.data_ptr(), _stream())
-    _count()
-    return out
 
 
 def ce_fwd(logits: Tensor, C: int, target: Tensor, ignore_index: int, smoothing: float, mix: Optional[Tensor] = None,

@@ -49,7 +49,7 @@ def na_loss(x_aug: Tensor, x: Tensor, target_mse: float, alpha: float = 100.0) -
 
 
 def mixed(x: Tensor, mix) -> Tensor:
-    """The batch mixing of cvb_stem_im2col_mix: mix = (mode, lam, x1, y1, x2, y2), partner x.roll(1, 0)."""
+    """The batch mixing of cvb_stem_im2col: mix = (mode, lam, x1, y1, x2, y2), partner x.roll(1, 0)."""
     mode, lam, x1, y1, x2, y2 = [float(v) for v in mix]
     xp = x.roll(1, 0)
     if mode == 1:

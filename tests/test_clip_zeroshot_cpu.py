@@ -1,6 +1,6 @@
 """CPU checks for CLIP zero-shot evaluation: the fp32 restatement (tests/clip_zeroshot_ref.py) reproduces the real reference's class table,
 zero-shot logits, top-k and 3-D text output (tests/golden/make_golden_clip_zeroshot.py); encoding a causal prefix equals full-length
-encoding to fp32 rounding; the library exports the zero-shot kernels at ABI 11."""
+encoding to fp32 rounding; the library exports the zero-shot kernels at ABI 12."""
 import os
 import re
 import sys
@@ -63,12 +63,12 @@ def test_causal_prefix_equals_full_length(golden_dir):
     assert _rel(exact, full) <= 1e-6
 
 
-def test_abi_11_exports_zero_shot_kernels():
+def test_abi_12_exports_zero_shot_kernels():
     import __graft_entry__ as ge
     ge.build()
     from ml_cvnets_b200 import _lib
     lib = _lib.load()
-    assert _lib.ABI_VERSION == 11 and lib.cvb_abi_version() == 11
+    assert _lib.ABI_VERSION == 12 and lib.cvb_abi_version() == 12
     hdr = open(os.path.join(REPO, "include", "cvnets_b200.h")).read()
     for name in ("cvb_zs_class_embed", "cvb_zs_logits_topk"):
         assert re.search(r"CVB_API\s+int\s+" + name + r"\s*\(", hdr), name

@@ -56,19 +56,21 @@ def test_struct_layouts_match_c_compiler(tmp_path):
     assert got == want
 
 
-def test_derived_signatures():
-    """Spot checks of the header -> ctypes mapping: int64_t, double, struct pointers, device descriptor tables, pointer arrays, const char*."""
+def test_derived_signatures_at_abi_12():
+    """Spot checks of the header -> ctypes mapping: int64_t, double, struct pointers, device descriptor tables, pointer arrays, const char*,
+    and the ABI 12 constants."""
     import ctypes
     from ml_cvnets_b200 import _lib
     sigs = _lib._PROTOTYPES
     assert sigs["cvb_stem_im2col"][1][1:5] == [ctypes.c_int64] * 4 and sigs["cvb_stem_im2col"][1][5] is ctypes.c_int
+    assert sigs["cvb_stem_im2col"][1][8:] == [ctypes.c_void_p] * 3  # A, mix (device float[6] or NULL), stream
     assert sigs["cvb_bn_finalize"][1][2] is ctypes.c_double and sigs["cvb_bn_finalize"][1][5] is ctypes.c_float
     assert sigs["cvb_na_compose"][1][3] is ctypes.POINTER(ctypes.c_void_p)
     assert sigs["cvb_na_param_grad"][1][4] is sigs["cvb_na_param_grad"][1][6] is ctypes.POINTER(ctypes.c_void_p)
     assert sigs["cvb_pw_gemm"] == (ctypes.c_int, [ctypes.POINTER(_lib.cvb_gemm_args), ctypes.c_void_p])
     assert sigs["cvb_prep_weights"][1][0] is ctypes.c_void_p  # descs_device: an address in device memory
     assert sigs["cvb_last_error"] == (ctypes.c_char_p, [])
-    assert (_lib.ABI_VERSION, _lib.A_BNB, _lib.E_LIN_BWD, _lib.ACT_SIGMOID, _lib.PREP_PATCH_T) == (11, 5, 4, 5, 5)
+    assert (_lib.ABI_VERSION, _lib.A_BNB, _lib.E_LIN_BWD, _lib.ACT_SIGMOID, _lib.PREP_PATCH_T) == (12, 5, 4, 5, 5)
 
 
 def test_header_parser_rejects_unknown_input(tmp_path):
@@ -88,6 +90,19 @@ def test_failed_status_raises_with_the_library_message():
     from ml_cvnets_b200 import _lib
     with pytest.raises(_lib.CvbError, match=r"^cvb_act_fwd failed \(rc=1\): cvb_act_fwd: bad arguments$"):
         _lib.load().cvb_act_fwd(None, None, 8, _lib.ACT_GELU, None)  # argument validation fails before any CUDA call
+
+
+def test_apply_load_mode_rejects_shapes_past_its_row_kernel():
+    """cvb_apply_load_mode runs a row-block kernel (a thread per 8 channels of a row, int row index): more than 8192 channels or 2^31 rows
+    are rejected before any CUDA call."""
+    import __graft_entry__ as ge
+    ge.build()
+    from ml_cvnets_b200 import _lib
+    lib, p = _lib.load(), 256  # p: a non-NULL address that is never dereferenced
+    with pytest.raises(_lib.CvbError, match=r"cvb_apply_load_mode: K = 8200, M = 100 "):
+        lib.cvb_apply_load_mode(p, 8200, None, 0, _lib.A_AFF, p, p, None, None, None, 0, p, 8200, 100, 8200, None)
+    with pytest.raises(_lib.CvbError, match=r"cvb_apply_load_mode: K = 64, M = 2147483648 "):
+        lib.cvb_apply_load_mode(p, 64, None, 0, _lib.A_AFF, p, p, None, None, None, 0, p, 64, 1 << 31, 64, None)
 
 
 def test_state_dict_contract_and_signatures(golden_dir):

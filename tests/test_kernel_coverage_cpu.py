@@ -53,7 +53,7 @@ def test_exemptions_are_real_exports():
     assert all(reason.strip() for reason in EXEMPT.values())
 
 
-def test_nondeterministic_exceptions_are_real_exports():
+def test_nondeterministic_list_names_only_real_exports():
     """test_reproducible_gpu.py leaves the entry points in its NONDETERMINISTIC dict out of the bitwise checks: each must be an export, with a reason"""
     tree = ast.parse(open(os.path.join(REPO, "tests", "test_reproducible_gpu.py")).read())
     found = [ast.literal_eval(n.value) for n in tree.body

@@ -539,7 +539,7 @@ def test_linattn_cross(ops, Mp, N, d):
 # ------------------------------------------------------------------------------------------- stem gather with batch mixing
 @pytest.mark.parametrize("B,H,W", [(1, 16, 20), (4, 16, 20), (3, 10, 14)])
 @pytest.mark.parametrize("layout", ["nchw", "channels_last"])
-def test_stem_im2col_mix(ops, lib, B, H, W, layout):
+def test_stem_im2col_with_mix(ops, lib, B, H, W, layout):
     x = rnd(B, 3, H, W, seed=621)
     if layout == "channels_last":
         x = x.contiguous(memory_format=torch.channels_last)
@@ -549,11 +549,11 @@ def test_stem_im2col_mix(ops, lib, B, H, W, layout):
         u = F.unfold(img, kernel_size=3, stride=2, padding=1)
         return u.permute(0, 2, 1).reshape(-1, 27)
 
-    # the plain entry point equals the mixing one with mix = NULL, and with mode 0
+    # mix = NULL, through the wrapper and directly, equals mode 0
     plain = ops.stem_im2col(x)
     A0 = torch.empty_like(plain)
     sn, sc, sh, sw = x.stride()
-    lib.cvb_stem_im2col(x.data_ptr(), sn, sc, sh, sw, B, H, W, A0.data_ptr(), _stream())
+    lib.cvb_stem_im2col(x.data_ptr(), sn, sc, sh, sw, B, H, W, A0.data_ptr(), None, _stream())
     same(A0, plain, "cvb_stem_im2col")
     same(ops.stem_im2col(x, torch.tensor([0.0, 0.3, 1, 1, 5, 5], device="cuda")), plain, "mode 0")
     # mixup: fp32 blend, then one bf16 rounding

@@ -527,16 +527,13 @@ def test_linattn(ops, B, H, W, d):
     close(db[:2 * d], DQKV[:, :2 * d].float().sum(0), rtol=2e-3, atol=2e-3 * float(db.abs().max()) + 1e-5, what="dbias")
 
 
-def test_pool_colsum_im2col_prep(ops):
+def test_pool_im2col_prep(ops):
     B, HW, C = 5, 64, 96
     X = bf(rnd(B * HW, C, seed=101))
     p = ops.global_pool_fwd(X, B, HW)
     close(p, X.float().view(B, HW, C).mean(1), what="pool fwd")
     dx = ops.global_pool_bwd(p, B, HW)
     close(dx, (p.float() / HW)[:, None, :].expand(B, HW, C).reshape(-1, C), what="pool bwd")
-    close(ops.col_sum(X), X.float().sum(0), rtol=2e-3, atol=1e-2, what="col_sum bf16")
-    Xf = rnd(77, 1000, seed=102)
-    close(ops.col_sum(Xf), Xf.sum(0), rtol=1e-4, atol=1e-4, what="col_sum fp32")
     # stem im2col, NCHW and channels_last images
     img = rnd(2, 3, 16, 20, seed=103)
     for im in (img, img.contiguous(memory_format=torch.channels_last)):

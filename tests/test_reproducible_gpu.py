@@ -36,7 +36,6 @@ NONDETERMINISTIC = {
     "cvb_mha_bwd": "the register-resident (S <= 256) attention backward sums dQ with shared-memory float atomics",
     "cvb_embedding_bwd": "token-embedding gradients add repeated token ids with fp32 atomics",
     "cvb_ce_bwd": "the CLIP logit-scale gradient dlogit_scale is an fp32 atomic sum over rows (dlogits themselves have one writer)",
-    "cvb_col_sum": "fp32 atomic column sums; no training step calls it",
 }
 
 

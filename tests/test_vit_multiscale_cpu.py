@@ -1,6 +1,6 @@
 """CPU checks for multi-scale ViT training: the oracle's ViT with interpolated positional embeddings (tests/vit_multiscale_ref.py) reproduces the
 real reference at the sampler's crops (tests/golden/make_golden_vit_multiscale.py), and the library exports the interpolating token kernels
-at ABI 11."""
+at ABI 12."""
 import os
 import re
 import sys
@@ -48,12 +48,12 @@ def test_positional_table_is_resized_only_when_needed():
         assert torch.equal(vit_pos_embed(pe, n), F.interpolate(pe, size=(n, 8), mode="bilinear").reshape(1, n, 8))
 
 
-def test_abi_11_exports_interpolating_token_kernels():
+def test_abi_12_exports_interpolating_token_kernels():
     import __graft_entry__ as ge
     ge.build()
     from ml_cvnets_b200 import _lib
     lib = _lib.load()
-    assert _lib.ABI_VERSION == 11 and lib.cvb_abi_version() == 11
+    assert _lib.ABI_VERSION == 12 and lib.cvb_abi_version() == 12
     hdr = open(os.path.join(REPO, "include", "cvnets_b200.h")).read()
     for name in ("cvb_vit_tokens_interp_fwd", "cvb_vit_tokens_interp_bwd"):
         assert re.search(r"CVB_API\s+int\s+" + name + r"\s*\(", hdr), name
