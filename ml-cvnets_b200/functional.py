@@ -69,7 +69,22 @@ class LazyBN:
 
 
 def _lazy_modes(lz):
+    """(load mode, input-gradient epilogue, their parameters) of a module input: the producer's BatchNorm (+SiLU) when it is lazy, else raw."""
+    if lz is None:
+        return A_RAW, E_STORE, (None, None)
     return (A_AFF_SILU if lz.act else A_AFF), (E_SILU_BWD if lz.act else ops.E_LIN_BWD), (lz.bn[2], lz.bn[3])
+
+
+def _bn_out_grad(lz_out, D, dout, y, bn, act):
+    """(dz, sums) of a module output y -> BatchNorm [-> SiLU if ``act``] given its gradient ``dout``: dz is the gradient w.r.t. the BatchNorm
+    output and sums the BatchNorm-backward sums (sum dz, sum dz*y).  A lazy output's consumer already took dout through the activation and
+    wrote the sums."""
+    if lz_out is not None:
+        assert lz_out.stats is not None, "lazy module output was consumed by a module that does not know the protocol"
+        return dout, lz_out.stats
+    sums = D.ar.f64(2, y.shape[1])
+    dz = ops.bn_bwd_reduce(dout, y, sums, bn, act=act, store_dz=act)
+    return (dz if act else dout), sums
 
 
 def _ws_of(cfg, params):
@@ -116,15 +131,23 @@ class _Dst:
         self.grads[i] = v.view(self.params[i].shape)
         return v
 
-    def pair(self, i: int, j: int):
-        """(dgamma, dbeta) destinations for bn_bwd_finalize, or None (it allocates)."""
-        if self.ws is not None:
-            return (self.ws.gview(self.params[i]), self.ws.gview(self.params[j]))
-        return None
+    def padded(self, i: int, rows: int, cols: int, npad: int) -> torch.Tensor:
+        """zeroed fp32 [npad, cols] accumulator whose first ``rows`` rows are the gradient of params[i] ([rows, cols]; the kernel writes
+        ``npad`` >= ``rows`` rows).  Padded rows only outside workspace mode: the scratch is sliced, not copied, into the gradient."""
+        if npad == rows:
+            return self.mat(i, rows, cols)
+        assert self.ws is None, "padded gradient rows cannot be written into the flat gradient buffer"
+        v = self.ar.f32(npad, cols)
+        self.grads[i] = v[:rows].view(self.params[i].shape)
+        return v
 
-    def set_pair(self, i: int, j: int, dgb):
+    def bn_bwd(self, stats, count, gamma, bn, eval_mode: bool, i: int, j: int) -> torch.Tensor:
+        """BatchNorm-backward finalize: writes (dgamma, dbeta) as the gradients of params i, j and returns the input-gradient coefficients."""
+        out = (self.ws.gview(self.params[i]), self.ws.gview(self.params[j])) if self.ws is not None else None
+        dgb, coef = ops.bn_bwd_finalize(stats, count, gamma, bn, eval_mode=eval_mode, out=out)
         if self.ws is None:
             self.grads[i], self.grads[j] = dgb[0], dgb[1]
+        return coef
 
     def unprep(self, i: int, src, rows: int, cols: int, lds: int, kind: int, rot: int = 0, side: bool = False):
         """kernel-layout gradient (rotated / padded / tap-major) -> the parameter's own layout."""
@@ -186,14 +209,8 @@ class StemFn(torch.autograd.Function):
         (gamma,) = ctx.saved_tensors
         g2 = as_2d(to_bf16_cl(gout))
         D = _Dst(cfg, ctx.plist, g2.device, True)
-        if ctx.lz_out is not None:  # the consumer already went through the activation and took the BatchNorm-backward sums
-            assert ctx.lz_out.stats is not None, "lazy module output was consumed by a module that does not know the protocol"
-            dz, sd = g2, ctx.lz_out.stats
-        else:
-            sd = D.ar.f64(2, C0)
-            dz = ops.bn_bwd_reduce(g2, y, sd, bn, act=True, store_dz=True)
-        dgb, coef = ops.bn_bwd_finalize(sd, M, gamma, bn, eval_mode=ctx.ev[0], out=D.pair(1, 2))
-        D.set_pair(1, 2, dgb)
+        dz, sd = _bn_out_grad(ctx.lz_out, D, g2, y, bn, True)
+        coef = D.bn_bwd(sd, M, gamma, bn, ctx.ev[0], 1, 2)
         dW = ops.pw_wgrad_side(dz, A0, C0, 32, g_mode=A_BNB, G2=y, g_p=coef, dW=D.ar.f32(C0, 32))
         D.unprep(0, dW, C0, 27, 32, PW.KIND_ROWMAJOR, side=True)
         # the image's gradient exists only when something upstream learns (the RangeAugment sampler parameters)
@@ -294,12 +311,9 @@ class InvertedResidualFn(torch.autograd.Function):
         st1, st2, st3 = fa.f64(2, hid), fa.f64(2, hid), fa.f64(2, cout)
         bs = [c.batch_stats for c in cfg.bn]  # per layer: individual BatchNorms may be frozen (base_model.py:139-165)
         lz = ctx.lz_in = cfg.lazy_in
-        if lz is not None:
-            assert not cfg.residual, "a lazily normalised input cannot also be the residual"
-            am, _, ap = _lazy_modes(lz)
-            y1 = ops.pw_gemm(x2, P.get(cfg.i_w1), hid, a_mode=am, a_p=ap, col_stats=st1 if bs[0] else None)
-        else:
-            y1 = ops.pw_gemm(x2, P.get(cfg.i_w1), hid, col_stats=st1 if bs[0] else None)
+        assert lz is None or not cfg.residual, "a lazily normalised input cannot also be the residual"
+        am, _, ap = _lazy_modes(lz)
+        y1 = ops.pw_gemm(x2, P.get(cfg.i_w1), hid, a_mode=am, a_p=ap, col_stats=st1 if bs[0] else None)
         bn1 = _bn_forward(st1, M, g1, b1, cfg.bn[0])
         y2 = ops.dw_fwd(y1, B, H, W, hid, s, P.get(cfg.i_wd), x_mode=A_AFF_SILU, x_p=(bn1[2], bn1[3]), col_stats=st2 if bs[1] else None,
                         dilation=cfg.dilation)
@@ -329,36 +343,27 @@ class InvertedResidualFn(torch.autograd.Function):
         # parameter order: (w1, g1, b1, wd, g2, b2, w3, g3, b3)
         D = _Dst(cfg, ctx.plist, dout.device, True)
         ar = D.ar
-        sd3, sd2, sd1 = ar.f64(2, cout), ar.f64(2, hid), ar.f64(2, hid)
         # red_1x1 + BN3 (no activation): dz3 = dout
-        if ctx.lz_out is not None:
-            assert ctx.lz_out.stats is not None, "lazy module output was consumed by a module that does not know the protocol"
-            sd3 = ctx.lz_out.stats
-        else:
-            ops.bn_bwd_reduce(dout, y3, sd3)
-        dgb3, c3 = ops.bn_bwd_finalize(sd3, M2, g3, bn3, ev[2], out=D.pair(7, 8))
-        D.set_pair(7, 8, dgb3)
+        _, sd3 = _bn_out_grad(ctx.lz_out, D, dout, y3, bn3, False)
+        sd2, sd1 = ar.f64(2, hid), ar.f64(2, hid)
+        c3 = D.bn_bwd(sd3, M2, g3, bn3, ev[2], 7, 8)
         dz2 = ops.pw_gemm(dout, P.get(cfg.i_w3t), hid, K=cout, a_mode=A_BNB, A2=y3, a_p=c3, e_mode=E_SILU_BWD, Y=y2,
                           e_p=(bn2[2], bn2[3]), col_stats=sd2)
         ops.pw_wgrad_side(dout, y2, cout, hid, g_mode=A_BNB, G2=y3, g_p=c3, a_mode=A_AFF_SILU, a_p=(bn2[2], bn2[3]), dW=D.mat(6, cout, hid))
         # depthwise + BN2
-        dgb2, c2 = ops.bn_bwd_finalize(sd2, M2, g2, bn2, ev[1], out=D.pair(4, 5))
-        D.set_pair(4, 5, dgb2)
+        c2 = D.bn_bwd(sd2, M2, g2, bn2, ev[1], 4, 5)
         dz1, dWt = ops.dw_bwd(dz2, y1, B, H, W, hid, s, P.get(cfg.i_wd), g_mode=A_BNB, Y2=y2, g_p=c2, x_mode=A_AFF_SILU,
                               x_p=(bn1[2], bn1[3]), col_stats=sd1, dWt=ar.f32(9, hid), dilation=cfg.dilation)
         D.unprep(3, dWt, hid, 9, hid, PW.KIND_TAPMAJOR_F32)
         # exp_1x1 + BN1
-        dgb1, c1 = ops.bn_bwd_finalize(sd1, M, g1, bn1, ev[0], out=D.pair(1, 2))
-        D.set_pair(1, 2, dgb1)
+        c1 = D.bn_bwd(sd1, M, g1, bn1, ev[0], 1, 2)
         lz = ctx.lz_in
+        am, em, ap = _lazy_modes(lz)
         if lz is not None:  # the producer's BatchNorm (+SiLU) lives in this module's load mode: emit dz and its BN-backward sums for it
-            am, em, ap = _lazy_modes(lz)
             lz.stats = ar.f64(2, Cin)
-            dx = ops.pw_gemm(dz1, P.get(cfg.i_w1t), Cin, K=hid, a_mode=A_BNB, A2=y1, a_p=c1, e_mode=em, Y=x2, e_p=ap, col_stats=lz.stats)
-            ops.pw_wgrad_side(dz1, x2, hid, Cin, g_mode=A_BNB, G2=y1, g_p=c1, a_mode=am, a_p=ap, dW=D.mat(0, hid, Cin))
-        else:
-            dx = ops.pw_gemm(dz1, P.get(cfg.i_w1t), Cin, K=hid, a_mode=A_BNB, A2=y1, a_p=c1, R=dout if cfg.residual else None)
-            ops.pw_wgrad_side(dz1, x2, hid, Cin, g_mode=A_BNB, G2=y1, g_p=c1, dW=D.mat(0, hid, Cin))
+        dx = ops.pw_gemm(dz1, P.get(cfg.i_w1t), Cin, K=hid, a_mode=A_BNB, A2=y1, a_p=c1, e_mode=em, Y=x2 if lz is not None else None, e_p=ap,
+                         R=dout if cfg.residual else None, col_stats=lz.stats if lz is not None else None)
+        ops.pw_wgrad_side(dz1, x2, hid, Cin, g_mode=A_BNB, G2=y1, g_p=c1, a_mode=am, a_p=ap, dW=D.mat(0, hid, Cin))
         ops.join_side()
         return (to_4d(dx, B, H, W), None) + D.finish()
 
@@ -385,12 +390,9 @@ class MobileViTBlockv2Fn(torch.autograd.Function):
         samp = [fa.f64(2, B) for _ in range(2 * n + 1)]
         gcount = HW * d
         # local_rep: dw3x3 + BN + SiLU -> 1x1 (C -> d)
-        lz = ctx.lz_in = cfg.lazy_in
-        if lz is not None:
-            am, _, ap = _lazy_modes(lz)
-            y0 = ops.dw_fwd(x2, B, H, W, C, 1, P.get(cfg.i_wd0), x_mode=am, x_p=ap, col_stats=st0 if bs[0] else None, dilation=cfg.dilation)
-        else:
-            y0 = ops.dw_fwd(x2, B, H, W, C, 1, P.get(cfg.i_wd0), col_stats=st0 if bs[0] else None, dilation=cfg.dilation)
+        ctx.lz_in = cfg.lazy_in
+        am, _, ap = _lazy_modes(cfg.lazy_in)
+        y0 = ops.dw_fwd(x2, B, H, W, C, 1, P.get(cfg.i_wd0), x_mode=am, x_p=ap, col_stats=st0 if bs[0] else None, dilation=cfg.dilation)
         bn0 = _bn_forward(st0, M, g0, b0, cfg.bn[0])
         X = ops.pw_gemm(y0, P.get(cfg.i_wl), d, a_mode=A_AFF_SILU, a_p=(bn0[2], bn0[3]), samp_stats=samp[0], rows_per_sample=HW)
         blocks = []
@@ -437,16 +439,11 @@ class MobileViTBlockv2Fn(torch.autograd.Function):
         dout = as_2d(to_bf16_cl(gout))
         D = _Dst(cfg, ctx.plist, dev, True)
         ar = D.ar
-        sdp, sd0 = ar.f64(2, C), ar.f64(2, C)
         # ---- conv_proj (GN -> 1x1 -> BN, no act)
         base = 4 + 12 * n
-        if ctx.lz_out is not None:
-            assert ctx.lz_out.stats is not None, "lazy module output was consumed by a module that does not know the protocol"
-            sdp = ctx.lz_out.stats
-        else:
-            ops.bn_bwd_reduce(dout, yp, sdp)
-        dgbp, cp = ops.bn_bwd_finalize(sdp, M, gp, bnp, ev[1], out=D.pair(base + 3, base + 4))
-        D.set_pair(base + 3, base + 4, dgbp)
+        _, sdp = _bn_out_grad(ctx.lz_out, D, dout, yp, bnp, False)
+        sd0 = ar.f64(2, C)
+        cp = D.bn_bwd(sdp, M, gp, bnp, ev[1], base + 3, base + 4)
         cs, ss = ar.f64(2, d), ar.f64(2, B)
         g = ops.pw_gemm(dout, P.get(cfg.i_wpt), d, K=C, a_mode=A_BNB, A2=yp, a_p=cp, e_mode=E_GN_BWD, Y=XL, e_p=(gL, None),
                         row_stats=(gnL[0], gnL[1]), rows_per_sample=HW, col_stats=cs, samp_stats=ss, gn_ws=ar.f64(2, B, d))
@@ -493,17 +490,13 @@ class MobileViTBlockv2Fn(torch.autograd.Function):
         # ---- local_rep: 1x1 (no bias / norm) <- SiLU <- BN0 <- dw3x3
         ops.pw_wgrad_side(dX, y0, d, C, a_mode=A_AFF_SILU, a_p=(bn0[2], bn0[3]), dW=D.mat(3, d, C))
         dz0 = ops.pw_gemm(dX, P.get(cfg.i_wlt), C, K=d, e_mode=E_SILU_BWD, Y=y0, e_p=(bn0[2], bn0[3]), col_stats=sd0)
-        dgb0, c0 = ops.bn_bwd_finalize(sd0, M, g0, bn0, ev[0], out=D.pair(1, 2))
-        D.set_pair(1, 2, dgb0)
+        c0 = D.bn_bwd(sd0, M, g0, bn0, ev[0], 1, 2)
         lz = ctx.lz_in
+        am, _, ap = _lazy_modes(lz)
         if lz is not None:
-            am, _, ap = _lazy_modes(lz)
             lz.stats = ar.f64(2, C)
-            dx, dWt = ops.dw_bwd(dz0, x2, B, H, W, C, 1, P.get(cfg.i_wd0), g_mode=A_BNB, Y2=y0, g_p=c0, x_mode=am, x_p=ap, col_stats=lz.stats,
-                                 dWt=ar.f32(9, C), dilation=cfg.dilation)
-        else:
-            dx, dWt = ops.dw_bwd(dz0, x2, B, H, W, C, 1, P.get(cfg.i_wd0), g_mode=A_BNB, Y2=y0, g_p=c0, x_mode=A_RAW, dWt=ar.f32(9, C),
-                                 dilation=cfg.dilation)
+        dx, dWt = ops.dw_bwd(dz0, x2, B, H, W, C, 1, P.get(cfg.i_wd0), g_mode=A_BNB, Y2=y0, g_p=c0, x_mode=am, x_p=ap,
+                             col_stats=lz.stats if lz is not None else None, dWt=ar.f32(9, C), dilation=cfg.dilation)
         D.unprep(0, dWt, C, 9, C, PW.KIND_TAPMAJOR_F32)
         ops.join_side()
         return (to_4d(dx, B, H, W), None) + D.finish()
@@ -538,13 +531,7 @@ class PoolLinearFn(torch.autograd.Function):
             g = torch.zeros((B, npad), device=pooled.device, dtype=BF16)
             g[:, :ncls] = gout
         D = _Dst(cfg, ctx.plist, pooled.device, npad == ncls)
-        if npad == ncls:
-            dW, db = D.mat(0, npad, C), D.mat(1, 1, npad).view(npad)
-            ops.pw_wgrad_side(g, pooled, npad, C, dW=dW, dbias=db)
-        else:
-            dW, db = D.ar.f32(npad, C), D.ar.f32(npad)
-            ops.pw_wgrad_side(g, pooled, npad, C, dW=dW, dbias=db)
-            D.grads[0], D.grads[1] = dW[:ncls], db[:ncls]
+        ops.pw_wgrad_side(g, pooled, npad, C, dW=D.padded(0, ncls, C, npad), dbias=D.padded(1, ncls, 1, npad).view(npad))
         dp = ops.pw_gemm(g, cfg.prep.get(cfg.i_wt), C, K=npad)
         dx = ops.global_pool_bwd(dp, B, H * W)
         ops.join_side()
@@ -650,16 +637,11 @@ class PointwiseConvFn(torch.autograd.Function):
         if cfg.bn is not None:
             _, y, bn, ob = ctx.saved
             (gamma,) = ctx.saved_tensors
-            sd = D.ar.f64(2, cout)
             if ob is not None:
                 dout = ops.act_bwd(dout, ob, cfg.act)
-            act = cfg.act == ops.ACT_SILU
-            dz = ops.bn_bwd_reduce(dout, y, sd, bn, act=act, store_dz=act)
-            if not act:
-                dz = dout
-            gi, bi = (2, 3) if has_bias else (1, 2)
-            dgb, c = ops.bn_bwd_finalize(sd, M, gamma, bn, ctx.ev[0], out=D.pair(gi, bi))
-            D.set_pair(gi, bi, dgb)
+            dz, sd = _bn_out_grad(None, D, dout, y, bn, cfg.act == ops.ACT_SILU)
+            gi = 2 if has_bias else 1  # (gamma, beta) follow (w[, bias]) in plist
+            c = D.bn_bwd(sd, M, gamma, bn, ctx.ev[0], gi, gi + 1)
             if patch_stem:
                 dx = ops.patch_stem_dgrad(dz, y, c, P.get(cfg.i_w), B, Ho, Wo)
             elif need_dx:
@@ -720,13 +702,8 @@ class DepthwiseConvFn(torch.autograd.Function):
         if cfg.bn is not None:
             x2, y, bn = ctx.saved
             (gamma,) = ctx.saved_tensors
-            act = cfg.act is not None
-            sd = D.ar.f64(2, C)
-            dz = ops.bn_bwd_reduce(dout, y, sd, bn, act=act, store_dz=act)
-            if not act:
-                dz = dout
-            dgb, c = ops.bn_bwd_finalize(sd, M2, gamma, bn, ctx.ev[0], out=D.pair(1, 2))
-            D.set_pair(1, 2, dgb)
+            dz, sd = _bn_out_grad(None, D, dout, y, bn, cfg.act is not None)
+            c = D.bn_bwd(sd, M2, gamma, bn, ctx.ev[0], 1, 2)
             dx, dWt = ops.dw_bwd(dz, x2, B, H, W, C, cfg.stride, cfg.prep.get(cfg.i_w), g_mode=A_BNB, Y2=y, g_p=c, dWt=D.ar.f32(taps, C),
                                  dilation=cfg.dilation, ksize=cfg.k)
         else:
@@ -779,9 +756,7 @@ class LayerNormFn(torch.autograd.Function):
     def forward(ctx, x, cfg, gamma, beta):
         shape = x.shape
         C = shape[-1]
-        x2 = x.reshape(-1, C)
-        if x2.dtype != BF16 or not x2.is_contiguous():
-            x2 = x2.to(BF16).contiguous()
+        x2 = x.reshape(-1, C).to(BF16).contiguous()
         ln = ops.ln_stats(x2, cfg.eps)
         out = ops.apply_load_mode(x2, ops.A_GN, C, a_p=(gamma, beta, None), row_stats=(ln[0], ln[1]), rows_per_sample=1)
         ctx.cfg, ctx.shape, ctx.saved, ctx.plist = cfg, shape, (x2, ln), cfg.plist
@@ -794,9 +769,7 @@ class LayerNormFn(torch.autograd.Function):
         C = ctx.shape[-1]
         x2, ln = ctx.saved
         (gamma,) = ctx.saved_tensors
-        dy = gout.reshape(-1, C)
-        if dy.dtype != BF16 or not dy.is_contiguous():
-            dy = dy.to(BF16).contiguous()
+        dy = gout.reshape(-1, C).to(BF16).contiguous()
         D = _Dst(cfg, ctx.plist, dy.device, True)
         cs = D.ar.f64(2, C)
         dx = ops.ln_bwd(dy, x2, ln, gamma, cs)
@@ -869,9 +842,7 @@ class LinearFn(torch.autograd.Function):
     def forward(ctx, x, cfg, w, b):
         shape = x.shape
         cin, cout, npad = shape[-1], cfg.cout, cfg.npad
-        x2 = x.reshape(-1, cin)
-        if x2.dtype != BF16 or not x2.is_contiguous():
-            x2 = x2.to(BF16).contiguous()
+        x2 = x.reshape(-1, cin).to(BF16).contiguous()
         y = ops.pw_gemm(x2, cfg.prep.get(cfg.i_w), npad, bias=cfg.prep.get(cfg.i_b) if b is not None else None)
         ctx.cfg, ctx.shape, ctx.saved, ctx.plist = cfg, shape, (x2,), cfg.plist
         return y[:, :cout].view(*shape[:-1], cout)
@@ -887,18 +858,11 @@ class LinearFn(torch.autograd.Function):
             gp = torch.zeros((M, npad), device=g.device, dtype=BF16)
             gp[:, :cout] = g
             g = gp
-        elif g.dtype != BF16 or not g.is_contiguous():
+        else:
             g = g.to(BF16).contiguous()
         has_b = len(ctx.plist) > 1
         D = _Dst(cfg, ctx.plist, g.device, npad == cout)
-        if npad == cout:
-            ops.pw_wgrad_side(g, x2, npad, cin, dW=D.mat(0, npad, cin), dbias=D.mat(1, 1, npad).view(npad) if has_b else None)
-        else:
-            dW, db = D.ar.f32(npad, cin), D.ar.f32(npad)
-            ops.pw_wgrad_side(g, x2, npad, cin, dW=dW, dbias=db if has_b else None)
-            D.grads[0] = dW[:cout]
-            if has_b:
-                D.grads[1] = db[:cout]
+        ops.pw_wgrad_side(g, x2, npad, cin, dW=D.padded(0, cout, cin, npad), dbias=D.padded(1, cout, 1, npad).view(npad) if has_b else None)
         dx = ops.pw_gemm(g, cfg.prep.get(cfg.i_wt), cin, K=npad)
         ops.join_side()
         grads = D.finish()
@@ -918,9 +882,7 @@ class GlobalPoolFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, gout):
         B, C, H, W = ctx.dims
-        g = gout.reshape(B, C)
-        if g.dtype != BF16 or not g.is_contiguous():
-            g = g.to(BF16).contiguous()
+        g = gout.reshape(B, C).to(BF16).contiguous()
         return to_4d(ops.global_pool_bwd(g, B, H * W), B, H, W), None
 
 
@@ -951,18 +913,14 @@ class DropoutFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x, p):
-        x2 = x.reshape(-1, x.shape[-1])
-        if x2.dtype != BF16 or not x2.is_contiguous():
-            x2 = x2.to(BF16).contiguous()
+        x2 = x.reshape(-1, x.shape[-1]).to(BF16).contiguous()
         key = ops.rng_next(x.device)
         ctx.p, ctx.key, ctx.shape = p, key, x.shape
         return ops.dropout_fwd(x2, None, p, key).view(x.shape)
 
     @staticmethod
     def backward(ctx, gout):
-        g = gout.reshape(-1, ctx.shape[-1])
-        if g.dtype != BF16 or not g.is_contiguous():
-            g = g.to(BF16).contiguous()
+        g = gout.reshape(-1, ctx.shape[-1]).to(BF16).contiguous()
         return ops.dropout_bwd(g, ctx.p, ctx.key).view(ctx.shape), None
 
 
@@ -990,9 +948,7 @@ class SeScaleFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, s):
         B, C, H, W = x.shape
-        s2 = s.reshape(B, C)
-        if s2.dtype != BF16 or not s2.is_contiguous():
-            s2 = s2.to(BF16).contiguous()
+        s2 = s.reshape(B, C).to(BF16).contiguous()
         x2 = as_2d(x)
         ctx.saved, ctx.dims = (x2, s2), (B, C, H, W)
         return to_4d(ops.se_scale_fwd(x2, s2, B, H * W), B, H, W)
@@ -1019,9 +975,7 @@ class UnfoldFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g):
         B, C, H, W, ph, pw = ctx.dims
-        g2 = g.reshape(-1, C)
-        if g2.dtype != BF16 or not g2.is_contiguous():
-            g2 = g2.to(BF16).contiguous()
+        g2 = g.reshape(-1, C).to(BF16).contiguous()
         return to_4d(ops.patch_permute(g2, B, H, W, ph, pw, True), B, H, W), None, None
 
 
@@ -1031,9 +985,7 @@ class FoldFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, t, B, H, W, ph, pw):
         C = t.shape[-1]
-        t2 = t.reshape(-1, C)
-        if t2.dtype != BF16 or not t2.is_contiguous():
-            t2 = t2.to(BF16).contiguous()
+        t2 = t.reshape(-1, C).to(BF16).contiguous()
         ctx.dims = (B, C, H, W, ph, pw, tuple(t.shape))
         return to_4d(ops.patch_permute(t2, B, H, W, ph, pw, True), B, H, W)
 
@@ -1078,7 +1030,7 @@ class VitTokensFn(torch.autograd.Function):
     def backward(ctx, gout):
         B, C, nh, nw, n_pos = ctx.dims
         N = nh * nw
-        g = gout if (gout.dtype == BF16 and gout.is_contiguous()) else gout.to(BF16).contiguous()
+        g = gout.to(BF16).contiguous()
         D = _Dst(ctx.cfg, ctx.plist, g.device, True)
         dpos = D.mat(0, n_pos, C)
         dcls = D.mat(1, 1, C).view(C) if ctx.has_cls else None
@@ -1103,7 +1055,7 @@ class EmbeddingFn(torch.autograd.Function):
     def backward(ctx, g):
         V, C = ctx.shape
         B, S = ctx.tokens.shape
-        g = g if (g.dtype == BF16 and g.is_contiguous()) else g.to(BF16).contiguous()
+        g = g.to(BF16).contiguous()
         D = _Dst(ctx.cfg, ctx.plist, g.device, True)
         dtable = D.mat(0, V, C)
         dpos = D.mat(1, S, C) if ctx.has_pos else None
@@ -1118,7 +1070,7 @@ class EotGatherFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, tokens):
         B, S, C = x.shape
-        x = x if (x.dtype == BF16 and x.is_contiguous()) else x.to(BF16).contiguous()
+        x = x.to(BF16).contiguous()
         out, idx = ops.eot_gather_fwd(x, tokens)
         ctx.dims, ctx.idx = (B, S, C), idx
         return out
@@ -1126,7 +1078,7 @@ class EotGatherFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g):
         B, S, C = ctx.dims
-        g = g if (g.dtype == BF16 and g.is_contiguous()) else g.to(BF16).contiguous()
+        g = g.to(BF16).contiguous()
         return ops.eot_gather_bwd(g, ctx.idx, B, S, C), None
 
 
@@ -1144,7 +1096,7 @@ class ProjectionFn(torch.autograd.Function):
     def backward(ctx, g):
         din, dout = ctx.shape
         (x2,) = ctx.saved
-        g = g if (g.dtype == BF16 and g.is_contiguous()) else g.to(BF16).contiguous()
+        g = g.to(BF16).contiguous()
         D = _Dst(ctx.cfg, ctx.plist, g.device, True)
         ops.pw_wgrad_side(x2, g, din, dout, dW=D.mat(0, din, dout))
         dx = ops.pw_gemm(g, ctx.cfg.prep.get(ctx.cfg.i_p), din, K=dout)
@@ -1157,7 +1109,7 @@ class L2NormFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x):
-        x = x if (x.dtype == BF16 and x.is_contiguous()) else x.to(BF16).contiguous()
+        x = x.to(BF16).contiguous()
         y, inv = ops.l2norm_fwd(x)
         # y is also the OUTPUT: keeping that very object on ctx would close a reference cycle (output -> grad_fn -> ctx -> output) that keeps the
         # whole step's autograd graph -- and the leaf accumulators with the stream they were created on -- alive into the next step
@@ -1167,7 +1119,7 @@ class L2NormFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g):
         y, inv = ctx.saved
-        g = g if (g.dtype == BF16 and g.is_contiguous()) else g.to(BF16).contiguous()
+        g = g.to(BF16).contiguous()
         return ops.l2norm_bwd(g, y, inv)
 
 
@@ -1181,8 +1133,8 @@ class ClipLossFn(torch.autograd.Function):
     def forward(ctx, img, txt, logit_scale, cfg):
         import torch.distributed as dist
         N, d = img.shape
-        img = img if (img.dtype == BF16 and img.is_contiguous()) else img.to(BF16).contiguous()
-        txt = txt if (txt.dtype == BF16 and txt.is_contiguous()) else txt.to(BF16).contiguous()
+        img = img.to(BF16).contiguous()
+        txt = txt.to(BF16).contiguous()
         world, rank = cfg.world, cfg.rank
         if world > 1:
             I_all = torch.empty((world * N, d), device=img.device, dtype=BF16)
@@ -1306,30 +1258,21 @@ class TransformerEncoderFn(torch.autograd.Function):
         # pw_gemm would apply internally) and the normalised tokens are KEPT for the weight gradient of the same projection, which would otherwise
         # re-normalise them (one extra pass over the tokens per weight-gradient block)
         keep_n = C >= ops.WIDE_K and 3 * C >= ops.WIDE_N_WGRAD and ffn >= ops.WIDE_N_WGRAD
-        xn1 = xn2 = None
-        if keep_n:
-            xn1 = ops.apply_load_mode(x2, A_GN, C, a_p=(g1, b1), row_stats=(ln1[0], ln1[1]), rows_per_sample=1)
-            qkv = ops.pw_gemm(xn1, P.get(cfg.i_wqkv), 3 * C, bias=bqkv)
-        else:
-            qkv = ops.pw_gemm(x2, P.get(cfg.i_wqkv), 3 * C, a_mode=A_GN, a_p=(g1, b1), row_stats=(ln1[0], ln1[1]), rows_per_sample=1, bias=bqkv)
+
+        def ln_proj(X, ln, gamma, beta, weight, N, bias):
+            """(LayerNorm(X) @ weight^T + bias, the kept normalised tokens or None)."""
+            if not keep_n:
+                return ops.pw_gemm(X, weight, N, a_mode=A_GN, a_p=(gamma, beta), row_stats=(ln[0], ln[1]), rows_per_sample=1, bias=bias), None
+            xn = ops.apply_load_mode(X, A_GN, C, a_p=(gamma, beta), row_stats=(ln[0], ln[1]), rows_per_sample=1)
+            return ops.pw_gemm(xn, weight, N, bias=bias), xn
+
+        qkv, xn1 = ln_proj(x2, ln1, g1, b1, P.get(cfg.i_wqkv), 3 * C, bqkv)
         O, LSE = ops.mha_fwd(qkv, N, S, cfg.heads, cfg.head_dim, cfg.scale, amask, kpm)
         drop = getattr(cfg, "drop", None)  # (p, p_ffn, p_row) in training with dropout / stochastic depth > 0 (transformer.py:97-100, 139-156)
-        keys = None
         if drop is None:
             samp = _fwd_arena(cfg, x.device).f64(2, M)
             X1 = ops.pw_gemm(O, P.get(cfg.i_wo), C, bias=bo, R=x2, samp_stats=samp, rows_per_sample=1)
             ln2 = ops.gn_finalize(samp, C, cfg.eps)
-            if keep_n:
-                xn2 = ops.apply_load_mode(X1, A_GN, C, a_p=(g2, b2), row_stats=(ln2[0], ln2[1]), rows_per_sample=1)
-                h = ops.pw_gemm(xn2, P.get(cfg.i_w1), ffn, bias=bb1)
-            else:
-                h = ops.pw_gemm(X1, P.get(cfg.i_w1), ffn, a_mode=A_GN, a_p=(g2, b2), row_stats=(ln2[0], ln2[1]), rows_per_sample=1, bias=bb1)
-            if cfg.act == ops.ACT_SILU:
-                ha = None
-                X2 = ops.pw_gemm(h, P.get(cfg.i_w2), C, a_mode=A_SILU, bias=bb2, R=X1)
-            else:
-                ha = ops.act_fwd(h, cfg.act)
-                X2 = ops.pw_gemm(ha, P.get(cfg.i_w2), C, bias=bb2, R=X1)
         else:
             # the residual adds leave the GEMM epilogues: x + DropPath(Dropout(branch)) is one element-wise pass with hashed masks
             p, p_ffn, p_row = drop
@@ -1337,11 +1280,16 @@ class TransformerEncoderFn(torch.autograd.Function):
             A = ops.pw_gemm(O, P.get(cfg.i_wo), C, bias=bo)
             X1 = ops.dropout_fwd(A, x2, p, k1, p_row=p_row, rows_per_sample=S)
             ln2 = ops.ln_stats(X1, cfg.eps)
-            if keep_n:
-                xn2 = ops.apply_load_mode(X1, A_GN, C, a_p=(g2, b2), row_stats=(ln2[0], ln2[1]), rows_per_sample=1)
-                h = ops.pw_gemm(xn2, P.get(cfg.i_w1), ffn, bias=bb1)
+        h, xn2 = ln_proj(X1, ln2, g2, b2, P.get(cfg.i_w1), ffn, bb1)
+        keys = None
+        if drop is None:
+            if cfg.act == ops.ACT_SILU:
+                ha = None
+                X2 = ops.pw_gemm(h, P.get(cfg.i_w2), C, a_mode=A_SILU, bias=bb2, R=X1)
             else:
-                h = ops.pw_gemm(X1, P.get(cfg.i_w1), ffn, a_mode=A_GN, a_p=(g2, b2), row_stats=(ln2[0], ln2[1]), rows_per_sample=1, bias=bb1)
+                ha = ops.act_fwd(h, cfg.act)
+                X2 = ops.pw_gemm(ha, P.get(cfg.i_w2), C, bias=bb2, R=X1)
+        else:
             ha = ops.act_fwd(h, cfg.act)
             k3 = None
             if p_ffn > 0:
@@ -1370,6 +1318,13 @@ class TransformerEncoderFn(torch.autograd.Function):
         D = _Dst(cfg, ctx.plist, dev, True)
         ar = D.ar
         vec = lambda i, n: D.mat(i, 1, n).view(n)  # noqa: E731
+
+        def ln_wgrad(G, xn, X, ln, gamma, beta, N, dW, dbias):
+            """Weight gradient of the forward's ln_proj: on the kept normalised tokens, else through the LayerNorm load mode on X."""
+            if xn is not None:
+                return ops.pw_wgrad_side(G, xn, N, C, dW=dW, dbias=dbias)
+            return ops.pw_wgrad_side(G, X, N, C, a_mode=A_GN, a_p=(gamma, beta), row_stats=(ln[0], ln[1]), rows_per_sample=1, dW=dW, dbias=dbias)
+
         # ---- FFN
         db2, db1 = vec(11, C), vec(9, ffn)
         drop = ctx.drop
@@ -1389,10 +1344,7 @@ class TransformerEncoderFn(torch.autograd.Function):
             ops.pw_wgrad_side(dY, ha, C, ffn, dW=D.mat(10, C, ffn), dbias=db2)
             dh = ops.act_bwd(ops.pw_gemm(dY, P.get(cfg.i_w2t), ffn, K=C), h, cfg.act)
         xn1, xn2 = ctx.xn
-        if xn2 is not None:
-            ops.pw_wgrad_side(dh, xn2, ffn, C, dW=D.mat(8, ffn, C), dbias=db1)
-        else:
-            ops.pw_wgrad_side(dh, X1, ffn, C, a_mode=A_GN, a_p=(g2, b2), row_stats=(ln2[0], ln2[1]), rows_per_sample=1, dW=D.mat(8, ffn, C), dbias=db1)
+        ln_wgrad(dh, xn2, X1, ln2, g2, b2, ffn, D.mat(8, ffn, C), db1)
         csf = ar.f64(2, C)
         vF = ops.pw_gemm(dh, P.get(cfg.i_w1t), C, K=ffn)
         if drop is None:
@@ -1411,11 +1363,7 @@ class TransformerEncoderFn(torch.autograd.Function):
         ops.pw_wgrad_side(dA, O, C, C, dW=D.mat(4, C, C), dbias=dbo)
         dO = ops.pw_gemm(dA, P.get(cfg.i_wot), C, K=C)
         dqkv = ops.mha_bwd(qkv, O, dO, LSE, N, S, cfg.heads, cfg.head_dim, cfg.scale, amask, kpm)
-        if xn1 is not None:
-            ops.pw_wgrad_side(dqkv, xn1, 3 * C, C, dW=D.mat(2, 3 * C, C), dbias=vec(3, 3 * C))
-        else:
-            ops.pw_wgrad_side(dqkv, x2, 3 * C, C, a_mode=A_GN, a_p=(g1, b1), row_stats=(ln1[0], ln1[1]), rows_per_sample=1, dW=D.mat(2, 3 * C, C),
-                              dbias=vec(3, 3 * C))
+        ln_wgrad(dqkv, xn1, x2, ln1, g1, b1, 3 * C, D.mat(2, 3 * C, C), vec(3, 3 * C))
         csa = ar.f64(2, C)
         vA = ops.pw_gemm(dqkv, P.get(cfg.i_wqkvt), C, K=3 * C)
         dx = ops.ln_bwd(vA, x2, ln1, g1, csa, DRES=dX1)

@@ -125,7 +125,8 @@ class LayerNorm2D_NCHW(nn.GroupNorm):
         cfg = getattr(self, "_cfg", None)
         if cfg is None:  # ONE cfg object per module: its id keys the module's slice of the step workspace
             cfg = self._cfg = SimpleNamespace()
-        cfg.eps, cfg.ws, cfg.plist = float(self.eps), getattr(self, "_ws", None), [self.weight, self.bias]
+        cfg.eps = float(self.eps)
+        _bind(self, cfg, [self.weight, self.bias])
         return Fn.GroupNorm1Fn.apply(Fn.to_bf16_cl(x), cfg, self.weight, self.bias)
 
     def __repr__(self):
@@ -152,7 +153,8 @@ class LayerNorm(nn.LayerNorm):
         cfg = getattr(self, "_cfg", None)
         if cfg is None:
             cfg = self._cfg = SimpleNamespace()
-        cfg.eps, cfg.ws, cfg.plist = float(self.eps), getattr(self, "_ws", None), [self.weight, self.bias]
+        cfg.eps = float(self.eps)
+        _bind(self, cfg, [self.weight, self.bias])
         return Fn.LayerNormFn.apply(x, cfg, self.weight, self.bias)
 
 
@@ -227,6 +229,16 @@ _ACT_CLASSES = {}
 def _need_cuda(x: Tensor, who: str):
     if not x.is_cuda:
         raise RuntimeError(f"{who}: ml-cvnets_b200 runs on CUDA (sm_90a) only and has no CPU fallback; got a {x.device} tensor")
+
+
+def _bind(module: nn.Module, cfg, plist):
+    """Ready ``cfg`` for one call of its autograd function: the module's step workspace (if any), the parameters in the function's order,
+    and the kernel-layout weight copies ``cfg.prep`` (for functions that have them) refreshed."""
+    cfg.ws = getattr(module, "_ws", None)
+    cfg.plist = plist
+    if hasattr(cfg, "prep"):
+        cfg.prep.prepare(force=module.training)
+    return cfg
 
 
 def get_normalization_layer(opts, num_features: int, norm_type: Optional[str] = None, *args, **kwargs) -> nn.Module:
@@ -346,19 +358,16 @@ class ConvLayer2d(BaseLayer):
             self._stem = cfg
         cfg = self._stem
         cfg.bn = Fn.bn_cfg(norm) if norm is not None else None
-        cfg.ws = getattr(self, "_ws", None)
-        cfg.prep.prepare(force=self.training)
+        g, b = (norm.weight, norm.bias) if norm is not None else (None, None)
+        _bind(self, cfg, [conv.weight] + ([conv.bias] if conv.bias is not None else []) + ([g, b] if norm is not None else []))
         if not (pointwise and cfg.k > 1 and x.dtype == torch.float32 and self.in_channels % 8):
             x = Fn.to_bf16_cl(x)  # (fp32 images with few channels go through the gather kernel as they are)
-        g, b = (norm.weight, norm.bias) if norm is not None else (None, None)
         if pointwise:
-            cfg.plist = [conv.weight] + ([conv.bias] if conv.bias is not None else []) + ([g, b] if norm is not None else [])
             return Fn.PointwiseConvFn.apply(x, cfg, Fn.to_bf16_cl(residual) if residual is not None else None, conv.weight, conv.bias, g, b)
         if residual is not None:
             raise NotImplementedError("residual is supported for 1x1 convs only")
         if act not in (None, ops.ACT_SILU):
             raise NotImplementedError("depthwise conv followed by an activation other than Swish")
-        cfg.plist = [conv.weight] + ([g, b] if norm is not None else [])
         return Fn.DepthwiseConvFn.apply(x, cfg, conv.weight, g, b)
 
     def __repr__(self):
@@ -402,10 +411,7 @@ class LinearLayer(BaseLayer):
             if self.bias is not None:
                 cfg.i_b = prep.add(self.bias, PW.KIND_VECTOR_F32, dst_rows=npad)
             self._cfg = cfg
-        cfg = self._cfg
-        cfg.ws = getattr(self, "_ws", None)
-        cfg.plist = [self.weight] + ([self.bias] if self.bias is not None else [])
-        cfg.prep.prepare(force=self.training)
+        cfg = _bind(self, self._cfg, [self.weight] + ([self.bias] if self.bias is not None else []))
         return Fn.LinearFn.apply(x, cfg, self.weight, self.bias)
 
     def __repr__(self):
@@ -466,10 +472,8 @@ class LinearSelfAttention(BaseLayer):
                                         i_wqkvt=prep.add(wq, PW.KIND_TRANSPOSED, rot=1, ldd=2 * d + 8),
                                         i_bqkv=prep.add(bq, PW.KIND_VECTOR_F32, rot=1, dst_rows=2 * d + 8),
                                         i_wo=prep.add(wo, PW.KIND_ROWMAJOR), i_wot=prep.add(wo, PW.KIND_TRANSPOSED))
-        cfg = self._cfg
-        cfg.ws = getattr(self, "_ws", None)
-        cfg.plist = [self.qkv_proj.block.conv.weight, self.qkv_proj.block.conv.bias, self.out_proj.block.conv.weight, self.out_proj.block.conv.bias]
-        cfg.prep.prepare(force=self.training)
+        cfg = _bind(self, self._cfg, [self.qkv_proj.block.conv.weight, self.qkv_proj.block.conv.bias, self.out_proj.block.conv.weight,
+                                      self.out_proj.block.conv.bias])
         xp = Fn.to_bf16_cl(x_prev) if x_prev is not None else None
         res = Fn.to_bf16_cl(residual) if residual is not None else None
         return Fn.LinearSelfAttentionFn.apply(Fn.to_bf16_cl(x), cfg, xp, res, *cfg.plist)

@@ -14,8 +14,8 @@ import torch
 from torch import Tensor, nn
 
 from . import functional as Fn
-from .layers import ConvLayer2d, GlobalPool, Identity, LinearLayer, norm_layers_tuple
-from .modules import InvertedResidual, MobileViTBlockv2, _require_cuda, make_divisible
+from .layers import ConvLayer2d, GlobalPool, Identity, LinearLayer, _bind, _need_cuda, norm_layers_tuple
+from .modules import InvertedResidual, MobileViTBlockv2, make_divisible
 from .neural_aug import augmented_forward, build_neural_augmentor
 from .ops import PreparedWeights as PW
 
@@ -209,7 +209,7 @@ class MobileViTv2(nn.Module):
 
     # ---- feature maps for down-stream heads (base_image_encoder.py:206-276); every returned map is materialised (no lazy boundaries)
     def extract_end_points_all(self, x: Tensor, use_l5: Optional[bool] = True, use_l5_exp: Optional[bool] = False, *args, **kwargs) -> Dict[str, Tensor]:
-        _require_cuda(x, "MobileViTv2")
+        _need_cuda(x, "MobileViTv2")
         out_dict = {}
         x = self.layer_1(self.conv_1(x))
         out_dict["out_l1"] = x
@@ -239,13 +239,11 @@ class MobileViTv2(nn.Module):
                                          i_w=prep.add(lin.weight, PW.KIND_ROWMAJOR, dst_rows=npad),
                                          i_wt=prep.add(lin.weight, PW.KIND_TRANSPOSED, ldd=npad),
                                          i_b=prep.add(lin.bias, PW.KIND_VECTOR_F32, dst_rows=npad))
-        self._head.ws = getattr(self, "_ws", None)
-        self._head.plist = [lin.weight, lin.bias]
-        self._head.prep.prepare(force=self.training)
-        return Fn.PoolLinearFn.apply(Fn.to_bf16_cl(x), self._head, lin.weight, lin.bias)
+        head = _bind(self, self._head, [lin.weight, lin.bias])
+        return Fn.PoolLinearFn.apply(Fn.to_bf16_cl(x), head, lin.weight, lin.bias)
 
     def forward(self, x: Tensor, *args, **kwargs) -> Union[Tensor, Dict[str, Optional[Tensor]]]:
-        _require_cuda(x, "MobileViTv2")
+        _need_cuda(x, "MobileViTv2")
         if self.neural_augmentor is not None:
             return augmented_forward(self, x)
         return self.forward_classifier(x)

@@ -28,9 +28,9 @@ from torch import Tensor, nn
 
 from . import functional as Fn
 from . import ops
-from .layers import Dropout, get_normalization_layer
+from .layers import Dropout, _bind, _need_cuda, get_normalization_layer
 from .models_vit import PositionalEmbedding, VisionTransformer, default_vit_opts
-from .modules import TransformerEncoder, _require_cuda
+from .modules import TransformerEncoder
 from .ops import PreparedWeights as PW
 
 
@@ -71,10 +71,7 @@ class _Projection(nn.Module):
         if self._cfg is None:
             prep = PW()
             self._cfg = SimpleNamespace(prep=prep, i_p=prep.add(P, PW.KIND_ROWMAJOR), i_pt=prep.add(P, PW.KIND_TRANSPOSED))
-        cfg = self._cfg
-        cfg.ws, cfg.plist = getattr(owner, "_ws", None), [P]
-        cfg.prep.prepare(force=owner.training)
-        return Fn.ProjectionFn.apply(x, cfg, P)
+        return Fn.ProjectionFn.apply(x, _bind(owner, self._cfg, [P]), P)
 
 
 class TextTransformer(nn.Module):
@@ -136,7 +133,7 @@ class TextTransformer(nn.Module):
     def forward(self, text_tokens: Tensor, key_padding_mask: Optional[Tensor] = None, *args, **kwargs) -> Tensor:
         """transformer.py:506-551: [B, L] -> [B, d] features; [B, N, L] (several captions per image) -> [B, N, d]; [B, Cl, M, L] (zero-shot
         prompts: M captions per class, eval mode only) -> the fp32 [d, Cl] class table of ``forward_zero_shot``."""
-        _require_cuda(text_tokens, "TextTransformer")
+        _need_cuda(text_tokens, "TextTransformer")
         if text_tokens.dim() == 4:
             return self.forward_zero_shot(text_tokens, key_padding_mask)
         if text_tokens.dim() == 3:
@@ -162,8 +159,7 @@ class TextTransformer(nn.Module):
     def _tower(self, tokens: Tensor, pe: Optional[Tensor], key_padding_mask: Optional[Tensor]) -> Tensor:
         """transformer.py:354-423 up to the projection: bf16 [b, projection_dim] features of the end-of-text tokens, not yet normalised.
         ``pe`` holds the first tokens.shape[1] rows of the positional table."""
-        emb = self._emb
-        emb.ws, emb.plist = getattr(self, "_ws", None), [self.embedding_layer.weight] + ([pe] if pe is not None else [])
+        emb = _bind(self, self._emb, [self.embedding_layer.weight] + ([pe] if pe is not None else []))
         x = Fn.EmbeddingFn.apply(tokens, emb, self.embedding_layer.weight, pe)
         attn_mask = None
         if self.causal_masking:

@@ -13,8 +13,8 @@ from typing import Dict, List, Optional, Tuple, Union
 
 from torch import Tensor, nn
 
-from .layers import ConvLayer2d, Dropout, GlobalPool, LinearLayer, norm_layers_tuple
-from .modules import EfficientNetBlock, _require_cuda, make_divisible
+from .layers import ConvLayer2d, Dropout, GlobalPool, LinearLayer, _need_cuda, norm_layers_tuple
+from .modules import EfficientNetBlock, make_divisible
 from .neural_aug import augmented_forward, build_neural_augmentor
 
 # mode: (width_mult, depth_mult, train_resolution)
@@ -126,7 +126,7 @@ class EfficientNet(nn.Module):
 
     def extract_end_points_all(self, x: Tensor, use_l5: Optional[bool] = True, use_l5_exp: Optional[bool] = False, *args, **kwargs) -> Dict[str, Tensor]:
         """base_image_encoder.py:extract_end_points_all."""
-        _require_cuda(x, "EfficientNet")
+        _need_cuda(x, "EfficientNet")
         out = {}
         x = self.layer_1(self.conv_1(x))
         out["out_l1"] = x
@@ -144,7 +144,7 @@ class EfficientNet(nn.Module):
         return out
 
     def forward_classifier(self, x: Tensor, *args, **kwargs) -> Tensor:
-        _require_cuda(x, "EfficientNet")
+        _need_cuda(x, "EfficientNet")
         x = self.classifier.global_pool(self.extract_features(x))
         if hasattr(self.classifier, "classifier_dropout"):
             x = self.classifier.classifier_dropout(x)

@@ -9,8 +9,8 @@ from typing import Dict, Optional, Tuple, Union
 
 from torch import Tensor, nn
 
-from .layers import ConvLayer2d, Dropout, GlobalPool, LinearLayer, norm_layers_tuple
-from .modules import InvertedResidual, MobileViTBlock, _require_cuda
+from .layers import ConvLayer2d, Dropout, GlobalPool, LinearLayer, _need_cuda, norm_layers_tuple
+from .modules import InvertedResidual, MobileViTBlock
 from .neural_aug import augmented_forward, build_neural_augmentor
 
 
@@ -132,7 +132,7 @@ class MobileViT(nn.Module):
         return self.forward_classifier(x)
 
     def forward_classifier(self, x: Tensor, *args, **kwargs) -> Tensor:
-        _require_cuda(x, "MobileViT")
+        _need_cuda(x, "MobileViT")
         x = self.extract_features(x)
         x = self.classifier.global_pool(x)
         if hasattr(self.classifier, "dropout"):

@@ -22,8 +22,8 @@ from torch import Tensor, nn
 
 from . import functional as Fn
 from . import ops
-from .layers import ConvLayer2d, Dropout, LinearLayer, get_normalization_layer, norm_layers_tuple
-from .modules import TransformerEncoder, _require_cuda
+from .layers import ConvLayer2d, Dropout, LinearLayer, _bind, _need_cuda, get_normalization_layer, norm_layers_tuple
+from .modules import TransformerEncoder
 from .neural_aug import augmented_forward, build_neural_augmentor
 
 
@@ -152,9 +152,7 @@ class VisionTransformer(nn.Module):
         patch = self.patch_emb(x)  # [B, d, nh, nw], channels-last == token-major [B*N, d]
         n_h, n_w = patch.shape[-2:]
         pe = self.pos_embed.pos_embed.pos_embed  # resampled to n_h * n_w rows inside the token kernel when the counts differ
-        tok = self._tok
-        tok.ws = getattr(self, "_ws", None)
-        tok.plist = [pe] + ([self.cls_token] if self.cls_token is not None else [])
+        tok = _bind(self, self._tok, [pe] + ([self.cls_token] if self.cls_token is not None else []))
         # emb_dropout (vit.py: positional-embedding dropout, 0.1 in the 'tiny' config): hashed-mask kernel in training, identity otherwise
         return self.emb_dropout(Fn.VitTokensFn.apply(patch, tok, pe, self.cls_token)), (n_h, n_w)
 
@@ -168,7 +166,7 @@ class VisionTransformer(nn.Module):
         return self.post_transformer_norm(x)
 
     def forward_classifier(self, x: Tensor, *args, **kwargs) -> Tensor:
-        _require_cuda(x, "VisionTransformer")
+        _need_cuda(x, "VisionTransformer")
         return self.classifier(self.extract_features(x))
 
     def forward(self, x: Tensor, *args, **kwargs) -> Union[Tensor, Dict[str, Optional[Tensor]]]:

@@ -15,7 +15,7 @@ from torch import Tensor, nn
 
 from . import functional as Fn
 from .layers import (AdaptiveAvgPool2d, ConvLayer2d, Dropout, Identity, LinearLayer, LinearSelfAttention, MultiHeadAttention, StochasticDepth,
-                     build_activation_layer, get_normalization_layer)
+                     _bind, _need_cuda, build_activation_layer, get_normalization_layer)
 from .ops import PreparedWeights as PW
 
 
@@ -27,11 +27,6 @@ def make_divisible(v, divisor: int = 8, min_value=None):
     if new_v < 0.9 * v:
         new_v += divisor
     return new_v
-
-
-def _require_cuda(x: Tensor, who: str):
-    if not x.is_cuda:
-        raise RuntimeError(f"{who}: ml-cvnets_b200 runs on CUDA (sm_90a) only and has no CPU fallback; got a {x.device} tensor")
 
 
 class BaseModule(nn.Module):
@@ -62,17 +57,15 @@ def _lazy_in(x: Tensor):
 
 # -------------------------------------------------------------------------------------------------------------- stem
 def _stem_forward(layer: ConvLayer2d, x: Tensor) -> Tensor:
-    _require_cuda(x, "ConvLayer2d(stem)")
+    _need_cuda(x, "ConvLayer2d(stem)")
     if layer._stem is None:
         prep = PW()
         cfg = SimpleNamespace(prep=prep, i_w=prep.add(layer.block.conv.weight, PW.KIND_ROWMAJOR, ldd=32))
         layer._stem = cfg
     cfg = layer._stem
     cfg.bn = Fn.bn_cfg(layer.block.norm)
-    cfg.ws = getattr(layer, "_ws", None)
-    cfg.plist = [layer.block.conv.weight, layer.block.norm.weight, layer.block.norm.bias]
     cfg.lazy_out = _lazy_out(layer)
-    cfg.prep.prepare(force=layer.training)
+    _bind(layer, cfg, [layer.block.conv.weight, layer.block.norm.weight, layer.block.norm.bias])
     return _tag(Fn.StemFn.apply(x, cfg, *cfg.plist), cfg)
 
 
@@ -116,17 +109,15 @@ class InvertedResidual(BaseModule):
         self._cfg = cfg
 
     def forward(self, x: Tensor, *args, **kwargs) -> Tensor:
-        _require_cuda(x, "InvertedResidual")
+        _need_cuda(x, "InvertedResidual")
         if self._cfg is None:
             self._build_cfg()
         cfg, b = self._cfg, self.block
         cfg.bn = [Fn.bn_cfg(b.exp_1x1.block.norm), Fn.bn_cfg(b.conv_3x3.block.norm), Fn.bn_cfg(b.red_1x1.block.norm)]
-        cfg.ws = getattr(self, "_ws", None)
-        cfg.plist = [b.exp_1x1.block.conv.weight, b.exp_1x1.block.norm.weight, b.exp_1x1.block.norm.bias,
-                     b.conv_3x3.block.conv.weight, b.conv_3x3.block.norm.weight, b.conv_3x3.block.norm.bias,
-                     b.red_1x1.block.conv.weight, b.red_1x1.block.norm.weight, b.red_1x1.block.norm.bias]
         cfg.lazy_in, cfg.lazy_out = _lazy_in(x), _lazy_out(self) and not self.use_res_connect
-        cfg.prep.prepare(force=self.training)
+        _bind(self, cfg, [b.exp_1x1.block.conv.weight, b.exp_1x1.block.norm.weight, b.exp_1x1.block.norm.bias,
+                          b.conv_3x3.block.conv.weight, b.conv_3x3.block.norm.weight, b.conv_3x3.block.norm.bias,
+                          b.red_1x1.block.conv.weight, b.red_1x1.block.norm.weight, b.red_1x1.block.norm.bias])
         return _tag(Fn.InvertedResidualFn.apply(Fn.to_bf16_cl(x), cfg, *cfg.plist), cfg)
 
     def __repr__(self) -> str:
@@ -155,7 +146,7 @@ class SqueezeExcitation(BaseModule):
         self.in_channels, self.squeeze_factor, self.scale_fn = in_channels, squeeze_factor, scale_fn_name
 
     def forward(self, x: Tensor, *args, **kwargs) -> Tensor:
-        _require_cuda(x, "SqueezeExcitation")
+        _need_cuda(x, "SqueezeExcitation")
         x = Fn.to_bf16_cl(x)
         return Fn.SeScaleFn.apply(x, self.se_layer(x))
 
@@ -192,7 +183,7 @@ class InvertedResidualSE(BaseModule):
         self.use_res_connect = self.stride == 1 and in_channels == out_channels
 
     def forward(self, x: Tensor, *args, **kwargs) -> Tensor:
-        _require_cuda(x, "InvertedResidualSE")
+        _need_cuda(x, "InvertedResidualSE")
         x = Fn.to_bf16_cl(x)
         y = x
         for name, m in self.block._modules.items():  # (named_children() would de-duplicate the shared activation module)
@@ -223,7 +214,7 @@ class EfficientNetBlock(InvertedResidualSE):
         p = float(self.stochastic_depth.p)
         if not (self.use_res_connect and self.training and p > 0.0):
             return super().forward(x)
-        _require_cuda(x, "EfficientNetBlock")
+        _need_cuda(x, "EfficientNetBlock")
         x = Fn.to_bf16_cl(x)
         y = x
         for m in self.block._modules.values():
@@ -261,7 +252,7 @@ class LinearAttnFFN(BaseModule):
         """Stand-alone use on the unfolded tensor [B, d, P, N] (transformer.py:248-264), self- or cross-attention: the layers' own
         kernel paths composed, residual additions inside the out_proj / second FFN conv epilogues.  Inside MobileViTBlockv2 the unit runs
         in the block's fused function instead."""
-        _require_cuda(x, "LinearAttnFFN")
+        _need_cuda(x, "LinearAttnFFN")
         if self.std_dropout or self.ffn_dropout or self.attn_dropout_p:
             raise NotImplementedError("dropout > 0 is not implemented")
         norm1, attn = self.pre_norm_attn[0], self.pre_norm_attn[1]
@@ -373,7 +364,7 @@ class MobileViTBlockv2(BaseModule):
         return out
 
     def forward_spatial(self, x: Tensor, *args, **kwargs) -> Tensor:
-        _require_cuda(x, "MobileViTBlockv2")
+        _need_cuda(x, "MobileViTBlockv2")
         if x.shape[2] % self.patch_h or x.shape[3] % self.patch_w:
             raise NotImplementedError("H, W must be multiples of the patch size (the bilinear resize_input_if_needed path, "
                                       "mobilevit_block.py:595-603, never fires at 256x256 and is out of scope)")
@@ -381,10 +372,8 @@ class MobileViTBlockv2(BaseModule):
             self._build_cfg()
         cfg = self._cfg
         cfg.bn = [Fn.bn_cfg(self.local_rep[0].block.norm), Fn.bn_cfg(self.conv_proj.block.norm)]
-        cfg.ws = getattr(self, "_ws", None)
-        cfg.plist = self._params()
         cfg.lazy_in, cfg.lazy_out = _lazy_in(x), _lazy_out(self)
-        cfg.prep.prepare(force=self.training)
+        _bind(self, cfg, self._params())
         return _tag(Fn.MobileViTBlockv2Fn.apply(Fn.to_bf16_cl(x), cfg, *cfg.plist), cfg)
 
     def forward(self, x: Union[Tensor, Tuple[Tensor]], *args, **kwargs) -> Union[Tensor, Tuple[Tensor, Tensor]]:
@@ -438,7 +427,7 @@ class MobileViTBlock(BaseModule):
         self.dilation, self.n_blocks, self.conv_ksize = dilation, n_transformer_blocks, conv_ksize
 
     def forward_spatial(self, x: Tensor) -> Tensor:
-        _require_cuda(x, "MobileViTBlock")
+        _need_cuda(x, "MobileViTBlock")
         res = Fn.to_bf16_cl(x)
         fm = self.local_rep(res)
         B, _, H, W = fm.shape
@@ -517,7 +506,7 @@ class TransformerEncoder(BaseModule):
 
     def forward(self, x: Tensor, x_prev: Optional[Tensor] = None, key_padding_mask: Optional[Tensor] = None,
                 attn_mask: Optional[Tensor] = None, *args, **kwargs) -> Tensor:
-        _require_cuda(x, "TransformerEncoder")
+        _need_cuda(x, "TransformerEncoder")
         if x_prev is not None:
             raise NotImplementedError("cross-attention (x_prev) is not implemented on the GPU path")
         if self.training and self.pre_norm_mha[1].attn_dropout.p:
@@ -540,10 +529,8 @@ class TransformerEncoder(BaseModule):
         p, pf, pr = float(self.pre_norm_mha[2].p), float(self.pre_norm_ffn[3].p), float(self.stochastic_dropout)
         cfg.drop = (p, pf, pr) if (self.training and (p > 0 or pf > 0 or pr > 0)) else None
         cfg.eps = float(self.pre_norm_mha[0].eps)  # VisionTransformer.update_layer_norm_eps rewrites it after construction (vit.py:204-208)
-        cfg.prep.prepare(force=self.training)
         n1, mha, n2 = self.pre_norm_mha[0], self.pre_norm_mha[1], self.pre_norm_ffn[0]
         l1, l2 = self.pre_norm_ffn[1], self.pre_norm_ffn[4]
-        cfg.ws = getattr(self, "_ws", None)
-        cfg.plist = [n1.weight, n1.bias, mha.qkv_proj.weight, mha.qkv_proj.bias, mha.out_proj.weight, mha.out_proj.bias, n2.weight, n2.bias,
-                     l1.weight, l1.bias, l2.weight, l2.bias]
+        _bind(self, cfg, [n1.weight, n1.bias, mha.qkv_proj.weight, mha.qkv_proj.bias, mha.out_proj.weight, mha.out_proj.bias, n2.weight, n2.bias,
+                          l1.weight, l1.bias, l2.weight, l2.bias])
         return Fn.TransformerEncoderFn.apply(x.to(torch.bfloat16).contiguous(), cfg, *cfg.plist)
