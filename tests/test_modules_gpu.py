@@ -145,7 +145,13 @@ def _model_and_oracle(pkg, width, seed):
 
 @pytest.mark.parametrize("width", ["1.0", "0.5"])
 def test_model_against_reference_golden(pkg, golden_dir, width):
-    fx = torch.load(os.path.join(golden_dir, "mobilevit_v2_fp32.pt"), weights_only=False)[width]
+    check_model_against_fixture(pkg, torch.load(os.path.join(golden_dir, "mobilevit_v2_fp32.pt"), weights_only=False)[width])
+
+
+def check_model_against_fixture(pkg, fx):
+    """A train-mode forward / backward of MobileViTv2 at the fixture's width against the real reference's fp32 record, bounded by the oracle
+    run under torch bf16 autocast on this GPU."""
+    width = str(fx["width"])
     model, P = _model_and_oracle(pkg, fx["width"], fx["seed"])
     x = O.seeded_input((2, 3, fx["res"], fx["res"]), fx["x_seed"]).cuda()
     logits = model(x)

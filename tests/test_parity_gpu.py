@@ -46,9 +46,9 @@ def cosine(a, b):
     return float(torch.dot(a, b) / (a.norm() * b.norm() + 1e-30))
 
 
-def _setup(pkg, seed):
-    model = pkg.MobileViTv2(pkg.default_opts(width_multiplier=1.0))
-    P = O.seeded_fill_(O.mobilevit_v2_shapes(1.0), seed)
+def _setup(pkg, seed, width=1.0):
+    model = pkg.MobileViTv2(pkg.default_opts(width_multiplier=width))
+    P = O.seeded_fill_(O.mobilevit_v2_shapes(width), seed)
     model.load_state_dict(P, strict=True)
     return model.cuda(), P
 
@@ -63,9 +63,10 @@ def _record(name, d):
         pass
 
 
-@pytest.mark.parametrize("B", [128, 32])
-def test_benchmark_config_train_parity(pkg, B):
-    model, P = _setup(pkg, 2024)
+def train_parity_record(pkg, B, width=1.0):
+    """One train-mode forward / backward of ours, the fp32 oracle and the oracle under torch bf16 autocast on the same seeded batch:
+    the record of their distances, and the per-parameter tuples of the parameters carrying a non-negligible share of the gradient."""
+    model, P = _setup(pkg, 2024, width)
     model.train()
     x = O.seeded_input((B, 3, 256, 256), 31).cuda()
     y = (torch.arange(B, device="cuda") * 37) % 1000
@@ -79,7 +80,7 @@ def test_benchmark_config_train_parity(pkg, B):
     torch.cuda.empty_cache()
     # truth: fp32 oracle on this GPU
     P32 = O.clone_params(P, device="cuda")
-    l32 = O.mobilevit_v2_forward(P32, x, width_multiplier=1.0, training=True)
+    l32 = O.mobilevit_v2_forward(P32, x, width_multiplier=width, training=True)
     loss32 = F.cross_entropy(l32, y, label_smoothing=0.1)
     loss32.backward()
     g32 = {k: v.grad.detach().clone() for k, v in P32.items() if v.requires_grad and v.grad is not None}
@@ -90,7 +91,7 @@ def test_benchmark_config_train_parity(pkg, B):
     # same-precision comparator: the oracle under torch bf16 autocast
     Pa = O.clone_params(P, device="cuda")
     with torch.autocast("cuda", dtype=torch.bfloat16):
-        la = O.mobilevit_v2_forward(Pa, x, width_multiplier=1.0, training=True)
+        la = O.mobilevit_v2_forward(Pa, x, width_multiplier=width, training=True)
         lossa = F.cross_entropy(la, y, label_smoothing=0.1)
     lossa.backward()
     ga = {k: v.grad.detach().float().clone() for k, v in Pa.items() if v.requires_grad and v.grad is not None}
@@ -112,10 +113,20 @@ def test_benchmark_config_train_parity(pkg, B):
     worst = min(sig, key=lambda t: t[2])
     med_rel = sorted(t[4] for t in sig)[len(sig) // 2]
     med_rel_a = sorted(t[5] for t in sig)[len(sig) // 2]
-    rec = {"B": B, "logits_rel_l2": e_log, "autocast_logits_rel_l2": a_log, "north_star_1e-3_x": e_log / 1e-3, "loss": ours_loss, "loss_fp32": loss32,
+    rec = {"width": width, "B": B, "logits_rel_l2": e_log, "autocast_logits_rel_l2": a_log, "north_star_1e-3_x": e_log / 1e-3, "loss": ours_loss,
+           "loss_fp32": loss32, "loss_autocast": float(lossa),
            "grad_cosine_all": cos_all, "autocast_grad_cosine_all": cos_all_a, "grad_rel_l2_all": rel_all, "autocast_grad_rel_l2_all": rel_all_a,
            "median_param_grad_rel_l2": med_rel, "autocast_median_param_grad_rel_l2": med_rel_a,
            "worst_param": {"name": worst[0], "cosine": worst[2], "autocast_cosine": worst[3]}, "n_params": len(keys), "n_significant": len(sig)}
+    return rec, sig
+
+
+@pytest.mark.parametrize("B", [128, 32])
+def test_benchmark_config_train_parity(pkg, B):
+    rec, sig = train_parity_record(pkg, B)
+    e_log, a_log, ours_loss, loss32 = rec["logits_rel_l2"], rec["autocast_logits_rel_l2"], rec["loss"], rec["loss_fp32"]
+    cos_all, rel_all, rel_all_a = rec["grad_cosine_all"], rec["grad_rel_l2_all"], rec["autocast_grad_rel_l2_all"]
+    worst = min(sig, key=lambda t: t[2])
     print("\n[parity B=%d train] " % B + json.dumps(rec))
     _record(f"train_B{B}", rec)
     assert e_log <= 8e-2, rec
@@ -149,17 +160,16 @@ def test_benchmark_config_eval_parity(pkg):
     assert top1 >= 0.95, rec
 
 
-def test_benchmark_config_stagewise_parity(pkg):
-    """(1) of the module docstring: each module on the oracle's own stage input, batch 128 @ 256x256, train mode."""
-    B = 128
-    model, P = _setup(pkg, 2024)
+def stagewise_record(pkg, width=1.0, B=128):
+    """Each module fed the fp32 oracle's input of its stage, train mode at 256x256: rel-L2 of its output against the oracle's, per stage."""
+    model, P = _setup(pkg, 2024, width)
     model.train()
     model.fuse_boundaries = False
     x = O.seeded_input((B, 3, 256, 256), 31).cuda()
     Pg = O.clone_params(P, requires_grad=False, device="cuda")
     with torch.no_grad():
-        ref_logits, stages = O.mobilevit_v2_forward(Pg, x, width_multiplier=1.0, training=True, return_stages=True)
-        names = [pre for _, pre, _ in O.mobilevit_v2_layout(1.0)]
+        ref_logits, stages = O.mobilevit_v2_forward(Pg, x, width_multiplier=width, training=True, return_stages=True)
+        names = [pre for _, pre, _ in O.mobilevit_v2_layout(width)]
         rec, prev = {}, x
         for pre in names:
             mod = model
@@ -178,6 +188,12 @@ def test_benchmark_config_stagewise_parity(pkg):
         finally:
             model.extract_features = saved
         rec["classifier"] = rel_l2(head_out, ref_logits)
+    return rec
+
+
+def test_benchmark_config_stagewise_parity(pkg):
+    """(1) of the module docstring: each module on the oracle's own stage input, batch 128 @ 256x256, train mode."""
+    rec = stagewise_record(pkg)
     print("\n[stage-wise parity B=128 train] " + json.dumps(rec))
     _record("stagewise_B128", rec)
     for k, e in rec.items():

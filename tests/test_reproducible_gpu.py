@@ -88,13 +88,13 @@ def _state(ts, model):
     return st
 
 
-def _train(pkg, ops, xs, ys, *, pdl=True, side=True, graph=False):
+def _train(pkg, ops, xs, ys, *, pdl=True, side=True, graph=False, width=1.0):
     from test_engine_gpu import _small_model
     lr = 2e-3
     prev_pdl, prev_side = ops.set_pdl_enabled(pdl), ops._SIDE["on"]
     ops._SIDE["on"] = side
     try:
-        model = _small_model(pkg, width=1.0)
+        model = _small_model(pkg, width=width)
         # weight decay is set from the start: at lr = 0 the capture's warm-up steps leave the weights bit-for-bit unchanged (p * (1 - 0 * wd) - 0 * u)
         ts = pkg.TrainStep(model, lr=0.0 if graph else lr, weight_decay=0.05, max_norm=10.0, label_smoothing=0.1)
         if graph:
@@ -574,7 +574,8 @@ def test_linattn_bitwise(ops, H, d):
     close(db[:2 * d + 1], sums, rtol=2e-3, atol=2e-3 * float(sums.abs().max()) + 1e-5, what="dbias")
 
 
-@pytest.mark.parametrize("Mp,d", [(256, 128), (64, 192), (16, 256)])
+# d = 336 / 448 (MobileViTv2-1.75): the 8-channel groups of one row span three warps, so linattn_bwd sums three warp pieces of ds
+@pytest.mark.parametrize("Mp,d", [(256, 128), (64, 192), (16, 256), (64, 336), (16, 448)])
 def test_linattn_cross_bitwise(ops, Mp, d):
     B, P, N = 128, 4, Mp
     ld = 2 * d + 8
