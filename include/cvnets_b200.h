@@ -261,7 +261,7 @@ CVB_API int cvb_set_mha_impl(int mode);
 /* LayerNorm backward of a [M, C] token matrix in one pass (autograd of nn.LayerNorm as used at transformer.py:77-95):
  * V = gradient w.r.t. the LayerNorm OUTPUT (bf16), X = its input, mean/rstd from cvb_ln_stats or cvb_gn_finalize(count = C);
  * DX = rstd * (V*gamma - mean_c(V*gamma) - xhat * mean_c(V*gamma*xhat)) + DRES (optional residual-stream gradient);
- * dgamma[c] += sum_m V*xhat, dbeta[c] += sum_m V, col_sum[c] += sum_m DX (optional: bias gradient of the producer).  C <= 1024. */
+ * dgamma[c] += sum_m V*xhat, dbeta[c] += sum_m V, col_sum[c] += sum_m DX (optional: bias gradient of the producer).  C <= 1280. */
 CVB_API int cvb_ln_bwd(const void* V, const void* X, const float* mean, const float* rstd, const float* gamma, const void* DRES, void* DX,
                int64_t M, int C, double* dgamma, double* dbeta, double* col_sum, cvb_stream_t stream);
 /* element-wise activation passes over contiguous bf16 tensors of n elements (n % 8 == 0): Y = act(X);  DX = DY * act'(X), act = kind.

@@ -424,8 +424,10 @@ __global__ void __launch_bounds__(NT) gn_bwd_stats_kernel(const bf16* __restrict
 // LayerNorm backward in ONE pass (a "sample" is a single token row, so both phases of the GroupNorm backward fit in a warp):
 //   g = v * gamma;  dx = rstd * (g - mean_c(g) - xhat * mean_c(g * xhat)) + dres;   dbeta += v;  dgamma += v * xhat;  col_sum += dx
 // (autograd of nn.LayerNorm, cvnets/layers/normalization/layer_norm.py:14-72).  One warp per row, rows grid-strided; the per-channel
-// sums live in registers (lane owns chunks lane, lane+32, ...: C <= 1024) and are flushed once per CTA.
-constexpr int LNB_MAXCH = 4;
+// sums live in shared memory and are flushed once per CTA.  A row stays in registers: lane owns 8-channel chunks lane, lane+32, ..., MAXCH of
+// them, so C <= 256 * MAXCH.  MAXCH = 4 serves C <= 1024; MAXCH = 5 the 1280-wide ViT-H rows (the widest LayerNorm of any recipe).
+constexpr int LNB_MAXCH = 5;
+template <int MAXCH>
 __global__ void __launch_bounds__(NT) ln_bwd_kernel(const bf16* __restrict__ V, const bf16* __restrict__ X, const float* __restrict__ mean,
                                                     const float* __restrict__ rstd, const float* __restrict__ gamma, const bf16* __restrict__ DRES,
                                                     bf16* __restrict__ DX, int64_t M, int C, double* dgamma, double* dbeta, double* col_sum) {
@@ -443,11 +445,11 @@ __global__ void __launch_bounds__(NT) ln_bwd_kernel(const bf16* __restrict__ V, 
   const float invC = 1.0f / (float)C;
   for (int64_t row = (int64_t)blockIdx.x * (NT / 32) + warp; row < M; row += (int64_t)gridDim.x * (NT / 32)) {
     const float mu = mean[row], rs = rstd[row];
-    float v[LNB_MAXCH][8], xh[LNB_MAXCH][8];
-    uint4 dres[LNB_MAXCH];
+    float v[MAXCH][8], xh[MAXCH][8];
+    uint4 dres[MAXCH];
     float s1 = 0.f, s2 = 0.f;
 #pragma unroll
-    for (int q = 0; q < LNB_MAXCH; ++q) {
+    for (int q = 0; q < MAXCH; ++q) {
       const int ch = lane + 32 * q;
       if (ch < nch) {
         unpack8(ldg16_stream(V + row * C + ch * 8), v[q]);
@@ -456,7 +458,7 @@ __global__ void __launch_bounds__(NT) ln_bwd_kernel(const bf16* __restrict__ V, 
       }
     }
 #pragma unroll
-    for (int q = 0; q < LNB_MAXCH; ++q) {
+    for (int q = 0; q < MAXCH; ++q) {
       const int ch = lane + 32 * q;
       if (ch < nch) {
         float gq[8];
@@ -476,7 +478,7 @@ __global__ void __launch_bounds__(NT) ln_bwd_kernel(const bf16* __restrict__ V, 
     s1 = warp_sum(s1) * invC;
     s2 = warp_sum(s2) * invC;
 #pragma unroll
-    for (int q = 0; q < LNB_MAXCH; ++q) {
+    for (int q = 0; q < MAXCH; ++q) {
       const int ch = lane + 32 * q;
       if (ch < nch) {
         float d[8];
@@ -912,7 +914,7 @@ extern "C" int cvb_ln_bwd(const void* V, const void* X, const float* mean, const
   int64_t ctas = (M + NT / 32 - 1) / (NT / 32);
   const int64_t cap = 4 * (int64_t)cvb_num_sms();
   if (ctas > cap) ctas = cap;
-  CVB_CUDA(cvb_launch(ln_bwd_kernel, (unsigned)ctas, NT, (size_t)4 * C * sizeof(float), static_cast<cudaStream_t>(stream), static_cast<const bf16*>(V),
+  CVB_CUDA(cvb_launch(C <= 1024 ? ln_bwd_kernel<4> : ln_bwd_kernel<LNB_MAXCH>, (unsigned)ctas, NT, (size_t)4 * C * sizeof(float), static_cast<cudaStream_t>(stream), static_cast<const bf16*>(V),
                       static_cast<const bf16*>(X), mean, rstd, gamma, static_cast<const bf16*>(DRES), static_cast<bf16*>(DX), M, C, dgamma, dbeta,
                       col_sum));
   CVB_LAUNCH_CHECK();

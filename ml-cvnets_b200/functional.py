@@ -102,10 +102,11 @@ def _arena(cfg, kind: str, ws, device) -> Arena:
     return ws.arena((id(cfg), kind), rec) if ws is not None else Arena(rec, device)
 
 
-def _fwd_arena(cfg, device) -> Arena:
-    """fp64 statistics accumulators of one forward: one memset per module, or a slice of the step arena (no launch at all)."""
+def _fwd_arena(cfg, device, kind: str = "fwd") -> Arena:
+    """fp64 statistics accumulators of one forward: one memset per module, or a slice of the step arena (no launch at all).  ``kind``
+    "rfwd": a forward recomputed inside the backward, which must not reuse the slice the step's forward already carved."""
     ws = getattr(cfg, "ws", None)
-    return _arena(cfg, "fwd", ws if ws is not None and ws.active else None, device)
+    return _arena(cfg, kind, ws if ws is not None and ws.active else None, device)
 
 
 class _Dst:
@@ -1243,131 +1244,181 @@ class MultiHeadAttentionFn(torch.autograd.Function):
         return dx.view(N, S, C), None, dWq, dbq, dWo, dbo
 
 
+def _encoder_forward(x2, N, S, cfg, amask, kpm, drop, keys=None, arena="fwd"):
+    """One TransformerEncoder forward on the token matrix x2 [M = N*S, C] -> (output [M, C], what its backward needs).
+
+    ``drop``: (p, p_ffn, p_row) in training with dropout / stochastic depth > 0, else None.  ``keys``: the mask keys an earlier forward of the
+    same layer drew, to replay it bit for bit (a recompute), else new keys are drawn from the device generator.  ``arena``: the key of the
+    call's statistics scratch (a recompute inside the backward carves a slice of its own)."""
+    M, C = x2.shape
+    ffn = cfg.ffn
+    P = cfg.prep
+    ln1 = ops.ln_stats(x2, cfg.eps)
+    # wide layers (ViT / CLIP: K = 768 under 18-24 N tiles): the LayerNorm prologue is applied ONCE by a pre-pass (ops.WIDE_K / WIDE_N policy, which
+    # pw_gemm would apply internally) and the normalised tokens are KEPT for the weight gradient of the same projection, which would otherwise
+    # re-normalise them (one extra pass over the tokens per weight-gradient block)
+    keep_n = C >= ops.WIDE_K and 3 * C >= ops.WIDE_N_WGRAD and ffn >= ops.WIDE_N_WGRAD
+    g1, b1, _, bqkv, _, bo, g2, b2, _, bb1, _, bb2 = cfg.plist
+
+    def ln_proj(X, ln, gamma, beta, weight, N, bias):
+        """(LayerNorm(X) @ weight^T + bias, the kept normalised tokens or None)."""
+        if not keep_n:
+            return ops.pw_gemm(X, weight, N, a_mode=A_GN, a_p=(gamma, beta), row_stats=(ln[0], ln[1]), rows_per_sample=1, bias=bias), None
+        xn = ops.apply_load_mode(X, A_GN, C, a_p=(gamma, beta), row_stats=(ln[0], ln[1]), rows_per_sample=1)
+        return ops.pw_gemm(xn, weight, N, bias=bias), xn
+
+    qkv, xn1 = ln_proj(x2, ln1, g1, b1, P.get(cfg.i_wqkv), 3 * C, bqkv)
+    O, LSE = ops.mha_fwd(qkv, N, S, cfg.heads, cfg.head_dim, cfg.scale, amask, kpm)
+    if drop is None:
+        samp = _fwd_arena(cfg, x2.device, arena).f64(2, M)
+        X1 = ops.pw_gemm(O, P.get(cfg.i_wo), C, bias=bo, R=x2, samp_stats=samp, rows_per_sample=1)
+        ln2 = ops.gn_finalize(samp, C, cfg.eps)
+    else:
+        # the residual adds leave the GEMM epilogues: x + DropPath(Dropout(branch)) is one element-wise pass with hashed masks
+        p, p_ffn, p_row = drop
+        if keys is None:
+            keys = (ops.rng_next(x2.device), ops.rng_next(x2.device), ops.rng_next(x2.device) if p_ffn > 0 else None)
+        k1, k2, k3 = keys
+        A = ops.pw_gemm(O, P.get(cfg.i_wo), C, bias=bo)
+        X1 = ops.dropout_fwd(A, x2, p, k1, p_row=p_row, rows_per_sample=S)
+        ln2 = ops.ln_stats(X1, cfg.eps)
+    h, xn2 = ln_proj(X1, ln2, g2, b2, P.get(cfg.i_w1), ffn, bb1)
+    if drop is None:
+        if cfg.act == ops.ACT_SILU:
+            ha = None
+            X2 = ops.pw_gemm(h, P.get(cfg.i_w2), C, a_mode=A_SILU, bias=bb2, R=X1)
+        else:
+            ha = ops.act_fwd(h, cfg.act)
+            X2 = ops.pw_gemm(ha, P.get(cfg.i_w2), C, bias=bb2, R=X1)
+    else:
+        ha = ops.act_fwd(h, cfg.act)
+        if k3 is not None:
+            ha = ops.dropout_fwd(ha, None, p_ffn, k3)
+        Fo = ops.pw_gemm(ha, P.get(cfg.i_w2), C, bias=bb2)
+        X2 = ops.dropout_fwd(Fo, X1, p, k2, p_row=p_row, rows_per_sample=S)
+    return X2, SimpleNamespace(N=N, S=S, x2=x2, ln1=ln1, qkv=qkv, O=O, LSE=LSE, X1=X1, ln2=ln2, h=h, ha=ha, xn1=xn1, xn2=xn2,
+                               amask=amask, kpm=kpm, drop=drop, keys=keys)
+
+
+def _encoder_backward(st, dY, cfg, plist):
+    """Backward of one ``_encoder_forward`` (``st``: what it returned) for the output gradient dY bf16 [M, C] -> (input gradient [M, C], the
+    parameter gradients as ``_Dst.finish`` returns them).  ``plist``: the layer's parameters in TransformerEncoder._bind order."""
+    N, S = st.N, st.S
+    M, C = dY.shape
+    ffn = cfg.ffn
+    P = cfg.prep
+    x2, ln1, qkv, O, LSE, X1, ln2, h, ha, amask, kpm = st.x2, st.ln1, st.qkv, st.O, st.LSE, st.X1, st.ln2, st.h, st.ha, st.amask, st.kpm
+    g1, b1, g2, b2 = plist[0], plist[1], plist[6], plist[7]
+    dev = x2.device
+    # parameter order: (g1, b1, wqkv, bqkv, wo, bo, g2, b2, w1, bb1, w2, bb2)
+    D = _Dst(cfg, plist, dev, True)
+    ar = D.ar
+    vec = lambda i, n: D.mat(i, 1, n).view(n)  # noqa: E731
+
+    def ln_wgrad(G, xn, X, ln, gamma, beta, N, dW, dbias):
+        """Weight gradient of the forward's ln_proj: on the kept normalised tokens, else through the LayerNorm load mode on X."""
+        if xn is not None:
+            return ops.pw_wgrad_side(G, xn, N, C, dW=dW, dbias=dbias)
+        return ops.pw_wgrad_side(G, X, N, C, a_mode=A_GN, a_p=(gamma, beta), row_stats=(ln[0], ln[1]), rows_per_sample=1, dW=dW, dbias=dbias)
+
+    # ---- FFN
+    db2, db1 = vec(11, C), vec(9, ffn)
+    drop = st.drop
+    if drop is not None:
+        p, p_ffn, p_row = drop
+        k1, k2, k3 = st.keys
+        dF = ops.dropout_bwd(dY, p, k2, p_row=p_row, rows_per_sample=S)  # gradient of the FFN branch; the residual path keeps dY
+        ops.pw_wgrad_side(dF, ha, C, ffn, dW=D.mat(10, C, ffn), dbias=db2)
+        dha = ops.pw_gemm(dF, P.get(cfg.i_w2t), ffn, K=C)
+        if k3 is not None:
+            dha = ops.dropout_bwd(dha, p_ffn, k3)
+        dh = ops.act_bwd(dha, h, cfg.act)
+    elif cfg.act == ops.ACT_SILU:
+        ops.pw_wgrad_side(dY, h, C, ffn, a_mode=A_SILU, dW=D.mat(10, C, ffn), dbias=db2)
+        dh = ops.pw_gemm(dY, P.get(cfg.i_w2t), ffn, K=C, e_mode=E_SILU_BWD, Y=h)
+    else:
+        ops.pw_wgrad_side(dY, ha, C, ffn, dW=D.mat(10, C, ffn), dbias=db2)
+        dh = ops.act_bwd(ops.pw_gemm(dY, P.get(cfg.i_w2t), ffn, K=C), h, cfg.act)
+    ln_wgrad(dh, st.xn2, X1, ln2, g2, b2, ffn, D.mat(8, ffn, C), db1)
+    csf = ar.f64(2, C)
+    vF = ops.pw_gemm(dh, P.get(cfg.i_w1t), C, K=ffn)
+    if drop is None:
+        bsum1 = ar.f64(C)
+        dX1 = ops.ln_bwd(vF, X1, ln2, g2, csf, DRES=dY, col_sum=bsum1)  # bsum1 = column sums of dX1 = d(out_proj bias)
+        D.late64(5, bsum1)
+        dA = dX1
+        dbo = None
+    else:
+        dX1 = ops.ln_bwd(vF, X1, ln2, g2, csf, DRES=dY)
+        dA = ops.dropout_bwd(dX1, p, k1, p_row=p_row, rows_per_sample=S)  # gradient of the attention branch (out_proj output)
+        dbo = vec(5, C)
+    D.late64(6, csf[1])
+    D.late64(7, csf[0])
+    # ---- attention
+    ops.pw_wgrad_side(dA, O, C, C, dW=D.mat(4, C, C), dbias=dbo)
+    dO = ops.pw_gemm(dA, P.get(cfg.i_wot), C, K=C)
+    dqkv = ops.mha_bwd(qkv, O, dO, LSE, N, S, cfg.heads, cfg.head_dim, cfg.scale, amask, kpm)
+    ln_wgrad(dqkv, st.xn1, x2, ln1, g1, b1, 3 * C, D.mat(2, 3 * C, C), vec(3, 3 * C))
+    csa = ar.f64(2, C)
+    vA = ops.pw_gemm(dqkv, P.get(cfg.i_wqkvt), C, K=3 * C)
+    dx = ops.ln_bwd(vA, x2, ln1, g1, csa, DRES=dX1)
+    D.late64(0, csa[1])
+    D.late64(1, csa[0])
+    ops.join_side()
+    return dx, D.finish()
+
+
 class TransformerEncoderFn(torch.autograd.Function):
     """x = x + MHA(LN1(x));  x = x + W2 act(W1 LN2(x) + b1) + b2   (transformer.py:139-156)."""
 
     @staticmethod
-    def forward(ctx, x, cfg, g1, b1, wqkv, bqkv, wo, bo, g2, b2, w1, bb1, w2, bb2):
+    def forward(ctx, x, cfg, *params):
         N, S, C = x.shape
-        M, ffn = N * S, cfg.ffn
-        P = cfg.prep
-        x2 = x.reshape(M, C)
         amask, kpm = _masks(cfg.masks, N, S, x.device)
-        ln1 = ops.ln_stats(x2, cfg.eps)
-        # wide layers (ViT / CLIP: K = 768 under 18-24 N tiles): the LayerNorm prologue is applied ONCE by a pre-pass (ops.WIDE_K / WIDE_N policy, which
-        # pw_gemm would apply internally) and the normalised tokens are KEPT for the weight gradient of the same projection, which would otherwise
-        # re-normalise them (one extra pass over the tokens per weight-gradient block)
-        keep_n = C >= ops.WIDE_K and 3 * C >= ops.WIDE_N_WGRAD and ffn >= ops.WIDE_N_WGRAD
-
-        def ln_proj(X, ln, gamma, beta, weight, N, bias):
-            """(LayerNorm(X) @ weight^T + bias, the kept normalised tokens or None)."""
-            if not keep_n:
-                return ops.pw_gemm(X, weight, N, a_mode=A_GN, a_p=(gamma, beta), row_stats=(ln[0], ln[1]), rows_per_sample=1, bias=bias), None
-            xn = ops.apply_load_mode(X, A_GN, C, a_p=(gamma, beta), row_stats=(ln[0], ln[1]), rows_per_sample=1)
-            return ops.pw_gemm(xn, weight, N, bias=bias), xn
-
-        qkv, xn1 = ln_proj(x2, ln1, g1, b1, P.get(cfg.i_wqkv), 3 * C, bqkv)
-        O, LSE = ops.mha_fwd(qkv, N, S, cfg.heads, cfg.head_dim, cfg.scale, amask, kpm)
-        drop = getattr(cfg, "drop", None)  # (p, p_ffn, p_row) in training with dropout / stochastic depth > 0 (transformer.py:97-100, 139-156)
-        if drop is None:
-            samp = _fwd_arena(cfg, x.device).f64(2, M)
-            X1 = ops.pw_gemm(O, P.get(cfg.i_wo), C, bias=bo, R=x2, samp_stats=samp, rows_per_sample=1)
-            ln2 = ops.gn_finalize(samp, C, cfg.eps)
-        else:
-            # the residual adds leave the GEMM epilogues: x + DropPath(Dropout(branch)) is one element-wise pass with hashed masks
-            p, p_ffn, p_row = drop
-            k1, k2 = ops.rng_next(x.device), ops.rng_next(x.device)
-            A = ops.pw_gemm(O, P.get(cfg.i_wo), C, bias=bo)
-            X1 = ops.dropout_fwd(A, x2, p, k1, p_row=p_row, rows_per_sample=S)
-            ln2 = ops.ln_stats(X1, cfg.eps)
-        h, xn2 = ln_proj(X1, ln2, g2, b2, P.get(cfg.i_w1), ffn, bb1)
-        keys = None
-        if drop is None:
-            if cfg.act == ops.ACT_SILU:
-                ha = None
-                X2 = ops.pw_gemm(h, P.get(cfg.i_w2), C, a_mode=A_SILU, bias=bb2, R=X1)
-            else:
-                ha = ops.act_fwd(h, cfg.act)
-                X2 = ops.pw_gemm(ha, P.get(cfg.i_w2), C, bias=bb2, R=X1)
-        else:
-            ha = ops.act_fwd(h, cfg.act)
-            k3 = None
-            if p_ffn > 0:
-                k3 = ops.rng_next(x.device)
-                ha = ops.dropout_fwd(ha, None, p_ffn, k3)
-            Fo = ops.pw_gemm(ha, P.get(cfg.i_w2), C, bias=bb2)
-            X2 = ops.dropout_fwd(Fo, X1, p, k2, p_row=p_row, rows_per_sample=S)
-            keys = (k1, k2, k3)
-        ctx.keys, ctx.drop, ctx.xn = keys, drop, (xn1, xn2)
-        ctx.cfg, ctx.dims, ctx.plist = cfg, (N, S, C), cfg.plist
-        ctx.saved = (x2, ln1, qkv, O, LSE, X1, ln2, h, ha, amask, kpm)
-        ctx.save_for_backward(g1, b1, g2, b2)
+        X2, ctx.st = _encoder_forward(x.reshape(N * S, C), N, S, cfg, amask, kpm, getattr(cfg, "drop", None))
+        ctx.cfg, ctx.plist = cfg, cfg.plist
         return X2.view(N, S, C)
 
     @staticmethod
     def backward(ctx, gout):
-        cfg = ctx.cfg
-        N, S, C = ctx.dims
-        M, ffn = N * S, cfg.ffn
-        P = cfg.prep
-        x2, ln1, qkv, O, LSE, X1, ln2, h, ha, amask, kpm = ctx.saved
-        g1, b1, g2, b2 = ctx.saved_tensors
-        dev = x2.device
-        dY = gout.reshape(M, C).to(BF16).contiguous()
-        # parameter order: (g1, b1, wqkv, bqkv, wo, bo, g2, b2, w1, bb1, w2, bb2)
-        D = _Dst(cfg, ctx.plist, dev, True)
-        ar = D.ar
-        vec = lambda i, n: D.mat(i, 1, n).view(n)  # noqa: E731
+        N, S, C = gout.shape
+        dx, grads = _encoder_backward(ctx.st, gout.reshape(N * S, C).to(BF16).contiguous(), ctx.cfg, ctx.plist)
+        return (dx.view(N, S, C), None) + grads
 
-        def ln_wgrad(G, xn, X, ln, gamma, beta, N, dW, dbias):
-            """Weight gradient of the forward's ln_proj: on the kept normalised tokens, else through the LayerNorm load mode on X."""
-            if xn is not None:
-                return ops.pw_wgrad_side(G, xn, N, C, dW=dW, dbias=dbias)
-            return ops.pw_wgrad_side(G, X, N, C, a_mode=A_GN, a_p=(gamma, beta), row_stats=(ln[0], ln[1]), rows_per_sample=1, dW=dW, dbias=dbias)
 
-        # ---- FFN
-        db2, db1 = vec(11, C), vec(9, ffn)
-        drop = ctx.drop
-        if drop is not None:
-            p, p_ffn, p_row = drop
-            k1, k2, k3 = ctx.keys
-            dF = ops.dropout_bwd(dY, p, k2, p_row=p_row, rows_per_sample=S)  # gradient of the FFN branch; the residual path keeps dY
-            ops.pw_wgrad_side(dF, ha, C, ffn, dW=D.mat(10, C, ffn), dbias=db2)
-            dha = ops.pw_gemm(dF, P.get(cfg.i_w2t), ffn, K=C)
-            if k3 is not None:
-                dha = ops.dropout_bwd(dha, p_ffn, k3)
-            dh = ops.act_bwd(dha, h, cfg.act)
-        elif cfg.act == ops.ACT_SILU:
-            ops.pw_wgrad_side(dY, h, C, ffn, a_mode=A_SILU, dW=D.mat(10, C, ffn), dbias=db2)
-            dh = ops.pw_gemm(dY, P.get(cfg.i_w2t), ffn, K=C, e_mode=E_SILU_BWD, Y=h)
-        else:
-            ops.pw_wgrad_side(dY, ha, C, ffn, dW=D.mat(10, C, ffn), dbias=db2)
-            dh = ops.act_bwd(ops.pw_gemm(dY, P.get(cfg.i_w2t), ffn, K=C), h, cfg.act)
-        xn1, xn2 = ctx.xn
-        ln_wgrad(dh, xn2, X1, ln2, g2, b2, ffn, D.mat(8, ffn, C), db1)
-        csf = ar.f64(2, C)
-        vF = ops.pw_gemm(dh, P.get(cfg.i_w1t), C, K=ffn)
-        if drop is None:
-            bsum1 = ar.f64(C)
-            dX1 = ops.ln_bwd(vF, X1, ln2, g2, csf, DRES=dY, col_sum=bsum1)  # bsum1 = column sums of dX1 = d(out_proj bias)
-            D.late64(5, bsum1)
-            dA = dX1
-            dbo = None
-        else:
-            dX1 = ops.ln_bwd(vF, X1, ln2, g2, csf, DRES=dY)
-            dA = ops.dropout_bwd(dX1, p, k1, p_row=p_row, rows_per_sample=S)  # gradient of the attention branch (out_proj output)
-            dbo = vec(5, C)
-        D.late64(6, csf[1])
-        D.late64(7, csf[0])
-        # ---- attention
-        ops.pw_wgrad_side(dA, O, C, C, dW=D.mat(4, C, C), dbias=dbo)
-        dO = ops.pw_gemm(dA, P.get(cfg.i_wot), C, K=C)
-        dqkv = ops.mha_bwd(qkv, O, dO, LSE, N, S, cfg.heads, cfg.head_dim, cfg.scale, amask, kpm)
-        ln_wgrad(dqkv, xn1, x2, ln1, g1, b1, 3 * C, D.mat(2, 3 * C, C), vec(3, 3 * C))
-        csa = ar.f64(2, C)
-        vA = ops.pw_gemm(dqkv, P.get(cfg.i_wqkvt), C, K=3 * C)
-        dx = ops.ln_bwd(vA, x2, ln1, g1, csa, DRES=dX1)
-        D.late64(0, csa[1])
-        D.late64(1, csa[0])
-        ops.join_side()
-        return (dx.view(N, S, C), None) + D.finish()
+class EncoderRunFn(torch.autograd.Function):
+    """A run of TransformerEncoder layers with recomputing gradient checkpointing (what torch.utils.checkpoint does for the reference,
+    vit.py:526-533, text_encoders/transformer.py:390-401): the forward keeps only the run's input and each layer's mask keys, the backward
+    re-runs the run's forward from them -- bit for bit the same activations, every forward kernel being deterministic -- and then each
+    layer's backward, last layer first.  torch's checkpoint would restore torch's RNG state, not the library's device-side generator, so the
+    dropout / stochastic-depth masks are replayed from the saved keys instead.  ``run.cfgs``: the layers' cfgs as TransformerEncoder.prepare
+    left them; ``params``: their parameter lists, concatenated."""
+
+    @staticmethod
+    def forward(ctx, x, run, *params):
+        N, S, C = x.shape
+        x2 = y = x.reshape(N * S, C)
+        layers = []
+        for cfg in run.cfgs:
+            amask, kpm = _masks(cfg.masks, N, S, x.device)
+            drop = getattr(cfg, "drop", None)
+            y, st = _encoder_forward(y, N, S, cfg, amask, kpm, drop)
+            layers.append((cfg, cfg.plist, amask, kpm, drop, st.keys))
+            del st
+        ctx.x2, ctx.layers = x2, layers
+        return y.view(N, S, C)
+
+    @staticmethod
+    def backward(ctx, gout):
+        N, S, C = gout.shape
+        y, sts = ctx.x2, []
+        for cfg, _, amask, kpm, drop, keys in ctx.layers:
+            y, st = _encoder_forward(y, N, S, cfg, amask, kpm, drop, keys=keys, arena="rfwd")
+            sts.append(st)
+        del y
+        dY = gout.reshape(N * S, C).to(BF16).contiguous()
+        grads = []
+        for cfg, plist, *_ in reversed(ctx.layers):
+            dY, g = _encoder_backward(sts.pop(), dY, cfg, plist)  # the layer's activations are released as soon as its backward is issued
+            grads.append(g)
+        return (dY.view(N, S, C), None) + tuple(gp for g in reversed(grads) for gp in g)

@@ -146,8 +146,8 @@ class LayerNorm(nn.LayerNorm):
         from . import functional as Fn
         _need_cuda(x, self.__class__.__name__)
         C = self.normalized_shape[0]
-        if len(self.normalized_shape) != 1 or x.shape[-1] != C or C % 8 or C > 1024 or not self.elementwise_affine:
-            raise NotImplementedError("LayerNorm: last-dimension normalisation with C % 8 == 0, C <= 1024 and affine weights is implemented")
+        if len(self.normalized_shape) != 1 or x.shape[-1] != C or C % 8 or C > 1280 or not self.elementwise_affine:
+            raise NotImplementedError("LayerNorm: last-dimension normalisation with C % 8 == 0, C <= 1280 and affine weights is implemented")
         if x.dim() > 2 and x.shape[1] == C:
             raise NotImplementedError("LayerNorm on a channel-first tensor (x.shape[1] == C, layer_norm.py:52-65) is not implemented")
         cfg = getattr(self, "_cfg", None)

@@ -30,13 +30,15 @@ from . import functional as Fn
 from . import ops
 from .layers import Dropout, _bind, _need_cuda, get_normalization_layer
 from .models_vit import PositionalEmbedding, VisionTransformer, default_vit_opts
-from .modules import TransformerEncoder
+from .modules import TransformerEncoder, checkpointed_encoders
 from .ops import PreparedWeights as PW
 
 
 def default_clip_opts(vit_mode: str = "base", projection_dim: int = 512, text_dim: int = 512, text_layers: int = 12, text_heads: int = 8,
                       vocab_size: int = 49408, context_length: int = 77, **extra) -> argparse.Namespace:
-    """config/multi_modal_img_text/clip_vit.yaml model section."""
+    """config/multi_modal_img_text/clip_vit.yaml model section.  The ViT-H/16 recipe (examples/range_augment/clip/clip_vit_huge.yaml):
+    ``vit_mode="huge", text_dim=768, text_heads=12`` and gradient checkpointing of both towers (``model.classification.gradient_checkpointing``,
+    ``model.text.transformer.gradient_checkpoint``)."""
     opts = default_vit_opts(vit_mode)
     kv = {
         "model.multi_modal_image_text.name": "clip", "model.multi_modal_image_text.clip.projection_dim": projection_dim,
@@ -44,7 +46,7 @@ def default_clip_opts(vit_mode: str = "base", projection_dim: int = 512, text_di
         "model.text.transformer.n_heads_per_layer": text_heads, "model.text.transformer.ffn_multiplier_per_layer": 4.0,
         "model.text.transformer.causal_masking": True, "model.text.transformer.norm_layer": "layer_norm_fp32",
         "model.text.transformer.dropout": 0.0, "model.text.transformer.attn_dropout": 0.0, "model.text.transformer.ffn_dropout": 0.0,
-        "model.text.transformer.no_pos_embedding": False, "dataset.text_vocab_size": vocab_size, "dataset.text_context_length": context_length,
+        "model.text.transformer.no_pos_embedding": False, "model.text.transformer.gradient_checkpoint": False, "dataset.text_vocab_size": vocab_size, "dataset.text_context_length": context_length,
         "dataset.padding_index": None,
     }
     kv.update(extra)
@@ -109,6 +111,8 @@ class TextTransformer(nn.Module):
         self._emb = SimpleNamespace()
         self._proj = _Projection()
         self._mask = None
+        # every layer's activations are recomputed in the backward (transformer.py:390-401); nothing to recompute in eval mode
+        self.gradient_checkpoint = bool(getattr(opts, "model.text.transformer.gradient_checkpoint", False))
 
     def reset_parameters_clip_style(self):
         """transformer.py:181-211."""
@@ -165,8 +169,12 @@ class TextTransformer(nn.Module):
         if self.causal_masking:
             attn_mask = self.build_attention_mask(tokens.shape[1], tokens.shape[0], tokens.device)
             key_padding_mask = None
+        ckpt = self.gradient_checkpoint and self.training and torch.is_grad_enabled()
         for layer in self.transformer:
-            x = layer(x, key_padding_mask=key_padding_mask, attn_mask=attn_mask)
+            if ckpt:
+                x = checkpointed_encoders([layer], x, key_padding_mask=key_padding_mask, attn_mask=attn_mask)
+            else:
+                x = layer(x, key_padding_mask=key_padding_mask, attn_mask=attn_mask)
         x = Fn.EotGatherFn.apply(x, tokens)       # LayerNorm is per token: normalising only the gathered token equals norm-then-gather
         x = self.final_layer_norm(x)
         return self._proj.apply_to(x, self.projection_layer, self)

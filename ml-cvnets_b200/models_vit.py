@@ -7,8 +7,11 @@ backward kernel is the library's.  BASELINE.json configs[2]: ViT-B/16, bf16, 224
 Any input resolution whose sides are multiples of 16 works, square or not (the multi-scale recipes feed 128-320 px crops): when the patch
 grid does not hold the table's 196 entries, the positional table is linearly resampled in the token-assembly kernel exactly as the
 reference's F.interpolate does (cvnets/layers/positional_embedding.py:90-95), and sequences over 256 tokens run on the streaming attention
-kernels (every ViT mode has head_dim 64).  Not implemented (raises): SimpleFPN (detection), sinusoidal positional embeddings,
-output_stride, gradient checkpointing, attention-probability dropout > 0 in training.
+kernels (every ViT mode has head_dim 64).  With ``model.classification.gradient_checkpointing`` (the ViT-H recipes), training splits the
+encoder stack as torch's checkpoint_sequential does for the reference (vit.py:526-533) into ``model.classification.vit.checkpoint_segments``
+segments; the first segments - 1 runs keep only their input and are recomputed in the backward (modules.checkpointed_encoders), the
+remaining layers run normally.  The option does nothing in eval mode.  Not implemented (raises): SimpleFPN (detection), sinusoidal
+positional embeddings, output_stride, attention-probability dropout > 0 in training.
 """
 from __future__ import annotations
 
@@ -23,18 +26,19 @@ from torch import Tensor, nn
 from . import functional as Fn
 from . import ops
 from .layers import ConvLayer2d, Dropout, LinearLayer, _bind, _need_cuda, get_normalization_layer, norm_layers_tuple
-from .modules import TransformerEncoder
+from .modules import TransformerEncoder, checkpointed_encoders
 from .neural_aug import augmented_forward, build_neural_augmentor
 
 
 def default_vit_opts(mode: str = "base", n_classes: int = 1000, **extra) -> argparse.Namespace:
-    """The recipe's model options (examples/vit/classification/vit_base.yaml:80-97)."""
+    """The recipe's model options (examples/vit/classification/vit_base.yaml:80-97; the ViT-H recipes set gradient_checkpointing)."""
     opts = argparse.Namespace()
     kv = {
         "model.classification.name": "vit", "model.classification.n_classes": n_classes, "model.classification.vit.mode": mode,
         "model.classification.vit.norm_layer": "layer_norm_fp32", "model.classification.vit.dropout": 0.0,
         "model.classification.vit.stochastic_dropout": 0.0, "model.classification.vit.no_cls_token": False,
         "model.classification.vit.sinusoidal_pos_emb": False, "model.classification.vit.use_simple_fpn": False,
+        "model.classification.gradient_checkpointing": False, "model.classification.vit.checkpoint_segments": 4,
         "model.activation.name": "gelu", "model.normalization.name": "batch_norm", "model.normalization.momentum": 0.1,
         "model.layer.conv_init": "kaiming_normal", "model.layer.linear_init": "trunc_normal", "model.layer.linear_init_std_dev": 0.02,
     }
@@ -114,6 +118,10 @@ class VisionTransformer(nn.Module):
             if isinstance(m, nn.LayerNorm):
                 m.eps = 1e-6
         self._tok = SimpleNamespace()
+        self.gradient_checkpointing = bool(getattr(opts, "model.classification.gradient_checkpointing", False))
+        self.checkpoint_segments = int(getattr(opts, "model.classification.vit.checkpoint_segments", 4))
+        if self.gradient_checkpointing and not 1 <= self.checkpoint_segments <= n_layers:
+            raise ValueError(f"checkpoint_segments must be in 1..{n_layers}, got {self.checkpoint_segments}")
 
     @classmethod
     def build_model(cls, opts, *args, **kwargs):
@@ -158,7 +166,16 @@ class VisionTransformer(nn.Module):
 
     def extract_features(self, x: Tensor, *args, **kwargs) -> Tensor:
         x, _ = self.extract_patch_embeddings(x)
-        x = self.transformer(x)
+        if self.training and self.gradient_checkpointing and torch.is_grad_enabled():
+            layers = list(self.transformer)
+            size = len(layers) // self.checkpoint_segments  # torch.utils.checkpoint.checkpoint_sequential's split
+            end = size * (self.checkpoint_segments - 1)
+            for start in range(0, end, size):
+                x = checkpointed_encoders(layers[start:start + size], x)
+            for layer in layers[end:]:
+                x = layer(x)
+        else:
+            x = self.transformer(x)
         # LayerNorm is per token, so normalising only the token the classifier reads equals the reference's norm-then-select
         x = x[:, 0] if self.cls_token is not None else None
         if x is None:

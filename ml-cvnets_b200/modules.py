@@ -506,9 +506,14 @@ class TransformerEncoder(BaseModule):
 
     def forward(self, x: Tensor, x_prev: Optional[Tensor] = None, key_padding_mask: Optional[Tensor] = None,
                 attn_mask: Optional[Tensor] = None, *args, **kwargs) -> Tensor:
-        _need_cuda(x, "TransformerEncoder")
         if x_prev is not None:
             raise NotImplementedError("cross-attention (x_prev) is not implemented on the GPU path")
+        cfg = self.prepare(x, key_padding_mask, attn_mask)
+        return Fn.TransformerEncoderFn.apply(x.to(torch.bfloat16).contiguous(), cfg, *cfg.plist)
+
+    def prepare(self, x: Tensor, key_padding_mask: Optional[Tensor] = None, attn_mask: Optional[Tensor] = None):
+        """Checks the input and readies the layer's cfg (masks, dropout, parameters) for one call of its forward kernels."""
+        _need_cuda(x, "TransformerEncoder")
         if self.training and self.pre_norm_mha[1].attn_dropout.p:
             raise NotImplementedError("attention-probability dropout > 0 in training mode is not implemented (every recipe of the reference sets 0; "
                                       "it is the identity in eval mode, which works)")
@@ -533,4 +538,11 @@ class TransformerEncoder(BaseModule):
         l1, l2 = self.pre_norm_ffn[1], self.pre_norm_ffn[4]
         _bind(self, cfg, [n1.weight, n1.bias, mha.qkv_proj.weight, mha.qkv_proj.bias, mha.out_proj.weight, mha.out_proj.bias, n2.weight, n2.bias,
                           l1.weight, l1.bias, l2.weight, l2.bias])
-        return Fn.TransformerEncoderFn.apply(x.to(torch.bfloat16).contiguous(), cfg, *cfg.plist)
+        return cfg
+
+
+def checkpointed_encoders(layers, x: Tensor, key_padding_mask: Optional[Tensor] = None, attn_mask: Optional[Tensor] = None) -> Tensor:
+    """``x`` through the TransformerEncoder ``layers`` as one run whose activations are recomputed in the backward (functional.EncoderRunFn):
+    the gradient checkpointing of the ViT / CLIP recipes, with the same results as calling the layers one after another."""
+    cfgs = [layer.prepare(x, key_padding_mask, attn_mask) for layer in layers]
+    return Fn.EncoderRunFn.apply(x.to(torch.bfloat16).contiguous(), SimpleNamespace(cfgs=cfgs), *[p for c in cfgs for p in c.plist])
