@@ -175,7 +175,6 @@ extern "C" int cvb_embedding_fwd(const int64_t* tokens, const float* table, cons
   const int64_t ntok = (int64_t)B * S;
   CVB_CUDA(cvb_launch(embedding_fwd_kernel, kgrid(ntok * (C / 8)), KNT, 0, static_cast<cudaStream_t>(stream), tokens, table, pos, static_cast<bf16*>(out), ntok,
                       S, C, V));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -184,7 +183,6 @@ extern "C" int cvb_embedding_bwd(const void* dout, const int64_t* tokens, float*
   const int64_t ntok = (int64_t)B * S;
   CVB_CUDA(cvb_launch(embedding_bwd_kernel, kgrid(ntok * (C / 8)), KNT, 0, static_cast<cudaStream_t>(stream), static_cast<const bf16*>(dout), tokens, dtable,
                       dpos, ntok, S, C, V));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -192,7 +190,6 @@ extern "C" int cvb_eot_gather_fwd(const void* X, const int64_t* tokens, int B, i
   CVB_CHECK(X && tokens && out && idx && B > 0 && S > 0 && C > 0 && C % 8 == 0 && cvb_aligned16(X) && cvb_aligned16(out), "cvb_eot_gather_fwd: bad arguments");
   CVB_CUDA(cvb_launch(eot_gather_fwd_kernel, B, 128, 0, static_cast<cudaStream_t>(stream), static_cast<const bf16*>(X), tokens, S, C, static_cast<bf16*>(out),
                       idx));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -201,7 +198,6 @@ extern "C" int cvb_eot_gather_bwd(const void* dout, const int* idx, int B, int S
   const int64_t ntok = (int64_t)B * S;
   CVB_CUDA(cvb_launch(eot_gather_bwd_kernel, kgrid(ntok * (C / 8)), KNT, 0, static_cast<cudaStream_t>(stream), static_cast<const bf16*>(dout), idx, S, C,
                       static_cast<bf16*>(dX), ntok));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -209,7 +205,6 @@ extern "C" int cvb_l2norm_fwd(const void* X, void* Y, float* inv_norm, int M, in
   CVB_CHECK(X && Y && inv_norm && M > 0 && C > 0 && C % 8 == 0 && cvb_aligned16(X) && cvb_aligned16(Y), "cvb_l2norm_fwd: bad arguments");
   CVB_CUDA(cvb_launch(l2norm_fwd_kernel, (M + KNT / 32 - 1) / (KNT / 32), KNT, 0, static_cast<cudaStream_t>(stream), static_cast<const bf16*>(X),
                       static_cast<bf16*>(Y), inv_norm, M, C, eps));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -217,6 +212,5 @@ extern "C" int cvb_l2norm_bwd(const void* DY, const void* Y, const float* inv_no
   CVB_CHECK(DY && Y && inv_norm && DX && M > 0 && C > 0 && C % 8 == 0 && cvb_aligned16(DY) && cvb_aligned16(Y) && cvb_aligned16(DX), "cvb_l2norm_bwd: bad arguments");
   CVB_CUDA(cvb_launch(l2norm_bwd_kernel, (M + KNT / 32 - 1) / (KNT / 32), KNT, 0, static_cast<cudaStream_t>(stream), static_cast<const bf16*>(DY),
                       static_cast<const bf16*>(Y), inv_norm, static_cast<bf16*>(DX), M, C));
-  CVB_LAUNCH_CHECK();
   return 0;
 }

@@ -24,26 +24,38 @@ void cvb_set_error(const char* fmt, ...);
       return 1;                         \
     }                                   \
   } while (0)
-#define CVB_CUDA(call)                                                                   \
+// variadic: the call's template argument lists may hold commas
+#define CVB_CUDA(...)                                                                    \
   do {                                                                                   \
-    cudaError_t e_ = (call);                                                             \
+    cudaError_t e_ = (__VA_ARGS__);                                                      \
     if (e_ != cudaSuccess) {                                                             \
       (void)cudaGetLastError(); /* reported here: do not leave it for the next caller */ \
       cvb_set_error("%s:%d CUDA error: %s", __FILE__, __LINE__, cudaGetErrorString(e_)); \
       return 2;                                                                          \
     }                                                                                    \
   } while (0)
-#define CVB_LAUNCH_CHECK() CVB_CUDA(cudaGetLastError())
 
 static inline bool cvb_aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 int cvb_num_sms();
 // Order-independent gradient accumulation.  Partial sums that many CTAs (or warps) contribute are added in fp64: the few fp32 addends of
 // one element sum exactly there, so the result does not depend on the order in which they arrive and two runs of a step are bitwise equal.
-// cvb_det_alloc: zeroed fp64 scratch of n elements (stream-ordered, capturable); cvb_det_add: dst[r * ld + c] += scratch[r * cols + c];
-// cvb_det_free: release it after the adds.
-int cvb_det_alloc(double** scratch, size_t n, cudaStream_t st);
-int cvb_det_add(const double* scratch, float* dst, int rows, int cols, int ld, cudaStream_t st);
-int cvb_det_free(double* scratch, cudaStream_t st);
+// DetScratch holds that fp64 scratch, stream-ordered (capturable).  alloc: n zeroed elements; add: dst[r * ld + c] += scratch[offset +
+// r * cols + c]; release: free it after the adds.  An early return frees it in the destructor and keeps the first failure's message.
+class DetScratch {
+ public:
+  explicit DetScratch(cudaStream_t st) : st_(st) {}
+  DetScratch(const DetScratch&) = delete;
+  DetScratch& operator=(const DetScratch&) = delete;
+  ~DetScratch();
+  int alloc(size_t n);
+  int add(size_t offset, float* dst, int rows, int cols, int ld);
+  int release();
+  double* data() const { return p_; }
+
+ private:
+  cudaStream_t st_;
+  double* p_ = nullptr;
+};
 
 // ---------------------------------------------------------------------------------------------- small device helpers
 // SiLU through ONE special-function op: sigmoid(z) = 0.5 + 0.5 tanh(z/2) with tanh.approx.f32 (MUFU.TANH, max abs error 2^-11), instead of
@@ -153,6 +165,7 @@ __device__ __forceinline__ float apply_mode(int mode, float x, float p0, float p
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 int cvb_pdl_enabled();
+// Returns the launch's error, or the error pending after it (cudaGetLastError) when the launch itself succeeded.
 template <typename... KArgs, typename... Args>
 static inline cudaError_t cvb_launch(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
   cudaLaunchConfig_t cfg;
@@ -166,21 +179,32 @@ static inline cudaError_t cvb_launch(void (*kernel)(KArgs...), dim3 grid, dim3 b
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = cvb_pdl_enabled() ? 1 : 0;
-  return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
+  const cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
+  return e != cudaSuccess ? e : cudaGetLastError();
+}
+// Opts the kernel in to `bytes` of dynamic shared memory (past the default 48 KB) on its first call.  The flag is keyed on the kernel
+// itself, so kernels with the same parameter list keep their own.
+template <auto Kernel>
+static inline cudaError_t cvb_smem_optin(int bytes) {
+  static bool done = false;
+  if (done) return cudaSuccess;
+  const cudaError_t e = cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+  done = e == cudaSuccess;
+  return e;
 }
 
 // ---------------------------------------------------------------------------------------------- TMA + mbarrier (sm_90a)
 #include <cuda.h>  // CUtensorMap (types only; the encoder is fetched through cudaGetDriverEntryPoint, no -lcuda)
 
 // Host: tensor map of a channels-last bf16 feature map [B, H, W, C] with a [1, boxH, boxW, boxC] box (boxC * 2 bytes <= 128),
-// optional 128-byte swizzle, zero fill for out-of-bounds elements (the conv halo).
-int cvb_make_tmap_nhwc(CUtensorMap* map, const void* base, int B, int H, int W, int C, int boxH, int boxW, int boxC, int swizzle128);
-// Host: tensor map of a row-major bf16 matrix [rows, cols] (leading dimension ld elements) with a [box_rows, 32 cols] box and
-// 64-byte swizzle: the shared-memory image is exactly the 64-byte-row XOR layout (swz64) the GEMM's ldmatrix addressing uses.
-int cvb_make_tmap_2d_k32(CUtensorMap* map, const void* base, int64_t rows, int cols, int ld, int box_rows);
-// Same matrix view with a [box_rows, 64 cols] box and 128-byte swizzle: the image is the canonical MN-major SWIZZLE_128B wgmma
-// operand layout (8-row x 128-byte atoms) when the ROWS are the reduction dimension (weight-gradient GEMM).
-int cvb_make_tmap_2d_c64(CUtensorMap* map, const void* base, int64_t rows, int cols, int ld, int box_rows);
+// no swizzle, zero fill for out-of-bounds elements (the conv halo).
+int cvb_make_tmap_nhwc(CUtensorMap* map, const void* base, int B, int H, int W, int C, int boxH, int boxW, int boxC);
+// Host: tensor map of a row-major bf16 matrix [rows, cols] (leading dimension ld elements) with a [box_rows, box_cols] box.  The swizzle
+// follows from the box width:
+//   32 columns: 64-byte swizzle; the shared-memory image is exactly the 64-byte-row XOR layout (swz64) the GEMM's ldmatrix addressing uses.
+//   64 columns: 128-byte swizzle; the image is the canonical MN-major SWIZZLE_128B wgmma operand layout (8-row x 128-byte atoms) when the
+//               ROWS are the reduction dimension (weight-gradient GEMM).
+int cvb_make_tmap_2d(CUtensorMap* map, const void* base, int64_t rows, int cols, int ld, int box_rows, int box_cols);
 
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");

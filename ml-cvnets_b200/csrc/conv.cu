@@ -270,7 +270,6 @@ extern "C" int cvb_im2col(const void* X, int x_fp32, int64_t sxn, int64_t sxc, i
     CVB_CUDA(cvb_launch(im2col_generic_kernel, cgrid(M * lda), CNT, 0, st, X, x_fp32, sxn, sxc, sxh, sxw, Cin, H, W, k, stride, pad, Ho, Wo,
                         static_cast<bf16*>(A), lda, M));
   }
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -281,7 +280,6 @@ extern "C" int cvb_col2im(const void* dA, int lda, int B, int Cin, int H, int W,
   const int64_t npix = (int64_t)B * H * W;
   CVB_CUDA(cvb_launch(col2im_nhwc_kernel, cgrid(npix * (Cin / 8)), CNT, 0, static_cast<cudaStream_t>(stream), static_cast<const bf16*>(dA), lda, Cin, H, W, k,
                       stride, pad, Ho, Wo, static_cast<bf16*>(dX), npix));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -292,7 +290,6 @@ extern "C" int cvb_patch_permute(const void* X, void* OUT, int B, int H, int W, 
   const int64_t npix = (int64_t)B * H * W;
   CVB_CUDA(cvb_launch(patch_permute_kernel, cgrid(npix * (C / 8)), CNT, 0, static_cast<cudaStream_t>(stream), static_cast<const bf16*>(X),
                       static_cast<bf16*>(OUT), H, W, C, patch_h, patch_w, inverse, npix));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -300,7 +297,6 @@ extern "C" int cvb_concat2(const void* A, const void* B, int C1, int C2, int64_t
   CVB_CHECK(A && B && OUT && C1 > 0 && C2 > 0 && C1 % 8 == 0 && C2 % 8 == 0 && M > 0, "cvb_concat2: bad arguments");
   CVB_CUDA(cvb_launch(concat2_kernel, cgrid(M * ((C1 + C2) / 8)), CNT, 0, static_cast<cudaStream_t>(stream), static_cast<const bf16*>(A),
                       static_cast<const bf16*>(B), static_cast<bf16*>(OUT), C1, C2, 0, M, static_cast<bf16*>(nullptr), static_cast<bf16*>(nullptr)));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -309,7 +305,6 @@ extern "C" int cvb_split2(const void* G, int C1, int C2, int64_t M, void* DA, vo
   CVB_CUDA(cvb_launch(concat2_kernel, cgrid(M * ((C1 + C2) / 8)), CNT, 0, static_cast<cudaStream_t>(stream), static_cast<const bf16*>(nullptr),
                       static_cast<const bf16*>(nullptr), const_cast<bf16*>(static_cast<const bf16*>(G)), C1, C2, 1, M, static_cast<bf16*>(DA),
                       static_cast<bf16*>(DB)));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -320,7 +315,6 @@ extern "C" int cvb_vit_tokens_interp_fwd(const void* patch, const float* pos, in
   const int has_cls = cls != nullptr;
   CVB_CUDA(cvb_launch(vit_tokens_interp_fwd_kernel, cgrid((int64_t)B * (N + has_cls) * (C / 8)), CNT, 0, static_cast<cudaStream_t>(stream),
                       static_cast<const bf16*>(patch), pos, n_pos, (float)n_pos / (float)N, cls, static_cast<bf16*>(out), B, N, C, has_cls));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -330,14 +324,12 @@ extern "C" int cvb_vit_tokens_interp_bwd(const void* dout, void* dpatch, float* 
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int has_cls = dcls != nullptr;
   // batch sum per output token into a zeroed fp32 [N, C] scratch (vit_tokens_bwd_kernel, dpos = scratch), then the transposed stencil
-  double* ws = nullptr;
-  if (cvb_det_alloc(&ws, ((size_t)N * C + 1) / 2, st)) return 2;
-  float* g = reinterpret_cast<float*>(ws);
+  DetScratch ws(st);
+  if (ws.alloc(((size_t)N * C + 1) / 2)) return 2;
+  float* g = reinterpret_cast<float*>(ws.data());
   CVB_CUDA(cvb_launch(vit_tokens_bwd_kernel, cgrid((int64_t)(N + has_cls) * (C / 8)), CNT, 0, st, static_cast<const bf16*>(dout), static_cast<bf16*>(dpatch),
                       g, dcls, B, N, C, has_cls));
-  CVB_LAUNCH_CHECK();
   CVB_CUDA(cvb_launch(vit_pos_interp_bwd_kernel, cgrid((int64_t)n_pos * (C / 8)), CNT, 0, st, static_cast<const float*>(g), dpos, n_pos,
                       (float)n_pos / (float)N, N, C));
-  CVB_LAUNCH_CHECK();
-  return cvb_det_free(ws, st);
+  return ws.release();
 }

@@ -561,11 +561,10 @@ extern "C" int cvb_dw_fwd(const cvb_dw_fwd_args* args, cvb_stream_t stream) {
   dim3 grid(tiles_h * tiles_w, cblocks, gz);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   CUtensorMap tmX;
-  if (cvb_make_tmap_nhwc(&tmX, a.X, a.B, a.H, a.W, a.C, IH, IW, CB, 0)) return 1;
+  if (cvb_make_tmap_nhwc(&tmX, a.X, a.B, a.H, a.W, a.C, IH, IW, CB)) return 1;
 #define CVB_DW_FWD(MODE, S, KS)                                                                                          \
   {                                                                                                                      \
-    static bool attr = false;                                                                                            \
-    if (!attr) { CVB_CUDA(cudaFuncSetAttribute(dw_fwd_kernel<MODE, S, KS>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024)); attr = true; } \
+    CVB_CUDA(cvb_smem_optin<dw_fwd_kernel<MODE, S, KS>>(100 * 1024));                                                    \
     CVB_CUDA(cvb_launch(dw_fwd_kernel<MODE, S, KS>, grid, NT, smem, st, tmX, a, Ho, Wo, TH, TW, tiles_w, buf_bytes));     \
   }
 #define CVB_DW_FWD_X(S, KS)                                                  \
@@ -581,7 +580,6 @@ extern "C" int cvb_dw_fwd(const cvb_dw_fwd_args* args, cvb_stream_t stream) {
   }
 #undef CVB_DW_FWD_X
 #undef CVB_DW_FWD
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -600,14 +598,14 @@ extern "C" int cvb_dw_bwd(const cvb_dw_bwd_args* args, cvb_stream_t stream) {
   if (a.dilation > 1) {
     // the dilated kernel's per-block dW partials meet in the same fp64 scratch as the walk kernels' (order-independent, so reproducible)
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    double* ws = nullptr;
-    if (cvb_det_alloc(&ws, (size_t)9 * a.C, st)) return 2;
+    DetScratch ws(st);
+    if (ws.alloc((size_t)9 * a.C)) return 2;
     cvb_dw_bwd_args b = a;
-    b.dWt = reinterpret_cast<float*>(ws);
-    int rc = cvb_dw_bwd_dilated(b, st);
-    if (rc == 0) rc = cvb_det_add(ws, a.dWt, 9, a.C, a.C, st);
-    const int rf = cvb_det_free(ws, st);
-    return rc ? rc : rf;
+    b.dWt = reinterpret_cast<float*>(ws.data());
+    const int rc = cvb_dw_bwd_dilated(b, st);
+    if (rc) return rc;
+    if (ws.add(0, a.dWt, 9, a.C, a.C)) return 2;
+    return ws.release();
   }
   if (a.stride == 2) CVB_CHECK(a.H % 2 == 0 && a.W % 2 == 0, "cvb_dw_bwd: stride 2 needs even H, W");
   const int s = a.stride, K = a.ksize == 5 ? 5 : 3;
@@ -633,18 +631,17 @@ extern "C" int cvb_dw_bwd(const cvb_dw_bwd_args* args, cvb_stream_t stream) {
   dim3 grid(tiles_h * tiles_w, cblocks, gz);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   CUtensorMap tmDZ, tmY2, tmX;
-  if (cvb_make_tmap_nhwc(&tmDZ, a.DZ, a.B, Ho, Wo, a.C, GH, GW, CB, 0)) return 1;
-  if (cvb_make_tmap_nhwc(&tmY2, bnb ? a.Y2 : a.DZ, a.B, Ho, Wo, a.C, GH, GW, CB, 0)) return 1;
-  if (cvb_make_tmap_nhwc(&tmX, a.X, a.B, a.H, a.W, a.C, XH, XW, CB, 0)) return 1;
+  if (cvb_make_tmap_nhwc(&tmDZ, a.DZ, a.B, Ho, Wo, a.C, GH, GW, CB)) return 1;
+  if (cvb_make_tmap_nhwc(&tmY2, bnb ? a.Y2 : a.DZ, a.B, Ho, Wo, a.C, GH, GW, CB)) return 1;
+  if (cvb_make_tmap_nhwc(&tmX, a.X, a.B, a.H, a.W, a.C, XH, XW, CB)) return 1;
   // the CTAs' dW partials meet in an fp64 scratch (order-independent), added to dWt afterwards
-  double* ws = nullptr;
-  if (cvb_det_alloc(&ws, (size_t)K * K * a.C, st)) return 2;
+  DetScratch ws(st);
+  if (ws.alloc((size_t)K * K * a.C)) return 2;
   cvb_dw_bwd_args b = a;
-  b.dWt = reinterpret_cast<float*>(ws);
+  b.dWt = reinterpret_cast<float*>(ws.data());
 #define CVB_DW_BWD(GM, XM, S, KS)                                                                                        \
   {                                                                                                                      \
-    static bool attr = false;                                                                                            \
-    if (!attr) { CVB_CUDA(cudaFuncSetAttribute(dw_bwd_kernel<GM, XM, S, KS>, cudaFuncAttributeMaxDynamicSharedMemorySize, bwd_smem_cap<KS>())); attr = true; } \
+    CVB_CUDA(cvb_smem_optin<dw_bwd_kernel<GM, XM, S, KS>>(bwd_smem_cap<KS>()));                                          \
     CVB_CUDA(cvb_launch(dw_bwd_kernel<GM, XM, S, KS>, grid, bwd_threads<KS>(), smem, st, tmDZ, tmY2, tmX, b, Ho, Wo, TH, TW, tiles_w, g_bytes,   \
                         x_bytes));                                                                                       \
   }
@@ -666,7 +663,6 @@ extern "C" int cvb_dw_bwd(const cvb_dw_bwd_args* args, cvb_stream_t stream) {
 #undef CVB_DW_BWD_S
 #undef CVB_DW_BWD_X
 #undef CVB_DW_BWD
-  CVB_LAUNCH_CHECK();
-  if (cvb_det_add(ws, a.dWt, K * K, a.C, a.C, st)) return 2;
-  return cvb_det_free(ws, st);
+  if (ws.add(0, a.dWt, K * K, a.C, a.C)) return 2;
+  return ws.release();
 }

@@ -247,7 +247,6 @@ int cvb_dw_fwd_dilated(const cvb_dw_fwd_args& a, cudaStream_t st) {
   if (a.x_mode == CVB_A_RAW) CVB_CUDA(cvb_launch(dwd_fwd_kernel<CVB_A_RAW>, grid, block, 0, st, a, a.dilation, CC));
   else if (a.x_mode == CVB_A_AFF) CVB_CUDA(cvb_launch(dwd_fwd_kernel<CVB_A_AFF>, grid, block, 0, st, a, a.dilation, CC));
   else CVB_CUDA(cvb_launch(dwd_fwd_kernel<CVB_A_AFF_SILU>, grid, block, 0, st, a, a.dilation, CC));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -265,6 +264,5 @@ int cvb_dw_bwd_dilated(const cvb_dw_bwd_args& a, cudaStream_t st) {
   }
   if (bnb) CVB_DWD_BWD(CVB_A_BNB) else CVB_DWD_BWD(CVB_A_RAW)
 #undef CVB_DWD_BWD
-  CVB_LAUNCH_CHECK();
   return 0;
 }

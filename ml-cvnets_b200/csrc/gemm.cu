@@ -417,11 +417,7 @@ int launch_gemm(const cvb_gemm_args& a, cudaStream_t st, bool require_two_ctas) 
   // the transform-ahead pipeline waits for stage it+1 before issuing stage it+NST-1: it needs >= 3 stages
   if (nst < 3) return -1;  // caller retries with a narrower N tile (smaller resident weight panel)
   size_t smem = fixed + (size_t)nst * A_STAGE_ALL;
-  static bool attr_set = false;
-  if (!attr_set) {
-    CVB_CUDA(cudaFuncSetAttribute(pw_gemm_kernel<WM, AMODE, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, 216 * 1024));
-    attr_set = true;
-  }
+  CVB_CUDA(cvb_smem_optin<pw_gemm_kernel<WM, AMODE, EPI>>(216 * 1024));
   // resident CTAs per SM: registers allow 2 (launch bounds); shared memory: 228 KB per SM, ~5 KB static + reserved per CTA
   const int occ = (2 * (smem + 5 * 1024) <= (size_t)228 * 1024) ? 2 : 1;
   const int n_tiles = (a.N + BN - 1) / BN, m_tiles = (a.M + BM - 1) / BM;
@@ -429,12 +425,11 @@ int launch_gemm(const cvb_gemm_args& a, cudaStream_t st, bool require_two_ctas) 
   if (gy > m_tiles) gy = m_tiles;
   if (gy < 1) gy = 1;
   CUtensorMap tmA, tmA2, tmW;
-  if (cvb_make_tmap_2d_k32(&tmA, a.A, a.M, a.K, a.lda, BM)) return 1;
-  if (cvb_make_tmap_2d_k32(&tmA2, AMODE == CVB_A_BNB ? a.A2 : a.A, a.M, a.K, AMODE == CVB_A_BNB ? a.lda2 : a.lda, BM)) return 1;
-  if (cvb_make_tmap_2d_k32(&tmW, a.W, a.N, a.K, a.ldw, BN)) return 1;
+  if (cvb_make_tmap_2d(&tmA, a.A, a.M, a.K, a.lda, BM, 32)) return 1;
+  if (cvb_make_tmap_2d(&tmA2, AMODE == CVB_A_BNB ? a.A2 : a.A, a.M, a.K, AMODE == CVB_A_BNB ? a.lda2 : a.lda, BM, 32)) return 1;
+  if (cvb_make_tmap_2d(&tmW, a.W, a.N, a.K, a.ldw, BN, 32)) return 1;
   dim3 grid(n_tiles, gy);
   CVB_CUDA(cvb_launch(pw_gemm_kernel<WM, AMODE, EPI>, grid, NTHREADS, smem, st, tmA, tmA2, tmW, a, nst));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -662,14 +657,9 @@ int launch_wgrad(const cvb_wgrad_args& a, cudaStream_t st) {
   int m_per_cta = ((a.M + splits - 1) / splits + WG_MB - 1) / WG_MB * WG_MB;
   splits = (a.M + m_per_cta - 1) / m_per_cta;
   size_t smem = (size_t)WG_STAGES * WG_MB * 64 * 2 * (GMODE == CVB_A_BNB ? 3 : 2);
-  static bool attr_set = false;
-  if (!attr_set) {
-    CVB_CUDA(cudaFuncSetAttribute(pw_wgrad_kernel<GMODE, AMODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, 128 * 1024));
-    attr_set = true;
-  }
+  CVB_CUDA(cvb_smem_optin<pw_wgrad_kernel<GMODE, AMODE>>(128 * 1024));
   dim3 grid(kt, nt, splits);
   CVB_CUDA(cvb_launch(pw_wgrad_kernel<GMODE, AMODE>, grid, NTHREADS, smem, st, a, m_per_cta));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -728,14 +718,11 @@ extern "C" int cvb_pw_gemm(const cvb_gemm_args* args, cvb_stream_t stream) {
   int rc;
   switch (a.a_mode) {
     case CVB_A_RAW: rc = dispatch_epi<CVB_A_RAW>(a, epi, st); break;
-    case CVB_A_AFF: CVB_CHECK(a.a_p0 && a.a_p1, "cvb_pw_gemm: AFF needs p0/p1"); rc = dispatch_epi<CVB_A_AFF>(a, epi, st); break;
-    case CVB_A_AFF_SILU: CVB_CHECK(a.a_p0 && a.a_p1, "cvb_pw_gemm: AFF_SILU needs p0/p1"); rc = dispatch_epi<CVB_A_AFF_SILU>(a, epi, st); break;
+    case CVB_A_AFF: rc = dispatch_epi<CVB_A_AFF>(a, epi, st); break;
+    case CVB_A_AFF_SILU: rc = dispatch_epi<CVB_A_AFF_SILU>(a, epi, st); break;
     case CVB_A_SILU: rc = dispatch_epi<CVB_A_SILU>(a, epi, st); break;
-    case CVB_A_GN: CVB_CHECK(a.a_p0 && a.a_p1, "cvb_pw_gemm: GN needs gamma/beta"); rc = dispatch_epi<CVB_A_GN>(a, epi, st); break;
-    case CVB_A_BNB:
-      CVB_CHECK(a.A2 && a.a_p0 && a.a_p1 && a.a_p2 && a.lda2 % 8 == 0 && cvb_aligned16(a.A2), "cvb_pw_gemm: BNB needs A2 and p0/p1/p2");
-      rc = dispatch_epi<CVB_A_BNB>(a, epi, st);
-      break;
+    case CVB_A_GN: rc = dispatch_epi<CVB_A_GN>(a, epi, st); break;
+    case CVB_A_BNB: rc = dispatch_epi<CVB_A_BNB>(a, epi, st); break;
     default: cvb_set_error("cvb_pw_gemm: unsupported a_mode %d", a.a_mode); return 1;
   }
   // a narrow layer whose K does not fit the mma.sync kernel's resident weight panel (the EfficientNet-b6 / b7 squeeze-excitation reduce
@@ -758,18 +745,18 @@ extern "C" int cvb_pw_wgrad(const cvb_wgrad_args* args, cvb_stream_t stream) {
   if (a.g_mode == CVB_A_BNB) CVB_CHECK(a.G2 && a.g_p0 && a.g_p1 && a.g_p2 && a.ldg2 % 8 == 0 && cvb_aligned16(a.G2), "cvb_pw_wgrad: BNB needs G2 and p0/p1/p2");
   CVB_CHECK(a.g_mode == CVB_A_RAW || a.g_mode == CVB_A_BNB, "cvb_pw_wgrad: unsupported g_mode %d", a.g_mode);
   // the kernels reduce split partials with fp64 atomics into a scratch (order-independent), which is then added to dW / dbias
-  double* ws = nullptr;
+  DetScratch ws(st);
   const size_t nW = (size_t)a.N * a.K;
-  if (cvb_det_alloc(&ws, nW + (a.dbias ? a.N : 0), st)) return 2;
+  if (ws.alloc(nW + (a.dbias ? a.N : 0))) return 2;
   cvb_wgrad_args b = a;
-  b.dW = reinterpret_cast<float*>(ws);
+  b.dW = reinterpret_cast<float*>(ws.data());
   b.lddw = a.K;
-  b.dbias = a.dbias ? reinterpret_cast<float*>(ws + nW) : nullptr;
+  b.dbias = a.dbias ? reinterpret_cast<float*>(ws.data() + nW) : nullptr;
   int rc = -1;
   if (g_tc_enabled) rc = cvb_pw_wgrad_tc(b, st);  // wgmma kernel: whole [128 x 128] dW blocks in registers, operands read once
   if (rc < 0) rc = a.g_mode == CVB_A_RAW ? dispatch_wgrad_a<CVB_A_RAW>(b, st) : dispatch_wgrad_a<CVB_A_BNB>(b, st);
-  if (rc == 0) rc = cvb_det_add(ws, a.dW, a.N, a.K, a.lddw, st);
-  if (rc == 0 && a.dbias) rc = cvb_det_add(ws + nW, a.dbias, 1, a.N, a.N, st);
-  const int rf = cvb_det_free(ws, st);
-  return rc ? rc : rf;
+  if (rc) return rc;
+  if (ws.add(0, a.dW, a.N, a.K, a.lddw)) return 2;
+  if (a.dbias && ws.add(nW, a.dbias, 1, a.N, a.N)) return 2;
+  return ws.release();
 }

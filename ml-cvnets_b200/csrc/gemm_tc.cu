@@ -368,11 +368,7 @@ int launch_tc_impl(const cvb_gemm_args& a, cudaStream_t st, size_t fixed, int st
   int nst = (int)((budget - fixed) / stage_bytes);
   if (nst > TC_MAX_STAGES) nst = TC_MAX_STAGES;
   const size_t smem = fixed + (size_t)nst * stage_bytes;
-  static bool attr = false;
-  if (!attr) {
-    CVB_CUDA(cudaFuncSetAttribute(pw_gemm_tc_kernel<AMODE, EPI, WRES>, cudaFuncAttributeMaxDynamicSharedMemorySize, 216 * 1024));
-    attr = true;
-  }
+  CVB_CUDA(cvb_smem_optin<pw_gemm_tc_kernel<AMODE, EPI, WRES>>(216 * 1024));
   const int n_tiles = (a.N + TC_BN - 1) / TC_BN, m_tiles = (a.M + TC_BM - 1) / TC_BM;
   // one persistent CTA per SM, never more CTAs than SMs: rounding UP (e.g. 3 N tiles x 45 = 135 CTAs on 132 SMs) would put a few CTAs
   // into a second wave and double the time of the layer
@@ -380,13 +376,12 @@ int launch_tc_impl(const cvb_gemm_args& a, cudaStream_t st, size_t fixed, int st
   if (gy > m_tiles) gy = m_tiles;
   if (gy < 1) gy = 1;
   CUtensorMap tmA, tmA2, tmW;
-  if (cvb_make_tmap_2d_k32(&tmA, a.A, a.M, a.K, a.lda, TC_BM)) return 1;
-  if (cvb_make_tmap_2d_k32(&tmA2, AMODE == CVB_A_BNB ? a.A2 : a.A, a.M, a.K, AMODE == CVB_A_BNB ? a.lda2 : a.lda, TC_BM)) return 1;
-  if (cvb_make_tmap_2d_k32(&tmW, a.W, a.N, a.K, a.ldw, TC_BN)) return 1;
+  if (cvb_make_tmap_2d(&tmA, a.A, a.M, a.K, a.lda, TC_BM, 32)) return 1;
+  if (cvb_make_tmap_2d(&tmA2, AMODE == CVB_A_BNB ? a.A2 : a.A, a.M, a.K, AMODE == CVB_A_BNB ? a.lda2 : a.lda, TC_BM, 32)) return 1;
+  if (cvb_make_tmap_2d(&tmW, a.W, a.N, a.K, a.ldw, TC_BN, 32)) return 1;
   dim3 grid(n_tiles, gy);
   const int threads = TC_THREADS + XfCfg<AMODE>::THREADS;
   CVB_CUDA(cvb_launch(pw_gemm_tc_kernel<AMODE, EPI, WRES>, grid, threads, smem, st, tmA, tmA2, tmW, a, nst));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -464,7 +459,6 @@ int launch_tc_gn_bwd(const cvb_gemm_args& a, cudaStream_t st) {
   const int col_blocks = a.col_sum ? (a.N + 15) / 16 : 0;
   CVB_CUDA(cvb_launch(gn_bwd_ws_finalize_kernel, B + col_blocks, 128, 0, st, static_cast<const double*>(a.gn_ws), a.row_mean, a.row_rstd, a.e_p0, B, a.N, a.col_sum,
                       a.col_sq, a.samp_sum, a.samp_sq));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 

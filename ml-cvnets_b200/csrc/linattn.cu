@@ -345,11 +345,9 @@ static int linattn_fwd_impl(const void* QKV, int ldq, int B, int H, int W, int d
   const int nthreads = NT;  // a multiple of 32; threads beyond (d/8)*(NT/(d/8)) idle in the channel-grouped loops
   size_t smem = (size_t)(N + d + (size_t)(NT / (d / 8)) * d) * sizeof(float);
   CVB_CHECK(smem <= 200 * 1024, "cvb_linattn_fwd: N=%d too large", N);
-  static bool attr = false;
-  if (!attr) { CVB_CUDA(cudaFuncSetAttribute(linattn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); attr = true; }
+  CVB_CUDA(cvb_smem_optin<linattn_fwd_kernel>(200 * 1024));
   CVB_CUDA(cvb_launch(linattn_fwd_kernel, B * P, nthreads, smem, static_cast<cudaStream_t>(stream), static_cast<const bf16*>(QKV), ldq, H, W, d,
                       static_cast<bf16*>(O), ldo, S, CTX, patch == 0 ? 1 : 0, static_cast<const bf16*>(VX), ldvx, Nv));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -377,18 +375,16 @@ static int linattn_bwd_impl(const void* QKV, int ldq, const void* DO, int ldo, c
   const int cgs = d / 8;
   size_t smem = (size_t)(la_pieces(cgs) * N + 3 * d) * sizeof(double) + (size_t)(2 * (NT / cgs) * d + N + d) * sizeof(float);
   CVB_CHECK(smem <= 200 * 1024, "cvb_linattn_bwd: N=%d too large", N);
-  static bool attr = false;
-  if (!attr) { CVB_CUDA(cudaFuncSetAttribute(linattn_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); attr = true; }
+  CVB_CUDA(cvb_smem_optin<linattn_bwd_kernel>(200 * 1024));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  double* ws = nullptr;  // the CTAs' bias-gradient partials meet in fp64 (order-independent), added to dbias afterwards
-  if (dbias && cvb_det_alloc(&ws, (size_t)2 * d + 1, st)) return 2;
+  DetScratch ws(st);  // the CTAs' bias-gradient partials meet in fp64 (order-independent), added to dbias afterwards
+  if (dbias && ws.alloc((size_t)2 * d + 1)) return 2;
   CVB_CUDA(cvb_launch(linattn_bwd_kernel, B * P, nthreads, smem, st, static_cast<const bf16*>(QKV), ldq,
-                      static_cast<const bf16*>(DO), ldo, S, CTX, H, W, d, static_cast<bf16*>(DQKV), ws, patch == 0 ? 1 : 0,
+                      static_cast<const bf16*>(DO), ldo, S, CTX, H, W, d, static_cast<bf16*>(DQKV), ws.data(), patch == 0 ? 1 : 0,
                       static_cast<const bf16*>(VX), ldvx, Nv, static_cast<bf16*>(DVX)));
-  CVB_LAUNCH_CHECK();
   if (!dbias) return 0;
-  if (cvb_det_add(ws, dbias, 1, 2 * d + 1, 2 * d + 1, st)) return 2;
-  return cvb_det_free(ws, st);
+  if (ws.add(0, dbias, 1, 2 * d + 1, 2 * d + 1)) return 2;
+  return ws.release();
 }
 
 extern "C" int cvb_linattn_bwd(const void* QKV, int ldq, const void* DO, int ldo, const float* S, const float* CTX, int B, int H, int W, int d, int patch,

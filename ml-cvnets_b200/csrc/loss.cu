@@ -132,7 +132,6 @@ extern "C" int cvb_ce_fwd(const void* logits, int ld, int B, int C, const int64_
   CVB_CHECK(logits && target && lse && loss && n_valid && B > 0 && C > 0 && ld >= C, "cvb_ce_fwd: bad arguments");
   CVB_CUDA(cvb_launch(ce_fwd_kernel, 1, LNT, 0, static_cast<cudaStream_t>(stream), static_cast<const bf16*>(logits), ld, B, C, target, ignore_index,
                       label_smoothing, lse, loss, n_valid, mix, logit_scale));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -142,7 +141,6 @@ extern "C" int cvb_ce_bwd(const void* logits, int ld, int B, int C, const int64_
   CVB_CHECK(logits && target && lse && n_valid && dlogits && B > 0 && C > 0 && ld >= C && ldd >= C, "cvb_ce_bwd: bad arguments");
   CVB_CUDA(cvb_launch(ce_bwd_kernel, B, 256, 0, static_cast<cudaStream_t>(stream), static_cast<const bf16*>(logits), ld, B, C, target, ignore_index,
                       label_smoothing, lse, n_valid, grad_out, grad_scale, static_cast<bf16*>(dlogits), ldd, mix, logit_scale, dlogit_scale));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -152,7 +150,6 @@ extern "C" int cvb_cast_f64_f32(const cvb_cast_desc* descs_device, int n_desc, i
   int gx = (max_n + 255) / 256;
   if (gx > 16) gx = 16;
   CVB_CUDA(cvb_launch(cast_f64_f32_kernel, dim3(gx, n_desc), 256, 0, static_cast<cudaStream_t>(stream), reinterpret_cast<const CastDesc*>(descs_device)));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -181,7 +178,6 @@ extern "C" int cvb_transpose_bf16(const void* X, void* Y, int R, int C, cvb_stre
   CVB_CHECK(X && Y && R > 0 && C > 0, "cvb_transpose_bf16: bad arguments");
   CVB_CUDA(cvb_launch(transpose_bf16_kernel, dim3((C + 31) / 32, (R + 31) / 32), 256, 0, static_cast<cudaStream_t>(stream), static_cast<const bf16*>(X),
                       static_cast<bf16*>(Y), R, C));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -190,7 +186,6 @@ extern "C" int cvb_add_bf16_f32(const void* A, const float* B, void* OUT, int64_
   int64_t g = (n + 255) / 256;
   if (g > 4096) g = 4096;
   CVB_CUDA(cvb_launch(add_bf16_f32_kernel, (int)g, 256, 0, static_cast<cudaStream_t>(stream), static_cast<const bf16*>(A), B, static_cast<bf16*>(OUT), n));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 

@@ -383,10 +383,8 @@ int launch_fwd(const void* QKV, int ldq, int B, int S, int H, float scale, const
                cudaStream_t st, int hd) {
   const int Sp = (S + 63) / 64 * 64;
   const size_t smem = (size_t)3 * Sp * MhaCfg<HD>::LD * 2;
-  static bool attr = false;
-  if (!attr) { CVB_CUDA(cudaFuncSetAttribute(mha_fwd_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); attr = true; }
+  CVB_CUDA(cvb_smem_optin<mha_fwd_kernel<HD>>(200 * 1024));
   CVB_CUDA(cvb_launch(mha_fwd_kernel<HD>, B * H, 128, smem, st, static_cast<const bf16*>(QKV), ldq, S, H, scale, amask, kpm, static_cast<bf16*>(O), ldo, LSE, hd));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 template <int HD>
@@ -394,11 +392,9 @@ int launch_bwd(const void* QKV, int ldq, const void* O, const void* DO, int ldo,
                const float* amask, const uint8_t* kpm, void* DQKV, int lddq, cudaStream_t st, int hd) {
   const int Sp = (S + 63) / 64 * 64;
   const size_t smem = (size_t)4 * Sp * MhaCfg<HD>::LD * 2 + (size_t)2 * Sp * 4;
-  static bool attr = false;
-  if (!attr) { CVB_CUDA(cudaFuncSetAttribute(mha_bwd_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); attr = true; }
+  CVB_CUDA(cvb_smem_optin<mha_bwd_kernel<HD>>(200 * 1024));
   CVB_CUDA(cvb_launch(mha_bwd_kernel<HD>, B * H, 256, smem, st, static_cast<const bf16*>(QKV), ldq, static_cast<const bf16*>(O),
                       static_cast<const bf16*>(DO), ldo, LSE, S, H, scale, amask, kpm, static_cast<bf16*>(DQKV), lddq, hd));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 

@@ -366,22 +366,15 @@ __global__ void __launch_bounds__(THREADS, 1)
   store_acc(DQKV + (size_t)b * S * lddq + h * 64, lddq, dq, scale, q0, S);
 }
 
-int set_smem(const void* fn) {
-  CVB_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
-  return 0;
-}
-
 }  // namespace
 
 int cvb_mha_fwd_long(const void* QKV, int ldq, int B, int S, int H, float scale, const float* amask, const unsigned char* kpm, void* O, int ldo,
                      float* LSE, cudaStream_t st) {
   const int NQT = (S + 127) / 128;
   CUtensorMap tm;
-  if (cvb_make_tmap_2d_c64(&tm, QKV, (int64_t)B * S, 3 * H * 64, ldq, 64)) return 1;
-  static bool attr = false;
-  if (!attr) { if (set_smem((const void*)mha_long_fwd_kernel)) return 2; attr = true; }
+  if (cvb_make_tmap_2d(&tm, QKV, (int64_t)B * S, 3 * H * 64, ldq, 64, 64)) return 1;
+  CVB_CUDA(cvb_smem_optin<mha_long_fwd_kernel>((int)SMEM_BYTES));
   CVB_CUDA(cvb_launch(mha_long_fwd_kernel, B * H * NQT, THREADS, SMEM_BYTES, st, tm, S, H, NQT, scale, amask, kpm, static_cast<bf16*>(O), ldo, LSE));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -389,27 +382,21 @@ int cvb_mha_bwd_long(const void* QKV, int ldq, const void* O, const void* DO, in
                      const float* amask, const unsigned char* kpm, void* DQKV, int lddq, cudaStream_t st) {
   const int NT = (S + 127) / 128;
   CUtensorMap tmQKV, tmDO;
-  if (cvb_make_tmap_2d_c64(&tmQKV, QKV, (int64_t)B * S, 3 * H * 64, ldq, 64)) return 1;
-  if (cvb_make_tmap_2d_c64(&tmDO, DO, (int64_t)B * S, H * 64, ldo, 64)) return 1;
-  static bool attr = false;
-  if (!attr) {
-    if (set_smem((const void*)mha_long_dkv_kernel) || set_smem((const void*)mha_long_dq_kernel)) return 2;
-    attr = true;
-  }
-  // D: stream-ordered scratch from the device pool (cvb_det_alloc: fp64 elements, zero-filled; used here as B*H*S floats)
-  double* ws = nullptr;
-  if (cvb_det_alloc(&ws, ((size_t)B * H * S + 1) / 2, st)) return 2;
-  float* Dv = reinterpret_cast<float*>(ws);
+  if (cvb_make_tmap_2d(&tmQKV, QKV, (int64_t)B * S, 3 * H * 64, ldq, 64, 64)) return 1;
+  if (cvb_make_tmap_2d(&tmDO, DO, (int64_t)B * S, H * 64, ldo, 64, 64)) return 1;
+  CVB_CUDA(cvb_smem_optin<mha_long_dkv_kernel>((int)SMEM_BYTES));
+  CVB_CUDA(cvb_smem_optin<mha_long_dq_kernel>((int)SMEM_BYTES));
+  // D: stream-ordered scratch from the device pool (DetScratch: fp64 elements, zero-filled; used here as B*H*S floats)
+  DetScratch ws(st);
+  if (ws.alloc(((size_t)B * H * S + 1) / 2)) return 2;
+  float* Dv = reinterpret_cast<float*>(ws.data());
   const int64_t rows = (int64_t)B * S * H;
   int64_t grid = (rows + 255) / 256;
   if (grid > 16 * (int64_t)cvb_num_sms()) grid = 16 * (int64_t)cvb_num_sms();
   CVB_CUDA(cvb_launch(mha_long_d_kernel, (int)grid, 256, 0, st, static_cast<const bf16*>(O), static_cast<const bf16*>(DO), ldo, B, S, H, Dv));
-  CVB_LAUNCH_CHECK();
   CVB_CUDA(cvb_launch(mha_long_dkv_kernel, B * H * NT, THREADS, SMEM_BYTES, st, tmQKV, tmDO, LSE, static_cast<const float*>(Dv), S, H, NT, scale, amask,
                       kpm, static_cast<bf16*>(DQKV), lddq));
-  CVB_LAUNCH_CHECK();
   CVB_CUDA(cvb_launch(mha_long_dq_kernel, B * H * NT, THREADS, SMEM_BYTES, st, tmQKV, tmDO, LSE, static_cast<const float*>(Dv), S, H, NT, scale, amask,
                       kpm, static_cast<bf16*>(DQKV), lddq));
-  CVB_LAUNCH_CHECK();
-  return cvb_det_free(ws, st);
+  return ws.release();
 }

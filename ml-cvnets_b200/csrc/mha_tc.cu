@@ -299,13 +299,11 @@ int cvb_mha_fwd_tc(const void* QKV, int ldq, int B, int S, int H, float scale, c
   const int NCH = (S + 63) / 64;
   const int NQT = (S + 127) / 128;
   CUtensorMap tmQ, tmKV;
-  if (cvb_make_tmap_2d_c64(&tmQ, QKV, (int64_t)B * S, 3 * H * 64, ldq, 128)) return 1;
-  if (cvb_make_tmap_2d_c64(&tmKV, QKV, (int64_t)B * S, 3 * H * 64, ldq, NCH * 64)) return 1;
+  if (cvb_make_tmap_2d(&tmQ, QKV, (int64_t)B * S, 3 * H * 64, ldq, 128, 64)) return 1;
+  if (cvb_make_tmap_2d(&tmKV, QKV, (int64_t)B * S, 3 * H * 64, ldq, NCH * 64, 64)) return 1;
   const size_t smem = (size_t)2 * BOX64 + (size_t)2 * NCH * BOX64 + 1024;
-  static bool attr = false;
-  if (!attr) { CVB_CUDA(cudaFuncSetAttribute(mha_tc_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024)); attr = true; }
+  CVB_CUDA(cvb_smem_optin<mha_tc_fwd_kernel>(96 * 1024));
   CVB_CUDA(cvb_launch(mha_tc_fwd_kernel, B * H * NQT, FW_THREADS, smem, st, tmQ, tmKV, S, NCH, H, NQT, scale, kpm, static_cast<bf16*>(O), ldo, LSE));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -314,14 +312,12 @@ int cvb_mha_bwd_tc(const void* QKV, int ldq, const void* O, const void* DO, int 
   const int NB = (S + 63) / 64;
   const int R = NB * 64;
   CUtensorMap tmQKV, tmDO;
-  if (cvb_make_tmap_2d_c64(&tmQKV, QKV, (int64_t)B * S, 3 * H * 64, ldq, R)) return 1;
-  if (cvb_make_tmap_2d_c64(&tmDO, DO, (int64_t)B * S, H * 64, ldo, R)) return 1;
+  if (cvb_make_tmap_2d(&tmQKV, QKV, (int64_t)B * S, 3 * H * 64, ldq, R, 64)) return 1;
+  if (cvb_make_tmap_2d(&tmDO, DO, (int64_t)B * S, H * 64, ldo, R, 64)) return 1;
   // Q, K, V, dO images + two dS^T images + fp32 dQ + LSE / D
   const size_t smem = (size_t)4 * R * 128 + 2 * BOX64 + (size_t)R * 64 * 4 + (size_t)2 * R * 4 + 1024;
-  static bool attr = false;
-  if (!attr) { CVB_CUDA(cudaFuncSetAttribute(mha_tc_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024)); attr = true; }
+  CVB_CUDA(cvb_smem_optin<mha_tc_bwd_kernel>(224 * 1024));
   CVB_CUDA(cvb_launch(mha_tc_bwd_kernel, B * H, BW_THREADS, smem, st, tmQKV, tmDO, static_cast<const bf16*>(O), static_cast<const bf16*>(DO), ldo, LSE, S,
                       H, NB, scale, kpm, static_cast<bf16*>(DQKV), lddq));
-  CVB_LAUNCH_CHECK();
   return 0;
 }

@@ -598,7 +598,6 @@ extern "C" int cvb_na_plan(const void* key, int B, int enabled, float* tab, cvb_
   CVB_CHECK(key && tab && B > 0 && B <= NA_MAX_B && enabled > 0 && enabled < 8, "cvb_na_plan: bad arguments (1 <= B <= %d, enabled in 1..7)", NA_MAX_B);
   const int n = B / 2 > 1 ? B / 2 : 1;
   CVB_CUDA(cvb_launch(na_plan_kernel, 1, NA_PLAN_NT, 0, static_cast<cudaStream_t>(stream), static_cast<const unsigned long long*>(key), B, n, enabled, tab));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -606,7 +605,6 @@ extern "C" int cvb_na_noise(const void* key, int B, int H, int W, float* eps, cv
   CVB_CHECK(key && eps && B > 0 && H > 0 && W > 0, "cvb_na_noise: bad arguments");
   const int64_t total = (int64_t)B * 3 * H * W;
   CVB_CUDA(cvb_launch(na_noise_kernel, grid_for(total), NA_NT, 0, static_cast<cudaStream_t>(stream), static_cast<const unsigned long long*>(key), total, eps));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -615,7 +613,6 @@ extern "C" int cvb_na_stats(const float* X, const float* mix, const void* key, i
   CVB_CHECK(X && key && mu_x && mu_e && B > 0 && H > 0 && W > 0, "cvb_na_stats: bad arguments");
   CVB_CUDA(cvb_launch(na_stats_kernel, 3 * B, NA_NT, 0, static_cast<cudaStream_t>(stream), X, mix, static_cast<const unsigned long long*>(key), B, H, W,
                       need_eps, mu_x, mu_e));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -624,7 +621,6 @@ extern "C" int cvb_na_compose(const float* tab, const double* mu_x, const double
   CVB_CHECK(tab && mu_x && mu_e && raw && coef && B > 0, "cvb_na_compose: bad arguments");
   if (params_of(raw, &P, "cvb_na_compose")) return 1;
   CVB_CUDA(cvb_launch(na_compose_kernel, grid_for(3 * B), NA_NT, 0, static_cast<cudaStream_t>(stream), tab, mu_x, mu_e, P, B, coef));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -633,7 +629,6 @@ extern "C" int cvb_na_apply(const float* X, const float* mix, const void* key, c
   CVB_CHECK(X && key && coef && Y && sq && B > 0 && H > 0 && W > 0, "cvb_na_apply: bad arguments");
   CVB_CUDA(cvb_launch(na_apply_kernel, 3 * B, NA_NT, 0, static_cast<cudaStream_t>(stream), X, mix, static_cast<const unsigned long long*>(key), coef, B, H, W,
                       need_eps, Y, sq));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -642,7 +637,6 @@ extern "C" int cvb_na_bwd_reduce(const float* DY, const double* g_sq, const floa
   CVB_CHECK(X && key && coef && red && B > 0 && H > 0 && W > 0, "cvb_na_bwd_reduce: bad arguments");
   CVB_CUDA(cvb_launch(na_bwd_reduce_kernel, 3 * B, NA_NT, 0, static_cast<cudaStream_t>(stream), DY, g_sq, X, mix, static_cast<const unsigned long long*>(key),
                       coef, B, H, W, need_eps, red));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -657,7 +651,6 @@ extern "C" int cvb_na_param_grad(const float* tab, const double* mu_x, const dou
     G.raw[j] = grads[j];
   }
   CVB_CUDA(cvb_launch(na_param_grad_kernel, 1, NA_NT, 0, static_cast<cudaStream_t>(stream), tab, mu_x, mu_e, red, P, B, G));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -666,7 +659,6 @@ extern "C" int cvb_na_loss_fwd(const double* sq, int B, int H, int W, const floa
   CVB_CHECK(sq && target && loss && B > 0 && H > 0 && W > 0 && T > 0, "cvb_na_loss_fwd: bad arguments");
   CVB_CUDA(cvb_launch(na_loss_fwd_kernel, 1, NA_NT, 0, static_cast<cudaStream_t>(stream), sq, B, 1.0 / (3.0 * H * W), target, T,
                       reinterpret_cast<const long long*>(step), alpha, w_na, ce, w_ce, loss, parts));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -675,7 +667,6 @@ extern "C" int cvb_na_loss_bwd(const double* sq, int B, int H, int W, const floa
   CVB_CHECK(sq && target && g_sq && B > 0 && H > 0 && W > 0 && T > 0, "cvb_na_loss_bwd: bad arguments");
   CVB_CUDA(cvb_launch(na_loss_bwd_kernel, grid_for(B), NA_NT, 0, static_cast<cudaStream_t>(stream), sq, B, 1.0 / (3.0 * H * W), target, T,
                       reinterpret_cast<const long long*>(step), alpha, w_na, grad_out, grad_scale, g_sq, g_ce, w_ce));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -685,7 +676,6 @@ extern "C" int cvb_stem_dgrad(const void* dz, const void* y, const float* coef, 
   CVB_CHECK(cvb_aligned16(dz) && cvb_aligned16(y) && (reinterpret_cast<uintptr_t>(dX) & 7) == 0, "cvb_stem_dgrad: misaligned operand");
   CVB_CUDA(cvb_launch(stem_dgrad_kernel, grid_for((int64_t)B * Ho * Wo), NA_NT, 0, static_cast<cudaStream_t>(stream), static_cast<const bf16*>(dz),
                       static_cast<const bf16*>(y), coef, static_cast<const bf16*>(w), B, Ho, Wo, C0, dX));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -694,16 +684,11 @@ extern "C" int cvb_patch_stem_dgrad(const void* dz, const void* y, const float* 
   CVB_CHECK(dz && y && coef && w && dX && B > 0 && Ho > 0 && Wo > 0 && C0 >= 16 && C0 <= PS_MAX_C0 && C0 % 16 == 0,
             "cvb_patch_stem_dgrad: bad arguments (C0 a multiple of 16 up to %d)", PS_MAX_C0);
   CVB_CHECK(cvb_aligned16(dz) && cvb_aligned16(y) && cvb_aligned16(dX) && cvb_aligned16(coef), "cvb_patch_stem_dgrad: misaligned operand");
-  static bool attr = false;
-  if (!attr) {
-    CVB_CUDA(cudaFuncSetAttribute(patch_stem_dgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ps_smem(PS_MAX_C0)));
-    attr = true;
-  }
+  CVB_CUDA(cvb_smem_optin<patch_stem_dgrad_kernel>((int)ps_smem(PS_MAX_C0)));
   const int64_t tiles = (int64_t)B * Ho * ((Wo + PS_OWN - 1) / PS_OWN);
   const int64_t want = (tiles + PS_WARPS - 1) / PS_WARPS;
   const int grid = (int)(want < cvb_num_sms() ? want : cvb_num_sms());  // persistent: at most one CTA per SM
   CVB_CUDA(cvb_launch(patch_stem_dgrad_kernel, grid, PS_NT, ps_smem(C0), static_cast<cudaStream_t>(stream), static_cast<const bf16*>(dz),
                       static_cast<const bf16*>(y), coef, static_cast<const bf16*>(w), B, Ho, Wo, C0, dX));
-  CVB_LAUNCH_CHECK();
   return 0;
 }

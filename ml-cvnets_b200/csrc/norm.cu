@@ -41,7 +41,11 @@ __global__ void __launch_bounds__(256) det_add_kernel(const double* __restrict__
     dst[(size_t)r * ld + c] += (float)s[i];
   }
 }
-int cvb_det_alloc(double** scratch, size_t n, cudaStream_t st) {
+DetScratch::~DetScratch() {
+  // an early return: the failure that caused it has set the message, so a failed free here only clears its pending error
+  if (p_ && cudaFreeAsync(p_, st_) != cudaSuccess) (void)cudaGetLastError();
+}
+int DetScratch::alloc(size_t n) {
   static bool pool_set = false;
   if (!pool_set) {  // keep freed scratch in the device's default pool instead of returning it to the driver at every synchronisation
     int dev = 0;
@@ -52,19 +56,20 @@ int cvb_det_alloc(double** scratch, size_t n, cudaStream_t st) {
     CVB_CUDA(cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep));
     pool_set = true;
   }
-  CVB_CUDA(cudaMallocAsync(reinterpret_cast<void**>(scratch), n * sizeof(double), st));
-  CVB_CUDA(cudaMemsetAsync(*scratch, 0, n * sizeof(double), st));
+  CVB_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&p_), n * sizeof(double), st_));
+  CVB_CUDA(cudaMemsetAsync(p_, 0, n * sizeof(double), st_));
   return 0;
 }
-int cvb_det_add(const double* scratch, float* dst, int rows, int cols, int ld, cudaStream_t st) {
+int DetScratch::add(size_t offset, float* dst, int rows, int cols, int ld) {
   const int64_t n = (int64_t)rows * cols;
   const int grid = (int)std::min<int64_t>((n + 255) / 256, 4 * (int64_t)cvb_num_sms());
-  CVB_CUDA(cvb_launch(det_add_kernel, grid, 256, 0, st, scratch, dst, rows, cols, ld));
-  CVB_LAUNCH_CHECK();
+  CVB_CUDA(cvb_launch(det_add_kernel, grid, 256, 0, st_, static_cast<const double*>(p_ + offset), dst, rows, cols, ld));
   return 0;
 }
-int cvb_det_free(double* scratch, cudaStream_t st) {
-  CVB_CUDA(cudaFreeAsync(scratch, st));
+int DetScratch::release() {
+  double* p = p_;
+  p_ = nullptr;
+  CVB_CUDA(cudaFreeAsync(p, st_));
   return 0;
 }
 extern "C" int cvb_device_info(int* sm_count, int* cc_major, int* cc_minor) {
@@ -80,57 +85,36 @@ extern "C" int cvb_device_info(int* sm_count, int* cc_major, int* cc_minor) {
 typedef CUresult (*cvb_encode_tiled_fn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                         const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                         CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static cvb_encode_tiled_fn cvb_get_encoder() {
-  static cvb_encode_tiled_fn fn = nullptr;
-  if (!fn) {
+// bf16 tiled tensor map of `rank` dimensions (innermost first), unit element strides, 128-byte L2 promotion, zero fill out of bounds
+static int encode_bf16(CUtensorMap* map, cuuint32_t rank, const void* base, const cuuint64_t* dims, const cuuint64_t* strides, const cuuint32_t* box,
+                       CUtensorMapSwizzle swizzle) {
+  static cvb_encode_tiled_fn enc = nullptr;
+  if (!enc) {
     void* p = nullptr;
     cudaDriverEntryPointQueryResult q;
     if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<cvb_encode_tiled_fn>(p);
+      enc = reinterpret_cast<cvb_encode_tiled_fn>(p);
   }
-  return fn;
-}
-int cvb_make_tmap_nhwc(CUtensorMap* map, const void* base, int B, int H, int W, int C, int boxH, int boxW, int boxC, int swizzle128) {
-  cvb_encode_tiled_fn enc = cvb_get_encoder();
   CVB_CHECK(enc != nullptr, "cuTensorMapEncodeTiled is not available from the driver");
+  const cuuint32_t estr[4] = {1, 1, 1, 1};
+  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, rank, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                   swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  CVB_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled (%u-D) failed with %d", rank, (int)r);
+  return 0;
+}
+int cvb_make_tmap_nhwc(CUtensorMap* map, const void* base, int B, int H, int W, int C, int boxH, int boxW, int boxC) {
   CVB_CHECK(boxC * 2 <= 128 && boxW <= 256 && boxH <= 256 && C % 8 == 0, "bad TMA box (%d,%d,%d) for C=%d", boxH, boxW, boxC, C);
-  cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
-  cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
-  cuuint32_t box[4] = {(cuuint32_t)boxC, (cuuint32_t)boxW, (cuuint32_t)boxH, 1};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   swizzle128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  CVB_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed with %d", (int)r);
-  return 0;
+  const cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
+  const cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
+  const cuuint32_t box[4] = {(cuuint32_t)boxC, (cuuint32_t)boxW, (cuuint32_t)boxH, 1};
+  return encode_bf16(map, 4, base, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_NONE);
 }
-
-int cvb_make_tmap_2d_k32(CUtensorMap* map, const void* base, int64_t rows, int cols, int ld, int box_rows) {
-  cvb_encode_tiled_fn enc = cvb_get_encoder();
-  CVB_CHECK(enc != nullptr, "cuTensorMapEncodeTiled is not available from the driver");
-  CVB_CHECK(box_rows > 0 && box_rows <= 256 && ld % 8 == 0 && cols > 0 && rows > 0, "bad 2-D TMA box");
-  cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
-  cuuint32_t box[2] = {32, (cuuint32_t)box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  CVB_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled (2-D) failed with %d", (int)r);
-  return 0;
-}
-
-int cvb_make_tmap_2d_c64(CUtensorMap* map, const void* base, int64_t rows, int cols, int ld, int box_rows) {
-  cvb_encode_tiled_fn enc = cvb_get_encoder();
-  CVB_CHECK(enc != nullptr, "cuTensorMapEncodeTiled is not available from the driver");
-  CVB_CHECK(box_rows > 0 && box_rows <= 256 && ld % 8 == 0 && cols > 0 && rows > 0, "bad 2-D TMA box");
-  cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
-  cuuint32_t box[2] = {64, (cuuint32_t)box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  CVB_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled (2-D, 64-column box) failed with %d", (int)r);
-  return 0;
+int cvb_make_tmap_2d(CUtensorMap* map, const void* base, int64_t rows, int cols, int ld, int box_rows, int box_cols) {
+  CVB_CHECK(box_rows > 0 && box_rows <= 256 && (box_cols == 32 || box_cols == 64) && ld % 8 == 0 && cols > 0 && rows > 0, "bad 2-D TMA box");
+  const cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
+  const cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
+  const cuuint32_t box[2] = {(cuuint32_t)box_cols, (cuuint32_t)box_rows};
+  return encode_bf16(map, 2, base, dims, strides, box, box_cols == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B);
 }
 
 namespace {
@@ -826,7 +810,6 @@ extern "C" int cvb_bn_finalize(const double* sum, const double* sq, double count
   CVB_CHECK(sum && sq && mean && rstd && scale && shift && C > 0 && count > 0, "cvb_bn_finalize: bad arguments");
   CVB_CUDA(cvb_launch(bn_finalize_kernel, (C + 127) / 128, 128, 0, static_cast<cudaStream_t>(stream), sum, sq, count, gamma, beta, eps, momentum, running_mean,
                                                                                      running_var, nbt, mean, rstd, scale, shift, C));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -834,7 +817,6 @@ extern "C" int cvb_bn_eval_scale_shift(const float* gamma, const float* beta, co
                                        float* mean, float* rstd, float* scale, float* shift, int C, cvb_stream_t stream) {
   CVB_CHECK(running_mean && running_var && mean && rstd && scale && shift && C > 0, "cvb_bn_eval_scale_shift: bad arguments");
   CVB_CUDA(cvb_launch(bn_eval_kernel, (C + 127) / 128, 128, 0, static_cast<cudaStream_t>(stream), gamma, beta, running_mean, running_var, eps, mean, rstd, scale, shift, C));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -843,7 +825,6 @@ extern "C" int cvb_bn_bwd_finalize(const double* sum_dz, const double* sum_dzy, 
   CVB_CHECK(sum_dz && sum_dzy && mean && rstd && c1 && c2 && c3 && C > 0 && count > 0, "cvb_bn_bwd_finalize: bad arguments");
   CVB_CUDA(cvb_launch(bn_bwd_finalize_kernel, (C + 127) / 128, 128, 0, static_cast<cudaStream_t>(stream), sum_dz, sum_dzy, count, gamma, mean, rstd, eval_mode, dgamma,
                                                                                          dbeta, c1, c2, c3, C));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -853,7 +834,6 @@ extern "C" int cvb_bn_apply(const void* Y, const float* scale, const float* shif
   int64_t nvec = M * (C / 8);
   CVB_CUDA(cvb_launch(bn_apply_kernel, grid_for(nvec), NT, 0, static_cast<cudaStream_t>(stream), static_cast<const bf16*>(Y), scale, shift, act,
                                                                                static_cast<const bf16*>(R), static_cast<bf16*>(OUT), nvec, C / 8));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -870,7 +850,6 @@ extern "C" int cvb_apply_load_mode(const void* A, int lda, const void* A2, int l
   CVB_CUDA(cvb_launch(apply_load_mode_rows_kernel, g.ctas, g.nthreads, 0, static_cast<cudaStream_t>(stream), static_cast<const bf16*>(A),
                       static_cast<const bf16*>(A2), mode, p0, p1, p2, row_mean, row_rstd, rows_per_sample > 0 ? rows_per_sample : 1,
                       static_cast<bf16*>(OUT), (int)M, g.cgs, g.rpp, g.rows_per_cta, lda, lda2, ldo));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -883,7 +862,6 @@ extern "C" int cvb_bn_bwd_reduce(const void* DOUT, const void* Y, const float* s
   CVB_CUDA(cvb_launch(bn_bwd_reduce_kernel, dim3(g.ctas, (C + CH_CHUNK - 1) / CH_CHUNK), g.nthreads, 2 * nc * sizeof(double),
       static_cast<cudaStream_t>(stream), static_cast<const bf16*>(DOUT), static_cast<const bf16*>(Y), scale, shift, act, static_cast<bf16*>(DZ), sum_dz,
       sum_dzy, M, C, g.rows_per_cta));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -891,7 +869,6 @@ extern "C" int cvb_gn_finalize(const double* samp_sum, const double* samp_sq, do
                                cvb_stream_t stream) {
   CVB_CHECK(samp_sum && samp_sq && mean && rstd && B > 0 && count > 0, "cvb_gn_finalize: bad arguments");
   CVB_CUDA(cvb_launch(gn_finalize_kernel, (B + 127) / 128, 128, 0, static_cast<cudaStream_t>(stream), samp_sum, samp_sq, count, eps, mean, rstd, B));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -902,7 +879,6 @@ extern "C" int cvb_gn_stats(const void* X, int ldx, int B, int rows_per_sample, 
   if (chunks < 1) chunks = 1;
   CVB_CUDA(cvb_launch(gn_stats_kernel, B * chunks, NT, 0, static_cast<cudaStream_t>(stream), static_cast<const bf16*>(X), ldx, rows_per_sample, C, chunks, samp_sum,
                                                                            samp_sq));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -917,7 +893,6 @@ extern "C" int cvb_ln_bwd(const void* V, const void* X, const float* mean, const
   CVB_CUDA(cvb_launch(C <= 1024 ? ln_bwd_kernel<4> : ln_bwd_kernel<LNB_MAXCH>, (unsigned)ctas, NT, (size_t)4 * C * sizeof(float), static_cast<cudaStream_t>(stream), static_cast<const bf16*>(V),
                       static_cast<const bf16*>(X), mean, rstd, gamma, static_cast<const bf16*>(DRES), static_cast<bf16*>(DX), M, C, dgamma, dbeta,
                       col_sum));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -925,7 +900,6 @@ extern "C" int cvb_act_fwd(const void* X, void* Y, int64_t n, int kind, cvb_stre
   CVB_CHECK(X && Y && n > 0 && n % 8 == 0 && cvb_aligned16(X) && cvb_aligned16(Y) && kind >= CVB_ACT_SILU && kind <= CVB_ACT_SIGMOID,
             "cvb_act_fwd: bad arguments");
   CVB_CUDA(cvb_launch(act_fwd_kernel, grid_for(n / 8), NT, 0, static_cast<cudaStream_t>(stream), static_cast<const bf16*>(X), static_cast<bf16*>(Y), n / 8, kind));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 extern "C" int cvb_act_bwd(const void* DY, const void* X, void* DX, int64_t n, int kind, cvb_stream_t stream) {
@@ -934,7 +908,6 @@ extern "C" int cvb_act_bwd(const void* DY, const void* X, void* DX, int64_t n, i
             "cvb_act_bwd: bad arguments");
   CVB_CUDA(cvb_launch(act_bwd_kernel, grid_for(n / 8), NT, 0, static_cast<cudaStream_t>(stream), static_cast<const bf16*>(DY), static_cast<const bf16*>(X),
                       static_cast<bf16*>(DX), n / 8, kind));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -943,7 +916,6 @@ extern "C" int cvb_ln_stats(const void* X, int ldx, int64_t M, int C, float eps,
   const int rows_per_cta = NT / 32;
   CVB_CUDA(cvb_launch(ln_stats_kernel, (unsigned)((M + rows_per_cta - 1) / rows_per_cta), NT, 0, static_cast<cudaStream_t>(stream),
                       static_cast<const bf16*>(X), ldx, M, C, eps, mean, rstd));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -956,7 +928,6 @@ extern "C" int cvb_gn_bwd_apply(const void* G, const void* X, const float* mean,
   CVB_CUDA(cvb_launch(gn_bwd_apply_kernel, g.ctas, g.nthreads, col_sum ? g.rpp * C * sizeof(float) : 0, static_cast<cudaStream_t>(stream),
       static_cast<const bf16*>(G), static_cast<const bf16*>(X), mean, rstd, sg, sgx, count, static_cast<const bf16*>(DRES), static_cast<bf16*>(DX), M,
       rows_per_sample, C, col_sum, g.cgs, g.rpp, g.rows_per_cta, static_cast<const float*>(nullptr)));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -976,13 +947,11 @@ extern "C" int cvb_gn_bwd(const void* V, const void* X, const float* mean, const
   CVB_CUDA(cvb_launch(gn_bwd_stats_kernel, dim3(chunks, B), nthreads1, 2 * C * sizeof(double), static_cast<cudaStream_t>(stream),
                       static_cast<const bf16*>(V), static_cast<const bf16*>(X), mean, rstd, gamma, rows_per_sample, C, g1.cgs, g1.rpp, rows_per_cta, dgamma,
                       dbeta, samp_ws, samp_ws + B));
-  CVB_LAUNCH_CHECK();
   RowGeom g = row_geom(M, C);
   CVB_CUDA(cvb_launch(gn_bwd_apply_kernel, g.ctas, g.nthreads, 0, static_cast<cudaStream_t>(stream), static_cast<const bf16*>(V),
                       static_cast<const bf16*>(X), mean, rstd, static_cast<const double*>(samp_ws), static_cast<const double*>(samp_ws + B), count,
                       static_cast<const bf16*>(DRES), static_cast<bf16*>(DX), M, rows_per_sample, C, static_cast<double*>(nullptr), g.cgs, g.rpp,
                       g.rows_per_cta, gamma));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -993,7 +962,6 @@ extern "C" int cvb_global_pool_fwd(const void* X, int B, int HW, int C, void* OU
   int rpp = NT / cgs; if (rpp < 1) rpp = 1;
   CVB_CUDA(cvb_launch(pool_fwd_kernel, dim3(B, (C + CH_CHUNK - 1) / CH_CHUNK), cgs * rpp, nc * sizeof(double), static_cast<cudaStream_t>(stream),
                       static_cast<const bf16*>(X), HW, C, static_cast<bf16*>(OUT)));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -1001,7 +969,6 @@ extern "C" int cvb_global_pool_bwd(const void* DOUT, int B, int HW, int C, void*
   CVB_CHECK(DOUT && DX && B > 0 && HW > 0 && C > 0 && C % 8 == 0, "cvb_global_pool_bwd: bad arguments");
   int64_t nvec = (int64_t)B * HW * (C / 8);
   CVB_CUDA(cvb_launch(pool_bwd_kernel, grid_for(nvec), NT, 0, static_cast<cudaStream_t>(stream), static_cast<const bf16*>(DOUT), HW, C, static_cast<bf16*>(DX), nvec));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -1011,7 +978,6 @@ extern "C" int cvb_stem_im2col(const float* X, int64_t sxn, int64_t sxc, int64_t
   int64_t total = (int64_t)B * (H / 2) * (W / 2) * 4;
   CVB_CUDA(cvb_launch(stem_im2col_kernel, grid_for(total), NT, 0, static_cast<cudaStream_t>(stream), X, sxn, sxc, sxh, sxw, B, H, W, static_cast<bf16*>(A),
                       mix));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -1022,13 +988,11 @@ extern "C" int cvb_prep_weights(const cvb_prep_desc* descs_device, int n_desc, i
   if (gx > 64) gx = 64;
   dim3 grid(gx, n_desc);
   CVB_CUDA(cvb_launch(prep_weights_kernel, grid, NT, 0, static_cast<cudaStream_t>(stream), descs_device));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
 extern "C" int cvb_unprep_grad(const float* src, float* dst, int rows, int cols, int lds, int kind, int rot, cvb_stream_t stream) {
   CVB_CHECK(src && dst && rows > 0 && cols > 0, "cvb_unprep_grad: bad arguments");
   CVB_CUDA(cvb_launch(unprep_grad_kernel, grid_for((int64_t)rows * cols), NT, 0, static_cast<cudaStream_t>(stream), src, dst, rows, cols, lds, kind, rot));
-  CVB_LAUNCH_CHECK();
   return 0;
 }

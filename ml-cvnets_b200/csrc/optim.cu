@@ -188,7 +188,6 @@ extern "C" int cvb_grad_norm_blocks(int64_t n) {
 extern "C" int cvb_grad_norm(const float* grads, int64_t n, const float* scale, float grad_div, float* stats, float* partials, cvb_stream_t stream) {
   CVB_CHECK(grads && scale && stats && partials && n > 0 && grad_div > 0.f && cvb_aligned16(grads), "cvb_grad_norm: bad arguments");
   CVB_CUDA(cvb_launch(grad_norm_kernel, cvb_grad_norm_blocks(n), ONT, 0, static_cast<cudaStream_t>(stream), grads, n, scale, grad_div, stats, partials));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -203,7 +202,6 @@ extern "C" int cvb_adamw_step(float* params, const float* grads, float* exp_avg,
   CVB_CUDA(cvb_launch(adamw_step_kernel, blocks, ONT, 0, static_cast<cudaStream_t>(stream), params, grads, exp_avg, exp_avg_sq, weight_decay, n, hp, beta1,
                       beta2, eps, max_norm, stats, scale, step, growth_factor, backoff_factor, growth_interval, ema, ema_momentum, partials,
                       cvb_grad_norm_blocks(n)));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -218,6 +216,5 @@ extern "C" int cvb_sgd_step(float* params, const float* grads, float* momentum_b
   CVB_CUDA(cvb_launch(sgd_step_kernel, blocks, ONT, 0, static_cast<cudaStream_t>(stream), params, grads, momentum_buf, weight_decay, n, hp, momentum,
                       nesterov, max_norm, stats, scale, step, growth_factor, backoff_factor, growth_interval, ema, ema_momentum, partials,
                       cvb_grad_norm_blocks(n)));
-  CVB_LAUNCH_CHECK();
   return 0;
 }

@@ -5,7 +5,7 @@
 //
 // Pure bandwidth: one pass over the map with 16-byte accesses.  A CTA owns a strip of pixels of one sample and a chunk of at most 2048
 // channels; a thread keeps one 8-channel group, so its scale vector and its DS partial stay in registers.  The DS partials of a CTA's pixel
-// lanes are summed in a fixed order in shared memory, and the CTAs' sums meet in an fp64 scratch (cvb_det_alloc), so DS is reproducible
+// lanes are summed in a fixed order in shared memory, and the CTAs' sums meet in an fp64 scratch (DetScratch), so DS is reproducible
 // run to run.  The pooled vector / the two 1x1 convs of the SE unit are the library's pool and GEMM kernels.
 #include "common.cuh"
 
@@ -89,7 +89,6 @@ int se_geometry(const char* who, int B, int HW, int C, int* rows_per_cta, int* s
 int se_bwd_launch(const void* DY, const void* X, const void* S, void* DX, double* ws, int B, int HW, int C, int rpc, int strips, cudaStream_t st) {
   CVB_CUDA(cvb_launch(se_scale_bwd_kernel, dim3(strips, B, (C + SE_CHUNK - 1) / SE_CHUNK), SE_NT, 0, st, static_cast<const bf16*>(DY),
                       static_cast<const bf16*>(X), static_cast<const bf16*>(S), static_cast<bf16*>(DX), ws, HW, C, rpc));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -101,7 +100,6 @@ extern "C" int cvb_se_scale_fwd(const void* X, const void* S, void* Y, int B, in
   CVB_CHECK(X && S && Y && cvb_aligned16(X) && cvb_aligned16(S) && cvb_aligned16(Y), "cvb_se_scale_fwd: null / misaligned operand");
   CVB_CUDA(cvb_launch(se_scale_fwd_kernel, dim3(strips, B, (C + SE_CHUNK - 1) / SE_CHUNK), SE_NT, 0, static_cast<cudaStream_t>(stream), static_cast<const bf16*>(X),
                       static_cast<const bf16*>(S), static_cast<bf16*>(Y), HW, C, rpc));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -111,10 +109,10 @@ extern "C" int cvb_se_scale_bwd(const void* DY, const void* X, const void* S, vo
   CVB_CHECK(DY && X && S && DX && DS && cvb_aligned16(DY) && cvb_aligned16(X) && cvb_aligned16(S) && cvb_aligned16(DX),
             "cvb_se_scale_bwd: null / misaligned operand");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  double* ws = nullptr;
-  if (cvb_det_alloc(&ws, (size_t)B * C, st)) return 2;
-  int rc = se_bwd_launch(DY, X, S, DX, ws, B, HW, C, rpc, strips, st);
-  if (rc == 0) rc = cvb_det_add(ws, DS, B, C, C, st);
-  const int rf = cvb_det_free(ws, st);
-  return rc ? rc : rf;
+  DetScratch ws(st);
+  if (ws.alloc((size_t)B * C)) return 2;
+  const int rc = se_bwd_launch(DY, X, S, DX, ws.data(), B, HW, C, rpc, strips, st);
+  if (rc) return rc;
+  if (ws.add(0, DS, B, C, C)) return 2;
+  return ws.release();
 }

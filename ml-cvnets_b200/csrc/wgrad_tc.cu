@@ -7,7 +7,7 @@
 // every activation / gradient element is read ONCE per (N-block, K-block) instead of once per 64x64 tile (the mma.sync kernel is
 // L2-bandwidth bound on exactly that re-reading).  Warp roles:
 //   warps 0-7   consumers     : 4 x wgmma.m64nKBk16 (K = 16 pixels each) per stage, both operands MN-major; after the last stage
-//                               fp64 reductions of the accumulator registers into the dW scratch (see cvb_det_alloc)
+//                               fp64 reductions of the accumulator registers into the dW scratch (see DetScratch)
 //   warp 8      TMA producer  : per stage [64 pixels] x {G: 128 ch (+ G2 for BN-backward), A: <=128 ch}, 64-channel boxes
 //   warps 9-16  transform     : in-place operand prologues in shared memory (BN-backward on G, BN+SiLU / SiLU / GroupNorm on A),
 //                               bias-gradient column sums, fence.proxy.async, hand the stage to the consumers
@@ -223,17 +223,12 @@ int launch_wgrad_tc(const cvb_wgrad_args& a, cudaStream_t st) {
   splits = (a.M + m_per_cta - 1) / m_per_cta;
   const size_t smem = (size_t)nst * stage_bytes + 1024;
   CUtensorMap tmG, tmG2, tmA;
-  if (cvb_make_tmap_2d_c64(&tmG, a.G, a.M, a.N, a.ldg, WT_BMP)) return 1;
-  if (cvb_make_tmap_2d_c64(&tmG2, GMODE == CVB_A_BNB ? a.G2 : a.G, a.M, a.N, GMODE == CVB_A_BNB ? a.ldg2 : a.ldg, WT_BMP)) return 1;
-  if (cvb_make_tmap_2d_c64(&tmA, a.A, a.M, a.K, a.lda, WT_BMP)) return 1;
-  static bool attr = false;
-  if (!attr) {
-    CVB_CUDA(cudaFuncSetAttribute(pw_wgrad_tc_kernel<GMODE, AMODE, KB>, cudaFuncAttributeMaxDynamicSharedMemorySize, 216 * 1024));
-    attr = true;
-  }
+  if (cvb_make_tmap_2d(&tmG, a.G, a.M, a.N, a.ldg, WT_BMP, 64)) return 1;
+  if (cvb_make_tmap_2d(&tmG2, GMODE == CVB_A_BNB ? a.G2 : a.G, a.M, a.N, GMODE == CVB_A_BNB ? a.ldg2 : a.ldg, WT_BMP, 64)) return 1;
+  if (cvb_make_tmap_2d(&tmA, a.A, a.M, a.K, a.lda, WT_BMP, 64)) return 1;
+  CVB_CUDA(cvb_smem_optin<pw_wgrad_tc_kernel<GMODE, AMODE, KB>>(216 * 1024));
   dim3 grid(nb, kb, splits);
   CVB_CUDA(cvb_launch(pw_wgrad_tc_kernel<GMODE, AMODE, KB>, grid, WT_THREADS, smem, st, tmG, tmG2, tmA, a, m_per_cta, nst, stage_bytes));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 

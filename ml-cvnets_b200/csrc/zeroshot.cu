@@ -151,7 +151,6 @@ extern "C" int cvb_zs_class_embed(const void* X, int ldx, int R, const int* perm
             "cvb_zs_class_embed: bad arguments (d %% 8 == 0, d <= %d, ldx >= d, ldx %% 8 == 0, 16-byte aligned rows)", CE_MAX_CHUNK * 256);
   CVB_CUDA(cvb_launch(zs_class_embed_kernel, (Cl + CE_WARPS - 1) / CE_WARPS, CE_WARPS * 32, 0, static_cast<cudaStream_t>(stream),
                       static_cast<const bf16*>(X), ldx, R, perm, Cl, M, d, table));
-  CVB_LAUNCH_CHECK();
   return 0;
 }
 
@@ -160,9 +159,8 @@ extern "C" int cvb_zs_logits_topk(const void* img, int ldi, const float* table, 
   CVB_CHECK(img && table && B > 0 && d > 0 && d <= 4096 && ldi >= d && Cl > 0, "cvb_zs_logits_topk: bad arguments (d <= 4096, ldi >= d)");
   CVB_CHECK(logits || (targets && hits), "cvb_zs_logits_topk: nothing to compute (no logits output, no targets + hits)");
   const size_t smem = sizeof(float) * LT_ROWS * d;
-  if (smem > 48 * 1024) CVB_CUDA(cudaFuncSetAttribute(zs_logits_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  if (smem > 48 * 1024) CVB_CUDA(cvb_smem_optin<zs_logits_topk_kernel>((int)sizeof(float) * LT_ROWS * 4096));  // the largest d
   CVB_CUDA(cvb_launch(zs_logits_topk_kernel, (B + LT_ROWS - 1) / LT_ROWS, LT_THREADS, smem, static_cast<cudaStream_t>(stream),
                       static_cast<const bf16*>(img), ldi, table, B, d, Cl, scale, targets, logits, reinterpret_cast<unsigned long long*>(hits)));
-  CVB_LAUNCH_CHECK();
   return 0;
 }

@@ -105,6 +105,24 @@ def test_apply_load_mode_rejects_shapes_past_its_row_kernel():
         lib.cvb_apply_load_mode(p, 64, None, 0, _lib.A_AFF, p, p, None, None, None, 0, p, 64, 1 << 31, 64, None)
 
 
+@pytest.mark.parametrize("mode, given, msg", [
+    ("A_AFF", {"a_p0": 256}, r"cvb_pw_gemm: load mode 1 needs p0/p1$"),
+    ("A_GN", {"row_mean": 256, "row_rstd": 256, "rows_per_sample": 64}, r"cvb_pw_gemm: load mode 4 needs p0/p1$"),
+    ("A_BNB", {"A2": 256, "lda2": 64, "a_p0": 256, "a_p1": 256}, r"cvb_pw_gemm: BNB needs A2 and p0/p1/p2$"),
+])
+def test_pw_gemm_rejects_a_load_mode_without_its_parameters(mode, given, msg):
+    """cvb_pw_gemm checks a load mode's per-channel vectors (and BNB's second operand) once, before any CUDA call and before it picks
+    a kernel."""
+    import ctypes
+    import __graft_entry__ as ge
+    ge.build()
+    from ml_cvnets_b200 import _lib
+    p = 256  # a 16-byte-aligned address that is never dereferenced
+    args = _lib.cvb_gemm_args(M=128, N=64, K=64, A=p, lda=64, a_mode=getattr(_lib, mode), W=p, ldw=64, C=p, ldc=64, **given)
+    with pytest.raises(_lib.CvbError, match=msg):
+        _lib.load().cvb_pw_gemm(ctypes.byref(args), None)
+
+
 def test_state_dict_contract_and_signatures(golden_dir):
     import ml_cvnets_b200 as m
     with open(os.path.join(golden_dir, "state_dict_contract.json")) as f:

@@ -1,7 +1,7 @@
 """Bitwise run-to-run reproducibility (-m gpu), at the grid sizes training uses.
 
 A MobileViTv2 training step is meant to be bitwise reproducible: every reduction that several CTAs add into sums fp32 partials in fp64, and
-weight gradients meet in an fp64 scratch (cvb_det_alloc / cvb_det_add).  One last-bit difference flips a bf16 rounding somewhere in the
+weight gradients meet in an fp64 scratch (DetScratch in csrc/common.cuh).  One last-bit difference flips a bf16 rounding somewhere in the
 network, and AdamW turns the noise gradients of analytically-zero parameters into +-lr steps, so "close" is not enough: two runs must be
 torch.equal.
 
