@@ -408,8 +408,11 @@ __global__ void __launch_bounds__(NT) gn_bwd_stats_kernel(const bf16* __restrict
 // LayerNorm backward in ONE pass (a "sample" is a single token row, so both phases of the GroupNorm backward fit in a warp):
 //   g = v * gamma;  dx = rstd * (g - mean_c(g) - xhat * mean_c(g * xhat)) + dres;   dbeta += v;  dgamma += v * xhat;  col_sum += dx
 // (autograd of nn.LayerNorm, cvnets/layers/normalization/layer_norm.py:14-72).  One warp per row, rows grid-strided; the per-channel
-// sums live in shared memory and are flushed once per CTA.  A row stays in registers: lane owns 8-channel chunks lane, lane+32, ..., MAXCH of
-// them, so C <= 256 * MAXCH.  MAXCH = 4 serves C <= 1024; MAXCH = 5 the 1280-wide ViT-H rows (the widest LayerNorm of any recipe).
+// sums live in shared memory, one slice per warp, and are flushed once per CTA.  A row stays in registers: lane owns 8-channel chunks lane,
+// lane+32, ..., MAXCH of them, so C <= 256 * MAXCH.  MAXCH = 4 serves C <= 1024; MAXCH = 5 the 1280-wide ViT-H rows (the widest LayerNorm of
+// any recipe).  Every channel of a warp's slice has one owning lane, which adds its rows in grid order, and the CTA adds the slices in warp
+// order before one fp64 atomic per channel: dgamma / dbeta / the column sums are bitwise the same run to run (shared-memory float atomics,
+// whose order depends on warp scheduling, made them differ in the last bits and a TrainStep of the MobileViT-v1 models non-reproducible).
 constexpr int LNB_MAXCH = 5;
 template <int MAXCH>
 __global__ void __launch_bounds__(NT) ln_bwd_kernel(const bf16* __restrict__ V, const bf16* __restrict__ X, const float* __restrict__ mean,
@@ -417,10 +420,12 @@ __global__ void __launch_bounds__(NT) ln_bwd_kernel(const bf16* __restrict__ V, 
                                                     bf16* __restrict__ DX, int64_t M, int C, double* dgamma, double* dbeta, double* col_sum) {
   pdl_wait();
   pdl_trigger();
-  extern __shared__ float sred[];  // [3][C] per-channel sums of the CTA (dbeta, dgamma, column sums of DX) + [C] gamma
-  float* sgam = sred + 3 * C;
+  constexpr int NW = NT / 32;
+  extern __shared__ float sred[];  // [NW][3][C] per-warp per-channel sums (dbeta, dgamma, column sums of DX) + [C] gamma
+  float* sgam = sred + NW * 3 * C;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  for (int i = tid; i < 3 * C; i += NT) sred[i] = 0.f;
+  float* wred = sred + warp * 3 * C;  // this warp's slice: [element][chunk] layout, the 32 lanes of an update hit 32 different banks
+  for (int i = tid; i < NW * 3 * C; i += NT) sred[i] = 0.f;
   for (int i = tid; i < C; i += NT) sgam[i] = gamma[i];
   __syncthreads();
   const int nch = C / 8;
@@ -451,8 +456,8 @@ __global__ void __launch_bounds__(NT) ln_bwd_kernel(const bf16* __restrict__ V, 
 #pragma unroll
         for (int e = 0; e < 8; ++e) {
           xh[q][e] = (xh[q][e] - mu) * rs;
-          atomicAdd(&sred[e * nch + ch], v[q][e]);  // [element][chunk] layout: the 32 lanes of a reduction hit 32 different banks
-          atomicAdd(&sred[C + e * nch + ch], v[q][e] * xh[q][e]);
+          wred[e * nch + ch] += v[q][e];
+          wred[C + e * nch + ch] += v[q][e] * xh[q][e];
           v[q][e] *= gq[e];  // from here on v holds g = V * gamma
           s1 += v[q][e];
           s2 = fmaf(v[q][e], xh[q][e], s2);
@@ -472,7 +477,7 @@ __global__ void __launch_bounds__(NT) ln_bwd_kernel(const bf16* __restrict__ V, 
           float o = rs * (v[q][e] - s1 - xh[q][e] * s2);
           if (DRES) o += d[e];
           d[e] = o;
-          if (col_sum) atomicAdd(&sred[2 * C + e * nch + ch], o);
+          if (col_sum) wred[2 * C + e * nch + ch] += o;
         }
         stg16(DX + row * C + ch * 8, pack8(d));
       }
@@ -481,9 +486,15 @@ __global__ void __launch_bounds__(NT) ln_bwd_kernel(const bf16* __restrict__ V, 
   __syncthreads();
   for (int i = tid; i < C; i += NT) {
     const int t = (i & 7) * (C / 8) + (i >> 3);  // channel i lives at [element i % 8][chunk i / 8]
-    atomicAdd(dbeta + i, (double)sred[t]);
-    atomicAdd(dgamma + i, (double)sred[C + t]);
-    if (col_sum) atomicAdd(col_sum + i, (double)sred[2 * C + t]);
+    float b = 0.f, g = 0.f, s = 0.f;
+    for (int w = 0; w < NW; ++w) {
+      b += sred[w * 3 * C + t];
+      g += sred[w * 3 * C + C + t];
+      s += sred[w * 3 * C + 2 * C + t];
+    }
+    atomicAdd(dbeta + i, (double)b);
+    atomicAdd(dgamma + i, (double)g);
+    if (col_sum) atomicAdd(col_sum + i, (double)s);
   }
 }
 
@@ -890,7 +901,11 @@ extern "C" int cvb_ln_bwd(const void* V, const void* X, const float* mean, const
   int64_t ctas = (M + NT / 32 - 1) / (NT / 32);
   const int64_t cap = 4 * (int64_t)cvb_num_sms();
   if (ctas > cap) ctas = cap;
-  CVB_CUDA(cvb_launch(C <= 1024 ? ln_bwd_kernel<4> : ln_bwd_kernel<LNB_MAXCH>, (unsigned)ctas, NT, (size_t)4 * C * sizeof(float), static_cast<cudaStream_t>(stream), static_cast<const bf16*>(V),
+  // per-warp sums + gamma: 100 C bytes (125 KB at the widest C); the opt-in covers every supported C
+  const int smem = (3 * (NT / 32) + 1) * C * (int)sizeof(float), smem_max = (3 * (NT / 32) + 1) * 256 * LNB_MAXCH * (int)sizeof(float);
+  CVB_CUDA(cvb_smem_optin<ln_bwd_kernel<4>>(smem_max));
+  CVB_CUDA(cvb_smem_optin<ln_bwd_kernel<LNB_MAXCH>>(smem_max));
+  CVB_CUDA(cvb_launch(C <= 1024 ? ln_bwd_kernel<4> : ln_bwd_kernel<LNB_MAXCH>, (unsigned)ctas, NT, (size_t)smem, static_cast<cudaStream_t>(stream), static_cast<const bf16*>(V),
                       static_cast<const bf16*>(X), mean, rstd, gamma, static_cast<const bf16*>(DRES), static_cast<bf16*>(DX), M, C, dgamma, dbeta,
                       col_sum));
   return 0;

@@ -398,18 +398,34 @@ def mobilevit_block_v1(P: Params, pre: str, x: Tensor, *, n_blocks: int, num_hea
     return conv_layer_2d(P, pre + ".fusion", torch.cat((res, fm), dim=1), training=training)
 
 
-def mobilevit_v1_forward(P: Params, x: Tensor, *, mode: str = "xx_small", training: bool = True) -> Tensor:
-    """MobileViT.forward (mobilevit.py:19-300 + base_image_encoder.py:261-301), every dropout p = 0."""
+def mobilevit_v1_layout(mode: str = "xx_small") -> List[Tuple[str, str, Dict]]:
+    """Stage wiring of MobileViT.__init__/_make_layer (mobilevit.py:19-300) as a flat list of (kind, state_dict prefix, kwargs):
+    the stem, the InvertedResiduals and MobileViTBlocks, and conv_1x1_exp (part of extract_features, before the classifier)."""
     _, _, _, mits = MIT_MODES[mode]
-    x = conv_layer_2d(P, "conv_1", x, stride=2, training=training)
-    x = inverted_residual(P, "layer_1.0", x, stride=1, training=training)
-    for i in range(3):
-        x = inverted_residual(P, f"layer_2.{i}", x, stride=2 if i == 0 else 1, training=training)
+    out: List[Tuple[str, str, Dict]] = [("stem", "conv_1", {}), ("ir", "layer_1.0", {"stride": 1})]
+    out += [("ir", f"layer_2.{i}", {"stride": 2 if i == 0 else 1}) for i in range(3)]
     for li, (_, _, _, n) in enumerate(mits):
-        x = inverted_residual(P, f"layer_{3 + li}.0", x, stride=2, training=training)
-        x = mobilevit_block_v1(P, f"layer_{3 + li}.1", x, n_blocks=n, training=training)
-    x = conv_layer_2d(P, "conv_1x1_exp", x, training=training)
-    return F.linear(x.mean(dim=[-2, -1]), P["classifier.fc.weight"], P["classifier.fc.bias"])
+        out += [("ir", f"layer_{3 + li}.0", {"stride": 2}), ("mvit", f"layer_{3 + li}.1", {"n_blocks": n})]
+    out.append(("exp", "conv_1x1_exp", {}))
+    return out
+
+
+def mobilevit_v1_forward(P: Params, x: Tensor, *, mode: str = "xx_small", training: bool = True, return_stages: bool = False):
+    """MobileViT.forward (mobilevit.py:19-300 + base_image_encoder.py:261-301), every dropout p = 0.  ``return_stages``: also the output of
+    every entry of ``mobilevit_v1_layout``, keyed by its prefix."""
+    stages = {}
+    for kind, pre, kw in mobilevit_v1_layout(mode):
+        if kind == "stem":
+            x = conv_layer_2d(P, pre, x, stride=2, training=training)
+        elif kind == "ir":
+            x = inverted_residual(P, pre, x, stride=kw["stride"], training=training)
+        elif kind == "mvit":
+            x = mobilevit_block_v1(P, pre, x, n_blocks=kw["n_blocks"], training=training)
+        else:
+            x = conv_layer_2d(P, pre, x, training=training)
+        stages[pre] = x
+    logits = F.linear(x.mean(dim=[-2, -1]), P["classifier.fc.weight"], P["classifier.fc.bias"])
+    return (logits, stages) if return_stages else logits
 
 
 # --------------------------------------------------------------------------------------------

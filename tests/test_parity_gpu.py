@@ -18,6 +18,7 @@ re-normalisations of a randomly initialised net.  So the tests assert three thin
 """
 import json
 import os
+from types import SimpleNamespace
 
 import pytest
 import torch
@@ -46,9 +47,18 @@ def cosine(a, b):
     return float(torch.dot(a, b) / (a.norm() * b.norm() + 1e-30))
 
 
-def _setup(pkg, seed, width=1.0):
-    model = pkg.MobileViTv2(pkg.default_opts(width_multiplier=width))
-    P = O.seeded_fill_(O.mobilevit_v2_shapes(width), seed)
+def mobilevit_v2_arch(width=1.0):
+    """what the parity measurements need of a model family: its drop-in model, its parameter shapes, its oracle forward (with
+    ``return_stages``) and its stage layout -- here MobileViTv2 at one width"""
+    return SimpleNamespace(build=lambda pkg: pkg.MobileViTv2(pkg.default_opts(width_multiplier=width)), shapes=lambda: O.mobilevit_v2_shapes(width),
+                           forward=lambda P, x, **kw: O.mobilevit_v2_forward(P, x, width_multiplier=width, **kw),
+                           layout=lambda: O.mobilevit_v2_layout(width))
+
+
+def _setup(pkg, seed, width=1.0, arch=None):
+    arch = arch or mobilevit_v2_arch(width)
+    model = arch.build(pkg)
+    P = O.seeded_fill_(arch.shapes(), seed)
     model.load_state_dict(P, strict=True)
     return model.cuda(), P
 
@@ -63,10 +73,12 @@ def _record(name, d):
         pass
 
 
-def train_parity_record(pkg, B, width=1.0):
+def train_parity_record(pkg, B, width=1.0, arch=None):
     """One train-mode forward / backward of ours, the fp32 oracle and the oracle under torch bf16 autocast on the same seeded batch:
-    the record of their distances, and the per-parameter tuples of the parameters carrying a non-negligible share of the gradient."""
-    model, P = _setup(pkg, 2024, width)
+    the record of their distances, and the per-parameter tuples of the parameters carrying a non-negligible share of the gradient.
+    ``arch``: the model family (``mobilevit_v2_arch``); MobileViTv2 at ``width`` when not given."""
+    arch = arch or mobilevit_v2_arch(width)
+    model, P = _setup(pkg, 2024, arch=arch)
     model.train()
     x = O.seeded_input((B, 3, 256, 256), 31).cuda()
     y = (torch.arange(B, device="cuda") * 37) % 1000
@@ -80,7 +92,7 @@ def train_parity_record(pkg, B, width=1.0):
     torch.cuda.empty_cache()
     # truth: fp32 oracle on this GPU
     P32 = O.clone_params(P, device="cuda")
-    l32 = O.mobilevit_v2_forward(P32, x, width_multiplier=width, training=True)
+    l32 = arch.forward(P32, x, training=True)
     loss32 = F.cross_entropy(l32, y, label_smoothing=0.1)
     loss32.backward()
     g32 = {k: v.grad.detach().clone() for k, v in P32.items() if v.requires_grad and v.grad is not None}
@@ -91,7 +103,7 @@ def train_parity_record(pkg, B, width=1.0):
     # same-precision comparator: the oracle under torch bf16 autocast
     Pa = O.clone_params(P, device="cuda")
     with torch.autocast("cuda", dtype=torch.bfloat16):
-        la = O.mobilevit_v2_forward(Pa, x, width_multiplier=width, training=True)
+        la = arch.forward(Pa, x, training=True)
         lossa = F.cross_entropy(la, y, label_smoothing=0.1)
     lossa.backward()
     ga = {k: v.grad.detach().float().clone() for k, v in Pa.items() if v.requires_grad and v.grad is not None}
@@ -160,16 +172,18 @@ def test_benchmark_config_eval_parity(pkg):
     assert top1 >= 0.95, rec
 
 
-def stagewise_record(pkg, width=1.0, B=128):
-    """Each module fed the fp32 oracle's input of its stage, train mode at 256x256: rel-L2 of its output against the oracle's, per stage."""
-    model, P = _setup(pkg, 2024, width)
+def stagewise_record(pkg, width=1.0, B=128, arch=None):
+    """Each module fed the fp32 oracle's input of its stage, train mode at 256x256: rel-L2 of its output against the oracle's, per stage.
+    ``arch``: the model family (``mobilevit_v2_arch``); MobileViTv2 at ``width`` when not given."""
+    arch = arch or mobilevit_v2_arch(width)
+    model, P = _setup(pkg, 2024, arch=arch)
     model.train()
     model.fuse_boundaries = False
     x = O.seeded_input((B, 3, 256, 256), 31).cuda()
     Pg = O.clone_params(P, requires_grad=False, device="cuda")
     with torch.no_grad():
-        ref_logits, stages = O.mobilevit_v2_forward(Pg, x, width_multiplier=width, training=True, return_stages=True)
-        names = [pre for _, pre, _ in O.mobilevit_v2_layout(width)]
+        ref_logits, stages = arch.forward(Pg, x, training=True, return_stages=True)
+        names = [pre for _, pre, _ in arch.layout()]
         rec, prev = {}, x
         for pre in names:
             mod = model

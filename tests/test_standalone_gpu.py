@@ -265,8 +265,15 @@ def test_mobilevit_v1_xxs_against_reference_fixture(pkg, golden_dir):
     """SURVEY.md 8a row a9 / BASELINE.json configs[0]: MobileViT-v1 XXS -- state_dict contract, eval forward at 1x3x256x256 and a train-mode
     forward/backward (dropouts 0) against the REAL reference (dense 3x3 convs via im2col + GEMM, unfold / fold permutations, head dims
     16 / 20 / 24 in the attention core)."""
+    check_mobilevit_v1_against_fixture(pkg, torch.load(os.path.join(golden_dir, "mobilevit_v1_xxs_fp32.pt"), weights_only=False), (4, 3, 192, 192))
+
+
+def check_mobilevit_v1_against_fixture(pkg, fx, train_shape):
+    """One MobileViT-v1 mode against the real reference's fp32 record: the state_dict keys, the eval logits at 1x3x256x256 and a train-mode
+    forward / backward (dropouts 0) on a ``train_shape`` batch, each bounded by the oracle under torch bf16 autocast on this GPU.  Gradients
+    the fixture stores as a sample (tests/golden_sample.py) are compared at the sampled positions."""
     import torch.nn.functional as F
-    fx = torch.load(os.path.join(golden_dir, "mobilevit_v1_xxs_fp32.pt"), weights_only=False)
+    mode = fx["mode"]
     opts = pkg.default_mit_opts(fx["mode"], **{"model.classification.mit.dropout": 0.0, "model.classification.classifier_dropout": 0.0})
     model = pkg.MobileViT(opts)
     assert {k: list(v.shape) for k, v in model.state_dict().items()} == {k: s for k, s in fx["keys"]}
@@ -279,11 +286,11 @@ def test_mobilevit_v1_xxs_against_reference_fixture(pkg, golden_dir):
         with torch.autocast("cuda", dtype=torch.bfloat16):
             eva = O.mobilevit_v1_forward(Pa, x1, mode=fx["mode"], training=False)
     e, ea = rel_l2(ev, fx["eval_logits"]), rel_l2(eva, fx["eval_logits"])
-    print(f"[mobilevit v1 xxs] eval logits rel-L2 vs the reference: ours {e:.4g}, torch-autocast {ea:.4g}")
+    print(f"[mobilevit v1 {mode}] eval logits rel-L2 vs the reference: ours {e:.4g}, torch-autocast {ea:.4g}")
     assert e <= max(3e-2, 1.5 * ea)
     assert int(ev.argmax()) == int(fx["eval_logits"].argmax()) or e <= 1e-2
     model.train()
-    x = O.seeded_input((4, 3, 192, 192), fx["x_seed"]).cuda()
+    x = O.seeded_input(train_shape, fx["x_seed"]).cuda()
     logits = model(x)
     loss = F.cross_entropy(logits.float(), fx["labels"].cuda(), label_smoothing=0.1)
     loss.backward()
@@ -292,7 +299,7 @@ def test_mobilevit_v1_xxs_against_reference_fixture(pkg, golden_dir):
         lt = O.mobilevit_v1_forward(Pt, x, mode=fx["mode"], training=True)
         F.cross_entropy(lt, fx["labels"].cuda(), label_smoothing=0.1).backward()
     et, eta = rel_l2(logits, fx["logits"]), rel_l2(lt, fx["logits"])
-    print(f"[mobilevit v1 xxs] train logits rel-L2 vs the reference: ours {et:.4g}, torch-autocast {eta:.4g}; loss {float(loss):.5f} vs {float(fx['loss']):.5f}")
+    print(f"[mobilevit v1 {mode}] train logits rel-L2 vs the reference: ours {et:.4g}, torch-autocast {eta:.4g}; loss {float(loss):.5f} vs {float(fx['loss']):.5f}")
     assert et <= max(5e-2, 1.5 * eta)
     named = dict(model.named_parameters())
     total = sum(n * n for n in fx["grad_norms"].values()) ** 0.5
@@ -300,10 +307,11 @@ def test_mobilevit_v1_xxs_against_reference_fixture(pkg, golden_dir):
     for k, g in fx["grads"].items():
         if fx["grad_norms"][k] < 1e-3 * total:
             continue
-        eo, eau = rel_l2(named[k].grad, g), rel_l2(Pt[k].grad, g)
+        eo, eau = rel_l2(*at_sample(named[k].grad, g)), rel_l2(*at_sample(Pt[k].grad, g))
         if eo > max(0.1, 2.0 * eau):
             bad.append((k, eo, eau))
     assert not bad, bad[:8]
+    return e, et
 
 
 def test_mobilevit_v1_trains_with_recipe_dropouts(pkg):

@@ -135,8 +135,8 @@ def test_vit_huge_against_reference(m, golden_dir, crop):
 
 # ------------------------------------------------------------------------------------------------ checkpointing equivalence
 def _nondeterministic(name):
-    """Gradients reduced with fp32 atomics (test_reproducible_gpu.NONDETERMINISTIC): LayerNorm gains / biases and the out_proj bias (the column
-    sums of cvb_ln_bwd's dx), and the token-embedding table (cvb_embedding_bwd)."""
+    """Gradients compared with a tolerance: LayerNorm gains / biases and the out_proj bias (the column sums of cvb_ln_bwd's dx), and the
+    token-embedding table (cvb_embedding_bwd, fp32 atomics: test_reproducible_gpu.NONDETERMINISTIC)."""
     return (".pre_norm_mha.0." in name or ".pre_norm_ffn.0." in name or name.startswith("post_transformer_norm.")
             or "final_layer_norm." in name or name.endswith("out_proj.bias") or name == "embedding_layer.weight")
 
