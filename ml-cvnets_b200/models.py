@@ -8,21 +8,19 @@ from __future__ import annotations
 
 import argparse
 from types import SimpleNamespace
-from typing import Dict, List, Optional, Tuple, Union
+from typing import Dict, Optional, Tuple
 
-import torch
 from torch import Tensor, nn
 
 from . import functional as Fn
-from .layers import ConvLayer2d, GlobalPool, Identity, LinearLayer, _bind, _need_cuda, norm_layers_tuple
+from .layers import ConvLayer2d, GlobalPool, Identity, LinearLayer, _bind
+from .models_base import ImageEncoder, extract_end_points_all, init_weights, make_mobilenet_layer
 from .modules import InvertedResidual, MobileViTBlockv2, make_divisible
-from .neural_aug import augmented_forward, build_neural_augmentor
 from .ops import PreparedWeights as PW
 
 
 def default_opts(width_multiplier: float = 1.0, n_classes: int = 1000, **extra) -> argparse.Namespace:
     """The subset of the reference's flat dotted-key namespace the hot path reads (options/utils.py:34-42)."""
-    opts = argparse.Namespace()
     kv = {
         "model.classification.name": "mobilevit_v2",
         "model.classification.n_classes": n_classes,
@@ -39,10 +37,7 @@ def default_opts(width_multiplier: float = 1.0, n_classes: int = 1000, **extra) 
         "model.layer.linear_init": "trunc_normal",
         "model.layer.linear_init_std_dev": 0.02,
     }
-    kv.update(extra)
-    for k, v in kv.items():
-        setattr(opts, k, v)
-    return opts
+    return argparse.Namespace(**{**kv, **extra})
 
 
 def get_configuration(opts) -> Dict:
@@ -64,15 +59,14 @@ def get_configuration(opts) -> Dict:
     }
 
 
-class MobileViTv2(nn.Module):
+class MobileViTv2(ImageEncoder):
     """Same attribute names / state_dict keys as the reference model: conv_1, layer_1..layer_5, conv_1x1_exp, classifier."""
 
     def __init__(self, opts, *args, **kwargs) -> None:
-        super().__init__()
+        super().__init__(opts)
         num_classes = getattr(opts, "model.classification.n_classes", 1000)
         pool_type = getattr(opts, "model.layer.global_pool", "mean")
         cfg = get_configuration(opts)
-        self.opts = opts
         # segmentation heads (DeepLabv3 / PSPNet) ask for output_stride 8 / 16: the stride of layer_4 / layer_5 becomes dilation
         # (base_image_encoder.py:38-47)
         self.dilation = 1
@@ -81,7 +75,6 @@ class MobileViTv2(nn.Module):
         self.output_stride = output_stride
         self.model_conf_dict = dict()
         c0 = cfg["layer0"]["out_channels"]
-        self.neural_augmentor = build_neural_augmentor(opts)  # before conv_1: its parameters come first (base_image_encoder.py:50)
         self.conv_1 = ConvLayer2d(opts=opts, in_channels=cfg["layer0"]["img_channels"], out_channels=c0, kernel_size=3, stride=2,
                                   use_norm=True, use_act=True)
         self.model_conf_dict["conv1"] = {"in": 3, "out": c0}
@@ -111,18 +104,7 @@ class MobileViTv2(nn.Module):
     def _make_layer(self, opts, input_channel, cfg: Dict, dilate: Optional[bool] = False) -> Tuple[nn.Sequential, int]:
         if cfg.get("block_type", "mobilevit").lower() == "mobilevit":
             return self._make_mit_layer(opts=opts, input_channel=input_channel, cfg=cfg, dilate=dilate)
-        return self._make_mobilenet_layer(opts=opts, input_channel=input_channel, cfg=cfg)
-
-    @staticmethod
-    def _make_mobilenet_layer(opts, input_channel: int, cfg: Dict) -> Tuple[nn.Sequential, int]:
-        output_channels = cfg.get("out_channels")
-        block = []
-        for i in range(cfg.get("num_blocks", 2)):
-            stride = cfg.get("stride", 1) if i == 0 else 1
-            block.append(InvertedResidual(opts=opts, in_channels=input_channel, out_channels=output_channels, stride=stride,
-                                          expand_ratio=cfg.get("expand_ratio", 4)))
-            input_channel = output_channels
-        return nn.Sequential(*block), input_channel
+        return make_mobilenet_layer(opts=opts, input_channel=input_channel, cfg=cfg)
 
     def _make_mit_layer(self, opts, input_channel, cfg: Dict, dilate: Optional[bool] = False) -> Tuple[nn.Sequential, int]:
         prev_dilation = self.dilation
@@ -144,52 +126,10 @@ class MobileViTv2(nn.Module):
             attn_norm_layer=getattr(opts, "model.classification.mitv2.attn_norm_layer", "layer_norm_2d"), dilation=self.dilation))
         return nn.Sequential(*block), input_channel
 
-    @classmethod
-    def build_model(cls, opts, *args, **kwargs):
-        return cls(opts, *args, **kwargs)
-
     # ---- weight init (cvnets/misc/init_utils.py:110-150, called from base_model.py:69-71)
     def reset_parameters(self, opts) -> None:
-        conv_init = getattr(opts, "model.layer.conv_init", "kaiming_normal")
-        lin_init = getattr(opts, "model.layer.linear_init", "normal")
-        lin_std = getattr(opts, "model.layer.linear_init_std_dev", 0.01)
-        for m in self.modules():
-            if isinstance(m, nn.Conv2d):
-                if conv_init == "kaiming_normal":
-                    nn.init.kaiming_normal_(m.weight, mode="fan_out")
-                elif conv_init == "kaiming_uniform":
-                    nn.init.kaiming_uniform_(m.weight, mode="fan_out")
-                else:
-                    nn.init.xavier_uniform_(m.weight)
-                if m.bias is not None:
-                    nn.init.zeros_(m.bias)
-            elif isinstance(m, norm_layers_tuple):
-                if m.weight is not None:
-                    nn.init.ones_(m.weight)
-                if m.bias is not None:
-                    nn.init.zeros_(m.bias)
-            elif isinstance(m, LinearLayer):
-                if lin_init == "trunc_normal":
-                    nn.init.trunc_normal_(m.weight, mean=0.0, std=lin_std)
-                elif lin_init == "normal":
-                    nn.init.normal_(m.weight, mean=0.0, std=lin_std)
-                else:
-                    nn.init.xavier_uniform_(m.weight)
-                if m.bias is not None:
-                    nn.init.zeros_(m.bias)
-
-    # ---- optimizer grouping (cvnets/misc/common.py:122-176 via base_model.py:92-123)
-    def get_trainable_parameters(self, weight_decay: Optional[float] = 0.0, no_decay_bn_filter_bias: Optional[bool] = False,
-                                 *args, **kwargs) -> Tuple[List[Dict], List[float]]:
-        with_decay, without_decay = [], []
-        for p in self.parameters():
-            if not p.requires_grad:
-                continue
-            (without_decay if (no_decay_bn_filter_bias and p.dim() == 1) else with_decay).append(p)
-        groups = [{"params": with_decay, "weight_decay": weight_decay}]
-        if without_decay:
-            groups.append({"params": without_decay, "weight_decay": 0.0})
-        return groups, [1.0] * len(groups)
+        init_weights(self.modules(), getattr(opts, "model.layer.conv_init", "kaiming_normal"), getattr(opts, "model.layer.linear_init", "normal"),
+                     getattr(opts, "model.layer.linear_init_std_dev", 0.01))
 
     # ---- forward (base_image_encoder.py:261-301)
     def extract_features(self, x: Tensor, *args, **kwargs) -> Tensor:
@@ -207,24 +147,7 @@ class MobileViTv2(nn.Module):
                 object.__setattr__(m, "_lazy_active", False)
         return self.conv_1x1_exp(x)
 
-    # ---- feature maps for down-stream heads (base_image_encoder.py:206-276); every returned map is materialised (no lazy boundaries)
-    def extract_end_points_all(self, x: Tensor, use_l5: Optional[bool] = True, use_l5_exp: Optional[bool] = False, *args, **kwargs) -> Dict[str, Tensor]:
-        _need_cuda(x, "MobileViTv2")
-        out_dict = {}
-        x = self.layer_1(self.conv_1(x))
-        out_dict["out_l1"] = x
-        x = self.layer_2(x)
-        out_dict["out_l2"] = x
-        x = self.layer_3(x)
-        out_dict["out_l3"] = x
-        x = self.layer_4(x)
-        out_dict["out_l4"] = x
-        if use_l5:
-            x = self.layer_5(x)
-            out_dict["out_l5"] = x
-            if use_l5_exp:
-                out_dict["out_l5_exp"] = self.conv_1x1_exp(x)
-        return out_dict
+    extract_end_points_all = extract_end_points_all
 
     def extract_end_points_l4(self, x: Tensor, *args, **kwargs) -> Dict[str, Tensor]:
         return self.extract_end_points_all(x, use_l5=False)
@@ -241,9 +164,3 @@ class MobileViTv2(nn.Module):
                                          i_b=prep.add(lin.bias, PW.KIND_VECTOR_F32, dst_rows=npad))
         head = _bind(self, self._head, [lin.weight, lin.bias])
         return Fn.PoolLinearFn.apply(Fn.to_bf16_cl(x), head, lin.weight, lin.bias)
-
-    def forward(self, x: Tensor, *args, **kwargs) -> Union[Tensor, Dict[str, Optional[Tensor]]]:
-        _need_cuda(x, "MobileViTv2")
-        if self.neural_augmentor is not None:
-            return augmented_forward(self, x)
-        return self.forward_classifier(x)

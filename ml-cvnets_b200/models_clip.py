@@ -49,9 +49,7 @@ def default_clip_opts(vit_mode: str = "base", projection_dim: int = 512, text_di
         "model.text.transformer.no_pos_embedding": False, "model.text.transformer.gradient_checkpoint": False, "dataset.text_vocab_size": vocab_size, "dataset.text_context_length": context_length,
         "dataset.padding_index": None,
     }
-    kv.update(extra)
-    for k, v in kv.items():
-        setattr(opts, k, v)
+    vars(opts).update({**kv, **extra})
     return opts
 
 

@@ -9,13 +9,13 @@ from __future__ import annotations
 
 import argparse
 import math
-from typing import Dict, List, Optional, Tuple, Union
+from typing import Dict, List, Tuple
 
 from torch import Tensor, nn
 
-from .layers import ConvLayer2d, Dropout, GlobalPool, LinearLayer, _need_cuda, norm_layers_tuple
+from .layers import ConvLayer2d, Dropout, GlobalPool, LinearLayer
+from .models_base import ImageEncoder, extract_end_points_all, init_weights
 from .modules import EfficientNetBlock, make_divisible
-from .neural_aug import augmented_forward, build_neural_augmentor
 
 # mode: (width_mult, depth_mult, train_resolution)
 _COMPOUND_SCALING = {"b0": (1.0, 1.0, 224), "b1": (1.0, 1.1, 240), "b2": (1.1, 1.2, 260), "b3": (1.2, 1.4, 300), "b4": (1.4, 1.8, 380),
@@ -29,7 +29,6 @@ LAYERS = ["layer_1", "layer_2", "layer_3", "layer_4", "layer_5"]
 def default_effnet_opts(mode: str = "b0", n_classes: int = 1000, **extra) -> argparse.Namespace:
     """Model section of examples/range_augment/classification/efficientnet_b0.yaml (swish, batch_norm momentum 0.1, no stochastic depth, no
     classifier dropout)."""
-    opts = argparse.Namespace()
     kv = {
         "model.classification.name": "efficientnet", "model.classification.n_classes": n_classes, "model.classification.efficientnet.mode": mode,
         "model.classification.efficientnet.stochastic_depth_prob": 0.0, "model.classification.classifier_dropout": 0.0,
@@ -37,10 +36,7 @@ def default_effnet_opts(mode: str = "b0", n_classes: int = 1000, **extra) -> arg
         "model.layer.global_pool": "mean", "model.layer.conv_init": "kaiming_normal", "model.layer.linear_init": "normal",
         "model.layer.linear_init_std_dev": 0.01,
     }
-    kv.update(extra)
-    for k, v in kv.items():
-        setattr(opts, k, v)
-    return opts
+    return argparse.Namespace(**{**kv, **extra})
 
 
 def get_effnet_configuration(opts) -> Dict:
@@ -59,16 +55,15 @@ def get_effnet_configuration(opts) -> Dict:
     return cfg
 
 
-class EfficientNet(nn.Module):
+class EfficientNet(ImageEncoder):
     def __init__(self, opts, *args, **kwargs) -> None:
-        super().__init__()
+        super().__init__(opts)
         num_classes = getattr(opts, "model.classification.n_classes", 1000)
         classifier_dropout = getattr(opts, "model.classification.classifier_dropout", 0.0)
         sd_prob = getattr(opts, "model.classification.efficientnet.stochastic_depth_prob", 0.2)
         cfg = get_effnet_configuration(opts)
-        self.opts, self.dilation = opts, 1
+        self.dilation = 1
         c = cfg["layer_1"][0][3]
-        self.neural_augmentor = build_neural_augmentor(opts)  # before conv_1: its parameters come first (base_image_encoder.py:50)
         self.conv_1 = ConvLayer2d(opts=opts, in_channels=3, out_channels=c, kernel_size=3, stride=2, use_norm=True, use_act=True)
         prev = 0
         for name in LAYERS:
@@ -96,27 +91,9 @@ class EfficientNet(nn.Module):
                 ci = co
         return nn.Sequential(*block), prev + count
 
-    @classmethod
-    def build_model(cls, opts, *args, **kwargs):
-        return cls(opts, *args, **kwargs)
-
     def reset_parameters(self, opts) -> None:
         """cvnets/misc/init_utils.py with the recipe's kaiming_normal convs / normal(0.01) linear."""
-        lin_std = getattr(opts, "model.layer.linear_init_std_dev", 0.01)
-        for m in self.modules():
-            if isinstance(m, nn.Conv2d):
-                nn.init.kaiming_normal_(m.weight, mode="fan_out")
-                if m.bias is not None:
-                    nn.init.zeros_(m.bias)
-            elif isinstance(m, norm_layers_tuple):
-                if m.weight is not None:
-                    nn.init.ones_(m.weight)
-                if m.bias is not None:
-                    nn.init.zeros_(m.bias)
-            elif isinstance(m, LinearLayer):
-                nn.init.normal_(m.weight, mean=0.0, std=lin_std)
-                if m.bias is not None:
-                    nn.init.zeros_(m.bias)
+        init_weights(self.modules(), "kaiming_normal", "normal", getattr(opts, "model.layer.linear_init_std_dev", 0.01))
 
     def extract_features(self, x: Tensor, *args, **kwargs) -> Tensor:
         x = self.conv_1(x)
@@ -124,33 +101,10 @@ class EfficientNet(nn.Module):
             x = getattr(self, name)(x)
         return self.conv_1x1_exp(x)
 
-    def extract_end_points_all(self, x: Tensor, use_l5: Optional[bool] = True, use_l5_exp: Optional[bool] = False, *args, **kwargs) -> Dict[str, Tensor]:
-        """base_image_encoder.py:extract_end_points_all."""
-        _need_cuda(x, "EfficientNet")
-        out = {}
-        x = self.layer_1(self.conv_1(x))
-        out["out_l1"] = x
-        x = self.layer_2(x)
-        out["out_l2"] = x
-        x = self.layer_3(x)
-        out["out_l3"] = x
-        x = self.layer_4(x)
-        out["out_l4"] = x
-        if use_l5:
-            x = self.layer_5(x)
-            out["out_l5"] = x
-            if use_l5_exp:
-                out["out_l5_exp"] = self.conv_1x1_exp(x)
-        return out
+    extract_end_points_all = extract_end_points_all
 
     def forward_classifier(self, x: Tensor, *args, **kwargs) -> Tensor:
-        _need_cuda(x, "EfficientNet")
         x = self.classifier.global_pool(self.extract_features(x))
         if hasattr(self.classifier, "classifier_dropout"):
             x = self.classifier.classifier_dropout(x)
         return self.classifier.classifier_fc(x)
-
-    def forward(self, x: Tensor, *args, **kwargs) -> Union[Tensor, Dict[str, Optional[Tensor]]]:
-        if self.neural_augmentor is not None:
-            return augmented_forward(self, x)
-        return self.forward_classifier(x)

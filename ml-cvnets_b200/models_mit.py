@@ -5,18 +5,17 @@ conv_1, layer_1 .. layer_5, conv_1x1_exp, classifier.{global_pool, [dropout,] fc
 from __future__ import annotations
 
 import argparse
-from typing import Dict, Optional, Tuple, Union
+from typing import Dict, Tuple
 
 from torch import Tensor, nn
 
-from .layers import ConvLayer2d, Dropout, GlobalPool, LinearLayer, _need_cuda, norm_layers_tuple
+from .layers import ConvLayer2d, Dropout, GlobalPool, LinearLayer
+from .models_base import ImageEncoder, init_weights, make_mobilenet_layer
 from .modules import InvertedResidual, MobileViTBlock
-from .neural_aug import augmented_forward, build_neural_augmentor
 
 
 def default_mit_opts(mode: str = "xx_small", n_classes: int = 1000, **extra) -> argparse.Namespace:
     """config/classification/imagenet/mobilevit.yaml model section (dropout 0.1 / attn_dropout 0 / classifier_dropout 0.1, swish)."""
-    opts = argparse.Namespace()
     kv = {
         "model.classification.name": "mobilevit", "model.classification.n_classes": n_classes, "model.classification.mit.mode": mode,
         "model.classification.classifier_dropout": 0.1, "model.classification.mit.dropout": 0.1, "model.classification.mit.ffn_dropout": 0.0,
@@ -26,10 +25,7 @@ def default_mit_opts(mode: str = "xx_small", n_classes: int = 1000, **extra) -> 
         "model.layer.global_pool": "mean", "model.layer.conv_init": "kaiming_normal", "model.layer.linear_init": "trunc_normal",
         "model.layer.linear_init_std_dev": 0.02,
     }
-    kv.update(extra)
-    for k, v in kv.items():
-        setattr(opts, k, v)
-    return opts
+    return argparse.Namespace(**{**kv, **extra})
 
 
 def get_mit_configuration(opts) -> Dict:
@@ -54,14 +50,13 @@ def get_mit_configuration(opts) -> Dict:
     return cfg
 
 
-class MobileViT(nn.Module):
+class MobileViT(ImageEncoder):
     def __init__(self, opts, *args, **kwargs) -> None:
-        super().__init__()
+        super().__init__(opts)
         num_classes = getattr(opts, "model.classification.n_classes", 1000)
         classifier_dropout = getattr(opts, "model.classification.classifier_dropout", 0.0)
         cfg = get_mit_configuration(opts)
-        self.opts, self.dilation = opts, 1
-        self.neural_augmentor = build_neural_augmentor(opts)  # before conv_1: its parameters come first (base_image_encoder.py:50)
+        self.dilation = 1
         self.conv_1 = ConvLayer2d(opts=opts, in_channels=3, out_channels=16, kernel_size=3, stride=2, use_norm=True, use_act=True)
         c = 16
         for li in range(1, 6):
@@ -78,12 +73,7 @@ class MobileViT(nn.Module):
 
     def _make_layer(self, opts, input_channel: int, cfg: Dict) -> Tuple[nn.Sequential, int]:
         if cfg.get("block_type", "mobilevit").lower() != "mobilevit":
-            block, out_c = [], cfg["out_channels"]
-            for i in range(cfg.get("num_blocks", 2)):
-                block.append(InvertedResidual(opts=opts, in_channels=input_channel, out_channels=out_c, stride=cfg.get("stride", 1) if i == 0 else 1,
-                                              expand_ratio=cfg.get("expand_ratio", 4)))
-                input_channel = out_c
-            return nn.Sequential(*block), input_channel
+            return make_mobilenet_layer(opts, input_channel, cfg)
         block = []
         if cfg.get("stride", 1) == 2:
             block.append(InvertedResidual(opts=opts, in_channels=input_channel, out_channels=cfg["out_channels"], stride=2,
@@ -99,26 +89,8 @@ class MobileViT(nn.Module):
             conv_ksize=getattr(opts, "model.classification.mit.conv_kernel_size", 3)))
         return nn.Sequential(*block), input_channel
 
-    @classmethod
-    def build_model(cls, opts, *args, **kwargs):
-        return cls(opts, *args, **kwargs)
-
     def reset_parameters(self, opts) -> None:
-        lin_std = getattr(opts, "model.layer.linear_init_std_dev", 0.02)
-        for m in self.modules():
-            if isinstance(m, nn.Conv2d):
-                nn.init.kaiming_normal_(m.weight, mode="fan_out")
-                if m.bias is not None:
-                    nn.init.zeros_(m.bias)
-            elif isinstance(m, norm_layers_tuple):
-                if m.weight is not None:
-                    nn.init.ones_(m.weight)
-                if m.bias is not None:
-                    nn.init.zeros_(m.bias)
-            elif isinstance(m, LinearLayer):
-                nn.init.trunc_normal_(m.weight, mean=0.0, std=lin_std)
-                if m.bias is not None:
-                    nn.init.zeros_(m.bias)
+        init_weights(self.modules(), "kaiming_normal", "trunc_normal", getattr(opts, "model.layer.linear_init_std_dev", 0.02))
 
     def extract_features(self, x: Tensor, *args, **kwargs) -> Tensor:
         x = self.conv_1(x)
@@ -126,13 +98,7 @@ class MobileViT(nn.Module):
             x = getattr(self, f"layer_{li}")(x)
         return self.conv_1x1_exp(x)
 
-    def forward(self, x: Tensor, *args, **kwargs) -> Union[Tensor, Dict[str, Optional[Tensor]]]:
-        if self.neural_augmentor is not None:
-            return augmented_forward(self, x)
-        return self.forward_classifier(x)
-
     def forward_classifier(self, x: Tensor, *args, **kwargs) -> Tensor:
-        _need_cuda(x, "MobileViT")
         x = self.extract_features(x)
         x = self.classifier.global_pool(x)
         if hasattr(self.classifier, "dropout"):

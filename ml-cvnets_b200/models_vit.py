@@ -17,7 +17,7 @@ from __future__ import annotations
 
 import argparse
 from types import SimpleNamespace
-from typing import Dict, List, Optional, Tuple, Union
+from typing import Dict, Tuple
 
 import numpy as np
 import torch
@@ -25,14 +25,13 @@ from torch import Tensor, nn
 
 from . import functional as Fn
 from . import ops
-from .layers import ConvLayer2d, Dropout, LinearLayer, _bind, _need_cuda, get_normalization_layer, norm_layers_tuple
+from .layers import ConvLayer2d, Dropout, LinearLayer, _bind, get_normalization_layer
+from .models_base import ImageEncoder, init_weights
 from .modules import TransformerEncoder, checkpointed_encoders
-from .neural_aug import augmented_forward, build_neural_augmentor
 
 
 def default_vit_opts(mode: str = "base", n_classes: int = 1000, **extra) -> argparse.Namespace:
     """The recipe's model options (examples/vit/classification/vit_base.yaml:80-97; the ViT-H recipes set gradient_checkpointing)."""
-    opts = argparse.Namespace()
     kv = {
         "model.classification.name": "vit", "model.classification.n_classes": n_classes, "model.classification.vit.mode": mode,
         "model.classification.vit.norm_layer": "layer_norm_fp32", "model.classification.vit.dropout": 0.0,
@@ -42,10 +41,7 @@ def default_vit_opts(mode: str = "base", n_classes: int = 1000, **extra) -> argp
         "model.activation.name": "gelu", "model.normalization.name": "batch_norm", "model.normalization.momentum": 0.1,
         "model.layer.conv_init": "kaiming_normal", "model.layer.linear_init": "trunc_normal", "model.layer.linear_init_std_dev": 0.02,
     }
-    kv.update(extra)
-    for k, v in kv.items():
-        setattr(opts, k, v)
-    return opts
+    return argparse.Namespace(**{**kv, **extra})
 
 
 def get_vit_configuration(opts) -> Dict:
@@ -81,16 +77,14 @@ class PositionalEmbedding(nn.Module):
         self.pos_embed = LearnablePositionalEmbedding(num_embeddings, embedding_dim)
 
 
-class VisionTransformer(nn.Module):
+class VisionTransformer(ImageEncoder):
     def __init__(self, opts, *args, **kwargs) -> None:
-        super().__init__()
+        super().__init__(opts)
         num_classes = getattr(opts, "model.classification.n_classes", 1000)
         if getattr(opts, "model.classification.vit.use_simple_fpn", False):
             raise NotImplementedError("SimpleFPN (detection) is out of scope")
         cfg = get_vit_configuration(opts)
         d, ffn, n_layers, heads, norm_layer = cfg["embed_dim"], cfg["ffn_dim"], cfg["n_transformer_layers"], cfg["n_attn_heads"], cfg["norm_layer"]
-        self.opts = opts
-        self.neural_augmentor = build_neural_augmentor(opts)  # before patch_emb: its parameters come first (base_image_encoder.py:50)
         stem_dim = max(32, d // 4)
         self.patch_emb = nn.Sequential(
             ConvLayer2d(opts=opts, in_channels=3, out_channels=stem_dim, kernel_size=4, stride=4, bias=False, use_norm=True, use_act=True),
@@ -123,37 +117,9 @@ class VisionTransformer(nn.Module):
         if self.gradient_checkpointing and not 1 <= self.checkpoint_segments <= n_layers:
             raise ValueError(f"checkpoint_segments must be in 1..{n_layers}, got {self.checkpoint_segments}")
 
-    @classmethod
-    def build_model(cls, opts, *args, **kwargs):
-        return cls(opts, *args, **kwargs)
-
     def reset_parameters(self, opts) -> None:
         """cvnets/misc/init_utils.py:110-150."""
-        lin_std = getattr(opts, "model.layer.linear_init_std_dev", 0.02)
-        for m in self.modules():
-            if isinstance(m, nn.Conv2d):
-                nn.init.kaiming_normal_(m.weight, mode="fan_out")
-                if m.bias is not None:
-                    nn.init.zeros_(m.bias)
-            elif isinstance(m, norm_layers_tuple):
-                if m.weight is not None:
-                    nn.init.ones_(m.weight)
-                if m.bias is not None:
-                    nn.init.zeros_(m.bias)
-            elif isinstance(m, LinearLayer):
-                nn.init.trunc_normal_(m.weight, mean=0.0, std=lin_std)
-                if m.bias is not None:
-                    nn.init.zeros_(m.bias)
-
-    def get_trainable_parameters(self, weight_decay: Optional[float] = 0.0, no_decay_bn_filter_bias: Optional[bool] = False, *args, **kwargs):
-        with_decay, without_decay = [], []
-        for p in self.parameters():
-            if p.requires_grad:
-                (without_decay if (no_decay_bn_filter_bias and p.dim() == 1) else with_decay).append(p)
-        groups = [{"params": with_decay, "weight_decay": weight_decay}]
-        if without_decay:
-            groups.append({"params": without_decay, "weight_decay": 0.0})
-        return groups, [1.0] * len(groups)
+        init_weights(self.modules(), "kaiming_normal", "trunc_normal", getattr(opts, "model.layer.linear_init_std_dev", 0.02))
 
     # ---- forward (vit.py:476-560)
     def extract_patch_embeddings(self, x: Tensor) -> Tuple[Tensor, Tuple[int, int]]:
@@ -183,12 +149,4 @@ class VisionTransformer(nn.Module):
         return self.post_transformer_norm(x)
 
     def forward_classifier(self, x: Tensor, *args, **kwargs) -> Tensor:
-        _need_cuda(x, "VisionTransformer")
         return self.classifier(self.extract_features(x))
-
-    def forward(self, x: Tensor, *args, **kwargs) -> Union[Tensor, Dict[str, Optional[Tensor]]]:
-        """Logits; with a RangeAugment augmentor the reference's {"augmented_tensor", "logits"} (vit.py:592-610), augmented_tensor None in
-        eval mode."""
-        if self.neural_augmentor is not None:
-            return augmented_forward(self, x)
-        return self.forward_classifier(x)

@@ -113,10 +113,3 @@ def build_neural_augmentor(opts, *args, **kwargs) -> Optional[DistributionNeural
         raise NotImplementedError("model.learn_augmentation.mode = 'basic' (BasicNeuralAugmentor) is not implemented; no recipe uses it")
     return None
 
-
-def augmented_forward(model: nn.Module, x: Tensor):
-    """BaseImageEncoder.forward with an augmentor (base_image_encoder.py:282-298)."""
-    if model.training:
-        x_aug = model.neural_augmentor(x)
-        return {"augmented_tensor": x_aug, "logits": model.forward_classifier(x_aug)}
-    return {"augmented_tensor": None, "logits": model.forward_classifier(x)}

@@ -34,6 +34,8 @@ def _make_shell(ours_cls, base_cls, shell_name: str):
     parameters, buffers and private state are those of this package's model, and whose forward / feature-extraction methods are this package's."""
     import types
 
+    from torch import nn
+
     def __init__(self, opts, *args, **kwargs) -> None:
         base_cls.__init__(self, opts, *args, **kwargs)
         inner = ours_cls(opts, *args, **kwargs)
@@ -49,9 +51,12 @@ def _make_shell(ours_cls, base_cls, shell_name: str):
                 self.__dict__[k] = v
 
     ns = {"__init__": __init__, "__doc__": f"Reference-side shell around ml_cvnets_b200.{ours_cls.__name__}; forward goes straight to the CUDA path."}
-    for k, v in ours_cls.__dict__.items():
-        if isinstance(v, types.FunctionType) and not (k.startswith("__") and k.endswith("__")) and k not in _KEEP_REFERENCE:
-            ns[k] = v
+    for klass in ours_cls.__mro__:  # subclass first, so an override wins over what it inherits (ImageEncoder's forward, ...)
+        if klass is nn.Module:
+            break
+        for k, v in klass.__dict__.items():
+            if isinstance(v, types.FunctionType) and not (k.startswith("__") and k.endswith("__")) and k not in _KEEP_REFERENCE:
+                ns.setdefault(k, v)
     return type(shell_name, (base_cls,), ns)
 
 
