@@ -11,7 +11,7 @@ from .models_clip import CLIP, SimpleImageProjectionHead, TextTransformer, clip_
 from .models_mit import MobileViT, default_mit_opts, get_mit_configuration  # noqa: F401
 from .models_vit import VisionTransformer, default_vit_opts, get_vit_configuration  # noqa: F401
 from .modules import EfficientNetBlock, InvertedResidual, InvertedResidualSE, SqueezeExcitation, LinearAttnFFN, MobileViTBlock, MobileViTBlockv2, TransformerEncoder  # noqa: F401
-from .engine import NeuralAugmentationLoss, TrainStep, ZeroShotAccuracy, cross_entropy  # noqa: F401
+from .engine import NeuralAugmentationLoss, TrainStep, ZeroShotAccuracy, cross_entropy, variable_batch_pairs  # noqa: F401
 from .neural_aug import Clip, DistributionNeuralAugmentor, UniformSampler, build_neural_augmentor  # noqa: F401
 from .optim import FlatAdamW, FlatSGD  # noqa: F401
 from .workspace import StepWorkspace  # noqa: F401
@@ -21,4 +21,4 @@ __all__ = ["InvertedResidualSE", "SqueezeExcitation", "MobileViTv2", "default_op
            "Dropout", "Identity", "TransformerEncoder", "MultiHeadAttention", "LayerNorm", "GELU", "TrainStep", "cross_entropy", "FlatAdamW",
            "StepWorkspace", "LayerNormFP32", "VisionTransformer", "default_vit_opts", "get_vit_configuration", "MobileViT", "default_mit_opts", "get_mit_configuration", "MobileViTBlock", "CLIP", "TextTransformer", "SimpleImageProjectionHead", "clip_contrastive_loss", "default_clip_opts", "ZeroShotAccuracy",
            "EfficientNetBlock", "EfficientNet", "default_effnet_opts", "get_effnet_configuration", "FlatSGD", "NeuralAugmentationLoss",
-           "DistributionNeuralAugmentor", "UniformSampler", "Clip", "build_neural_augmentor"]
+           "DistributionNeuralAugmentor", "UniformSampler", "Clip", "build_neural_augmentor", "variable_batch_pairs"]

@@ -15,12 +15,19 @@ inside the step (zero-fills are memset nodes, the loss is cvb_ce_*).  Semantics 
     for x, y in loader:
         step.set_lr(scheduler_lr)             # device scalar: schedulers keep working under replay
         loss = step(x, y)                     # device tensor; no host sync
+
+A variable-batch sampler draws a (crop, batch) pair per iteration; ``capture_shapes`` captures one graph per pair in the same TrainStep
+(``variable_batch_pairs`` gives the reference sampler's table):
+
+    pairs = variable_batch_pairs(224, 224, 256, max_scales=5, check_scale=32, min_w=128, max_w=320, min_h=128, max_h=320)
+    step.capture_shapes([(torch.randn(b, 3, h, w, device="cuda"), torch.zeros(b, dtype=torch.long, device="cuda")) for h, w, b in pairs])
 """
 from __future__ import annotations
 
 import gc
+import math
 from types import SimpleNamespace
-from typing import Optional
+from typing import Dict, List, Optional, Sequence, Tuple
 
 import torch
 
@@ -81,7 +88,6 @@ class TrainStep:
             self.ws.broadcast_buffers()
         self.loss_cfg = SimpleNamespace(label_smoothing=float(label_smoothing), ignore_index=int(ignore_index), scale=self.opt.loss_scale(),
                                         mix=self.ws.mix)
-        self._mix_host = torch.tensor([0.0, 1.0, 0.0, 0.0, 0.0, 0.0]).pin_memory()
         self.forward_loss = forward_loss
         if aug_loss is None and ce_weight != 1.0:
             raise ValueError("ce_weight weighs the cross entropy against aug_loss; without aug_loss the loss is the cross entropy")
@@ -90,8 +96,8 @@ class TrainStep:
         self.loss_cfg.group = process_group
         self.loss_cfg.world, self.loss_cfg.rank = self.world, (dist.get_rank(process_group) if data_parallel else 0)
         self._one = torch.ones((), device=self.ws.device, dtype=torch.float32)
-        self._graph = None
-        self._static = None
+        self._graphs: Dict[tuple, tuple] = {}  # input signature -> (CUDA graph, static inputs, static loss), in capture order
+        self._pool = None
         self.eager_steps = 0
 
     # ---- scheduler / checkpoint hooks
@@ -112,9 +118,9 @@ class TrainStep:
         are applied inside the stem's gather kernel and the loss kernels: no mixed image or soft-target tensor exists.  The values live in
         a device buffer, so a captured step follows per-iteration changes."""
         mode = {None: 0.0, "mixup": 1.0, "cutmix": 2.0}[kind]
-        h = self._mix_host
-        h[0], h[1] = mode, float(lam)
-        h[2], h[3], h[4], h[5] = [float(v) for v in box]
+        # a fresh pinned buffer per call: the copy queued by an earlier call may not have run yet (replayed graphs let the host run ahead)
+        # and must still read its own values (the host allocator keeps the buffer until the copy is done)
+        h = torch.tensor([mode, float(lam)] + [float(v) for v in box], dtype=torch.float32).pin_memory()
         self.ws.mix.copy_(h, non_blocking=True)
 
     def state_dict(self):
@@ -159,46 +165,175 @@ class TrainStep:
         return loss
 
     def step(self, *inputs: torch.Tensor) -> torch.Tensor:
-        if self._graph is None:
+        """One training step on ``inputs``.  Before capture it runs eagerly; after capture it replays the graph captured for the inputs'
+        shapes (``ValueError`` for a shape that was not captured).  The returned loss is a static tensor of that graph: read or clone it
+        before the next step."""
+        if not self._graphs:
             self.eager_steps += 1
             return self._step(*inputs)
-        *statics, sloss = self._static
+        graph, statics, sloss = self._graph_for(inputs)
         for s_in, t in zip(statics, inputs):
             if t is not s_in:
                 s_in.copy_(t, non_blocking=True)
-        self._graph.replay()
+        graph.replay()
         ops.invalidate_prepared_weights()
         return sloss
 
     __call__ = step
 
-    # ---- whole step as one CUDA graph
+    def _graph_for(self, inputs) -> tuple:
+        entry = self._graphs.get(_signature(inputs))
+        if entry is None:  # same shapes, other dtypes: the copy into the static buffers converts them (as a single-shape capture always did)
+            shapes = _shapes(inputs)
+            entry = next((e for sig, e in self._graphs.items() if tuple(s for s, _ in sig) == shapes), None)
+        if entry is None:
+            # no eager fall-back: an eager step at a new shape could re-plan the step arena under the captured graphs
+            raise ValueError(f"TrainStep.step: no CUDA graph was captured for input shapes {list(_shapes(inputs))}; captured: "
+                             f"{[list(s) for s in self.captured_shapes]} (capture every shape the sampler draws with capture_shapes)")
+        return entry
+
+    # ---- whole step as one CUDA graph per input shape
     def capture(self, *inputs: torch.Tensor, warmup: int = 3):
-        """Warm up eagerly (workspace planning needs two steps), then capture fwd + loss + bwd (+ all-reduce) + optimizer tail."""
-        assert self._graph is None, "already captured"
+        """Warm up eagerly (workspace planning needs two steps), then capture fwd + loss + bwd (+ all-reduce) + optimizer tail: the
+        one-shape case of ``capture_shapes``."""
+        return self.capture_shapes([inputs], warmup=warmup)
+
+    def capture_shapes(self, examples: Sequence[Sequence[torch.Tensor]], warmup: int = 3):
+        """Capture one CUDA graph per distinct input signature (shapes and dtypes) of ``examples``: ``(x, y)`` tuples, or the inputs of
+        ``forward_loss`` (e.g. ``(images, text_tokens)``).  ``step()`` then replays the graph of its inputs' shapes.
+
+        Warm-up: ``max(warmup, 3)`` passes over the distinct examples in the order given, each step a real eager training step on that
+        example (with one shape, eager steps already taken count toward the passes, as ``capture`` always did).  The first pass raises every
+        arena key's record to its maximum over all shapes, the next re-plans the step arena once at that size and caches each shape's
+        descriptor tables at their final addresses.  The arena is then frozen: every graph bakes in its addresses, and a step that would
+        re-plan it raises.
+
+        The graphs are captured most demanding first (largest inputs) into ONE memory pool, so K shapes reserve about what the largest
+        needs: a graph's temporaries may reuse blocks another graph freed at the end of its capture, which is safe because the graphs replay
+        one at a time on one stream, and whatever outlives a capture (the static loss, per-shape caches such as the contrastive loss's
+        labels) stays allocated.  The static inputs of all shapes are views into one buffer per input position, sized for the largest.
+        Everything else is shared by all graphs because it already lives on the device: the flat parameters, gradients and optimizer
+        state, the learning rate, the mix buffer, the dropout generator, the RangeAugment curriculum position and the BatchNorm running
+        statistics; replaying shapes in any order follows the trajectory of eager steps in that order.
+
+        Data parallel: the bucket plan covers the flat gradient buffer, whose layout does not depend on the shape, so one plan serves every
+        graph; all ranks must replay the same shape at the same step (the variable-batch sampler draws the same (crop, batch) on every
+        rank), and a forward_loss that all-gathers features (CLIP) needs the same per-rank batch on every rank, as the reference's does.
+
+        ``launches_per_shape`` maps each captured tuple of input shapes to its launch count; ``launches_per_step`` is the largest of them
+        (the one count of a single-shape capture)."""
+        assert not self._graphs, "already captured"
+        by_sig: Dict[tuple, tuple] = {}
+        for ex in examples:
+            ex = tuple(ex)
+            by_sig.setdefault(_signature(ex), ex)
+        if not by_sig:
+            raise ValueError("capture_shapes: no examples")
+        if len({len(ex) for ex in by_sig.values()}) != 1:
+            raise ValueError("capture_shapes: every example must have the same number of inputs")
         dev = self.ws.device
-        statics = [t.to(dev).clone() for t in inputs]
+        statics = _static_buffers(list(by_sig.items()), dev)
+        passes = max(warmup, 3) - (self.eager_steps if len(by_sig) == 1 else 0)
         torch.cuda.synchronize(dev)
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):
-            for _ in range(max(0, max(warmup, 3) - self.eager_steps)):
-                self._step(*statics)
-                self.eager_steps += 1
+            for _ in range(max(0, passes)):
+                for sig, st in statics.items():
+                    for s_in, t in zip(st, by_sig[sig]):
+                        s_in.copy_(t)
+                    self._step(*st)
+                    self.eager_steps += 1
+            self._first = next(iter(by_sig))
+            for s_in, t in zip(statics[self._first], by_sig[self._first]):  # static_inputs hold the first example, as they always have
+                s_in.copy_(t)
         torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize(dev)
+        self.ws.freeze()
         gc.collect()  # no autograd graph of an eager step (leaf accumulators are bound to the stream they were created on) may survive into capture
-        graph = torch.cuda.CUDAGraph()
-        n0 = ops.launch_count
-        with torch.cuda.graph(graph):
-            sloss = self._step(*statics)
-        self.launches_per_step = ops.launch_count - n0
-        self._graph, self._static = graph, (*statics, sloss)
+        self._pool = torch.cuda.graph_pool_handle()
+        order = sorted(statics, key=lambda sig: -sum(math.prod(s) * d.itemsize for s, d in sig))  # stable: ties keep the given order
+        self.launches_per_shape: Dict[tuple, int] = {}
+        for sig in order:
+            graph = torch.cuda.CUDAGraph()
+            n0 = ops.launch_count
+            with torch.cuda.graph(graph, pool=self._pool):
+                # detached: the loss's autograd graph (and the activations its nodes hold) dies here, so the next capture can reuse them
+                sloss = self._step(*statics[sig]).detach()
+            gc.collect()
+            self.launches_per_shape[tuple(s for s, _ in sig)] = ops.launch_count - n0
+            self._graphs[sig] = (graph, statics[sig], sloss)
+        self.launches_per_step = max(self.launches_per_shape.values())
         return self
 
     @property
     def static_inputs(self):
-        return None if self._static is None else self._static[:-1]
+        """The static input buffers that ``step()`` copies into, those of the first example given to ``capture_shapes`` (with one shape they
+        hold the example until the next step with other inputs; with several, all shapes' buffers share memory)."""
+        return None if not self._graphs else self._graphs[self._first][1]
+
+    @property
+    def captured_shapes(self) -> List[tuple]:
+        """The captured tuples of input shapes, in capture order."""
+        return [tuple(s for s, _ in sig) for sig in self._graphs]
+
+    def graph_pool_bytes(self) -> int:
+        """Device memory the captured graphs' shared pool holds (0 before capture)."""
+        if self._pool is None:
+            return 0
+        segs = torch.cuda.memory_snapshot(mempool_id=self._pool, include_traces=False)
+        pool = tuple(self._pool)
+        return sum(s["total_size"] for s in segs if tuple(s.get("segment_pool_id", pool)) == pool)
+
+
+def _shapes(inputs) -> tuple:
+    return tuple(tuple(t.shape) for t in inputs)
+
+
+def _signature(inputs) -> tuple:
+    return tuple((tuple(t.shape), t.dtype) for t in inputs)
+
+
+def _static_buffers(examples: List[Tuple[tuple, tuple]], dev) -> Dict[tuple, tuple]:
+    """Per signature, static input buffers for its example: views into ONE buffer per input position, sized for the largest shape, with
+    the strides ``clone`` would give the example (channels-last stays channels-last).  The shapes share memory: a step copies its batch in."""
+    n_in = len(examples[0][1])
+    nbytes = [max(ex[i].numel() * ex[i].element_size() for _, ex in examples) for i in range(n_in)]
+    bufs = [torch.empty(max(n, 16), device=dev, dtype=torch.uint8) for n in nbytes]
+    out = {}
+    for sig, ex in examples:
+        views = []
+        for buf, t in zip(bufs, ex):
+            flat = buf[:t.numel() * t.element_size()].view(t.dtype)
+            views.append(flat.as_strided(t.shape, torch.empty_like(t, device="meta").stride()))
+        out[sig] = tuple(views)
+    return out
+
+
+def variable_batch_pairs(crop_w: int, crop_h: int, batch: int, max_scales: int = 5, check_scale: int = 32, min_w: int = 160, max_w: int = 320,
+                         min_h: int = 160, max_h: int = 320) -> List[Tuple[int, int, int]]:
+    """The sorted (h, w, batch) table the reference's variable-batch sampler draws from (``sampler.vbs``: crop_size_width / _height,
+    train_batch_size0, max_n_scales, check_scale, min/max_crop_size_width / _height).  Per axis, ``max_scales`` evenly spaced sizes from min
+    to max plus the base crop (exact duplicates merged), each rounded to the nearest multiple of ``check_scale`` (never below it, and one step
+    up where rounding lost more than 10 %), sorted.  The i-th height pairs with the i-th width, and each pair's batch keeps crop_h * crop_w *
+    batch pixels: max(1, int(round(pixels / (h * w), 2))).  Duplicate pairs are merged."""
+    def sizes(base, lo, hi):
+        vals = {float(v) for v in _linspace(lo, hi, max_scales)}
+        vals.add(base)
+        return sorted(_round_to(v, check_scale) for v in vals)
+    pixels = crop_w * crop_h * batch
+    pairs = {(h, w, max(1, int(round(pixels / (h * w), 2)))) for h, w in zip(sizes(crop_h, min_h, max_h), sizes(crop_w, min_w, max_w))}
+    return sorted(pairs)
+
+
+def _linspace(lo: float, hi: float, n: int) -> List[float]:
+    import numpy as np
+    return [float(v) for v in np.linspace(lo, hi, int(n))]
+
+
+def _round_to(v: float, d: int) -> int:
+    r = max(d, int(v + d / 2) // d * d)
+    return r + d if r < 0.9 * v else r
 
 
 def linear_curriculum(start: float, end: float, period: int) -> torch.Tensor:

@@ -1124,36 +1124,56 @@ class L2NormFn(torch.autograd.Function):
         return ops.l2norm_bwd(g, y, inv)
 
 
+def _padded_rows(G: int, G8: int, d: int, device) -> torch.Tensor:
+    """bf16 [G8, d] whose rows G..G8 are zero (one memset node); rows 0..G are the caller's to fill."""
+    t = torch.empty((G8, d), device=device, dtype=BF16)
+    if G8 > G:
+        ops._lib().cvb_memset_zero(t[G:].data_ptr(), (G8 - G) * d * 2, ops._stream())
+    return t
+
+
 class ClipLossFn(torch.autograd.Function):
     """ContrastiveLossClip._forward_clip (loss_fn/multi_modal_img_text/contrastive_loss_clip.py:56-97) with gather_all_features
     (utils/third_party/ddp_functional_utils.py:334-357): logits_per_image = s * img @ all_text^T, logits_per_text = s * text @ all_img^T,
     s = clamp(exp(logit_scale), 0, 100); loss = (CE(logits_per_image, arange + N*rank) + CE(logits_per_text, .)) / 2.
-    Data parallel: the features are all-gathered over NCCL in the forward and their gradients reduce-scattered in the backward."""
+    Data parallel: the features are all-gathered over NCCL in the forward and their gradients reduce-scattered in the backward (every rank
+    must bring the same batch N, as the reference's gather does).
+
+    Any global batch G = world * N: when G is not a multiple of 8 the gathered operands are [G8, d] buffers (G8 = G rounded up to 8) whose
+    last rows are zero, so the logits GEMMs run at N = G8; the loss kernels read C = G columns of the [N, G8] logits and write zeros into the
+    gradient's pad columns, so the pad adds nothing to the input gradients, and the weight gradients' pad rows are dropped (a view) before the
+    reduce-scatter.  The feature dimension d must be a multiple of 8."""
 
     @staticmethod
     def forward(ctx, img, txt, logit_scale, cfg):
         import torch.distributed as dist
         N, d = img.shape
+        if d % 8:
+            raise NotImplementedError(f"contrastive loss: the feature dim ({d}) must be a multiple of 8")
         img = img.to(BF16).contiguous()
         txt = txt.to(BF16).contiguous()
         world, rank = cfg.world, cfg.rank
-        if world > 1:
-            I_all = torch.empty((world * N, d), device=img.device, dtype=BF16)
-            T_all = torch.empty((world * N, d), device=img.device, dtype=BF16)
-            w1 = dist.all_gather_into_tensor(I_all, img, group=cfg.group, async_op=True)
-            w2 = dist.all_gather_into_tensor(T_all, txt, group=cfg.group, async_op=True)
-            w1.wait()
-            w2.wait()
+        G = world * N
+        G8 = (G + 7) // 8 * 8
+        if world > 1 or G8 != G:
+            I_all, T_all = _padded_rows(G, G8, d, img.device), _padded_rows(G, G8, d, img.device)
+            if world > 1:
+                w1 = dist.all_gather_into_tensor(I_all[:G], img, group=cfg.group, async_op=True)
+                w2 = dist.all_gather_into_tensor(T_all[:G], txt, group=cfg.group, async_op=True)
+                w1.wait()
+                w2.wait()
+            else:
+                I_all[:G].copy_(img)
+                T_all[:G].copy_(txt)
         else:
             I_all, T_all = img, txt
-        G = world * N
-        if G % 8 or d % 8:
-            raise NotImplementedError("contrastive loss: global batch and feature dim must be multiples of 8")
-        labels = getattr(cfg, "_labels", None)
-        if labels is None or labels.numel() != N:
-            labels = cfg._labels = torch.arange(N, device=img.device, dtype=torch.int64) + N * rank
-        Li = ops.pw_gemm(img, T_all, G)
-        Lt = ops.pw_gemm(txt, I_all, G)
+        # one labels tensor per (N, rank), kept: a CUDA graph captured at one batch reads its own labels while other batches run
+        cache = cfg.__dict__.setdefault("_labels", {})
+        labels = cache.get((N, rank))
+        if labels is None:
+            labels = cache[(N, rank)] = torch.arange(N, device=img.device, dtype=torch.int64) + N * rank
+        Li = ops.pw_gemm(img, T_all, G8)
+        Lt = ops.pw_gemm(txt, I_all, G8)
         li, lse_i, nv_i = ops.ce_fwd(Li, G, labels, -1, 0.0, logit_scale=logit_scale)
         lt, lse_t, nv_t = ops.ce_fwd(Lt, G, labels, -1, 0.0, logit_scale=logit_scale)
         ctx.cfg, ctx.plist, ctx.dims = cfg, [logit_scale], (N, d, G)
@@ -1170,12 +1190,13 @@ class ClipLossFn(torch.autograd.Function):
         D = _Dst(cfg, ctx.plist, img.device, True)
         dp = D.mat(0, 1, 1)
         scale = getattr(cfg, "scale", None)
-        dLi = ops.ce_bwd(Li, G, labels, -1, 0.0, lse_i, nv_i, g, scale, G, logit_scale=p, dlogit_scale=dp)
-        dLt = ops.ce_bwd(Lt, G, labels, -1, 0.0, lse_t, nv_t, g, scale, G, logit_scale=p, dlogit_scale=dp)
-        dI = ops.pw_gemm(dLi, ops.transpose_bf16(T_all), d, K=G)     # through the local rows of logits_per_image
-        dT = ops.pw_gemm(dLt, ops.transpose_bf16(I_all), d, K=G)
-        dT_all = ops.pw_wgrad(dLi, img, G, d)                         # fp32 [G, d]: through the gathered operand of logits_per_image
-        dI_all = ops.pw_wgrad(dLt, txt, G, d)
+        G8 = I_all.shape[0]
+        dLi = ops.ce_bwd(Li, G, labels, -1, 0.0, lse_i, nv_i, g, scale, G8, logit_scale=p, dlogit_scale=dp)
+        dLt = ops.ce_bwd(Lt, G, labels, -1, 0.0, lse_t, nv_t, g, scale, G8, logit_scale=p, dlogit_scale=dp)
+        dI = ops.pw_gemm(dLi, ops.transpose_bf16(T_all), d, K=G8)    # through the local rows of logits_per_image
+        dT = ops.pw_gemm(dLt, ops.transpose_bf16(I_all), d, K=G8)
+        dT_all = ops.pw_wgrad(dLi, img, G8, d)[:G]                    # fp32 [G, d]: through the gathered operand; pad rows dropped
+        dI_all = ops.pw_wgrad(dLt, txt, G8, d)[:G]
         if cfg.world > 1:
             dT_part = torch.empty((N, d), device=img.device, dtype=torch.float32)
             dI_part = torch.empty((N, d), device=img.device, dtype=torch.float32)

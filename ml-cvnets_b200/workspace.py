@@ -23,6 +23,7 @@ import torch
 from . import _lib as L
 
 ALIGN = 8  # every parameter starts at a multiple of 8 floats (32 B): the weight-gradient kernels use 16-byte vector reductions
+MAX_CAST_TABLES = 64  # descriptor tables kept per arena key before the first capture (one per input shape the step has seen)
 
 
 class Arena:
@@ -98,7 +99,9 @@ class StepWorkspace:
         self._plan: Dict[tuple, Tuple[List[int], int, int, int, int]] = {}  # arena key -> (record, o32, n32, o64, n64) of its slice
         self._used = set()
         self._buf32 = self._buf64 = None
-        self._cast_tables: Dict[tuple, Tuple[torch.Tensor, int, int]] = {}
+        # arena key -> {pointer signature -> (device descriptor table, count, max n, signature)}: one table per input shape of the step
+        self._cast_tables: Dict[tuple, Dict[tuple, tuple]] = {}
+        self.frozen = False           # set before the first CUDA-graph capture: the graphs bake in the arena's and the tables' addresses
         # data-parallel buckets
         self.group = None
         self.world = 1
@@ -156,10 +159,23 @@ class StepWorkspace:
         self._buf64 = torch.zeros(max(o64, 4), device=self.device, dtype=torch.float64)
         self._cast_tables.clear()
 
+    def _needs_replan(self) -> bool:
+        outgrown = any(r[0] > n32 or r[1] > n64 for r, _, n32, _, n64 in self._plan.values())
+        return bool(self._plan) and (self._buf32 is None or outgrown)
+
+    def freeze(self):
+        """No re-plan from now on (called before the first CUDA-graph capture).  Raises if the last eager step outgrew the plan."""
+        if self._needs_replan():
+            raise RuntimeError("StepWorkspace: the step arena is not planned for every shape yet (warm up every shape after the last "
+                               "one that raised a record)")
+        self.frozen = True
+
     def begin_step(self):
         """Zero the gradient buffer and the arena (two memset nodes), reset the per-step bookkeeping."""
-        outgrown = any(r[0] > n32 or r[1] > n64 for r, _, n32, _, n64 in self._plan.values())
-        if self._plan and (self._buf32 is None or outgrown):
+        if self._needs_replan():
+            if self.frozen:
+                raise RuntimeError("StepWorkspace: the step arena would be re-planned under captured CUDA graphs (a step's scratch outgrew "
+                                   "the plan made when the graphs were captured)")
             if torch.cuda.is_current_stream_capturing():
                 raise RuntimeError("StepWorkspace: run at least two eager steps before capturing the step in a CUDA graph")
             self._replan()
@@ -176,13 +192,15 @@ class StepWorkspace:
 
     # ------------------------------------------------------------------------------------------- fp64 statistics -> fp32 gradients
     def scatter64(self, key: tuple, pairs: Sequence[Tuple[torch.Tensor, torch.Tensor]]):
-        """dst32[i] = float(src64[i]) for every (src, dst) pair in ONE launch; the descriptor table is cached once the arena is planned
-        (all addresses are then static, which is what makes the step capturable)."""
+        """dst32[i] = float(src64[i]) for every (src, dst) pair in ONE launch; the descriptor table is cached per set of addresses once the
+        arena is planned (all addresses are then static, which is what makes the step capturable; a carve's offset may depend on the input
+        shape, so each captured shape keeps its own table)."""
         if not pairs:
             return
-        cached = self._cast_tables.get(key)
+        tables = self._cast_tables.setdefault(key, {})
         sig = tuple((s.data_ptr(), d.data_ptr(), s.numel()) for s, d in pairs)
-        if cached is None or cached[3] != sig:
+        cached = tables.get(sig)
+        if cached is None:
             if torch.cuda.is_current_stream_capturing():
                 raise RuntimeError("StepWorkspace: descriptor table missing during capture (run two eager warm-up steps first)")
             descs = (L.cvb_cast_desc * len(pairs))()
@@ -193,7 +211,9 @@ class StepWorkspace:
                 mx = max(mx, s.numel())
             table = torch.frombuffer(bytearray(bytes(descs)), dtype=torch.uint8).to(self.device)
             cached = (table, len(pairs), mx, sig)
-            self._cast_tables[key] = cached
+            if len(tables) >= MAX_CAST_TABLES and not self.frozen:  # carves of their own have fresh addresses: keep only recent tables
+                tables.pop(next(iter(tables)))
+            tables[sig] = cached
         from . import ops
         L.load().cvb_cast_f64_f32(cached[0].data_ptr(), cached[1], cached[2], torch.cuda.current_stream().cuda_stream)
         ops._count()
