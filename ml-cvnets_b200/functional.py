@@ -114,63 +114,76 @@ class _Dst:
 
     Workspace mode (inside ``engine.TrainStep``): straight into the flat gradient buffer -- ``p.grad`` is a view of it -- and the autograd
     function returns ``None`` for the parameters (no AccumulateGrad kernels, no gather for the optimizer / all-reduce).  Otherwise: fresh
-    slices of a per-call arena, returned to autograd as usual (what a plain ``loss.backward()`` on the drop-in modules gets)."""
+    slices of a per-call arena, returned to autograd as usual (what a plain ``loss.backward()`` on the drop-in modules gets).  Every method
+    names a destination by its parameter, which must be in ``params`` (the module's ``cfg.plist``)."""
 
     def __init__(self, cfg, params, device, use_ws: bool):
-        self.params = list(params)
+        self.cfg, self.params = cfg, list(params)
+        self.slot = {id(p): i for i, p in enumerate(self.params)}
+        assert len(self.slot) == len(self.params), f"a parameter appears twice in the plist of cfg {sorted(vars(cfg))}"
         self.ws = _ws_of(cfg, self.params) if use_ws else None
         self.key = (id(cfg), "bwd")
         self.ar = _arena(cfg, "bwd", self.ws, device)
         self.grads = [None] * len(self.params)
         self.late = []
 
-    def mat(self, i: int, rows: int, cols: int) -> torch.Tensor:
-        """zeroed fp32 [rows, cols] accumulator that IS the gradient of params[i] (same memory layout)."""
+    def _slot(self, p) -> int:
+        i = self.slot.get(id(p))
+        assert i is not None, f"gradient destination for a tensor that is not in the plist of cfg {sorted(vars(self.cfg))}"
+        return i
+
+    def mat(self, p, rows: int, cols: int) -> torch.Tensor:
+        """zeroed fp32 [rows, cols] accumulator that IS the gradient of ``p`` (same memory layout)."""
+        i = self._slot(p)
         if self.ws is not None:
-            return self.ws.gview(self.params[i]).view(rows, cols)
+            return self.ws.gview(p).view(rows, cols)
         v = self.ar.f32(rows, cols)
-        self.grads[i] = v.view(self.params[i].shape)
+        self.grads[i] = v.view(p.shape)
         return v
 
-    def padded(self, i: int, rows: int, cols: int, npad: int) -> torch.Tensor:
-        """zeroed fp32 [npad, cols] accumulator whose first ``rows`` rows are the gradient of params[i] ([rows, cols]; the kernel writes
+    def padded(self, p, rows: int, cols: int, npad: int) -> torch.Tensor:
+        """zeroed fp32 [npad, cols] accumulator whose first ``rows`` rows are the gradient of ``p`` ([rows, cols]; the kernel writes
         ``npad`` >= ``rows`` rows).  Padded rows only outside workspace mode: the scratch is sliced, not copied, into the gradient."""
         if npad == rows:
-            return self.mat(i, rows, cols)
+            return self.mat(p, rows, cols)
+        i = self._slot(p)
         assert self.ws is None, "padded gradient rows cannot be written into the flat gradient buffer"
         v = self.ar.f32(npad, cols)
-        self.grads[i] = v[:rows].view(self.params[i].shape)
+        self.grads[i] = v[:rows].view(p.shape)
         return v
 
-    def bn_bwd(self, stats, count, gamma, bn, eval_mode: bool, i: int, j: int) -> torch.Tensor:
-        """BatchNorm-backward finalize: writes (dgamma, dbeta) as the gradients of params i, j and returns the input-gradient coefficients."""
-        out = (self.ws.gview(self.params[i]), self.ws.gview(self.params[j])) if self.ws is not None else None
+    def bn_bwd(self, stats, count, bn, eval_mode: bool, gamma, beta) -> torch.Tensor:
+        """BatchNorm-backward finalize: writes (dgamma, dbeta) as the gradients of gamma, beta; returns the input-gradient coefficients."""
+        i, j = self._slot(gamma), self._slot(beta)
+        out = (self.ws.gview(gamma), self.ws.gview(beta)) if self.ws is not None else None
         dgb, coef = ops.bn_bwd_finalize(stats, count, gamma, bn, eval_mode=eval_mode, out=out)
         if self.ws is None:
             self.grads[i], self.grads[j] = dgb[0], dgb[1]
         return coef
 
-    def unprep(self, i: int, src, rows: int, cols: int, lds: int, kind: int, rot: int = 0, side: bool = False):
+    def unprep(self, p, src, rows: int, cols: int, lds: int, kind: int, rot: int = 0, side: bool = False):
         """kernel-layout gradient (rotated / padded / tap-major) -> the parameter's own layout."""
-        out = self.ws.gview(self.params[i]).view((rows, cols) if kind != PW.KIND_VECTOR_F32 else (rows,)) if self.ws is not None else None
+        i = self._slot(p)
+        out = self.ws.gview(p).view((rows, cols) if kind != PW.KIND_VECTOR_F32 else (rows,)) if self.ws is not None else None
         g = ops.unprep_grad(src, rows, cols, lds, kind, rot=rot, side=side, out=out)
         if self.ws is None:
-            self.grads[i] = g.view(self.params[i].shape)
+            self.grads[i] = g.view(p.shape)
 
-    def late64(self, i: int, v64: torch.Tensor):
-        """fp64 accumulator that is a gradient: converted after the last kernel that accumulates into it."""
-        self.late.append((i, v64))
+    def late64(self, p, v64: torch.Tensor):
+        """fp64 accumulator that is the gradient of ``p``: converted after the last kernel that accumulates into it."""
+        self.late.append((self._slot(p), v64))
 
-    def finish(self):
+    def finish(self, *params):
+        """The gradients of ``params`` in that order (``None`` for one that is ``None`` or not in the plist, and for all in workspace mode)."""
         if self.ws is not None:
             self.ws.scatter64(self.key, [(v, self.ws.gview(self.params[i]).view(v.shape)) for i, v in self.late])
             self.ws.unit_done(self.params)
-            return (None,) * len(self.params)
+            return (None,) * len(params)
         if self.late:
             self.ar.cast()
             for i, v in self.late:
                 self.grads[i] = self.ar.as_f32(v).view(self.params[i].shape)
-        return tuple(self.grads)
+        return tuple(self.grads[self.slot[id(p)]] if id(p) in self.slot else None for p in params)
 
 
 # ==================================================================================================================
@@ -199,7 +212,7 @@ class StemFn(torch.autograd.Function):
         ctx.cfg, ctx.dims, ctx.ev = cfg, (B, Ho, Wo, C0, M), (not cfg.bn.batch_stats,)
         ctx.saved = (A0, y, bn, Ws)
         ctx.plist = cfg.plist
-        ctx.save_for_backward(gamma)
+        ctx.save_for_backward(w, gamma, beta)
         return to_4d(out, B, Ho, Wo)
 
     @staticmethod
@@ -207,17 +220,17 @@ class StemFn(torch.autograd.Function):
         cfg = ctx.cfg
         B, Ho, Wo, C0, M = ctx.dims
         A0, y, bn, Ws = ctx.saved
-        (gamma,) = ctx.saved_tensors
+        w, gamma, beta = ctx.saved_tensors
         g2 = as_2d(to_bf16_cl(gout))
         D = _Dst(cfg, ctx.plist, g2.device, True)
         dz, sd = _bn_out_grad(ctx.lz_out, D, g2, y, bn, True)
-        coef = D.bn_bwd(sd, M, gamma, bn, ctx.ev[0], 1, 2)
+        coef = D.bn_bwd(sd, M, bn, ctx.ev[0], gamma, beta)
         dW = ops.pw_wgrad_side(dz, A0, C0, 32, g_mode=A_BNB, G2=y, g_p=coef, dW=D.ar.f32(C0, 32))
-        D.unprep(0, dW, C0, 27, 32, PW.KIND_ROWMAJOR, side=True)
+        D.unprep(w, dW, C0, 27, 32, PW.KIND_ROWMAJOR, side=True)
         # the image's gradient exists only when something upstream learns (the RangeAugment sampler parameters)
         dx = ops.stem_dgrad(dz, y, coef, Ws, B, Ho, Wo) if ctx.needs_input_grad[0] else None
         ops.join_side()
-        return (dx, None) + D.finish()
+        return (dx, None) + D.finish(w, gamma, beta)
 
 
 # ==================================================================================================================
@@ -265,13 +278,9 @@ class NeuralAugmentFn(torch.autograd.Function):
         red = D.ar.f64(3 * B, 3)
         ops.na_bwd_reduce(None if g_y is None else g_y.float().contiguous(), None if g_sq is None else g_sq.contiguous(), x, mix, key, coef, need_eps,
                           red)
-        dests, i = [None] * 6, 0
-        for j in range(6):
-            if full[j] is not None:
-                dests[j] = D.mat(i, 1, 1)
-                i += 1
+        dests = [None if p is None else D.mat(p, 1, 1) for p in full]
         ops.na_param_grad(tab, mu, red, full, B, dests)
-        return (None, None) + D.finish()
+        return (None, None) + D.finish(*ctx.plist)
 
 
 class NeuralAugLossFn(torch.autograd.Function):
@@ -327,7 +336,7 @@ class InvertedResidualFn(torch.autograd.Function):
         ctx.cfg, ctx.dims, ctx.ev = cfg, (B, Cin, H, W, Ho, Wo), tuple(not b for b in bs)  # BN modes snapshotted for backward
         ctx.saved = (x2, y1, bn1, y2, bn2, y3, bn3)
         ctx.plist = cfg.plist
-        ctx.save_for_backward(g1, g2, g3)
+        ctx.save_for_backward(w1, g1, b1, wd, g2, b2, w3, g3, b3)
         return to_4d(out, B, Ho, Wo)
 
     @staticmethod
@@ -337,42 +346,40 @@ class InvertedResidualFn(torch.autograd.Function):
         hid, cout, s = cfg.hid, cfg.cout, cfg.stride
         M, M2 = B * H * W, B * Ho * Wo
         x2, y1, bn1, y2, bn2, y3, bn3 = ctx.saved
-        g1, g2, g3 = ctx.saved_tensors
+        w1, g1, b1, wd, g2, b2, w3, g3, b3 = ctx.saved_tensors
         P = cfg.prep
         ev = ctx.ev
         dout = as_2d(to_bf16_cl(gout))
-        # parameter order: (w1, g1, b1, wd, g2, b2, w3, g3, b3)
         D = _Dst(cfg, ctx.plist, dout.device, True)
         ar = D.ar
         # red_1x1 + BN3 (no activation): dz3 = dout
         _, sd3 = _bn_out_grad(ctx.lz_out, D, dout, y3, bn3, False)
         sd2, sd1 = ar.f64(2, hid), ar.f64(2, hid)
-        c3 = D.bn_bwd(sd3, M2, g3, bn3, ev[2], 7, 8)
+        c3 = D.bn_bwd(sd3, M2, bn3, ev[2], g3, b3)
         dz2 = ops.pw_gemm(dout, P.get(cfg.i_w3t), hid, K=cout, a_mode=A_BNB, A2=y3, a_p=c3, e_mode=E_SILU_BWD, Y=y2,
                           e_p=(bn2[2], bn2[3]), col_stats=sd2)
-        ops.pw_wgrad_side(dout, y2, cout, hid, g_mode=A_BNB, G2=y3, g_p=c3, a_mode=A_AFF_SILU, a_p=(bn2[2], bn2[3]), dW=D.mat(6, cout, hid))
+        ops.pw_wgrad_side(dout, y2, cout, hid, g_mode=A_BNB, G2=y3, g_p=c3, a_mode=A_AFF_SILU, a_p=(bn2[2], bn2[3]), dW=D.mat(w3, cout, hid))
         # depthwise + BN2
-        c2 = D.bn_bwd(sd2, M2, g2, bn2, ev[1], 4, 5)
+        c2 = D.bn_bwd(sd2, M2, bn2, ev[1], g2, b2)
         dz1, dWt = ops.dw_bwd(dz2, y1, B, H, W, hid, s, P.get(cfg.i_wd), g_mode=A_BNB, Y2=y2, g_p=c2, x_mode=A_AFF_SILU,
                               x_p=(bn1[2], bn1[3]), col_stats=sd1, dWt=ar.f32(9, hid), dilation=cfg.dilation)
-        D.unprep(3, dWt, hid, 9, hid, PW.KIND_TAPMAJOR_F32)
+        D.unprep(wd, dWt, hid, 9, hid, PW.KIND_TAPMAJOR_F32)
         # exp_1x1 + BN1
-        c1 = D.bn_bwd(sd1, M, g1, bn1, ev[0], 1, 2)
+        c1 = D.bn_bwd(sd1, M, bn1, ev[0], g1, b1)
         lz = ctx.lz_in
         am, em, ap = _lazy_modes(lz)
         if lz is not None:  # the producer's BatchNorm (+SiLU) lives in this module's load mode: emit dz and its BN-backward sums for it
             lz.stats = ar.f64(2, Cin)
         dx = ops.pw_gemm(dz1, P.get(cfg.i_w1t), Cin, K=hid, a_mode=A_BNB, A2=y1, a_p=c1, e_mode=em, Y=x2 if lz is not None else None, e_p=ap,
                          R=dout if cfg.residual else None, col_stats=lz.stats if lz is not None else None)
-        ops.pw_wgrad_side(dz1, x2, hid, Cin, g_mode=A_BNB, G2=y1, g_p=c1, a_mode=am, a_p=ap, dW=D.mat(0, hid, Cin))
+        ops.pw_wgrad_side(dz1, x2, hid, Cin, g_mode=A_BNB, G2=y1, g_p=c1, a_mode=am, a_p=ap, dW=D.mat(w1, hid, Cin))
         ops.join_side()
-        return (to_4d(dx, B, H, W), None) + D.finish()
+        return (to_4d(dx, B, H, W), None) + D.finish(w1, g1, b1, wd, g2, b2, w3, g3, b3)
 
 
 # ==================================================================================================================
 # MobileViTBlockv2 (cvnets/modules/mobilevit_block.py:605-626) with LinearAttnFFN (cvnets/modules/transformer.py:248-264)
 # and LinearSelfAttention (cvnets/layers/linear_attention.py:134-161); unfold/fold live in the attention kernel's indexing.
-# Parameter order: [wd0, g0, b0, wl] + n x [ga, ba, wqkv, bqkv, wo, bo, gf, bf, w1, b1, w2, b2] + [gL, bL, wp, gp, bp]
 # ==================================================================================================================
 class MobileViTBlockv2Fn(torch.autograd.Function):
     @staticmethod
@@ -441,17 +448,16 @@ class MobileViTBlockv2Fn(torch.autograd.Function):
         D = _Dst(cfg, ctx.plist, dev, True)
         ar = D.ar
         # ---- conv_proj (GN -> 1x1 -> BN, no act)
-        base = 4 + 12 * n
         _, sdp = _bn_out_grad(ctx.lz_out, D, dout, yp, bnp, False)
         sd0 = ar.f64(2, C)
-        cp = D.bn_bwd(sdp, M, gp, bnp, ev[1], base + 3, base + 4)
+        cp = D.bn_bwd(sdp, M, bnp, ev[1], gp, bp)
         cs, ss = ar.f64(2, d), ar.f64(2, B)
         g = ops.pw_gemm(dout, P.get(cfg.i_wpt), d, K=C, a_mode=A_BNB, A2=yp, a_p=cp, e_mode=E_GN_BWD, Y=XL, e_p=(gL, None),
                         row_stats=(gnL[0], gnL[1]), rows_per_sample=HW, col_stats=cs, samp_stats=ss, gn_ws=ar.f64(2, B, d))
         ops.pw_wgrad_side(dout, XL, C, d, g_mode=A_BNB, G2=yp, g_p=cp, a_mode=A_GN, a_p=(gL, bL), row_stats=(gnL[0], gnL[1]),
-                          rows_per_sample=HW, dW=D.mat(base + 2, C, d))
-        D.late64(base + 0, cs[1])  # dgamma = sum v*xhat
-        D.late64(base + 1, cs[0])  # dbeta = sum v
+                          rows_per_sample=HW, dW=D.mat(wp, C, d))
+        D.late64(gL, cs[1])  # dgamma = sum v*xhat
+        D.late64(bL, cs[0])  # dbeta = sum v
         bsum = ar.f64(d)  # column sums of the residual-stream gradient = bias gradient of the producing conv
         dX = ops.gn_bwd_apply(g, XL, gnL, ss, gcount, B, HW, DRES=None, col_sum=bsum if n > 0 else None)
         # ---- attention/FFN units, last to first
@@ -459,48 +465,47 @@ class MobileViTBlockv2Fn(torch.autograd.Function):
             X, gnA, qkv, O, S, CTX, X1, gnF, h = blocks[i]
             ga, ba, wqkv, bqkv, wo, bo, gf, bf, w1, b1, w2, b2 = params[4 + 12 * i: 16 + 12 * i]
             ix = cfg.i_blk[i]
-            o = 4 + 12 * i
             # FFN: X2 = X1 + W2 silu(h) + b2 ; h = W1 GN(X1) + b1
-            D.late64(o + 11, bsum)  # db2
-            ops.pw_wgrad_side(dX, h, d, ffn, a_mode=A_SILU, dW=D.mat(o + 10, d, ffn))
+            D.late64(b2, bsum)
+            ops.pw_wgrad_side(dX, h, d, ffn, a_mode=A_SILU, dW=D.mat(w2, d, ffn))
             csh, csf, ssf, bsum1 = ar.f64(2, ffn), ar.f64(2, d), ar.f64(2, B), ar.f64(d)
             dh = ops.pw_gemm(dX, P.get(ix.w2t), ffn, K=d, e_mode=E_SILU_BWD, Y=h, col_stats=csh)
-            D.late64(o + 9, csh[0])  # db1 = column sums of dh
-            ops.pw_wgrad_side(dh, X1, ffn, d, a_mode=A_GN, a_p=(gf, bf), row_stats=(gnF[0], gnF[1]), rows_per_sample=HW, dW=D.mat(o + 8, ffn, d))
+            D.late64(b1, csh[0])  # column sums of dh
+            ops.pw_wgrad_side(dh, X1, ffn, d, a_mode=A_GN, a_p=(gf, bf), row_stats=(gnF[0], gnF[1]), rows_per_sample=HW, dW=D.mat(w1, ffn, d))
             gF = ops.pw_gemm(dh, P.get(ix.w1t), d, K=ffn, e_mode=E_GN_BWD, Y=X1, e_p=(gf, None), row_stats=(gnF[0], gnF[1]),
                              rows_per_sample=HW, col_stats=csf, samp_stats=ssf, gn_ws=ar.f64(2, B, d))
-            D.late64(o + 6, csf[1])
-            D.late64(o + 7, csf[0])
+            D.late64(gf, csf[1])
+            D.late64(bf, csf[0])
             dX1 = ops.gn_bwd_apply(gF, X1, gnF, ssf, gcount, B, HW, DRES=dX, col_sum=bsum1)
             # attention: X1 = X + Wo O + bo ; O = linattn(qkv) ; qkv = Wqkv GN(X) + bqkv
-            D.late64(o + 5, bsum1)  # dbo
-            ops.pw_wgrad_side(dX1, O, d, d, dW=D.mat(o + 4, d, d))
+            D.late64(bo, bsum1)
+            ops.pw_wgrad_side(dX1, O, d, d, dW=D.mat(wo, d, d))
             dO = ops.pw_gemm(dX1, P.get(ix.wot), d, K=d)
             dbq = ar.f32(2 * d + 8)
             dqkv = ops.linattn_bwd(qkv, dO, S, CTX, B, H, W, d, dbias=dbq)
             dWq = ops.pw_wgrad_side(dqkv, X, 2 * d + 8, d, a_mode=A_GN, a_p=(ga, ba), row_stats=(gnA[0], gnA[1]), rows_per_sample=HW,
                                     dW=ar.f32(2 * d + 8, d))
-            D.unprep(o + 2, dWq, 2 * d + 1, d, d, PW.KIND_ROWMAJOR, rot=1, side=True)
-            D.unprep(o + 3, dbq, 2 * d + 1, 1, 1, PW.KIND_VECTOR_F32, rot=1)
+            D.unprep(wqkv, dWq, 2 * d + 1, d, d, PW.KIND_ROWMAJOR, rot=1, side=True)
+            D.unprep(bqkv, dbq, 2 * d + 1, 1, 1, PW.KIND_VECTOR_F32, rot=1)
             csa, ssa, bsum = ar.f64(2, d), ar.f64(2, B), ar.f64(d)
             gA = ops.pw_gemm(dqkv, P.get(ix.wqkvt), d, K=2 * d + 8, e_mode=E_GN_BWD, Y=X, e_p=(ga, None), row_stats=(gnA[0], gnA[1]),
                              rows_per_sample=HW, col_stats=csa, samp_stats=ssa, gn_ws=ar.f64(2, B, d))
-            D.late64(o + 0, csa[1])
-            D.late64(o + 1, csa[0])
+            D.late64(ga, csa[1])
+            D.late64(ba, csa[0])
             dX = ops.gn_bwd_apply(gA, X, gnA, ssa, gcount, B, HW, DRES=dX1, col_sum=bsum if i > 0 else None)
         # ---- local_rep: 1x1 (no bias / norm) <- SiLU <- BN0 <- dw3x3
-        ops.pw_wgrad_side(dX, y0, d, C, a_mode=A_AFF_SILU, a_p=(bn0[2], bn0[3]), dW=D.mat(3, d, C))
+        ops.pw_wgrad_side(dX, y0, d, C, a_mode=A_AFF_SILU, a_p=(bn0[2], bn0[3]), dW=D.mat(wl, d, C))
         dz0 = ops.pw_gemm(dX, P.get(cfg.i_wlt), C, K=d, e_mode=E_SILU_BWD, Y=y0, e_p=(bn0[2], bn0[3]), col_stats=sd0)
-        c0 = D.bn_bwd(sd0, M, g0, bn0, ev[0], 1, 2)
+        c0 = D.bn_bwd(sd0, M, bn0, ev[0], g0, b0)
         lz = ctx.lz_in
         am, _, ap = _lazy_modes(lz)
         if lz is not None:
             lz.stats = ar.f64(2, C)
         dx, dWt = ops.dw_bwd(dz0, x2, B, H, W, C, 1, P.get(cfg.i_wd0), g_mode=A_BNB, Y2=y0, g_p=c0, x_mode=am, x_p=ap,
                              col_stats=lz.stats if lz is not None else None, dWt=ar.f32(9, C), dilation=cfg.dilation)
-        D.unprep(0, dWt, C, 9, C, PW.KIND_TAPMAJOR_F32)
+        D.unprep(wd0, dWt, C, 9, C, PW.KIND_TAPMAJOR_F32)
         ops.join_side()
-        return (to_4d(dx, B, H, W), None) + D.finish()
+        return (to_4d(dx, B, H, W), None) + D.finish(*params)
 
 
 # ==================================================================================================================
@@ -531,12 +536,13 @@ class PoolLinearFn(torch.autograd.Function):
         else:
             g = torch.zeros((B, npad), device=pooled.device, dtype=BF16)
             g[:, :ncls] = gout
+        w, b = ctx.plist
         D = _Dst(cfg, ctx.plist, pooled.device, npad == ncls)
-        ops.pw_wgrad_side(g, pooled, npad, C, dW=D.padded(0, ncls, C, npad), dbias=D.padded(1, ncls, 1, npad).view(npad))
+        ops.pw_wgrad_side(g, pooled, npad, C, dW=D.padded(w, ncls, C, npad), dbias=D.padded(b, ncls, 1, npad).view(npad))
         dp = ops.pw_gemm(g, cfg.prep.get(cfg.i_wt), C, K=npad)
         dx = ops.global_pool_bwd(dp, B, H * W)
         ops.join_side()
-        return (to_4d(dx, B, H, W), None) + D.finish()
+        return (to_4d(dx, B, H, W), None) + D.finish(w, b)
 
 
 # ==================================================================================================================
@@ -612,7 +618,7 @@ class PointwiseConvFn(torch.autograd.Function):
             ctx.saved = (x2,)
         ctx.cfg, ctx.dims, ctx.plist, ctx.has_res = cfg, (B, Cin, H, W, Ho, Wo), cfg.plist, residual is not None
         ctx.x_fp32_nchw = x.dtype == torch.float32 and x.is_contiguous()
-        ctx.save_for_backward(gamma) if gamma is not None else None
+        ctx.save_for_backward(w, bias, gamma, beta)
         return to_4d(out, B, Ho, Wo)
 
     @staticmethod
@@ -625,10 +631,10 @@ class PointwiseConvFn(torch.autograd.Function):
         dout = as_2d(to_bf16_cl(gout))
         x2 = ctx.saved[0]
         Kc = x2.shape[1]
+        w, bias, gamma, beta = ctx.saved_tensors
         D = _Dst(cfg, ctx.plist, dout.device, True)
-        has_bias = cfg.has_bias
-        db = D.mat(1, 1, cout).view(cout) if has_bias else None
-        dW = D.ar.f32(cout, Kc) if dense else D.mat(0, cout, Cin)
+        db = D.mat(bias, 1, cout).view(cout) if cfg.has_bias else None
+        dW = D.ar.f32(cout, Kc) if dense else D.mat(w, cout, Cin)
         need_dx = ctx.needs_input_grad[0]
         dA = dx = None
         # the ViT / CLIP image stem (fp32 3-channel image, 4x4 stride-4 pad-1 windows): its image gradient, which the RangeAugment augmentor
@@ -637,12 +643,10 @@ class PointwiseConvFn(torch.autograd.Function):
                       and H % 4 == 0 and W % 4 == 0 and cout % 16 == 0 and cout <= 320)
         if cfg.bn is not None:
             _, y, bn, ob = ctx.saved
-            (gamma,) = ctx.saved_tensors
             if ob is not None:
                 dout = ops.act_bwd(dout, ob, cfg.act)
             dz, sd = _bn_out_grad(None, D, dout, y, bn, cfg.act == ops.ACT_SILU)
-            gi = 2 if has_bias else 1  # (gamma, beta) follow (w[, bias]) in plist
-            c = D.bn_bwd(sd, M, gamma, bn, ctx.ev[0], gi, gi + 1)
+            c = D.bn_bwd(sd, M, bn, ctx.ev[0], gamma, beta)
             if patch_stem:
                 dx = ops.patch_stem_dgrad(dz, y, c, P.get(cfg.i_w), B, Ho, Wo)
             elif need_dx:
@@ -654,17 +658,11 @@ class PointwiseConvFn(torch.autograd.Function):
                 dA = ops.pw_gemm(dh, P.get(cfg.i_wt), Kc, K=cout)
             ops.pw_wgrad_side(dh, x2, cout, Kc, dW=dW, dbias=db)
         if dense:
-            D.unprep(0, dW, cout, cfg.k * cfg.k * Cin, Kc, PW.KIND_PATCH, rot=cfg.k * cfg.k, side=True)
+            D.unprep(w, dW, cout, cfg.k * cfg.k * Cin, Kc, PW.KIND_PATCH, rot=cfg.k * cfg.k, side=True)
         ops.join_side()
         if dA is not None:
             dx = to_4d(ops.col2im(dA, B, Cin, H, W, cfg.k, cfg.stride, cfg.pad) if dense else dA, B, H, W)
-        grads = D.finish()
-        full = [grads[0], None, None, None]
-        if has_bias:
-            full[1] = grads[1]
-        if cfg.bn is not None:
-            full[2], full[3] = grads[2 if has_bias else 1], grads[3 if has_bias else 2]
-        return (dx, None, gout if ctx.has_res else None) + tuple(full)
+        return (dx, None, gout if ctx.has_res else None) + D.finish(w, bias, gamma, beta)
 
 
 class DepthwiseConvFn(torch.autograd.Function):
@@ -689,7 +687,7 @@ class DepthwiseConvFn(torch.autograd.Function):
             out = ops.act_fwd(y, cfg.act) if cfg.act is not None else y
             ctx.saved = (x2, y)
         ctx.cfg, ctx.dims, ctx.plist = cfg, (B, C, H, W, Ho, Wo), cfg.plist
-        ctx.save_for_backward(gamma) if gamma is not None else None
+        ctx.save_for_backward(w, gamma, beta)
         return to_4d(out, B, Ho, Wo)
 
     @staticmethod
@@ -699,12 +697,12 @@ class DepthwiseConvFn(torch.autograd.Function):
         M2 = B * Ho * Wo
         dout = as_2d(to_bf16_cl(gout))
         taps = cfg.k * cfg.k
+        w, gamma, beta = ctx.saved_tensors
         D = _Dst(cfg, ctx.plist, dout.device, True)
         if cfg.bn is not None:
             x2, y, bn = ctx.saved
-            (gamma,) = ctx.saved_tensors
             dz, sd = _bn_out_grad(None, D, dout, y, bn, cfg.act is not None)
-            c = D.bn_bwd(sd, M2, gamma, bn, ctx.ev[0], 1, 2)
+            c = D.bn_bwd(sd, M2, bn, ctx.ev[0], gamma, beta)
             dx, dWt = ops.dw_bwd(dz, x2, B, H, W, C, cfg.stride, cfg.prep.get(cfg.i_w), g_mode=A_BNB, Y2=y, g_p=c, dWt=D.ar.f32(taps, C),
                                  dilation=cfg.dilation, ksize=cfg.k)
         else:
@@ -712,9 +710,8 @@ class DepthwiseConvFn(torch.autograd.Function):
             dz = ops.act_bwd(dout, y, cfg.act) if cfg.act is not None else dout
             dx, dWt = ops.dw_bwd(dz, x2, B, H, W, C, cfg.stride, cfg.prep.get(cfg.i_w), dWt=D.ar.f32(taps, C), dilation=cfg.dilation,
                                  ksize=cfg.k)
-        D.unprep(0, dWt, C, taps, C, PW.KIND_TAPMAJOR_F32)
-        grads = D.finish()
-        return (to_4d(dx, B, H, W), None, grads[0]) + ((grads[1], grads[2]) if cfg.bn is not None else (None, None))
+        D.unprep(w, dWt, C, taps, C, PW.KIND_TAPMAJOR_F32)
+        return (to_4d(dx, B, H, W), None) + D.finish(w, gamma, beta)
 
 
 class GroupNorm1Fn(torch.autograd.Function):
@@ -731,7 +728,7 @@ class GroupNorm1Fn(torch.autograd.Function):
         gn = ops.gn_finalize(st, rps * C, cfg.eps)
         out = ops.apply_load_mode(x2, ops.A_GN, C, a_p=(gamma, beta, None), row_stats=(gn[0], gn[1]), rows_per_sample=rps)
         ctx.cfg, ctx.dims, ctx.saved, ctx.plist = cfg, (B, C, H, W), (x2, gn), cfg.plist
-        ctx.save_for_backward(gamma)
+        ctx.save_for_backward(gamma, beta)
         return to_4d(out, B, H, W)
 
     @staticmethod
@@ -739,14 +736,14 @@ class GroupNorm1Fn(torch.autograd.Function):
         cfg = ctx.cfg
         B, C, H, W = ctx.dims
         x2, gn = ctx.saved
-        (gamma,) = ctx.saved_tensors
+        gamma, beta = ctx.saved_tensors
         dout = as_2d(to_bf16_cl(gout))
         D = _Dst(cfg, ctx.plist, dout.device, True)
         dgb, wsp = D.ar.f64(2, C), D.ar.f64(2, B)
         dx = ops.gn_bwd(dout, x2, gn, gamma, float(H * W * C), B, H * W, dgb[0], dgb[1], wsp)
-        D.late64(0, dgb[0])
-        D.late64(1, dgb[1])
-        return (to_4d(dx, B, H, W), None) + D.finish()
+        D.late64(gamma, dgb[0])
+        D.late64(beta, dgb[1])
+        return (to_4d(dx, B, H, W), None) + D.finish(gamma, beta)
 
 
 class LayerNormFn(torch.autograd.Function):
@@ -761,7 +758,7 @@ class LayerNormFn(torch.autograd.Function):
         ln = ops.ln_stats(x2, cfg.eps)
         out = ops.apply_load_mode(x2, ops.A_GN, C, a_p=(gamma, beta, None), row_stats=(ln[0], ln[1]), rows_per_sample=1)
         ctx.cfg, ctx.shape, ctx.saved, ctx.plist = cfg, shape, (x2, ln), cfg.plist
-        ctx.save_for_backward(gamma)
+        ctx.save_for_backward(gamma, beta)
         return out.view(shape)
 
     @staticmethod
@@ -769,14 +766,14 @@ class LayerNormFn(torch.autograd.Function):
         cfg = ctx.cfg
         C = ctx.shape[-1]
         x2, ln = ctx.saved
-        (gamma,) = ctx.saved_tensors
+        gamma, beta = ctx.saved_tensors
         dy = gout.reshape(-1, C).to(BF16).contiguous()
         D = _Dst(cfg, ctx.plist, dy.device, True)
         cs = D.ar.f64(2, C)
         dx = ops.ln_bwd(dy, x2, ln, gamma, cs)
-        D.late64(0, cs[1])
-        D.late64(1, cs[0])
-        return (dx.view(ctx.shape), None) + D.finish()
+        D.late64(gamma, cs[1])
+        D.late64(beta, cs[0])
+        return (dx.view(ctx.shape), None) + D.finish(gamma, beta)
 
 
 class LinearSelfAttentionFn(torch.autograd.Function):
@@ -812,10 +809,11 @@ class LinearSelfAttentionFn(torch.autograd.Function):
         B, d, Pp, N, Mp = ctx.dims
         Pw = cfg.prep
         x2, qkv, xp2, qkp, O, S, CTX = ctx.saved
+        wqkv, bqkv, wo, bo = ctx.plist
         dy = as_2d(to_bf16_cl(gout))
         D = _Dst(cfg, ctx.plist, dy.device, True)
         ar = D.ar
-        ops.pw_wgrad_side(dy, O, d, d, dW=D.mat(2, d, d), dbias=D.mat(3, 1, d).view(d))
+        ops.pw_wgrad_side(dy, O, d, d, dW=D.mat(wo, d, d), dbias=D.mat(bo, 1, d).view(d))
         dO = ops.pw_gemm(dy, Pw.get(cfg.i_wot), d, K=d)
         dbq = ar.f32(2 * d + 8)
         dWq = ar.f32(2 * d + 8, d)
@@ -830,10 +828,10 @@ class LinearSelfAttentionFn(torch.autograd.Function):
             ops.pw_wgrad_side(dqkv, x2, 2 * d + 8, d, dW=dWq)
             dx = ops.pw_gemm(dqkv, Pw.get(cfg.i_wqkvt), d, K=2 * d + 8)
             dxp = to_4d(ops.pw_gemm(dqkp, Pw.get(cfg.i_wqkvt), d, K=2 * d + 8), B, Pp, Mp)
-        D.unprep(0, dWq, 2 * d + 1, d, d, PW.KIND_ROWMAJOR, rot=1, side=True)
-        D.unprep(1, dbq, 2 * d + 1, 1, 1, PW.KIND_VECTOR_F32, rot=1)
+        D.unprep(wqkv, dWq, 2 * d + 1, d, d, PW.KIND_ROWMAJOR, rot=1, side=True)
+        D.unprep(bqkv, dbq, 2 * d + 1, 1, 1, PW.KIND_VECTOR_F32, rot=1)
         ops.join_side()
-        return (to_4d(dx, B, Pp, N), None, dxp, gout if ctx.has_res else None) + D.finish()
+        return (to_4d(dx, B, Pp, N), None, dxp, gout if ctx.has_res else None) + D.finish(wqkv, bqkv, wo, bo)
 
 
 class LinearFn(torch.autograd.Function):
@@ -846,6 +844,7 @@ class LinearFn(torch.autograd.Function):
         x2 = x.reshape(-1, cin).to(BF16).contiguous()
         y = ops.pw_gemm(x2, cfg.prep.get(cfg.i_w), npad, bias=cfg.prep.get(cfg.i_b) if b is not None else None)
         ctx.cfg, ctx.shape, ctx.saved, ctx.plist = cfg, shape, (x2,), cfg.plist
+        ctx.save_for_backward(w, b)
         return y[:, :cout].view(*shape[:-1], cout)
 
     @staticmethod
@@ -861,13 +860,12 @@ class LinearFn(torch.autograd.Function):
             g = gp
         else:
             g = g.to(BF16).contiguous()
-        has_b = len(ctx.plist) > 1
+        w, b = ctx.saved_tensors
         D = _Dst(cfg, ctx.plist, g.device, npad == cout)
-        ops.pw_wgrad_side(g, x2, npad, cin, dW=D.padded(0, cout, cin, npad), dbias=D.padded(1, cout, 1, npad).view(npad) if has_b else None)
+        ops.pw_wgrad_side(g, x2, npad, cin, dW=D.padded(w, cout, cin, npad), dbias=D.padded(b, cout, 1, npad).view(npad) if b is not None else None)
         dx = ops.pw_gemm(g, cfg.prep.get(cfg.i_wt), cin, K=npad)
         ops.join_side()
-        grads = D.finish()
-        return (dx.view(ctx.shape), None, grads[0], grads[1] if has_b else None)
+        return (dx.view(ctx.shape), None) + D.finish(w, b)
 
 
 class GlobalPoolFn(torch.autograd.Function):
@@ -1024,20 +1022,21 @@ class VitTokensFn(torch.autograd.Function):
         N, n_pos = nh * nw, pos.shape[-2]
         p2 = as_2d(to_bf16_cl(patch))
         out = ops.vit_tokens_interp_fwd(p2, pos, cls, B, N, C)
-        ctx.cfg, ctx.dims, ctx.plist, ctx.has_cls = cfg, (B, C, nh, nw, n_pos), cfg.plist, cls is not None
+        ctx.cfg, ctx.dims, ctx.plist = cfg, (B, C, nh, nw, n_pos), cfg.plist
+        ctx.save_for_backward(pos, cls)
         return out
 
     @staticmethod
     def backward(ctx, gout):
         B, C, nh, nw, n_pos = ctx.dims
         N = nh * nw
+        pos, cls = ctx.saved_tensors
         g = gout.to(BF16).contiguous()
         D = _Dst(ctx.cfg, ctx.plist, g.device, True)
-        dpos = D.mat(0, n_pos, C)
-        dcls = D.mat(1, 1, C).view(C) if ctx.has_cls else None
+        dpos = D.mat(pos, n_pos, C)
+        dcls = D.mat(cls, 1, C).view(C) if cls is not None else None
         dpatch = ops.vit_tokens_interp_bwd(g, dpos, dcls, B, N, C)
-        grads = D.finish()
-        return to_4d(dpatch, B, nh, nw), None, grads[0], grads[1] if ctx.has_cls else None
+        return (to_4d(dpatch, B, nh, nw), None) + D.finish(pos, cls)
 
 
 # ==================================================================================================================
@@ -1049,20 +1048,21 @@ class EmbeddingFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, tokens, cfg, table, pos):
         out = ops.embedding_fwd(tokens, table, pos)
-        ctx.cfg, ctx.plist, ctx.tokens, ctx.shape, ctx.has_pos = cfg, cfg.plist, tokens, tuple(table.shape), pos is not None
+        ctx.cfg, ctx.plist, ctx.tokens = cfg, cfg.plist, tokens
+        ctx.save_for_backward(table, pos)
         return out
 
     @staticmethod
     def backward(ctx, g):
-        V, C = ctx.shape
+        table, pos = ctx.saved_tensors
+        V, C = table.shape
         B, S = ctx.tokens.shape
         g = g.to(BF16).contiguous()
         D = _Dst(ctx.cfg, ctx.plist, g.device, True)
-        dtable = D.mat(0, V, C)
-        dpos = D.mat(1, S, C) if ctx.has_pos else None
+        dtable = D.mat(table, V, C)
+        dpos = D.mat(pos, S, C) if pos is not None else None
         ops.embedding_bwd(g, ctx.tokens, dtable, dpos)
-        grads = D.finish()
-        return None, None, grads[0], grads[1] if ctx.has_pos else None
+        return (None, None) + D.finish(table, pos)
 
 
 class EotGatherFn(torch.autograd.Function):
@@ -1097,12 +1097,13 @@ class ProjectionFn(torch.autograd.Function):
     def backward(ctx, g):
         din, dout = ctx.shape
         (x2,) = ctx.saved
+        (P,) = ctx.plist
         g = g.to(BF16).contiguous()
         D = _Dst(ctx.cfg, ctx.plist, g.device, True)
-        ops.pw_wgrad_side(x2, g, din, dout, dW=D.mat(0, din, dout))
+        ops.pw_wgrad_side(x2, g, din, dout, dW=D.mat(P, din, dout))
         dx = ops.pw_gemm(g, ctx.cfg.prep.get(ctx.cfg.i_p), din, K=dout)
         ops.join_side()
-        return (dx, None) + D.finish()
+        return (dx, None) + D.finish(P)
 
 
 class L2NormFn(torch.autograd.Function):
@@ -1188,7 +1189,7 @@ class ClipLossFn(torch.autograd.Function):
         img, txt, I_all, T_all, Li, Lt, labels, lse_i, nv_i, lse_t, nv_t, p = ctx.saved
         g = (gout.float() * 0.5).contiguous()
         D = _Dst(cfg, ctx.plist, img.device, True)
-        dp = D.mat(0, 1, 1)
+        dp = D.mat(p, 1, 1)
         scale = getattr(cfg, "scale", None)
         G8 = I_all.shape[0]
         dLi = ops.ce_bwd(Li, G, labels, -1, 0.0, lse_i, nv_i, g, scale, G8, logit_scale=p, dlogit_scale=dp)
@@ -1207,8 +1208,7 @@ class ClipLossFn(torch.autograd.Function):
         else:
             dT_part, dI_part = dT_all, dI_all
         dimg, dtxt = ops.add_bf16_f32(dI, dI_part), ops.add_bf16_f32(dT, dT_part)
-        grads = D.finish()
-        return dimg, dtxt, (grads[0].view(()) if grads[0] is not None else None), None
+        return (dimg, dtxt) + D.finish(p) + (None,)
 
 
 # ==================================================================================================================
@@ -1329,12 +1329,10 @@ def _encoder_backward(st, dY, cfg, plist):
     ffn = cfg.ffn
     P = cfg.prep
     x2, ln1, qkv, O, LSE, X1, ln2, h, ha, amask, kpm = st.x2, st.ln1, st.qkv, st.O, st.LSE, st.X1, st.ln2, st.h, st.ha, st.amask, st.kpm
-    g1, b1, g2, b2 = plist[0], plist[1], plist[6], plist[7]
-    dev = x2.device
-    # parameter order: (g1, b1, wqkv, bqkv, wo, bo, g2, b2, w1, bb1, w2, bb2)
-    D = _Dst(cfg, plist, dev, True)
+    g1, b1, wqkv, bqkv, wo, bo, g2, b2, w1, bb1, w2, bb2 = plist
+    D = _Dst(cfg, plist, x2.device, True)
     ar = D.ar
-    vec = lambda i, n: D.mat(i, 1, n).view(n)  # noqa: E731
+    vec = lambda p, n: D.mat(p, 1, n).view(n)  # noqa: E731
 
     def ln_wgrad(G, xn, X, ln, gamma, beta, N, dW, dbias):
         """Weight gradient of the forward's ln_proj: on the kept normalised tokens, else through the LayerNorm load mode on X."""
@@ -1343,50 +1341,50 @@ def _encoder_backward(st, dY, cfg, plist):
         return ops.pw_wgrad_side(G, X, N, C, a_mode=A_GN, a_p=(gamma, beta), row_stats=(ln[0], ln[1]), rows_per_sample=1, dW=dW, dbias=dbias)
 
     # ---- FFN
-    db2, db1 = vec(11, C), vec(9, ffn)
+    db2, db1 = vec(bb2, C), vec(bb1, ffn)
     drop = st.drop
     if drop is not None:
         p, p_ffn, p_row = drop
         k1, k2, k3 = st.keys
         dF = ops.dropout_bwd(dY, p, k2, p_row=p_row, rows_per_sample=S)  # gradient of the FFN branch; the residual path keeps dY
-        ops.pw_wgrad_side(dF, ha, C, ffn, dW=D.mat(10, C, ffn), dbias=db2)
+        ops.pw_wgrad_side(dF, ha, C, ffn, dW=D.mat(w2, C, ffn), dbias=db2)
         dha = ops.pw_gemm(dF, P.get(cfg.i_w2t), ffn, K=C)
         if k3 is not None:
             dha = ops.dropout_bwd(dha, p_ffn, k3)
         dh = ops.act_bwd(dha, h, cfg.act)
     elif cfg.act == ops.ACT_SILU:
-        ops.pw_wgrad_side(dY, h, C, ffn, a_mode=A_SILU, dW=D.mat(10, C, ffn), dbias=db2)
+        ops.pw_wgrad_side(dY, h, C, ffn, a_mode=A_SILU, dW=D.mat(w2, C, ffn), dbias=db2)
         dh = ops.pw_gemm(dY, P.get(cfg.i_w2t), ffn, K=C, e_mode=E_SILU_BWD, Y=h)
     else:
-        ops.pw_wgrad_side(dY, ha, C, ffn, dW=D.mat(10, C, ffn), dbias=db2)
+        ops.pw_wgrad_side(dY, ha, C, ffn, dW=D.mat(w2, C, ffn), dbias=db2)
         dh = ops.act_bwd(ops.pw_gemm(dY, P.get(cfg.i_w2t), ffn, K=C), h, cfg.act)
-    ln_wgrad(dh, st.xn2, X1, ln2, g2, b2, ffn, D.mat(8, ffn, C), db1)
+    ln_wgrad(dh, st.xn2, X1, ln2, g2, b2, ffn, D.mat(w1, ffn, C), db1)
     csf = ar.f64(2, C)
     vF = ops.pw_gemm(dh, P.get(cfg.i_w1t), C, K=ffn)
     if drop is None:
         bsum1 = ar.f64(C)
         dX1 = ops.ln_bwd(vF, X1, ln2, g2, csf, DRES=dY, col_sum=bsum1)  # bsum1 = column sums of dX1 = d(out_proj bias)
-        D.late64(5, bsum1)
+        D.late64(bo, bsum1)
         dA = dX1
         dbo = None
     else:
         dX1 = ops.ln_bwd(vF, X1, ln2, g2, csf, DRES=dY)
         dA = ops.dropout_bwd(dX1, p, k1, p_row=p_row, rows_per_sample=S)  # gradient of the attention branch (out_proj output)
-        dbo = vec(5, C)
-    D.late64(6, csf[1])
-    D.late64(7, csf[0])
+        dbo = vec(bo, C)
+    D.late64(g2, csf[1])
+    D.late64(b2, csf[0])
     # ---- attention
-    ops.pw_wgrad_side(dA, O, C, C, dW=D.mat(4, C, C), dbias=dbo)
+    ops.pw_wgrad_side(dA, O, C, C, dW=D.mat(wo, C, C), dbias=dbo)
     dO = ops.pw_gemm(dA, P.get(cfg.i_wot), C, K=C)
     dqkv = ops.mha_bwd(qkv, O, dO, LSE, N, S, cfg.heads, cfg.head_dim, cfg.scale, amask, kpm)
-    ln_wgrad(dqkv, st.xn1, x2, ln1, g1, b1, 3 * C, D.mat(2, 3 * C, C), vec(3, 3 * C))
+    ln_wgrad(dqkv, st.xn1, x2, ln1, g1, b1, 3 * C, D.mat(wqkv, 3 * C, C), vec(bqkv, 3 * C))
     csa = ar.f64(2, C)
     vA = ops.pw_gemm(dqkv, P.get(cfg.i_wqkvt), C, K=3 * C)
     dx = ops.ln_bwd(vA, x2, ln1, g1, csa, DRES=dX1)
-    D.late64(0, csa[1])
-    D.late64(1, csa[0])
+    D.late64(g1, csa[1])
+    D.late64(b1, csa[0])
     ops.join_side()
-    return dx, D.finish()
+    return dx, D.finish(*plist)
 
 
 class TransformerEncoderFn(torch.autograd.Function):

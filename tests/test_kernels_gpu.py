@@ -722,7 +722,7 @@ def test_ln_bwd(ops, M, C, res):
 
 
 # ------------------------------------------------------------------------------------------------- fused training-step tail
-def test_flat_adamw_matches_torch_pipeline():
+def test_flat_adamw_matches_torch_pipeline(ops):
     """cvb_grad_norm + cvb_adamw_step vs GradScaler.unscale_ -> clip_grad_norm_(10) -> torch.optim.AdamW -> GradScaler.update
     (engine/training_engine.py:289-312), including a step with an inf gradient (skipped, scale backed off)."""
     import copy

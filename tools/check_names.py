@@ -25,8 +25,9 @@ def check(path):
                 if node.args.kwarg:
                     bound.add(node.args.kwarg.arg)
         elif isinstance(node, ast.Lambda):
-            for a in node.args.args + node.args.kwonlyargs:
-                bound.add(a.arg)
+            for a in node.args.args + node.args.kwonlyargs + node.args.posonlyargs + [node.args.vararg, node.args.kwarg]:
+                if a is not None:
+                    bound.add(a.arg)
         elif isinstance(node, ast.Name) and isinstance(node.ctx, (ast.Store, ast.Del)):
             bound.add(node.id)
         elif isinstance(node, ast.ExceptHandler) and node.name:
