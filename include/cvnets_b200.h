@@ -425,6 +425,23 @@ CVB_API int cvb_add_bf16_f32(const void* A, const float* B, void* OUT, int64_t n
 CVB_API int cvb_zs_class_embed(const void* X, int ldx, int R, const int* perm, int Cl, int M, int d, float* table, cvb_stream_t stream);
 CVB_API int cvb_zs_logits_topk(const void* img, int ldi, const float* table, int B, int d, int Cl, float scale, const int64_t* targets,
                                float* logits, int64_t* hits, cvb_stream_t stream);
+/* ---------------------------------------------------------------------------------------------------------------
+ * Validation of the classification recipes (engine/training_engine.py:val_epoch: loss, top1, top5; csrc/metrics.cu)
+ *   cls metrics: logits bf16 [B, ld] (C valid columns, C >= 1), target int64 [B].  Per row whose target is not ignore_index: the cross
+ *              entropy log-sum-exp - logit[target] WITHOUT label smoothing (the reference's loss in eval mode), and the rank of the
+ *              target = the number of classes whose bf16 logit is STRICTLY greater than the target's; a row is a top-k hit iff rank < k
+ *              (ties at the k-th place count for the target; C < 5 makes every counted row a top-5 hit).  A target outside [0, C) that is
+ *              not ignore_index is a counted miss with a NaN loss.  Adds into device accumulators: loss_sum fp64[1] += sum of the
+ *              per-row losses, counts int64[3] += {top-1 hits, top-5 hits, counted rows}.  row_loss: fp32 [B] scratch; ticket: int[1]
+ *              scratch, zero before the first call (every call leaves it zero).  Bitwise deterministic: integer atomics, and the sum folds
+ *              the fp32 row losses into fp64 in an order fixed by the row index alone.  No allocation, no host sync: capturable.
+ *   EMA update: ema[i] = ema[i] * (1 - momentum) + momentum * src[i] over n fp32 elements, in the reference's operation order
+ *              (cvnets/misc/averaging_utils.py:55: two rounded fp32 products, one rounded sum; 1 - momentum formed in double and rounded
+ *              to fp32).  The EMA of the BatchNorm running statistics, one launch per training step.
+ * ------------------------------------------------------------------------------------------------------------- */
+CVB_API int cvb_cls_metrics(const void* logits, int ld, int B, int C, const int64_t* target, int ignore_index, double* loss_sum, int64_t* counts,
+                            float* row_loss, int* ticket, cvb_stream_t stream);
+CVB_API int cvb_ema_update(float* ema, const float* src, int64_t n, double momentum, cvb_stream_t stream);
 /* cudaMemsetAsync(ptr, 0, bytes): the step's ONE workspace clear (a memset node under graph capture, not a kernel) */
 CVB_API int cvb_memset_zero(void* ptr, int64_t bytes, cvb_stream_t stream);
 

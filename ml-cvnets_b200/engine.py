@@ -53,7 +53,7 @@ class TrainStep:
                  ema_momentum: Optional[float] = None, init_scale: float = 65536.0, growth_interval: int = 2000,
                  process_group=None, data_parallel: Optional[bool] = None, n_buckets: int = 3, broadcast_buffers: bool = True,
                  forward_loss=None, optimizer: str = "adamw", momentum: float = 0.9, nesterov: bool = True,
-                 aug_loss: Optional["NeuralAugmentationLoss"] = None, ce_weight: float = 1.0):
+                 aug_loss: Optional["NeuralAugmentationLoss"] = None, ce_weight: float = 1.0, ema_buffers: bool = False):
         """``forward_loss(model, *inputs, cfg) -> loss`` replaces the default ``cross_entropy(model(x), y)`` (e.g. CLIP's contrastive step);
         ``cfg.scale`` is the device-resident loss scale the loss's backward must multiply by, ``cfg.world / rank / group`` the process group.
         ``optimizer="sgd"`` swaps AdamW for SGD with ``momentum`` / ``nesterov`` (optim.FlatSGD; ``betas`` / ``eps`` are then unused and
@@ -62,7 +62,13 @@ class TrainStep:
         composite_loss); ``loss_parts`` (device fp32 [2]) then holds (CE, L_na) of the last step.  A ``forward_loss`` of such a model returns
         ``(loss, augmented_tensor)``; with ``aug_loss`` the step then minimises ``ce_weight * loss + aug_loss.weight * L_na`` and ``loss_parts``
         holds (loss, L_na).  ``loss`` must apply ``cfg.scale`` in its backward, as the built-in losses do; the composite hands it its weighted
-        gradient unscaled (the CLIP recipe's step: INTEGRATION.md)."""
+        gradient unscaled (the CLIP recipe's step: INTEGRATION.md).
+
+        ``ema_buffers=True`` (needs ``ema_momentum``) extends the EMA to the whole state, as the reference's EMA averages the whole
+        state_dict (averaging_utils.py:43-55): the model's floating-point buffers (BatchNorm running statistics) become views of one flat fp32
+        tensor, a second one holds their EMA (initialised from the buffers), and every step launches ``cvb_ema_update`` after its forward
+        has updated the statistics.  Data parallel: each rank averages its own post-forward statistics.  ``ema_model()`` is the evaluable
+        EMA twin."""
         import torch.distributed as dist
         if optimizer not in ("adamw", "sgd"):
             raise ValueError(f"optimizer must be 'adamw' or 'sgd', got {optimizer!r}")
@@ -95,6 +101,13 @@ class TrainStep:
         self.loss_parts = torch.zeros(2, device=self.ws.device, dtype=torch.float32) if aug_loss is not None else None
         self.loss_cfg.group = process_group
         self.loss_cfg.world, self.loss_cfg.rank = self.world, (dist.get_rank(process_group) if data_parallel else 0)
+        if ema_buffers and ema_momentum is None:
+            raise ValueError("ema_buffers=True averages the buffers alongside the weights: it needs ema_momentum")
+        # after the data-parallel set-up: the EMA starts from rank 0's buffers, as the reference's deepcopy of the synchronised model does
+        flat_buf = self.ws.flat_buffers() if ema_buffers else None
+        self.ema_buffers = flat_buf.clone() if flat_buf is not None else None
+        self._ema_buffers_on = bool(ema_buffers)
+        self._ema_model = None
         self._one = torch.ones((), device=self.ws.device, dtype=torch.float32)
         self._graphs: Dict[tuple, tuple] = {}  # input signature -> (CUDA graph, static inputs, static loss), in capture order
         self._pool = None
@@ -124,10 +137,53 @@ class TrainStep:
         self.ws.mix.copy_(h, non_blocking=True)
 
     def state_dict(self):
-        return self.opt.state_dict()
+        sd = self.opt.state_dict()
+        if self.ema_buffers is not None:
+            sd["ema_buffers"] = self.ema_buffers.clone()
+        return sd
 
     def load_state_dict(self, sd):
         self.opt.load_state_dict(sd)
+        if self.ema_buffers is not None:
+            self.ema_buffers.copy_(sd["ema_buffers"])
+        ops.invalidate_prepared_weights()  # the EMA weights were written behind the twin's parameters (no Tensor._version bump there)
+
+    def ema_model(self) -> torch.nn.Module:
+        """The EMA model (the reference's ``EMA.ema_model``) as an eval-mode twin of ``model`` that owns no copy of the state: its parameters
+        are views of the optimizer's flat EMA, its floating-point buffers views of the buffer EMA (``ema_buffers=True``), so it always shows
+        the latest step.  It has no gradients, and kernel-layout weight caches of its own.  Its ``state_dict()`` has the reference EMA
+        model's keys and values, except ``num_batches_tracked``: integer buffers are not averaged and the twin reports the live counter
+        (DESIGN.md).  Evaluate it with ``EvalStep(step.ema_model())``."""
+        if self.opt.ema is None:
+            raise RuntimeError("ema_model: this TrainStep keeps no EMA (ema_momentum=None)")
+        if self._ema_model is not None:
+            return self._ema_model
+        live_bufs = [b for b in self.model.buffers() if b.is_floating_point()]
+        if live_bufs and not self._ema_buffers_on:
+            raise RuntimeError("ema_model: the model has BatchNorm running statistics; construct the TrainStep with ema_buffers=True so the "
+                               "EMA model averages them as the reference's EMA does")
+        import copy
+        twin = copy.deepcopy(self.model)  # the workspace does not travel (StepWorkspace.__deepcopy__); the parameters are re-pointed below
+        live_params = dict(self.model.named_parameters())
+        for name, p in twin.named_parameters():
+            lp = live_params[name]
+            if id(lp) in self.ws.offsets:
+                o, k = self.ws.offsets[id(lp)]
+                p.data = self.opt.ema[o:o + k].view_as(p)
+            p.requires_grad_(False)
+            p.grad = None
+        live_named = dict(self.model.named_buffers())
+        o = 0
+        for name, b in twin.named_buffers():
+            lb = live_named[name]
+            if b.is_floating_point():
+                k = b.numel()
+                b.data = self.ema_buffers[o:o + k].view_as(b)
+                o += k
+            else:
+                b.data = lb.data  # num_batches_tracked: the live counter
+        self._ema_model = twin.eval()
+        return self._ema_model
 
     # ---- one iteration, eager launches
     def _step(self, *inputs: torch.Tensor) -> torch.Tensor:
@@ -162,6 +218,8 @@ class TrainStep:
             ws.active = False
         ws.finish_reduce()
         self.opt.step(grad_div=float(self.world))
+        if self.ema_buffers is not None:
+            ops.ema_update(self.ema_buffers, ws.flat_buffers(), self.opt.ema_momentum)
         return loss
 
     def step(self, *inputs: torch.Tensor) -> torch.Tensor:
@@ -279,11 +337,15 @@ class TrainStep:
 
     def graph_pool_bytes(self) -> int:
         """Device memory the captured graphs' shared pool holds (0 before capture)."""
-        if self._pool is None:
-            return 0
-        segs = torch.cuda.memory_snapshot(mempool_id=self._pool, include_traces=False)
-        pool = tuple(self._pool)
-        return sum(s["total_size"] for s in segs if tuple(s.get("segment_pool_id", pool)) == pool)
+        return _pool_bytes(self._pool)
+
+
+def _pool_bytes(pool_handle) -> int:
+    if pool_handle is None:
+        return 0
+    segs = torch.cuda.memory_snapshot(mempool_id=pool_handle, include_traces=False)
+    pool = tuple(pool_handle)
+    return sum(s["total_size"] for s in segs if tuple(s.get("segment_pool_id", pool)) == pool)
 
 
 def _shapes(inputs) -> tuple:
@@ -464,3 +526,168 @@ class ZeroShotAccuracy:
         top1, top5 = self.hits.tolist()
         n = max(self.count, 1)
         return {"top1": 100.0 * top1 / n, "top5": 100.0 * top5 / n}
+
+
+class EvalStep:
+    """The reference's ``val_epoch`` (engine/training_engine.py:608-640) for a classifier: the eval-mode forward and the recipes'
+    ``stats.val: [loss, top1, top5]``, counted on the device (``cvb_cls_metrics``), optionally one CUDA graph per crop.
+
+        ev = EvalStep(step.ema_model())          # or EvalStep(model): the live model, switched to eval for each pass and restored after
+        ev.capture(batch=100, crop=(256, 256))   # optional, one graph per crop; eager without it
+        for x, y in val_loader:
+            ev.update(x, y)                      # no host sync
+        metrics = ev.compute()                   # {"loss", "top1", "top5"}: one sync; summed over the process group
+        ev.reset()
+
+    ``loss`` is the cross entropy without label smoothing (the reference's loss in eval mode; RangeAugment's augmentation term is 0 there),
+    summed over the rows and divided by their number N at ``compute``; ``topk`` = 100 * hits / N.  A row is a top-k hit iff fewer than k
+    classes have a logit strictly greater than the target's, compared on the classifier's bf16 logits (ties count for the target; torch.topk
+    leaves tie order unspecified).  Rows whose target is ``ignore_index`` are not counted.
+
+    Captured: ``update`` copies a batch into the static buffers of its crop's graph; a smaller batch (the ragged last one) fills the first
+    rows and the rest get target ``ignore_index``, so it needs no graph of its own.  A batch larger than the captured one, or a crop that was
+    not captured, raises.  All graphs share one memory pool.
+
+    Weight refresh: the forward reads kernel-layout (bf16) copies of the weights, which an eval-mode forward refreshes only when a weight
+    changed -- a decision taken on the host, which a captured graph would freeze.  So before the first pass after any weight change (a
+    ``_WEIGHTS_GENERATION`` bump, which every TrainStep step or replay and every optimizer step makes, or a parameter's version moving)
+    ``update`` refreshes every kernel-layout copy of the evaluated model once, eagerly; the captured graphs contain no refresh and always read
+    current weights.
+
+    Data parallel: each rank counts its own shard; ``compute`` sums ``[loss_sum, top1, top5, n]`` over ``process_group`` with one
+    all-reduce."""
+
+    def __init__(self, model: torch.nn.Module, *, ignore_index: int = -1, process_group=None):
+        import torch.distributed as dist
+        self.model = model
+        self.device = next(model.parameters()).device
+        self.ignore_index = int(ignore_index)
+        self.group = process_group
+        self.world = dist.get_world_size(process_group) if dist.is_available() and dist.is_initialized() else 1
+        self.loss_sum = torch.zeros(1, device=self.device, dtype=torch.float64)
+        self.counts = torch.zeros(3, device=self.device, dtype=torch.int64)  # top-1 hits, top-5 hits, rows
+        self._ticket = torch.zeros(1, device=self.device, dtype=torch.int32)
+        self._row_loss = torch.zeros(0, device=self.device, dtype=torch.float32)
+        self._graphs: Dict[tuple, tuple] = {}  # (C, H, W) -> (CUDA graph, static images, static targets, static logits)
+        self._pool = None
+        self._weights_seen = None
+        self.logits: Optional[torch.Tensor] = None  # bf16 logits of the last batch (captured: the graph's static output; all its rows)
+        self.launches_per_crop: Dict[tuple, int] = {}  # (C, H, W) -> kernel launches of its captured pass
+
+    # ---- weights
+    def _prepared(self) -> list:
+        """Every kernel-layout weight cache of the model (the ``prep`` of each module's kernel configuration)."""
+        out, seen = [], set()
+        for m in self.model.modules():
+            for v in vars(m).values():
+                prep = getattr(v, "prep", None) if isinstance(v, SimpleNamespace) else None
+                if isinstance(prep, ops.PreparedWeights) and id(prep) not in seen:
+                    seen.add(id(prep))
+                    out.append(prep)
+        return out
+
+    def _refresh(self, force: bool = False) -> None:
+        key = (ops._WEIGHTS_GENERATION[0], sum(p._version for p in self.model.parameters()))
+        if force or key != self._weights_seen:
+            for prep in self._prepared():
+                prep.refresh()
+            self._weights_seen = key
+
+    # ---- one pass
+    def _scratch(self, B: int) -> torch.Tensor:
+        if self._row_loss.numel() < B:
+            if self._graphs:
+                raise ValueError(f"EvalStep: batch {B} exceeds the captured batch {self._row_loss.numel()}")
+            self._row_loss = torch.zeros(B, device=self.device, dtype=torch.float32)
+        return self._row_loss
+
+    def _pass(self, x: torch.Tensor, y: torch.Tensor) -> torch.Tensor:
+        training = self.model.training
+        if training:
+            self.model.eval()
+        try:
+            out = self.model(x)
+        finally:
+            if training:
+                self.model.train(True)
+        logits = out["logits"] if isinstance(out, dict) else out  # a RangeAugment model: {"augmented_tensor": None, "logits"} in eval
+        ops.cls_metrics(logits, y, self.loss_sum, self.counts, self._scratch(y.shape[0]), self._ticket, self.ignore_index)
+        return logits
+
+    def update(self, images: torch.Tensor, targets: torch.Tensor) -> None:
+        """Count one validation batch (no host sync)."""
+        targets = targets.to(device=self.device, dtype=torch.int64)
+        self._refresh()
+        with torch.no_grad():
+            if not self._graphs:
+                self.logits = self._pass(images.to(self.device), targets.contiguous())
+                return
+            key = tuple(images.shape[1:])
+            entry = self._graphs.get(key)
+            if entry is None:
+                raise ValueError(f"EvalStep.update: no CUDA graph was captured for images of shape [*, {', '.join(map(str, key))}]; captured: "
+                                 f"{[list(k) for k in self._graphs]}")
+            graph, sx, sy, logits = entry
+            b = images.shape[0]
+            if b > sx.shape[0]:
+                raise ValueError(f"EvalStep.update: batch {b} exceeds the captured batch {sx.shape[0]}")
+            sx[:b].copy_(images, non_blocking=True)
+            sy[:b].copy_(targets, non_blocking=True)
+            if b < sy.shape[0]:
+                sy[b:].fill_(self.ignore_index)
+            graph.replay()
+            self.logits = logits
+
+    # ---- capture
+    def capture(self, batch: int, crop: Tuple[int, int], channels: int = 3, warmup: int = 2) -> "EvalStep":
+        """Capture the eval pass of ``batch`` images of size ``crop`` (H, W) as one CUDA graph (call once per crop; the first capture fixes the
+        largest batch).  Warm-up passes run eagerly on rows that all carry ``ignore_index``, so they count nothing."""
+        H, W = int(crop[0]), int(crop[1])
+        key = (int(channels), H, W)
+        if key in self._graphs:
+            raise ValueError(f"EvalStep.capture: crop {crop} was already captured")
+        dev = self.device
+        sx = torch.zeros((batch,) + key, device=dev, dtype=torch.float32)
+        sy = torch.full((batch,), self.ignore_index, device=dev, dtype=torch.int64)
+        self._scratch(batch)
+        torch.cuda.synchronize(dev)
+        side = torch.cuda.Stream(device=dev)
+        side.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(side), torch.no_grad():
+            self._refresh()
+            for _ in range(max(1, warmup)):
+                self._pass(sx, sy)
+        torch.cuda.current_stream().wait_stream(side)
+        torch.cuda.synchronize(dev)
+        self._refresh(force=True)  # caches the warm-up created included: the graph's forward then skips every refresh
+        torch.cuda.synchronize(dev)
+        gc.collect()
+        if self._pool is None:
+            self._pool = torch.cuda.graph_pool_handle()
+        graph = torch.cuda.CUDAGraph()
+        n0 = ops.launch_count
+        with torch.cuda.graph(graph, pool=self._pool), torch.no_grad():
+            logits = self._pass(sx, sy)
+        self.launches_per_crop[key] = ops.launch_count - n0
+        self._graphs[key] = (graph, sx, sy, logits)
+        return self
+
+    def graph_pool_bytes(self) -> int:
+        """Device memory the captured eval graphs' shared pool holds (0 before capture)."""
+        return _pool_bytes(self._pool)
+
+    # ---- results
+    def compute(self) -> Dict[str, float]:
+        """{"loss", "top1", "top5"} over every row counted since the last ``reset`` (summed over the process group): one host sync."""
+        acc = torch.cat([self.loss_sum, self.counts.to(torch.float64)])
+        if self.world > 1:
+            import torch.distributed as dist
+            dist.all_reduce(acc, op=dist.ReduceOp.SUM, group=self.group)
+        loss, top1, top5, n = acc.tolist()
+        if n == 0:
+            return {"loss": float("nan"), "top1": float("nan"), "top5": float("nan")}
+        return {"loss": loss / n, "top1": 100.0 * top1 / n, "top5": 100.0 * top5 / n}
+
+    def reset(self) -> None:
+        self.loss_sum.zero_()
+        self.counts.zero_()

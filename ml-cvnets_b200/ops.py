@@ -368,6 +368,37 @@ def zs_logits_topk(img: Tensor, table: Tensor, scale: float = 100.0, targets: Op
     return logits
 
 
+def cls_metrics(logits: Tensor, target: Tensor, loss_sum: Tensor, counts: Tensor, row_loss: Tensor, ticket: Tensor,
+                ignore_index: int = -1) -> None:
+    """Validation metrics of one batch, added on the device (no host sync): ``loss_sum`` (fp64 [1]) += the summed cross entropy without
+    label smoothing, ``counts`` (int64 [3]) += {top-1 hits, top-5 hits, counted rows}.  logits: bf16 [B, C] with unit column stride (a view
+    of the classifier's padded output is fine); target: int64 [B], rows with ``ignore_index`` skipped.  Top-k rule: fewer than k classes with
+    a logit strictly greater than the target's.  ``row_loss`` (fp32, >= B elements) and ``ticket`` (int32 [1], zero before the first call)
+    are scratch."""
+    if logits.dim() != 2 or logits.dtype != torch.bfloat16 or logits.stride(1) != 1 or logits.stride(0) < logits.shape[1]:
+        raise ValueError("cls_metrics: logits must be a bf16 [B, C] matrix with unit column stride and row stride >= C")
+    B, C = logits.shape
+    if target.dtype != torch.int64 or tuple(target.shape) != (B,) or not target.is_contiguous():
+        raise ValueError(f"cls_metrics: target must be a contiguous int64 [{B}] tensor")
+    if loss_sum.dtype != torch.float64 or loss_sum.numel() != 1 or counts.dtype != torch.int64 or counts.numel() != 3:
+        raise ValueError("cls_metrics: loss_sum must be fp64 [1] and counts int64 [3]")
+    if row_loss.dtype != torch.float32 or row_loss.numel() < B or ticket.dtype != torch.int32 or ticket.numel() != 1:
+        raise ValueError(f"cls_metrics: row_loss must be fp32 with >= {B} elements and ticket int32 [1]")
+    _lib().cvb_cls_metrics(logits.data_ptr(), logits.stride(0), B, C, target.data_ptr(), int(ignore_index), loss_sum.data_ptr(),
+                           counts.data_ptr(), row_loss.data_ptr(), ticket.data_ptr(), _stream())
+    _count()
+
+
+def ema_update(ema: Tensor, src: Tensor, momentum: float) -> None:
+    """ema = ema * (1 - momentum) + momentum * src over two contiguous fp32 buffers of equal size (the reference's operation order)."""
+    if ema.dtype != torch.float32 or src.dtype != torch.float32 or ema.numel() != src.numel() or not (ema.is_contiguous() and src.is_contiguous()):
+        raise ValueError("ema_update: ema and src must be contiguous fp32 tensors of the same size")
+    if not 0.0 <= float(momentum) <= 1.0:
+        raise ValueError(f"ema_update: momentum {momentum} is outside [0, 1]")
+    _lib().cvb_ema_update(ema.data_ptr(), src.data_ptr(), ema.numel(), float(momentum), _stream())
+    _count()
+
+
 def patch_permute(X: Tensor, B: int, H: int, W: int, ph: int, pw: int, inverse: bool) -> Tensor:
     """MobileViT-v1 unfold (inverse=False: feature-map rows -> token rows [B*P*N, C]) / fold (inverse=True)."""
     out = torch.empty_like(X)
@@ -920,3 +951,9 @@ class PreparedWeights:
         _count()
         self._versions = versions
         self._forced_last = bool(force)
+
+    def refresh(self):
+        """Refresh all kernel-layout copies now, as an eval-mode forward would: later ``prepare(force=False)`` calls skip until a parameter
+        changes (engine.EvalStep refreshes eagerly so that its captured forwards contain no refresh)."""
+        self.prepare(force=True)
+        self._forced_last = False

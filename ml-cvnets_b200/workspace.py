@@ -307,16 +307,24 @@ class StepWorkspace:
         import torch.distributed as dist
         if self.world == 1:
             return
-        bufs = [b for b in self.model.buffers() if b.is_floating_point()]
-        if not bufs:
+        flat = self.flat_buffers()
+        if flat is None:
             return
+        dist.broadcast(flat, src=src, group=self.group)
+
+    def flat_buffers(self) -> Optional[torch.Tensor]:
+        """The model's floating-point buffers (BatchNorm running statistics) as ONE flat fp32 tensor, in ``model.buffers()`` order; on the
+        first call every such buffer becomes a view of it (state_dict / modules see no change).  None when the model has none."""
         if getattr(self, "_flat_buf", None) is None:
-            n = sum(b.numel() for b in bufs)
+            bufs = [b for b in self.model.buffers() if b.is_floating_point()]
+            if not bufs:
+                return None
+            n =sum(b.numel() for b in bufs)
             self._flat_buf = torch.empty(n, device=self.device, dtype=torch.float32)
             o = 0
             for b in bufs:
                 k = b.numel()
                 self._flat_buf[o:o + k].copy_(b.reshape(-1))
-                b.data = self._flat_buf[o:o + k].view_as(b)  # buffers become views of one flat tensor (state_dict / modules see no change)
+                b.data = self._flat_buf[o:o + k].view_as(b)
                 o += k
-        dist.broadcast(self._flat_buf, src=src, group=self.group)
+        return self._flat_buf
