@@ -370,6 +370,10 @@ CVB_API int cvb_adamw_step(float* params, const float* grads, float* exp_avg, fl
 CVB_API int cvb_sgd_step(float* params, const float* grads, float* momentum_buf, const float* weight_decay, int64_t n, const float* hp, float momentum,
                          int nesterov, float max_norm, float* stats, float* scale, float* step, float growth_factor, float backoff_factor,
                          int growth_interval, float* ema, float ema_momentum, const float* partials, cvb_stream_t stream);
+/* Gradient accumulation over micro-batches (engine/training_engine.py:286-312 with common.accum_freq > 1: gradients are SUMMED, the loss is
+ * not divided): acc[i] += g[i] over n fp32 elements, one IEEE add per element (round to nearest, subnormals kept), so the result is bitwise
+ * torch's fp32 add.  acc and g 16-byte aligned; grid of min(ceil(n / 1024), 4 * SMs) CTAs of 256 threads, grid-stride. */
+CVB_API int cvb_grad_accumulate(float* acc, const float* g, int64_t n, cvb_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
  * Classification loss of the step: F.cross_entropy(prediction, target, ignore_index, label_smoothing), mean over the non-ignored

@@ -10,6 +10,8 @@
 // iteration, scheduler.update_lr at engine/training_engine.py:246-249, without re-capturing the step's CUDA graph).
 // Optional: the EMA of the weights (cvnets/misc/averaging_utils.py:43-55: ema = ema*(1-momentum) + momentum*param, every iteration)
 // rides in the same pass, and grad_div folds DDP's division by the world size into the unscale.
+// With gradient accumulation (common.accum_freq > 1) cvb_grad_accumulate adds each micro-batch's gradients into an accumulator, and the
+// two launches above run once per accumulation window, over that accumulator.
 #include "common.cuh"
 
 namespace {
@@ -175,7 +177,43 @@ __global__ void __launch_bounds__(ONT) sgd_step_kernel(float* __restrict__ p, co
   finish_step(stats, scale, step, skip, s_tot, growth, backoff, growth_interval);
 }
 
+// one IEEE add, round to nearest, subnormals kept: the library builds with --use_fast_math, whose -ftz would flush them, and the sum must be
+// bitwise torch's fp32 add (and autograd's .grad +=)
+__device__ __forceinline__ float add_rn(float a, float b) {
+  float r;
+  asm("add.rn.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+  return r;
+}
+
+// gradient accumulation (engine.TrainStep(accum_freq > 1)): acc += g, 16-byte vectors, scalar tail, grid-stride
+__global__ void __launch_bounds__(ONT) grad_accumulate_kernel(float* __restrict__ acc, const float* __restrict__ g, int64_t n) {
+  pdl_wait();
+  pdl_trigger();
+  const int64_t nvec = n >> 2, stride = (int64_t)gridDim.x * ONT, first = (int64_t)blockIdx.x * ONT + threadIdx.x;
+  float4* a4 = reinterpret_cast<float4*>(acc);
+  const float4* g4 = reinterpret_cast<const float4*>(g);
+  for (int64_t i = first; i < nvec; i += stride) {
+    float4 a = a4[i];
+    const float4 b = __ldg(g4 + i);
+    a.x = add_rn(a.x, b.x);
+    a.y = add_rn(a.y, b.y);
+    a.z = add_rn(a.z, b.z);
+    a.w = add_rn(a.w, b.w);
+    a4[i] = a;
+  }
+  for (int64_t i = (nvec << 2) + first; i < n; i += stride) acc[i] = add_rn(acc[i], g[i]);
+}
+
 }  // namespace
+
+extern "C" int cvb_grad_accumulate(float* acc, const float* g, int64_t n, cvb_stream_t stream) {
+  CVB_CHECK(acc && g && n > 0 && cvb_aligned16(acc) && cvb_aligned16(g), "cvb_grad_accumulate: bad arguments (n > 0, 16-byte aligned buffers)");
+  int64_t blocks = ((n + 3) / 4 + ONT - 1) / ONT;
+  const int64_t cap = 4 * (int64_t)cvb_num_sms();
+  if (blocks > cap) blocks = cap;
+  CVB_CUDA(cvb_launch(grad_accumulate_kernel, (int)blocks, ONT, 0, static_cast<cudaStream_t>(stream), acc, g, n));
+  return 0;
+}
 
 extern "C" int cvb_grad_norm_blocks(int64_t n) {
   int blocks = (int)((n / 4 + ONT - 1) / ONT);

@@ -21,6 +21,17 @@ A variable-batch sampler draws a (crop, batch) pair per iteration; ``capture_sha
 
     pairs = variable_batch_pairs(224, 224, 256, max_scales=5, check_scale=32, min_w=128, max_w=320, min_h=128, max_h=320)
     step.capture_shapes([(torch.randn(b, 3, h, w, device="cuda"), torch.zeros(b, dtype=torch.long, device="cuda")) for h, w, b in pairs])
+
+Gradient accumulation (the reference's ``common.accum_freq``): every call is one micro-batch, and every ``accum_freq``-th call applies the
+update to the summed gradients; ``updated`` says whether the last call did (advance the scheduler and the iteration count then):
+
+    step = TrainStep(model, optimizer="sgd", lr=0.1, weight_decay=4e-5, max_norm=None, accum_freq=2)
+    for epoch in range(epochs):
+        step.zero_grad()                      # the reference's per-epoch _zero_grad(): drops a window left open by the last epoch
+        for x, y in loader:
+            loss = step(x, y)
+            if step.updated:
+                iteration += 1
 """
 from __future__ import annotations
 
@@ -53,7 +64,7 @@ class TrainStep:
                  ema_momentum: Optional[float] = None, init_scale: float = 65536.0, growth_interval: int = 2000,
                  process_group=None, data_parallel: Optional[bool] = None, n_buckets: int = 3, broadcast_buffers: bool = True,
                  forward_loss=None, optimizer: str = "adamw", momentum: float = 0.9, nesterov: bool = True,
-                 aug_loss: Optional["NeuralAugmentationLoss"] = None, ce_weight: float = 1.0, ema_buffers: bool = False):
+                 aug_loss: Optional["NeuralAugmentationLoss"] = None, ce_weight: float = 1.0, ema_buffers: bool = False, accum_freq: int = 1):
         """``forward_loss(model, *inputs, cfg) -> loss`` replaces the default ``cross_entropy(model(x), y)`` (e.g. CLIP's contrastive step);
         ``cfg.scale`` is the device-resident loss scale the loss's backward must multiply by, ``cfg.world / rank / group`` the process group.
         ``optimizer="sgd"`` swaps AdamW for SGD with ``momentum`` / ``nesterov`` (optim.FlatSGD; ``betas`` / ``eps`` are then unused and
@@ -68,14 +79,33 @@ class TrainStep:
         state_dict (averaging_utils.py:43-55): the model's floating-point buffers (BatchNorm running statistics) become views of one flat fp32
         tensor, a second one holds their EMA (initialised from the buffers), and every step launches ``cvb_ema_update`` after its forward
         has updated the statistics.  Data parallel: each rank averages its own post-forward statistics.  ``ema_model()`` is the evaluable
-        EMA twin."""
+        EMA twin.
+
+        ``accum_freq`` > 1 accumulates gradients over that many calls (micro-batches) per optimizer update, as the reference's
+        ``common.accum_freq`` does (engine/training_engine.py:286-312): each call runs forward, loss, backward and the data-parallel exchange
+        into the workspace's gradient buffer and adds it into one flat fp32 accumulator (``grad_acc``; ``p.grad`` become views of it), so the
+        gradients are summed, not averaged.  Every ``accum_freq``-th call then runs the optimizer tail over the accumulator, the buffer EMA,
+        and zeroes the accumulator: loss scale, step count and EMA change only there, and an inf / nan in any micro-batch skips that window's
+        update and backs the scale off once.  BatchNorm statistics update on every micro-batch.  ``updated`` is True after a call that
+        applied the update; ``zero_grad()`` discards an open window.  ``accum_freq`` 1 (the default) is the plain step, with no accumulator."""
         import torch.distributed as dist
         if optimizer not in ("adamw", "sgd"):
             raise ValueError(f"optimizer must be 'adamw' or 'sgd', got {optimizer!r}")
+        if isinstance(accum_freq, bool) or int(accum_freq) != accum_freq or accum_freq < 1:
+            raise ValueError(f"accum_freq must be an integer >= 1, got {accum_freq!r}")
         self.model = model
         self.ws = StepWorkspace(model)
+        self.accum_freq = int(accum_freq)
+        self.grad_acc = None
+        if self.accum_freq > 1:
+            self.grad_acc = torch.zeros_like(self.ws.flat_g)
+            for p in self.ws.params:
+                o, k = self.ws.offsets[id(p)]
+                p.grad = self.grad_acc[o:o + k].view_as(p)
+        self._window = 0        # micro-batches accumulated in the open window
+        self.updated = False    # whether the last call applied the optimizer update
         common = dict(lr=lr, weight_decay=weight_decay, no_decay_bn_filter_bias=no_decay_bn_filter_bias, max_norm=max_norm, init_scale=init_scale,
-                      growth_interval=growth_interval, ema_momentum=ema_momentum)
+                      growth_interval=growth_interval, ema_momentum=ema_momentum, grads=self.grad_acc)
         if optimizer == "adamw":
             self.opt = FlatAdamW(model, self.ws, betas=betas, eps=eps, **common)
         else:
@@ -110,6 +140,8 @@ class TrainStep:
         self._ema_model = None
         self._one = torch.ones((), device=self.ws.device, dtype=torch.float32)
         self._graphs: Dict[tuple, tuple] = {}  # input signature -> (CUDA graph, static inputs, static loss), in capture order
+        self._update_graph = None  # accum_freq > 1: the shape-independent update (optimizer tail, buffer EMA, accumulator clear)
+        self.launches_per_update: Optional[int] = None
         self._pool = None
         self.eager_steps = 0
 
@@ -185,8 +217,42 @@ class TrainStep:
         self._ema_model = twin.eval()
         return self._ema_model
 
+    def zero_grad(self) -> None:
+        """Discard the open accumulation window: zero the accumulator and restart the count (the reference's ``_zero_grad()`` at the start of
+        every epoch, which drops a partial window left by the previous one).  Nothing to discard with ``accum_freq`` 1."""
+        if self.grad_acc is not None:
+            self._clear_acc()
+        self._window = 0
+
+    def _clear_acc(self) -> None:
+        ops._lib().cvb_memset_zero(self.grad_acc.data_ptr(), self.grad_acc.numel() * 4, ops._stream())  # a memset node under capture
+
     # ---- one iteration, eager launches
     def _step(self, *inputs: torch.Tensor) -> torch.Tensor:
+        """One call's launches: the whole step, or with accum_freq > 1 one micro-batch up to and including its accumulate."""
+        loss = self._forward_backward(*inputs)
+        if self.grad_acc is None:
+            self._update()
+        else:
+            ops.grad_accumulate(self.grad_acc, self.ws.flat_g)
+        return loss
+
+    def _update(self) -> None:
+        self.opt.step(grad_div=float(self.world))
+        if self.ema_buffers is not None:
+            ops.ema_update(self.ema_buffers, self.ws.flat_buffers(), self.opt.ema_momentum)
+        if self.grad_acc is not None:
+            self._clear_acc()
+
+    def _end_window(self) -> bool:
+        """Count the call just made into the window; True when it completes the window (always with accum_freq 1)."""
+        self._window += 1
+        if self._window < self.accum_freq:
+            return False
+        self._window = 0
+        return True
+
+    def _forward_backward(self, *inputs: torch.Tensor) -> torch.Tensor:
         ws = self.ws
         ws.begin_step()
         if self.world > 1 and self.broadcast_buffers:
@@ -217,24 +283,30 @@ class TrainStep:
         finally:
             ws.active = False
         ws.finish_reduce()
-        self.opt.step(grad_div=float(self.world))
-        if self.ema_buffers is not None:
-            ops.ema_update(self.ema_buffers, ws.flat_buffers(), self.opt.ema_momentum)
         return loss
 
     def step(self, *inputs: torch.Tensor) -> torch.Tensor:
-        """One training step on ``inputs``.  Before capture it runs eagerly; after capture it replays the graph captured for the inputs'
-        shapes (``ValueError`` for a shape that was not captured).  The returned loss is a static tensor of that graph: read or clone it
-        before the next step."""
+        """One training step on ``inputs`` (with accum_freq > 1, one micro-batch; ``updated`` tells whether it applied the update).  Before
+        capture it runs eagerly; after capture it replays the graph captured for the inputs' shapes (``ValueError`` for a shape that was not
+        captured), and the update graph when the call completes a window.  The returned loss is this micro-batch's, a static tensor of the
+        graph: read or clone it before the next step."""
         if not self._graphs:
             self.eager_steps += 1
-            return self._step(*inputs)
+            loss = self._step(*inputs)
+            self.updated = self._end_window()
+            if self.updated and self.grad_acc is not None:
+                self._update()
+            return loss
         graph, statics, sloss = self._graph_for(inputs)
         for s_in, t in zip(statics, inputs):
             if t is not s_in:
                 s_in.copy_(t, non_blocking=True)
         graph.replay()
-        ops.invalidate_prepared_weights()
+        self.updated = self._end_window()
+        if self.updated and self._update_graph is not None:
+            self._update_graph.replay()
+        if self.updated:
+            ops.invalidate_prepared_weights()
         return sloss
 
     __call__ = step
@@ -258,7 +330,9 @@ class TrainStep:
 
     def capture_shapes(self, examples: Sequence[Sequence[torch.Tensor]], warmup: int = 3):
         """Capture one CUDA graph per distinct input signature (shapes and dtypes) of ``examples``: ``(x, y)`` tuples, or the inputs of
-        ``forward_loss`` (e.g. ``(images, text_tokens)``).  ``step()`` then replays the graph of its inputs' shapes.
+        ``forward_loss`` (e.g. ``(images, text_tokens)``).  ``step()`` then replays the graph of its inputs' shapes.  With accum_freq > 1
+        these are micro-step graphs (up to and including the accumulate), and ONE more graph, captured last into the same pool, holds the
+        shape-independent update that ``step()`` replays at the end of every window.
 
         Warm-up: ``max(warmup, 3)`` passes over the distinct examples in the order given, each step a real eager training step on that
         example (with one shape, eager steps already taken count toward the passes, as ``capture`` always did).  The first pass raises every
@@ -279,7 +353,7 @@ class TrainStep:
         rank), and a forward_loss that all-gathers features (CLIP) needs the same per-rank batch on every rank, as the reference's does.
 
         ``launches_per_shape`` maps each captured tuple of input shapes to its launch count; ``launches_per_step`` is the largest of them
-        (the one count of a single-shape capture)."""
+        (the one count of a single-shape capture).  ``launches_per_update`` counts the update graph's launches (None with accum_freq 1)."""
         assert not self._graphs, "already captured"
         by_sig: Dict[tuple, tuple] = {}
         for ex in examples:
@@ -300,8 +374,7 @@ class TrainStep:
                 for sig, st in statics.items():
                     for s_in, t in zip(st, by_sig[sig]):
                         s_in.copy_(t)
-                    self._step(*st)
-                    self.eager_steps += 1
+                    self.step(*st)  # real eager calls: with accum_freq > 1 they advance the window and update at its end
             self._first = next(iter(by_sig))
             for s_in, t in zip(statics[self._first], by_sig[self._first]):  # static_inputs hold the first example, as they always have
                 s_in.copy_(t)
@@ -322,6 +395,13 @@ class TrainStep:
             self.launches_per_shape[tuple(s for s, _ in sig)] = ops.launch_count - n0
             self._graphs[sig] = (graph, statics[sig], sloss)
         self.launches_per_step = max(self.launches_per_shape.values())
+        if self.grad_acc is not None:
+            graph = torch.cuda.CUDAGraph()
+            n0 = ops.launch_count
+            with torch.cuda.graph(graph, pool=self._pool):
+                self._update()
+            self.launches_per_update = ops.launch_count - n0
+            self._update_graph = graph
         return self
 
     @property

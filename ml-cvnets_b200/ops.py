@@ -399,6 +399,14 @@ def ema_update(ema: Tensor, src: Tensor, momentum: float) -> None:
     _count()
 
 
+def grad_accumulate(acc: Tensor, g: Tensor) -> None:
+    """acc += g over two contiguous, 16-byte aligned fp32 buffers of equal size (bitwise torch's fp32 add): gradient accumulation."""
+    if acc.dtype != torch.float32 or g.dtype != torch.float32 or acc.numel() != g.numel() or not (acc.is_contiguous() and g.is_contiguous()):
+        raise ValueError("grad_accumulate: acc and g must be contiguous fp32 tensors of the same size")
+    _lib().cvb_grad_accumulate(acc.data_ptr(), g.data_ptr(), acc.numel(), _stream())
+    _count()
+
+
 def patch_permute(X: Tensor, B: int, H: int, W: int, ph: int, pw: int, inverse: bool) -> Tensor:
     """MobileViT-v1 unfold (inverse=False: feature-map rows -> token rows [B*P*N, C]) / fold (inverse=True)."""
     out = torch.empty_like(X)

@@ -29,14 +29,15 @@ class _FlatStep:
 
     def __init__(self, model: torch.nn.Module, ws: Optional[StepWorkspace], lr: float, weight_decay: float, no_decay_bn_filter_bias: bool,
                  max_norm: Optional[float], init_scale: float, growth_factor: float, backoff_factor: float, growth_interval: int,
-                 ema_momentum: Optional[float]):
+                 ema_momentum: Optional[float], grads: Optional[torch.Tensor] = None):
         self.ws = ws if ws is not None else StepWorkspace(model)
         ws = self.ws
         self.params = ws.params
         dev, n = ws.device, ws.n
         self.n = n
         self.flat_p = torch.zeros(n, device=dev, dtype=torch.float32)
-        self.flat_g = ws.flat_g
+        self.flat_g = ws.flat_g if grads is None else grads  # the gradient buffer the step reads (TrainStep's accumulator with accum_freq > 1)
+        assert self.flat_g.shape == ws.flat_g.shape and self.flat_g.dtype == torch.float32 and self.flat_g.is_contiguous()
         for name in self._moments:
             setattr(self, name, torch.zeros(n, device=dev, dtype=torch.float32))
         self.wd = torch.zeros(n, device=dev, dtype=torch.float32)
@@ -70,7 +71,8 @@ class _FlatStep:
         return self.scale[0:1]
 
     def step(self, grad_div: float = 1.0) -> None:
-        """Gradients are read from the workspace's flat buffer (already summed over ranks when data parallel; grad_div = world size)."""
+        """Gradients are read from ``flat_g``: the workspace's flat buffer or the buffer given as ``grads`` (already summed over ranks when data
+        parallel; grad_div = world size)."""
         lr_now = self.param_groups[0]["lr"]
         if lr_now != float(self._hp_host[0]) and not torch.cuda.is_current_stream_capturing():
             self.set_lr(lr_now)
@@ -122,9 +124,10 @@ class FlatAdamW(_FlatStep):
 
     def __init__(self, model: torch.nn.Module, ws: Optional[StepWorkspace] = None, lr: float = 2e-3, betas=(0.9, 0.999), eps: float = 1e-8,
                  weight_decay: float = 0.05, no_decay_bn_filter_bias: bool = True, max_norm: float = 10.0, init_scale: float = 65536.0,
-                 growth_factor: float = 2.0, backoff_factor: float = 0.5, growth_interval: int = 2000, ema_momentum: Optional[float] = None):
+                 growth_factor: float = 2.0, backoff_factor: float = 0.5, growth_interval: int = 2000, ema_momentum: Optional[float] = None,
+                 grads: Optional[torch.Tensor] = None):
         super().__init__(model, ws, lr, weight_decay, no_decay_bn_filter_bias, max_norm, init_scale, growth_factor, backoff_factor, growth_interval,
-                         ema_momentum)
+                         ema_momentum, grads)
         self.consts = (float(betas[0]), float(betas[1]), float(eps))
 
     def _update(self) -> None:
@@ -141,11 +144,12 @@ class FlatSGD(_FlatStep):
 
     def __init__(self, model: torch.nn.Module, ws: Optional[StepWorkspace] = None, lr: float = 0.1, momentum: float = 0.9, nesterov: bool = True,
                  weight_decay: float = 4e-5, no_decay_bn_filter_bias: bool = True, max_norm: Optional[float] = None, init_scale: float = 65536.0,
-                 growth_factor: float = 2.0, backoff_factor: float = 0.5, growth_interval: int = 2000, ema_momentum: Optional[float] = None):
+                 growth_factor: float = 2.0, backoff_factor: float = 0.5, growth_interval: int = 2000, ema_momentum: Optional[float] = None,
+                 grads: Optional[torch.Tensor] = None):
         if nesterov and momentum <= 0.0:
             raise ValueError("Nesterov momentum requires momentum > 0 (torch.optim.SGD)")
         super().__init__(model, ws, lr, weight_decay, no_decay_bn_filter_bias, max_norm, init_scale, growth_factor, backoff_factor, growth_interval,
-                         ema_momentum)
+                         ema_momentum, grads)
         self.momentum, self.nesterov = float(momentum), bool(nesterov)
 
     def _update(self) -> None:
