@@ -244,14 +244,6 @@ class TrainStep:
         if self.grad_acc is not None:
             self._clear_acc()
 
-    def _end_window(self) -> bool:
-        """Count the call just made into the window; True when it completes the window (always with accum_freq 1)."""
-        self._window += 1
-        if self._window < self.accum_freq:
-            return False
-        self._window = 0
-        return True
-
     def _forward_backward(self, *inputs: torch.Tensor) -> torch.Tensor:
         ws = self.ws
         ws.begin_step()
@@ -290,37 +282,30 @@ class TrainStep:
         capture it runs eagerly; after capture it replays the graph captured for the inputs' shapes (``ValueError`` for a shape that was not
         captured), and the update graph when the call completes a window.  The returned loss is this micro-batch's, a static tensor of the
         graph: read or clone it before the next step."""
-        if not self._graphs:
+        replay = bool(self._graphs)
+        if replay:
+            graph, statics, loss = _graph_for(self._graphs, _signature(inputs), "TrainStep.step", lambda sig: list(_shapes(sig)),
+                                              "capture every input shape the sampler draws with capture_shapes")
+            for s_in, t in zip(statics, inputs):
+                if t is not s_in:
+                    s_in.copy_(t, non_blocking=True)
+            graph.replay()
+        else:
             self.eager_steps += 1
             loss = self._step(*inputs)
-            self.updated = self._end_window()
-            if self.updated and self.grad_acc is not None:
-                self._update()
-            return loss
-        graph, statics, sloss = self._graph_for(inputs)
-        for s_in, t in zip(statics, inputs):
-            if t is not s_in:
-                s_in.copy_(t, non_blocking=True)
-        graph.replay()
-        self.updated = self._end_window()
-        if self.updated and self._update_graph is not None:
-            self._update_graph.replay()
+        self._window += 1
+        self.updated = self._window == self.accum_freq
         if self.updated:
-            ops.invalidate_prepared_weights()
-        return sloss
+            self._window = 0
+            if replay:
+                if self._update_graph is not None:
+                    self._update_graph.replay()
+                ops.invalidate_prepared_weights()
+            elif self.grad_acc is not None:
+                self._update()
+        return loss
 
     __call__ = step
-
-    def _graph_for(self, inputs) -> tuple:
-        entry = self._graphs.get(_signature(inputs))
-        if entry is None:  # same shapes, other dtypes: the copy into the static buffers converts them (as a single-shape capture always did)
-            shapes = _shapes(inputs)
-            entry = next((e for sig, e in self._graphs.items() if tuple(s for s, _ in sig) == shapes), None)
-        if entry is None:
-            # no eager fall-back: an eager step at a new shape could re-plan the step arena under the captured graphs
-            raise ValueError(f"TrainStep.step: no CUDA graph was captured for input shapes {list(_shapes(inputs))}; captured: "
-                             f"{[list(s) for s in self.captured_shapes]} (capture every shape the sampler draws with capture_shapes)")
-        return entry
 
     # ---- whole step as one CUDA graph per input shape
     def capture(self, *inputs: torch.Tensor, warmup: int = 3):
@@ -366,42 +351,30 @@ class TrainStep:
         dev = self.ws.device
         statics = _static_buffers(list(by_sig.items()), dev)
         passes = max(warmup, 3) - (self.eager_steps if len(by_sig) == 1 else 0)
-        torch.cuda.synchronize(dev)
-        side = torch.cuda.Stream(device=dev)
-        side.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(side):
-            for _ in range(max(0, passes)):
-                for sig, st in statics.items():
-                    for s_in, t in zip(st, by_sig[sig]):
-                        s_in.copy_(t)
-                    self.step(*st)  # real eager calls: with accum_freq > 1 they advance the window and update at its end
-            self._first = next(iter(by_sig))
-            for s_in, t in zip(statics[self._first], by_sig[self._first]):  # static_inputs hold the first example, as they always have
+        self._first = next(iter(by_sig))
+
+        def fill(sig):
+            for s_in, t in zip(statics[sig], by_sig[sig]):
                 s_in.copy_(t)
-        torch.cuda.current_stream().wait_stream(side)
-        torch.cuda.synchronize(dev)
+
+        def warm_up():
+            for _ in range(max(0, passes)):
+                for sig in statics:
+                    fill(sig)
+                    self.step(*statics[sig])  # real eager calls: with accum_freq > 1 they advance the window and update at its end
+            fill(self._first)  # static_inputs hold the first example, as they always have
+        _warm_up(dev, warm_up)
         self.ws.freeze()
-        gc.collect()  # no autograd graph of an eager step (leaf accumulators are bound to the stream they were created on) may survive into capture
         self._pool = torch.cuda.graph_pool_handle()
         order = sorted(statics, key=lambda sig: -sum(math.prod(s) * d.itemsize for s, d in sig))  # stable: ties keep the given order
         self.launches_per_shape: Dict[tuple, int] = {}
         for sig in order:
-            graph = torch.cuda.CUDAGraph()
-            n0 = ops.launch_count
-            with torch.cuda.graph(graph, pool=self._pool):
-                # detached: the loss's autograd graph (and the activations its nodes hold) dies here, so the next capture can reuse them
-                sloss = self._step(*statics[sig]).detach()
-            gc.collect()
-            self.launches_per_shape[tuple(s for s, _ in sig)] = ops.launch_count - n0
+            # detached: the loss's autograd graph (and the activations its nodes hold) dies here, so the next capture can reuse them
+            graph, sloss, self.launches_per_shape[_shapes(sig)] = _capture(self._pool, lambda: self._step(*statics[sig]).detach())
             self._graphs[sig] = (graph, statics[sig], sloss)
         self.launches_per_step = max(self.launches_per_shape.values())
         if self.grad_acc is not None:
-            graph = torch.cuda.CUDAGraph()
-            n0 = ops.launch_count
-            with torch.cuda.graph(graph, pool=self._pool):
-                self._update()
-            self.launches_per_update = ops.launch_count - n0
-            self._update_graph = graph
+            self._update_graph, _, self.launches_per_update = _capture(self._pool, self._update)
         return self
 
     @property
@@ -413,7 +386,7 @@ class TrainStep:
     @property
     def captured_shapes(self) -> List[tuple]:
         """The captured tuples of input shapes, in capture order."""
-        return [tuple(s for s, _ in sig) for sig in self._graphs]
+        return [_shapes(sig) for sig in self._graphs]
 
     def graph_pool_bytes(self) -> int:
         """Device memory the captured graphs' shared pool holds (0 before capture)."""
@@ -428,12 +401,47 @@ def _pool_bytes(pool_handle) -> int:
     return sum(s["total_size"] for s in segs if tuple(s.get("segment_pool_id", pool)) == pool)
 
 
-def _shapes(inputs) -> tuple:
-    return tuple(tuple(t.shape) for t in inputs)
-
-
 def _signature(inputs) -> tuple:
     return tuple((tuple(t.shape), t.dtype) for t in inputs)
+
+
+def _shapes(sig) -> tuple:
+    return tuple(s for s, _ in sig)
+
+
+def _warm_up(dev, fn) -> None:
+    """Run ``fn`` (the eager passes before a capture) on a fresh side stream of ``dev``, fenced from the work before and after it, as
+    torch.cuda.graph's warm-up asks."""
+    torch.cuda.synchronize(dev)
+    side = torch.cuda.Stream(device=dev)
+    side.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(side):
+        fn()
+    torch.cuda.current_stream().wait_stream(side)
+    torch.cuda.synchronize(dev)
+
+
+def _capture(pool, fn) -> tuple:
+    """Capture ``fn()`` into the memory pool ``pool``: (CUDA graph, fn's output, library launches it made).  Garbage is collected on both
+    sides: before, because no autograd graph of an eager step (leaf accumulators are bound to the stream they were created on) may survive
+    into capture; after, so the blocks this capture's dropped temporaries held return to the pool for the next capture to reuse."""
+    gc.collect()
+    graph = torch.cuda.CUDAGraph()
+    n0 = ops.launch_count
+    with torch.cuda.graph(graph, pool=pool):
+        out = fn()
+    gc.collect()
+    return graph, out, ops.launch_count - n0
+
+
+def _graph_for(graphs: Dict[tuple, tuple], key: tuple, owner: str, fmt, hint: str) -> tuple:
+    """The (CUDA graph, static inputs, static output) captured for ``key``, else for the first captured key that ``fmt`` renders alike
+    (TrainStep: the same shapes with other dtypes, which the copy into the static buffers converts).  Otherwise ValueError, listing the
+    captured keys: there is no eager fall-back, as an eager pass at a new shape could re-plan the step arena under the captured graphs."""
+    entry = graphs.get(key) or next((e for k, e in graphs.items() if fmt(k) == fmt(key)), None)
+    if entry is None:
+        raise ValueError(f"{owner}: no CUDA graph was captured for {fmt(key)}; captured: {[fmt(k) for k in graphs]} ({hint})")
+    return entry
 
 
 def _static_buffers(examples: List[Tuple[tuple, tuple]], dev) -> Dict[tuple, tuple]:
@@ -648,7 +656,7 @@ class EvalStep:
         self.counts = torch.zeros(3, device=self.device, dtype=torch.int64)  # top-1 hits, top-5 hits, rows
         self._ticket = torch.zeros(1, device=self.device, dtype=torch.int32)
         self._row_loss = torch.zeros(0, device=self.device, dtype=torch.float32)
-        self._graphs: Dict[tuple, tuple] = {}  # (C, H, W) -> (CUDA graph, static images, static targets, static logits)
+        self._graphs: Dict[tuple, tuple] = {}  # (C, H, W) -> (CUDA graph, (static images, static targets), static logits)
         self._pool = None
         self._weights_seen = None
         self.logits: Optional[torch.Tensor] = None  # bf16 logits of the last batch (captured: the graph's static output; all its rows)
@@ -702,12 +710,8 @@ class EvalStep:
             if not self._graphs:
                 self.logits = self._pass(images.to(self.device), targets.contiguous())
                 return
-            key = tuple(images.shape[1:])
-            entry = self._graphs.get(key)
-            if entry is None:
-                raise ValueError(f"EvalStep.update: no CUDA graph was captured for images of shape [*, {', '.join(map(str, key))}]; captured: "
-                                 f"{[list(k) for k in self._graphs]}")
-            graph, sx, sy, logits = entry
+            graph, (sx, sy), logits = _graph_for(self._graphs, tuple(images.shape[1:]), "EvalStep.update", list,
+                                                 "capture every crop (C, H, W) the loader yields with capture")
             b = images.shape[0]
             if b > sx.shape[0]:
                 raise ValueError(f"EvalStep.update: batch {b} exceeds the captured batch {sx.shape[0]}")
@@ -730,26 +734,20 @@ class EvalStep:
         sx = torch.zeros((batch,) + key, device=dev, dtype=torch.float32)
         sy = torch.full((batch,), self.ignore_index, device=dev, dtype=torch.int64)
         self._scratch(batch)
-        torch.cuda.synchronize(dev)
-        side = torch.cuda.Stream(device=dev)
-        side.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(side), torch.no_grad():
-            self._refresh()
-            for _ in range(max(1, warmup)):
-                self._pass(sx, sy)
-        torch.cuda.current_stream().wait_stream(side)
-        torch.cuda.synchronize(dev)
+
+        def warm_up():
+            with torch.no_grad():
+                self._refresh()
+                for _ in range(max(1, warmup)):
+                    self._pass(sx, sy)
+        _warm_up(dev, warm_up)
         self._refresh(force=True)  # caches the warm-up created included: the graph's forward then skips every refresh
         torch.cuda.synchronize(dev)
-        gc.collect()
         if self._pool is None:
             self._pool = torch.cuda.graph_pool_handle()
-        graph = torch.cuda.CUDAGraph()
-        n0 = ops.launch_count
-        with torch.cuda.graph(graph, pool=self._pool), torch.no_grad():
-            logits = self._pass(sx, sy)
-        self.launches_per_crop[key] = ops.launch_count - n0
-        self._graphs[key] = (graph, sx, sy, logits)
+        with torch.no_grad():
+            graph, logits, self.launches_per_crop[key] = _capture(self._pool, lambda: self._pass(sx, sy))
+        self._graphs[key] = (graph, (sx, sy), logits)
         return self
 
     def graph_pool_bytes(self) -> int:
