@@ -83,7 +83,8 @@ typedef struct {
   const float* e_p0; const float* e_p1; /* per-N vectors (NULL => 1 / 0) */
   const void* R; int ldr;   /* bf16 [M, ldr] residual added to the output, or NULL */
   void* C; int ldc; int c_fp32; /* output bf16 (or fp32 if c_fp32) [M, ldc] */
-  double* col_sum; double* col_sq;   /* fp64 [N] accumulators or NULL (BatchNorm statistics of the stored output) */
+  double* col_sum; double* col_sq;   /* fp64 [N] accumulators or NULL (BatchNorm statistics of the stored output; the wgmma kernel's full
+                                        tiles without a residual sum the fp32 values before the bf16 rounding of the store) */
   double* samp_sum; double* samp_sq; /* fp64 [M/rows_per_sample] or NULL (GroupNorm statistics of the stored output) */
   double* gn_ws;            /* CVB_E_GN_BWD only, optional: ZEROED fp64 workspace [2][M/rows_per_sample][N].  When given (and
                                rows_per_sample % 64 == 0) the epilogue runs on the wgmma kernel: it accumulates the per-(sample, channel)
@@ -126,7 +127,8 @@ CVB_API int cvb_apply_load_mode(const void* A, int lda, const void* A2, int lda2
  * config/efficientnet.py).  dilation 0 / 1 = dense stencil (TMA walk kernels); dilation > 1 (stride 1 only) = the segmentation
  * backbones' output_stride 8 / 16 variants (base_image_encoder.py:38-47, mobilevit_v2.py:176-191), a direct-gather kernel.  The producer's BN(+SiLU) is applied on load (x_mode RAW/AFF/AFF_SILU); zero padding
  * is applied AFTER that transform, as in the reference where padding acts on the activated tensor.
- * Output: pre-BN y (bf16) + fp64 per-channel sum / sum of squares of the stored values.
+ * Output: pre-BN y (bf16) + fp64 per-channel sum / sum of squares of the stored values (interior tiles -- the whole tile and a full
+ * 64-channel block inside the map -- sum the fp32 values before the bf16 rounding of the store).
  * ------------------------------------------------------------------------------------------------------------- */
 typedef struct {
   int B, H, W, C, stride;
@@ -229,7 +231,8 @@ CVB_API int cvb_linattn_bwd(const void* QKV, int ldq, const void* DO, int ldo, c
  * Cross-attention (LinearSelfAttention._forward_cross_attn, linear_attention.py:163-207; LinearAttnFFN cross branch transformer.py:254-260):
  * query + key come from the projection of x_prev (QK_prev: [B, P, M, ldq], columns as above), the values from the projection of x
  * (V_x: [B, P, N, ldv], value columns [d, 2d)); softmax / context over M, output O [B, P, N, ldo].  S: [B, P, M], CTX: [B, P, d].
- * bwd writes the key/query columns of DQK_prev and the value columns of DV_x (the caller zero-fills the other columns of both). */
+ * bwd writes the key/query columns of DQK_prev and zeroes its pad columns [2d+1, ldq), and writes the value columns of DV_x; the value
+ * columns of DQK_prev and the other columns of DV_x are left alone (the caller zero-fills them). */
 CVB_API int cvb_linattn_cross_fwd(const void* QK_prev, int ldq, int B, int P, int M, int d, const void* V_x, int ldv, int N, void* O, int ldo,
                           float* S, float* CTX, cvb_stream_t stream);
 CVB_API int cvb_linattn_cross_bwd(const void* QK_prev, int ldq, const void* V_x, int ldv, const void* DO, int ldo, const float* S, const float* CTX,
@@ -343,12 +346,14 @@ CVB_API int cvb_patch_stem_dgrad(const void* dz, const void* y, const float* coe
 /* ---------------------------------------------------------------------------------------------------------------
  * Per-step tail of the training loop (engine/training_engine.py:289-312) on FLAT fp32 buffers of n elements: GradScaler unscale +
  * inf check, clip_grad_norm_, AdamW, GradScaler update -- two launches, all state on the device (CUDA-graph friendly).
- *   stats : fp32[4], zero-initialised once; [0] sum of squares of the unscaled gradients, [1] # non-finite elements,
- *           [2] 1/scale used by this step, [3] internal block counter (the step kernel clears [0], [1], [3] when it is done)
+ *   stats : fp32[4], zero-initialised once; [0] sum of squares of the unscaled gradients, [1] # non-finite elements (the step kernel
+ *           leaves both as the totals of the step just taken), [2] 1/scale used by this step, [3] internal block counter (the step
+ *           kernel leaves it zero)
  *   scale : fp32[2] = {loss scale, growth tracker}   (torch.amp.GradScaler: init 65536, growth 2.0, backoff 0.5, interval 2000)
  *   step  : fp32[1] optimizer step count
- * cvb_grad_norm must precede cvb_adamw_step.  AdamW follows torch.optim.AdamW exactly (decoupled weight decay p *= 1 - lr*wd[i],
- * bias-corrected moments, eps added after the sqrt); weight_decay is per ELEMENT so the reference's two parameter groups
+ * cvb_grad_norm must precede cvb_adamw_step.  AdamW follows torch.optim.AdamW (decoupled weight decay p *= 1 - lr*wd[i],
+ * bias-corrected moments, eps added after the sqrt) with its coefficients in fp32: 1 - beta1 and 1 - beta2 are formed from the fp32 betas
+ * (for beta2 = 0.999 that puts exp_avg_sq about 1.3e-5 relative off torch, which forms 1 - beta2 in double); weight_decay is per ELEMENT so the reference's two parameter groups
  * (cvnets/misc/common.py:122-176: 1-D parameters are not decayed) need no segment table.  max_norm <= 0 disables clipping.
  * hp    : fp32[1] DEVICE scalar = learning rate (written by the scheduler each iteration: scheduler.update_lr, training_engine.py:246-249)
  * grad_div : gradients are divided by loss_scale * grad_div (DDP's mean over ranks: grad_div = world size, main_train.py:90-96)
@@ -402,7 +407,8 @@ CVB_API int cvb_cast_f64_f32(const cvb_cast_desc* descs_device, int n_desc, int 
  * CLIP text tower edges and feature normalisation (BASELINE.json configs[4]; csrc/clip.cu)
  *   embedding: out[b,s,:] = bf16(table[tokens[b,s],:] + pos[s,:])  (cvnets/text_encoders/transformer.py:328-341); bwd: dtable[token] += dout
  *              (fp32 atomics), dpos[s] += sum_b dout[b,s]
- *   eot gather: out[b,:] = X[b, argmax_s tokens[b,s], :] (transformer.py:413-421); idx[b] saved; bwd scatters into a zero-filled dX
+ *   eot gather: out[b,:] = X[b, argmax_s tokens[b,s], :] (transformer.py:413-421); idx[b] saved; bwd writes every row of dX: dout at the
+ *              gathered rows, zeros elsewhere
  *   l2norm: Y = X / max(||X||_2, eps) per row (F.normalize, transformer.py:423-425); inv_norm saved; bwd dx = inv*(dy - y (y.dy))
  *   transpose / add: Y[c,r] = X[r,c];  OUT = bf16(A + B) (A bf16 or NULL, B fp32) -- glue of the contrastive loss's gradient assembly
  * ------------------------------------------------------------------------------------------------------------- */
