@@ -244,11 +244,14 @@ CVB_API int cvb_linattn_cross_bwd(const void* QK_prev, int ldq, const void* V_x,
  * QKV: bf16 [B*S, ldq] rows = tokens, columns [q (H*c) | k (H*c) | v (H*c)] exactly as qkv_proj writes them (:148-153);
  * O: bf16 [B*S, ldo] with head h at columns h*c.. (the layout out_proj reads, :236).  scale = head_dim^-0.5 (:70, :187).
  * attn_mask: fp32 [B, S, S] additive (or NULL, :197-208); key_padding_mask: uint8 [B, S], non-zero = masked with -inf (:210-224).
- * Softmax in fp32 (:226-228).  LSE: fp32 [B, H, S] log-sum-exp (base 2) saved for the backward.  Even c <= 64; S <= 256, or any S for c = 64.
+ * Softmax in fp32 (:226-228).  LSE: fp32 [B, H, S] log-sum-exp (base 2) saved for the backward.  Even c <= 64; any S for c = 64.  Other head
+ * dims keep a whole head in one CTA's shared memory (c padded to 16 / 32 / 48 / 64, S to a multiple of 64; forward 3*Sp*(c+8)*2 bytes,
+ * backward 4*Sp*(c+8)*2 + 8*Sp, at most 226 KB): S <= 1152 / 704 / 448 / 384 for c <= 16 / 32 / 48 / 62 in the backward (1600 / 960 / 640 /
+ * 512 in the forward); a longer sequence returns an error.
  * head_dim == 64 (ViT-B / CLIP image tower, key-padding masks included) runs on wgmma tensor cores: S <= 256 in mha_tc.cu (TMA-staged operands,
  * whole score rows in registers), S > 256 (ViT / CLIP at 256-512 px crops) in mha_long.cu (K/V and Q/dO streamed through shared memory in
- * 64-row tiles, online softmax; a backward without atomics, bitwise reproducible).  Every other head_dim, and heads with an additive mask at
- * S <= 256, run on the mma.sync kernels (mha.cu).
+ * 64-row tiles, online softmax; a backward without atomics, bitwise reproducible).  Every other head_dim, and head_dim-64 heads with an
+ * additive mask at S <= 256, run on the mma.sync kernels (mha.cu).
  * ------------------------------------------------------------------------------------------------------------- */
 CVB_API int cvb_mha_fwd(const void* QKV, int ldq, int B, int S, int H, int head_dim, float scale, const float* attn_mask,
                 const unsigned char* key_padding_mask, void* O, int ldo, float* LSE, cvb_stream_t stream);
@@ -256,7 +259,7 @@ CVB_API int cvb_mha_fwd(const void* QKV, int ldq, int B, int S, int H, int head_
 CVB_API int cvb_mha_bwd(const void* QKV, int ldq, const void* O, const void* DO, int ldo, const float* LSE, int B, int S, int H, int head_dim,
                 float scale, const float* attn_mask, const unsigned char* key_padding_mask, void* DQKV, int lddq, cvb_stream_t stream);
 /* Testing hook: which kernel family serves a head, forward and backward alike.  0 = automatic (default, as described above);
- * 1 = the mma.sync kernels wherever they can run (S <= 256); 2 = the streaming kernels for every head_dim-64 shape.  Modes 1 and 2
+ * 1 = the mma.sync kernels wherever they can run (head_dim 64: S <= 256); 2 = the streaming kernels for every head_dim-64 shape.  Modes 1 and 2
  * cross-check the families against each other; any other value selects 0.  Returns the previous mode. */
 CVB_API int cvb_set_mha_impl(int mode);
 /* per-token LayerNorm statistics of a bf16 [M, C] matrix: mean[m], rstd[m] = 1/sqrt(var + eps) (biased variance, fp32 math like
@@ -498,11 +501,22 @@ CVB_API int cvb_unprep_grad(const float* src, float* dst, int rows, int cols, in
 CVB_API int cvb_im2col(const void* X, int x_fp32, int64_t sxn, int64_t sxc, int64_t sxh, int64_t sxw, int B, int Cin, int H, int W, int k, int stride,
                int pad, void* A, int lda, cvb_stream_t stream);
 CVB_API int cvb_col2im(const void* dA, int lda, int B, int Cin, int H, int W, int k, int stride, int pad, void* dX, cvb_stream_t stream);
-/* MobileViT-v1 unfolding / folding (cvnets/modules/mobilevit_block.py:186-267) as a row permutation of the channels-last matrix:
- * feature-map row (b, h, w) <-> token row (b*P + p, n), p = (h % ph)*pw + (w % pw), n = (h / ph)*(W / pw) + (w / pw), P = ph*pw.
- * inverse = 0: X is the feature map [B*H*W, C], OUT the token matrix [B*P, N, C]; inverse = 1: the other way (folding).  The permutation
- * is its own adjoint with the flag flipped.  H, W must be multiples of the patch (the bilinear resize branch, :191-200, is not implemented). */
-CVB_API int cvb_patch_permute(const void* X, void* OUT, int B, int H, int W, int C, int patch_h, int patch_w, int inverse, cvb_stream_t stream);
+/* MobileViT-v1 unfolding / folding (cvnets/modules/mobilevit_block.py:186-267) on channels-last matrices.  The feature map is [B*H*W, C];
+ * the token matrix [B*P, N, C] covers the grid Hn x Wn, Hn = ceil(H / ph)*ph, Wn = ceil(W / pw)*pw: token row (b*P + p, n) is grid pixel
+ * (y, x) with p = (y % ph)*pw + (x % pw), n = (y / ph)*(Wn / pw) + (x / pw), P = ph*pw, N = (Hn / ph)*(Wn / pw).
+ * direction (cvb_patch_direction): UNFOLD maps the feature map to tokens, FOLD tokens to the feature map, UNFOLD_T and FOLD_T are their
+ * transposes (the backward of each: UNFOLD_T takes token gradients to the map, FOLD_T map gradients to tokens).
+ * H, W multiples of the patch: a row permutation (FOLD = UNFOLD_T, UNFOLD = FOLD_T, bit for bit).  Otherwise the reference's bilinear
+ * resize (F.interpolate, align_corners=False, :191-200 and :259-265) is fused in: UNFOLD samples the H x W map at the Hn x Wn grid, FOLD
+ * samples the token grid at H x W (4 source rows per output row, fp32, one bf16 rounding); the transposes are gathers over the rows whose
+ * stencil reads an output row, without atomics (bitwise reproducible).  Every row of OUT is written. */
+enum {
+  CVB_PATCH_UNFOLD = 0,   /* X feature map [B*H*W, C]  -> OUT tokens [B*P*N, C] */
+  CVB_PATCH_FOLD = 1,     /* X tokens [B*P*N, C]       -> OUT feature map [B*H*W, C] */
+  CVB_PATCH_UNFOLD_T = 2, /* X tokens [B*P*N, C]       -> OUT feature map [B*H*W, C]  (adjoint of UNFOLD) */
+  CVB_PATCH_FOLD_T = 3    /* X feature map [B*H*W, C]  -> OUT tokens [B*P*N, C]       (adjoint of FOLD) */
+};
+CVB_API int cvb_patch_permute(const void* X, void* OUT, int B, int H, int W, int C, int patch_h, int patch_w, int direction, cvb_stream_t stream);
 /* OUT[m, :] = [A[m, :C1] | B[m, :C2]] (torch.cat((res, fm), dim=1) on channels-last maps, mobilevit_block.py:287) and the adjoint split */
 CVB_API int cvb_concat2(const void* A, const void* B, int C1, int C2, int64_t M, void* OUT, cvb_stream_t stream);
 CVB_API int cvb_split2(const void* G, int C1, int C2, int64_t M, void* DA, void* DB, cvb_stream_t stream);

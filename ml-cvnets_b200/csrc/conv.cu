@@ -222,6 +222,99 @@ __global__ void __launch_bounds__(CNT) patch_permute_kernel(const bf16* __restri
   }
 }
 
+// MobileViT-v1 unfolding / folding of a map that is not a multiple of the patch (mobilevit_block.py:191-200, :259-265): the reference resizes
+// the H x W map bilinearly (align_corners=False) up to the Hn x Wn grid the patches tile before unfolding, and the folded Hn x Wn map back down
+// to H x W.  Each kernel thread owns one output row (8 channels) and fuses the resample with the row permutation; row indices on the Hn x Wn
+// grid are token rows (b*P + p, n).  interp_src is PyTorch's source-index rule per axis, scale = n_src / n_dst.
+//   dir 0 (unfold)  token (y, x) of Hn x Wn = the 4-tap stencil of map H x W             dir 2 = transpose of 0: map pixel (y, x) gathers
+//   dir 1 (fold)    map pixel (y, x) of H x W = the 4-tap stencil of the token grid        the tokens whose dir-0 stencil reads it
+//                                                                                          dir 3 = transpose of 1: token (y, x) gathers the map
+// Transposes are gathers over the few destinations whose stencil touches the row (like vit_pos_interp_bwd_kernel): no atomics, the same
+// bits every run.  fp32 arithmetic, one bf16 rounding.
+__device__ __forceinline__ int64_t grid_row(int64_t b, int y, int x, int Hg, int Wg, bool tok, int ph, int pw) {
+  if (!tok) return (b * Hg + y) * Wg + x;
+  const int nw = Wg / pw, N = (Hg / ph) * nw;
+  return (b * (ph * pw) + (y % ph) * pw + (x % pw)) * N + (y / ph) * nw + (x / pw);
+}
+// the weight with which destination d of a 1-D stencil (n_src sources, scale) reads source j; false if it does not read it
+__device__ __forceinline__ bool stencil_weight(int d, int j, float scale, int n_src, float& w) {
+  int i0, i1;
+  float lam;
+  interp_src(d, scale, n_src, i0, i1, lam);
+  if (i0 != j && i1 != j) return false;
+  w = i0 == j ? __fsub_rn(1.f, lam) : 0.f;
+  if (i1 == j) w = __fadd_rn(w, lam);
+  return true;
+}
+__global__ void __launch_bounds__(CNT) patch_resample_kernel(const bf16* __restrict__ X, bf16* __restrict__ OUT, int H, int W, int Hn, int Wn, int C,
+                                                             int ph, int pw, int dir, int64_t nrows) {
+  pdl_wait();
+  pdl_trigger();
+  // the stencil runs from its source grid (sh x sw) to its destination grid (dh x dw): map -> tokens for dirs 0 / 2, tokens -> map for 1 / 3
+  const bool up = dir == 0 || dir == 2, adjoint = dir >= 2;
+  const int sh = up ? H : Hn, sw = up ? W : Wn, dh = up ? Hn : H, dw = up ? Wn : W;
+  const float sy = (float)sh / (float)dh, sx = (float)sw / (float)dw;
+  // a forward direction writes the destination grid and reads the source grid; its transpose the other way round
+  const int oh = adjoint ? sh : dh, ow = adjoint ? sw : dw, ih = adjoint ? dh : sh, iw = adjoint ? dw : sw;
+  const bool out_tok = (dir == 0 || dir == 3), in_tok = !out_tok;
+  const int cg = C >> 3;
+  const int64_t total = nrows * cg;
+  for (int64_t idx = (int64_t)blockIdx.x * CNT + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * CNT) {
+    const int64_t pix = idx / cg;
+    const int c8 = (int)(idx % cg);
+    const int x = (int)(pix % ow), y = (int)((pix / ow) % oh);
+    const int64_t b = pix / ((int64_t)ow * oh);
+    float acc[8];
+#pragma unroll
+    for (int q = 0; q < 8; ++q) acc[q] = 0.f;
+    if (!adjoint) {
+      int y0, y1, x0, x1;
+      float ly, lx;
+      interp_src(y, sy, sh, y0, y1, ly);
+      interp_src(x, sx, sw, x0, x1, lx);
+      const int ys[2] = {y0, y1}, xs[2] = {x0, x1};
+      const float wy[2] = {__fsub_rn(1.f, ly), ly}, wx[2] = {__fsub_rn(1.f, lx), lx};
+#pragma unroll
+      for (int a = 0; a < 2; ++a) {
+        float row[8];
+#pragma unroll
+        for (int q = 0; q < 8; ++q) row[q] = 0.f;
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          float f[8];
+          unpack8(ldg16(X + grid_row(b, ys[a], xs[e], ih, iw, in_tok, ph, pw) * C + c8 * 8), f);
+#pragma unroll
+          for (int q = 0; q < 8; ++q) row[q] = __fadd_rn(row[q], __fmul_rn(wx[e], f[q]));
+        }
+#pragma unroll
+        for (int q = 0; q < 8; ++q) acc[q] = __fadd_rn(acc[q], __fmul_rn(wy[a], row[q]));
+      }
+    } else {
+      // destinations whose source index i0 lies in {j - 1, j}: src in [j - 1, j + 1), widened by 2 (vit_pos_interp_bwd_kernel)
+      const int d_lo = max(0, (int)((y - 1.0f) / sy) - 2), d_hi = min(dh - 1, (int)((y + 2.0f) / sy) + 2);
+      const int e_lo = max(0, (int)((x - 1.0f) / sx) - 2), e_hi = min(dw - 1, (int)((x + 2.0f) / sx) + 2);
+      for (int d = d_lo; d <= d_hi; ++d) {
+        float wy;
+        if (!stencil_weight(d, y, sy, sh, wy)) continue;
+        float row[8];
+#pragma unroll
+        for (int q = 0; q < 8; ++q) row[q] = 0.f;
+        for (int e = e_lo; e <= e_hi; ++e) {
+          float wx;
+          if (!stencil_weight(e, x, sx, sw, wx)) continue;
+          float f[8];
+          unpack8(ldg16(X + grid_row(b, d, e, ih, iw, in_tok, ph, pw) * C + c8 * 8), f);
+#pragma unroll
+          for (int q = 0; q < 8; ++q) row[q] = __fadd_rn(row[q], __fmul_rn(wx, f[q]));
+        }
+#pragma unroll
+        for (int q = 0; q < 8; ++q) acc[q] = __fadd_rn(acc[q], __fmul_rn(wy, row[q]));
+      }
+    }
+    stg16(OUT + grid_row(b, y, x, oh, ow, out_tok, ph, pw) * C + c8 * 8, pack8(acc));
+  }
+}
+
 // channel concatenation of two channels-last matrices (torch.cat((res, fm), dim=1), mobilevit_block.py:287) and its adjoint
 __global__ void __launch_bounds__(CNT) concat2_kernel(const bf16* __restrict__ A, const bf16* __restrict__ B, bf16* __restrict__ OUT, int C1, int C2,
                                                       int split, int64_t M, bf16* __restrict__ DA, bf16* __restrict__ DB) {
@@ -283,13 +376,24 @@ extern "C" int cvb_col2im(const void* dA, int lda, int B, int Cin, int H, int W,
   return 0;
 }
 
-extern "C" int cvb_patch_permute(const void* X, void* OUT, int B, int H, int W, int C, int patch_h, int patch_w, int inverse, cvb_stream_t stream) {
-  CVB_CHECK(X && OUT && B > 0 && H > 0 && W > 0 && C > 0 && C % 8 == 0 && patch_h > 0 && patch_w > 0 && H % patch_h == 0 && W % patch_w == 0,
-            "cvb_patch_permute: bad arguments (C %% 8 == 0, H, W multiples of the patch)");
+extern "C" int cvb_patch_permute(const void* X, void* OUT, int B, int H, int W, int C, int patch_h, int patch_w, int direction,
+                                 cvb_stream_t stream) {
+  CVB_CHECK(X && OUT && B > 0 && H > 0 && W > 0 && C > 0 && C % 8 == 0 && patch_h > 0 && patch_w > 0, "cvb_patch_permute: bad arguments (C %% 8 == 0)");
+  CVB_CHECK(direction >= CVB_PATCH_UNFOLD && direction <= CVB_PATCH_FOLD_T, "cvb_patch_permute: direction %d is not a cvb_patch_direction", direction);
   CVB_CHECK(cvb_aligned16(X) && cvb_aligned16(OUT), "cvb_patch_permute: misaligned operand");
-  const int64_t npix = (int64_t)B * H * W;
-  CVB_CUDA(cvb_launch(patch_permute_kernel, cgrid(npix * (C / 8)), CNT, 0, static_cast<cudaStream_t>(stream), static_cast<const bf16*>(X),
-                      static_cast<bf16*>(OUT), H, W, C, patch_h, patch_w, inverse, npix));
+  const int Hn = (H + patch_h - 1) / patch_h * patch_h, Wn = (W + patch_w - 1) / patch_w * patch_w;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (Hn == H && Wn == W) {  // a row permutation, its own adjoint with the direction flipped
+    const int64_t npix = (int64_t)B * H * W;
+    const int inverse = direction == CVB_PATCH_FOLD || direction == CVB_PATCH_UNFOLD_T;
+    CVB_CUDA(cvb_launch(patch_permute_kernel, cgrid(npix * (C / 8)), CNT, 0, st, static_cast<const bf16*>(X), static_cast<bf16*>(OUT), H, W, C, patch_h,
+                        patch_w, inverse, npix));
+    return 0;
+  }
+  const bool tok_out = direction == CVB_PATCH_UNFOLD || direction == CVB_PATCH_FOLD_T;
+  const int64_t nrows = (int64_t)B * (tok_out ? (int64_t)Hn * Wn : (int64_t)H * W);
+  CVB_CUDA(cvb_launch(patch_resample_kernel, cgrid(nrows * (C / 8)), CNT, 0, st, static_cast<const bf16*>(X), static_cast<bf16*>(OUT), H, W, Hn, Wn, C,
+                      patch_h, patch_w, direction, nrows));
   return 0;
 }
 

@@ -5,8 +5,10 @@
 // Q, K, V are strided views of the packed projection qkv[b*S + s, {0,1,2}*C + h*c + :] (the reference reshapes to [N,S,3,h,c],
 // :148-153), O is written straight into the [N*S, C] layout out_proj consumes (:236) -- no transposes, no [N,h,S,T] score
 // tensor in HBM (the reference materialises it twice, bf16 and fp32: 477 MB per ViT-B layer, SURVEY.md 8a a11).
-// One CTA per (sample, head); the whole K / V (and Q, dO in the backward) of that head live in shared memory (S <= 256,
-// head_dim in {16, 32, 64}: every hot-path config of SURVEY.md 8a: ViT-B 197x64, CLIP text 77x64, MobileViT-v1 256x16..).
+// One CTA per (sample, head); the whole K / V (and Q, dO in the backward) of that head live in shared memory, head_dim padded to
+// 16, 32, 48 or 64.  The key loops walk 64-row blocks, so S is bounded only by that shared memory (mha_smem_bytes): S <= 1152 / 704 / 448 /
+// 384 at the padded head dims 16 / 32 / 48 / 64 -- every MobileViT-v1 recipe crop (up to 400 tokens at head dims 16 - 36) and the CLIP text
+// tower (77x64).
 // Tensor cores: mma.sync.m16n8k16 bf16 -> fp32 (the score tiles are 16 x 64 per warp: far below a wgmma tile), online softmax
 // in the exp2 domain, probabilities kept in registers and re-used as the A operand of P.V.
 // Backward = two passes without atomics: pass A owns query rows (dQ), pass B owns key rows (dK, dV); P is recomputed from the
@@ -21,7 +23,8 @@ constexpr float LOG2E = 1.4426950408889634f;
 
 template <int HD>
 struct MhaCfg {
-  static constexpr int LD = HD + 8;       // smem row stride in elements (16-byte aligned rows, ldmatrix conflict-free)
+  static constexpr int LD = HD + 8;       // smem row stride in elements: 48 / 80 / 112 / 144 bytes, 16-byte aligned; the 8 rows of one
+                                          // ldmatrix phase land in 8 distinct 16-byte bank groups at each of them (conflict-free)
   static constexpr int KS = HD / 16;      // k-steps over the head dim
   static constexpr int NT = HD / 8;       // n-tiles over the head dim
 };
@@ -260,7 +263,7 @@ __global__ void __launch_bounds__(256) mha_bwd_kernel(const bf16* __restrict__ Q
   for (int q = tid; q < Sp; q += 256) {
     float d = 0.f;
     if (q < S) {
-      if (hd == HD) {
+      if (hd == HD && HD != 48) {  // HD 48 keeps the pair loop that served head_dim 48 when it ran on the HD-64 kernel: the same bits
 #pragma unroll
         for (int ch = 0; ch < HD / 8; ++ch) {
           float a[8], c[8];
@@ -378,21 +381,27 @@ __global__ void __launch_bounds__(256) mha_bwd_kernel(const bf16* __restrict__ Q
   }
 }
 
+// Dynamic shared memory of one CTA: Q, K, V rows (forward) plus dO rows and the fp32 LSE / D vectors (backward), S padded to 64.
+constexpr size_t MHA_SMEM_MAX = 226 * 1024;  // the sm_90 opt-in ceiling (227 KB) less the 1 KB NOTES.md reserves for static shared memory
+template <int HD>
+size_t mha_smem_bytes(int S, bool bwd) {
+  const size_t Sp = (size_t)(S + 63) / 64 * 64;
+  return bwd ? 4 * Sp * MhaCfg<HD>::LD * 2 + 8 * Sp : 3 * Sp * MhaCfg<HD>::LD * 2;
+}
+
 template <int HD>
 int launch_fwd(const void* QKV, int ldq, int B, int S, int H, float scale, const float* amask, const uint8_t* kpm, void* O, int ldo, float* LSE,
                cudaStream_t st, int hd) {
-  const int Sp = (S + 63) / 64 * 64;
-  const size_t smem = (size_t)3 * Sp * MhaCfg<HD>::LD * 2;
-  CVB_CUDA(cvb_smem_optin<mha_fwd_kernel<HD>>(200 * 1024));
+  const size_t smem = mha_smem_bytes<HD>(S, false);
+  CVB_CUDA(cvb_smem_optin<mha_fwd_kernel<HD>>((int)MHA_SMEM_MAX));
   CVB_CUDA(cvb_launch(mha_fwd_kernel<HD>, B * H, 128, smem, st, static_cast<const bf16*>(QKV), ldq, S, H, scale, amask, kpm, static_cast<bf16*>(O), ldo, LSE, hd));
   return 0;
 }
 template <int HD>
 int launch_bwd(const void* QKV, int ldq, const void* O, const void* DO, int ldo, const float* LSE, int B, int S, int H, float scale,
                const float* amask, const uint8_t* kpm, void* DQKV, int lddq, cudaStream_t st, int hd) {
-  const int Sp = (S + 63) / 64 * 64;
-  const size_t smem = (size_t)4 * Sp * MhaCfg<HD>::LD * 2 + (size_t)2 * Sp * 4;
-  CVB_CUDA(cvb_smem_optin<mha_bwd_kernel<HD>>(200 * 1024));
+  const size_t smem = mha_smem_bytes<HD>(S, true);
+  CVB_CUDA(cvb_smem_optin<mha_bwd_kernel<HD>>((int)MHA_SMEM_MAX));
   CVB_CUDA(cvb_launch(mha_bwd_kernel<HD>, B * H, 256, smem, st, static_cast<const bf16*>(QKV), ldq, static_cast<const bf16*>(O),
                       static_cast<const bf16*>(DO), ldo, LSE, S, H, scale, amask, kpm, static_cast<bf16*>(DQKV), lddq, hd));
   return 0;
@@ -401,19 +410,36 @@ int launch_bwd(const void* QKV, int ldq, const void* O, const void* DO, int ldo,
 int check_common(const char* who, const void* QKV, int ldq, int B, int S, int H, int head_dim, int ldo) {
   CVB_CHECK(QKV && B > 0 && S > 0 && H > 0, "%s: bad arguments", who);
   CVB_CHECK(head_dim >= 2 && head_dim <= 64 && head_dim % 2 == 0, "%s: head_dim %d not supported (even values up to 64)", who, head_dim);
-  CVB_CHECK(S <= 256 || head_dim == 64, "%s: sequence length %d > 256 needs head_dim 64 (got %d): the streaming kernels are head_dim-64 only, the "
-            "other head dims keep K/V of one head in shared memory", who, S, head_dim);
   CVB_CHECK(ldq % 8 == 0 && ldo % 8 == 0 && ldq >= 3 * H * head_dim && ldo >= H * head_dim && cvb_aligned16(QKV), "%s: bad leading dimensions / alignment", who);
   return 0;
 }
 
+// The mma.sync instantiation that serves a head dim: the smallest of 16 / 32 / 48 / 64 that holds it (pad columns are zero-filled).
+int mma_pad(int head_dim) { return head_dim <= 16 ? 16 : head_dim <= 32 ? 32 : head_dim <= 48 ? 48 : 64; }
+size_t mma_smem_bytes(int head_dim, int S, bool bwd) {
+  switch (mma_pad(head_dim)) {
+    case 16: return mha_smem_bytes<16>(S, bwd);
+    case 32: return mha_smem_bytes<32>(S, bwd);
+    case 48: return mha_smem_bytes<48>(S, bwd);
+    default: return mha_smem_bytes<64>(S, bwd);
+  }
+}
+// The longest sequence the mma.sync kernels run: the whole head must fit in one CTA's shared memory.
+int check_mma_fits(const char* who, int S, int head_dim, bool bwd) {
+  int smax = 0;
+  while (mma_smem_bytes(head_dim, smax + 64, bwd) <= MHA_SMEM_MAX) smax += 64;
+  CVB_CHECK(S <= smax, "%s: sequence length %d is too long for head_dim %d: the mma.sync kernels (head dim padded to %d) keep a whole head in "
+            "shared memory and take S <= %d in the %s", who, S, head_dim, mma_pad(head_dim), smax, bwd ? "backward" : "forward");
+  return 0;
+}
+
 // Which kernels serve a head.  Forward and backward ask the same question, so they always agree (the backward reads the forward's LSE).
-//   head_dim != 64                          mma.sync (this file; S <= 256, enforced by check_common)
+//   head_dim != 64                          mma.sync (this file; S up to the shared-memory limit, check_mma_fits)
 //   head_dim 64, S > 256                    streaming wgmma (mha_long.cu), with or without masks
 //   head_dim 64, S <= 256, additive mask    mma.sync: it reads the [S, S] mask in coalesced tiles, where the wgmma score fragments would
 //                                           gather single values (the causal CLIP text tower, S = 77)
 //   head_dim 64, S <= 256, otherwise        register-resident wgmma (mha_tc.cu)
-// g_mode (cvb_set_mha_impl, cross-checks only) overrides the choice where another family can run the shape.
+// g_mode (cvb_set_mha_impl, cross-checks only) overrides the choice where another family can run the shape (mode 1: head_dim 64 at S <= 256).
 enum class MhaPath { Mma, Tc, Long };
 int g_mode = 0;  // 0 automatic, 1 mma.sync wherever it runs, 2 streaming for every head_dim-64 shape
 
@@ -449,8 +475,10 @@ extern "C" int cvb_mha_fwd(const void* QKV, int ldq, int B, int S, int H, int he
   const MhaPath path = route(S, head_dim, attn_mask != nullptr);
   if (path == MhaPath::Long) return cvb_mha_fwd_long(QKV, ldq, B, S, H, scale, attn_mask, key_padding_mask, O, ldo, LSE, st);
   if (path == MhaPath::Tc) return cvb_mha_fwd_tc(QKV, ldq, B, S, H, scale, key_padding_mask, O, ldo, LSE, st);
+  if (check_mma_fits("cvb_mha_fwd", S, head_dim, false)) return 1;
   if (head_dim <= 16) return launch_fwd<16>(QKV, ldq, B, S, H, scale, attn_mask, key_padding_mask, O, ldo, LSE, st, head_dim);
   if (head_dim <= 32) return launch_fwd<32>(QKV, ldq, B, S, H, scale, attn_mask, key_padding_mask, O, ldo, LSE, st, head_dim);
+  if (head_dim <= 48) return launch_fwd<48>(QKV, ldq, B, S, H, scale, attn_mask, key_padding_mask, O, ldo, LSE, st, head_dim);
   return launch_fwd<64>(QKV, ldq, B, S, H, scale, attn_mask, key_padding_mask, O, ldo, LSE, st, head_dim);
 }
 
@@ -463,7 +491,9 @@ extern "C" int cvb_mha_bwd(const void* QKV, int ldq, const void* O, const void* 
   const MhaPath path = route(S, head_dim, attn_mask != nullptr);
   if (path == MhaPath::Long) return cvb_mha_bwd_long(QKV, ldq, O, DO, ldo, LSE, B, S, H, scale, attn_mask, key_padding_mask, DQKV, lddq, st);
   if (path == MhaPath::Tc) return cvb_mha_bwd_tc(QKV, ldq, O, DO, ldo, LSE, B, S, H, scale, key_padding_mask, DQKV, lddq, st);
+  if (check_mma_fits("cvb_mha_bwd", S, head_dim, true)) return 1;
   if (head_dim <= 16) return launch_bwd<16>(QKV, ldq, O, DO, ldo, LSE, B, S, H, scale, attn_mask, key_padding_mask, DQKV, lddq, st, head_dim);
   if (head_dim <= 32) return launch_bwd<32>(QKV, ldq, O, DO, ldo, LSE, B, S, H, scale, attn_mask, key_padding_mask, DQKV, lddq, st, head_dim);
+  if (head_dim <= 48) return launch_bwd<48>(QKV, ldq, O, DO, ldo, LSE, B, S, H, scale, attn_mask, key_padding_mask, DQKV, lddq, st, head_dim);
   return launch_bwd<64>(QKV, ldq, O, DO, ldo, LSE, B, S, H, scale, attn_mask, key_padding_mask, DQKV, lddq, st, head_dim);
 }

@@ -961,37 +961,38 @@ class SeScaleFn(torch.autograd.Function):
 
 
 class UnfoldFn(torch.autograd.Function):
-    """MobileViTBlock.unfolding (cvnets/modules/mobilevit_block.py:186-231): [B, C, H, W] -> [B*P, N, C] tokens (a row permutation)."""
+    """MobileViTBlock.unfolding (cvnets/modules/mobilevit_block.py:186-231): [B, C, H, W] -> [B*P, N, C] tokens.  A row permutation, with
+    the reference's bilinear resize to the (Hn, Wn) grid the patches tile fused in where H or W is not a multiple of the patch."""
 
     @staticmethod
-    def forward(ctx, x, ph, pw):
+    def forward(ctx, x, ph, pw, grid):
         B, C, H, W = x.shape
-        if H % ph or W % pw:
-            raise NotImplementedError("H, W must be multiples of the patch size (the bilinear resize branch, mobilevit_block.py:191-200, is not implemented)")
+        Hn, Wn = grid
         ctx.dims = (B, C, H, W, ph, pw)
-        return ops.patch_permute(as_2d(x), B, H, W, ph, pw, False).view(B * ph * pw, (H // ph) * (W // pw), C)
+        return ops.patch_permute(as_2d(x), B, H, W, ph, pw, direction=ops.PATCH_UNFOLD).view(B * ph * pw, (Hn // ph) * (Wn // pw), C)
 
     @staticmethod
     def backward(ctx, g):
         B, C, H, W, ph, pw = ctx.dims
         g2 = g.reshape(-1, C).to(BF16).contiguous()
-        return to_4d(ops.patch_permute(g2, B, H, W, ph, pw, True), B, H, W), None, None
+        return to_4d(ops.patch_permute(g2, B, H, W, ph, pw, direction=ops.PATCH_UNFOLD_T), B, H, W), None, None, None
 
 
 class FoldFn(torch.autograd.Function):
-    """MobileViTBlock.folding (mobilevit_block.py:233-267): [B*P, N, C] tokens -> [B, C, H, W]."""
+    """MobileViTBlock.folding (mobilevit_block.py:233-267): [B*P, N, C] tokens of the (Hn, Wn) grid -> [B, C, H, W], resized back down
+    bilinearly where the grid is larger than the map."""
 
     @staticmethod
     def forward(ctx, t, B, H, W, ph, pw):
         C = t.shape[-1]
         t2 = t.reshape(-1, C).to(BF16).contiguous()
         ctx.dims = (B, C, H, W, ph, pw, tuple(t.shape))
-        return to_4d(ops.patch_permute(t2, B, H, W, ph, pw, True), B, H, W)
+        return to_4d(ops.patch_permute(t2, B, H, W, ph, pw, direction=ops.PATCH_FOLD), B, H, W)
 
     @staticmethod
     def backward(ctx, g):
         B, C, H, W, ph, pw, shape = ctx.dims
-        return ops.patch_permute(as_2d(to_bf16_cl(g)), B, H, W, ph, pw, False).view(shape), None, None, None, None, None
+        return ops.patch_permute(as_2d(to_bf16_cl(g)), B, H, W, ph, pw, direction=ops.PATCH_FOLD_T).view(shape), None, None, None, None, None
 
 
 class Concat2Fn(torch.autograd.Function):

@@ -14,6 +14,7 @@ import torch
 from torch import Tensor, nn
 
 from . import functional as Fn
+from . import ops
 from .layers import (AdaptiveAvgPool2d, ConvLayer2d, Dropout, Identity, LinearLayer, LinearSelfAttention, MultiHeadAttention, StochasticDepth,
                      _bind, _need_cuda, build_activation_layer, get_normalization_layer)
 from .ops import PreparedWeights as PW
@@ -431,7 +432,8 @@ class MobileViTBlock(BaseModule):
         res = Fn.to_bf16_cl(x)
         fm = self.local_rep(res)
         B, _, H, W = fm.shape
-        patches = Fn.UnfoldFn.apply(fm, self.patch_h, self.patch_w)           # [B*P, N, d]
+        grid = ops.patch_grid(H, W, self.patch_h, self.patch_w)              # the bilinearly resized map where H, W are not patch multiples
+        patches = Fn.UnfoldFn.apply(fm, self.patch_h, self.patch_w, grid)     # [B*P, N, d]
         for layer in self.global_rep:
             patches = layer(patches)
         fm = Fn.FoldFn.apply(patches, B, H, W, self.patch_h, self.patch_w)
@@ -520,9 +522,10 @@ class TransformerEncoder(BaseModule):
         if x.dim() != 3:
             raise NotImplementedError("TransformerEncoder expects [N, S, C]")
         hd = self.pre_norm_mha[1].head_dim
-        if x.shape[1] > 256 and hd != 64:
-            raise NotImplementedError(f"TransformerEncoder: S = {x.shape[1]} > 256 needs head_dim 64 (the streaming attention kernels); "
-                                      f"head_dim {hd} keeps a head in shared memory and supports S <= 256")
+        smax = ops.mha_max_seq(hd)
+        if smax is not None and x.shape[1] > smax:
+            raise NotImplementedError(f"TransformerEncoder: S = {x.shape[1]} is too long for head_dim {hd}: the attention kernels keep a head in "
+                                      f"shared memory and take S <= {smax} there (any S at head_dim 64)")
         if x.shape[1] == x.shape[2]:
             raise NotImplementedError("S == C: the reference's LayerNorm would take its channel-first branch (layer_norm.py:52-65)")
         if self._cfg is None:

@@ -14,6 +14,7 @@ import torch
 from . import _lib as L
 from ._lib import (A_AFF, A_AFF_SILU, A_BNB, A_GN, A_RAW, A_SILU, E_GN_BWD, E_LIN_BWD, E_SILU, E_SILU_BWD, E_STORE,  # noqa: F401
                    ACT_GELU, ACT_HARDSIGMOID, ACT_HARDSWISH, ACT_RELU, ACT_SIGMOID, ACT_SILU,
+                   PATCH_FOLD, PATCH_FOLD_T, PATCH_UNFOLD, PATCH_UNFOLD_T,
                    cvb_dw_bwd_args, cvb_dw_fwd_args, cvb_gemm_args, cvb_prep_desc, cvb_wgrad_args)
 
 Tensor = torch.Tensor
@@ -407,10 +408,21 @@ def grad_accumulate(acc: Tensor, g: Tensor) -> None:
     _count()
 
 
-def patch_permute(X: Tensor, B: int, H: int, W: int, ph: int, pw: int, inverse: bool) -> Tensor:
-    """MobileViT-v1 unfold (inverse=False: feature-map rows -> token rows [B*P*N, C]) / fold (inverse=True)."""
-    out = torch.empty_like(X)
-    _lib().cvb_patch_permute(X.data_ptr(), out.data_ptr(), B, H, W, X.shape[1], ph, pw, int(inverse), _stream())
+def patch_grid(H: int, W: int, ph: int, pw: int):
+    """the Hn x Wn grid MobileViT-v1 tiles with patches: H, W rounded up to multiples of the patch (mobilevit_block.py:191-192)"""
+    return -(-H // ph) * ph, -(-W // pw) * pw
+
+
+def patch_permute(X: Tensor, B: int, H: int, W: int, ph: int, pw: int, inverse: bool = False, direction: Optional[int] = None) -> Tensor:
+    """MobileViT-v1 unfold (feature-map rows [B*H*W, C] -> token rows [B*P*N, C]) / fold, or their transposes; ``direction`` is a
+    PATCH_* constant and defaults to PATCH_FOLD if ``inverse`` else PATCH_UNFOLD.  Where H or W is not a multiple of the patch the tokens
+    cover the bilinearly up-resized Hn x Wn map (``patch_grid``), as in the reference."""
+    if direction is None:
+        direction = PATCH_FOLD if inverse else PATCH_UNFOLD
+    Hn, Wn = patch_grid(H, W, ph, pw)
+    rows = B * (Hn * Wn if direction in (PATCH_UNFOLD, PATCH_FOLD_T) else H * W)
+    out = torch.empty((rows, X.shape[1]), device=X.device, dtype=X.dtype)
+    _lib().cvb_patch_permute(X.data_ptr(), out.data_ptr(), B, H, W, X.shape[1], ph, pw, int(direction), _stream())
     _count()
     return out
 
@@ -619,6 +631,20 @@ def mha_bwd(QKV: Tensor, O: Tensor, DO: Tensor, LSE: Tensor, B: int, S: int, H: 
                     _p(attn_mask), _p(key_padding_mask), DQKV.data_ptr(), DQKV.stride(0), _stream())
     _count()
     return DQKV
+
+
+MHA_SMEM_MAX = 226 * 1024  # csrc/mha.cu: the dynamic shared memory one attention CTA may opt into
+
+
+def mha_max_seq(head_dim: int, backward: bool = True) -> Optional[int]:
+    """the longest sequence cvb_mha_fwd / cvb_mha_bwd take at ``head_dim``, or None (any length) for head_dim 64, whose long sequences run on
+    the streaming kernels.  Every other head dim runs on the mma.sync kernels, which keep one head's Q, K, V (and dO, LSE, D in the backward)
+    in shared memory, the head dim padded to 16 / 32 / 48 / 64 and S to a multiple of 64 (csrc/mha.cu mha_smem_bytes)."""
+    if head_dim == 64:
+        return None
+    ld = next(p for p in (16, 32, 48, 64) if head_dim <= p) + 8
+    per64 = 64 * ((4 * ld * 2 + 8) if backward else 3 * ld * 2)
+    return MHA_SMEM_MAX // per64 * 64
 
 
 def ln_bwd(V: Tensor, X: Tensor, ln: Tensor, gamma: Tensor, col_stats: Tensor, DRES: Optional[Tensor] = None,
